@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- image-pairs/sec of the DeMoN two-view inference path at 256x192 (BASELINE.json `metric`).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config b64|b1|refine1024]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config b64|b1|refine1024] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A step = one pass of the full pipeline (bootstrap + 3 x iterative + refinement, examples/example.py:87-99)
@@ -9,7 +9,7 @@ over one batch of 64 synthetic pairs per GPU: BASELINE.json configs[2] at N=1, c
 GPUs) at N=8 -- weak scaling, pairs are independent, the only collective is ONE NCCL all-gather (one call) of the final
 depth / motion tensors, inside the timed region and inside the CUDA graph of the step.
 --config b1 = configs[1] (one pair per step: latency); --config refine1024 = configs[4] (RefinementNet at 1024x768,
-batch 8; a step = one RefinementNet.eval).  The driver runs the default; the other two are recorded under profiles/.
+batch 8; a step = one RefinementNet.eval).
 
 One JSON line on stdout (rank 0):
   value        pairs/s, inputs resident in HBM, whole job; `--inflight` (default 2) batches per GPU are in flight on their
@@ -20,8 +20,12 @@ One JSON line on stdout (rank 0):
   roofline     the dominant kernel timed with CUDA events around its launches on the launching stream in a second,
                single-stream timed region; peak = a TF32 GEMM measured on this GPU in this run
   cpu_baseline the CPU oracle (torch-CPU fp32 + C geometry ops) on a bounded sample, host cores stated
-  check        after the timed regions: demon_check_errors() (a timed-out tcgen05 pipeline wait would have produced
+  check        after the timed regions: demon_check_errors() (a timed-out tensor-core pipeline wait would have produced
                garbage) and one sample of the LAST timed step against the CPU oracle (inverse-depth L1-rel)
+`--dump-outputs DIR` writes what the last step of the timed region behind `value` computed, as float32 .npy files
+(predict_depth0, predict_rotation, predict_translation; predict_depth0 for refine1024); above 64 MB in all, a fixed seeded
+subset of the pairs, with their indices in sample_indices.npy.  The inputs are seeded, so two
+builds run with the same arguments can be compared output for output.
 `--impl reference` times that CPU path alone with the same --steps / --warmup, 8 pairs per step (TensorFlow 1.4 cannot
 be installed here, DESIGN.md section 5).
 """
@@ -44,7 +48,7 @@ import torch
 PER_GPU_BATCH = 64
 ITERATIONS = 3
 METRIC = "image_pairs_per_sec_256x192"
-N_INPUT_SETS = 4     # rotating input batches: 4 x 75.5 MB > 126 MB L2 (plus a ~2.7 GB activation workspace per step)
+N_INPUT_SETS = 4     # rotating input batches: 4 x 75.5 MB > 50 MB L2 (plus a ~2.7 GB activation workspace per step)
 REF_PAIRS_PER_STEP = 8
 # conv1 / conv2 of netFlow2 and netDM2 depend only on the image pair: the pipeline runs them once per call instead of once
 # per iteration (2 nets x 2 saved iterations x 221.7 MMAC).  Throughput and roofline figures keep counting the
@@ -60,12 +64,13 @@ def peaks():
     if os.path.isfile(path):
         try:
             p = json.load(open(path))
-            burst = float(p.get("bf16_tflops", 1590.0))
-            return {"hbm_gbs": float(p.get("hbm_gbs", 6650.0)), "bf16_tflops": burst,
+            burst = float(p.get("bf16_tflops", 989.0))
+            return {"hbm_gbs": float(p.get("hbm_gbs", 3350.0)), "bf16_tflops": burst,
                     "bf16_tflops_sustained": float(p.get("bf16_tflops_sustained", burst)), "source": "measured"}
         except (OSError, ValueError, TypeError):
             pass
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # H100 SXM data sheet (dense, 700 W): never reached, only the denominator when nothing was measured
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 def measure_tf32_peak(dev, seconds=1.0):
@@ -100,7 +105,7 @@ def measure_tf32_peak(dev, seconds=1.0):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -260,12 +265,49 @@ def l1_rel(a, r):
     return float(np.abs(a - r).sum() / np.abs(r).sum())
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(directory, arrays, limit=DUMP_LIMIT_BYTES):
+    """The arrays a caller of the timed path receives (all with the batch as leading dimension), as float32 .npy files.
+    Over `limit` bytes in all, a fixed seeded subset of the batch is written instead (the same rows of every array, in
+    ascending order) and its row indices go to sample_indices.npy (float64, exact integers).  The size is checked before
+    anything is written."""
+    arrs = {name: (t.detach().float().cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t, dtype=np.float32))
+            for name, t in arrays.items()}
+    n = {a.shape[0] for a in arrs.values()}
+    assert len(n) == 1, "dumped arrays must share the leading (batch) dimension"
+    n = n.pop()
+    total = sum(a.nbytes for a in arrs.values())
+    if total > limit:
+        per_row = total // n
+        k = max(1, int((limit - 8 * n) // per_row))
+        idx = np.sort(np.random.RandomState(0).choice(n, k, replace=False))
+        arrs = {name: a[idx] for name, a in arrs.items()}
+        arrs["sample_indices"] = idx.astype(np.float64)
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrs.items():
+        np.save(os.path.join(directory, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64 if a.dtype == np.float64 else np.float32))
+
+
+def device_info(index):
+    """Name, power limit and maximum SM clock of the GPU the numbers were measured on."""
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None, "sm_max_mhz": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        info["power_limit_w"], info["sm_max_mhz"] = float(out[0]), float(out[1])
+    except Exception:
+        pass
+    return info
+
+
 def layer_roofline(lib, net_ptr, lm, B, steps, ms_local, precision, tf32_peak, pk):
     """Per-layer CUDA-event times (demon_net_profile_*) folded per kernel family -> roofline of the dominant kernel."""
     FAMILIES = {0: "conv_simt_kernel (fp32 CUDA-core implicit GEMM)",
-                1: "conv_tc_kernel (tcgen05 kind::tf32, operands in shared memory, %s)" % precision,
-                2: "conv_tc_halo_kernel<halo> (tcgen05 kind::tf32, TMA halo tile, A operand in TMEM, %s)" % precision,
-                3: "conv_tc_halo_kernel<per-tap> (tcgen05 kind::tf32, per-shift tiles, A operand in TMEM, %s)" % precision}
+                1: "conv_tc_kernel (unused)",
+                2: "conv_tc_halo_kernel<halo> (wgmma tf32, TMA halo tile, A operand in registers, %s)" % precision,
+                3: "conv_tc_halo_kernel<per-tap> (wgmma tf32, per-shift tiles, A operand in registers, %s)" % precision}
     fam = {k: [0.0, 0.0, 0] for k in FAMILIES}   # ms, MACs, launches
     top = []
     for i in range(lib.demon_net_num_layers(net_ptr)):
@@ -290,11 +332,11 @@ def layer_roofline(lib, net_ptr, lm, B, steps, ms_local, precision, tf32_peak, p
                          "for reference %s bf16 sustained %.1f / 2 = %.1f" % (tf32_peak, pk["source"], pk["bf16_tflops_sustained"], pk["bf16_tflops_sustained"] / 2))
         else:
             peak = pk["bf16_tflops_sustained"] / 2.0
-            peak_note = "DERIVED: %s bf16 sustained %.1f TF/s / 2 (kind::tf32 issues at half the bf16 rate); the TF32 GEMM measurement failed" % (pk["source"], pk["bf16_tflops_sustained"])
+            peak_note = "DERIVED: %s bf16 %.1f TF/s / 2 (tf32 issues at half the bf16 rate); the TF32 GEMM measurement failed" % (pk["source"], pk["bf16_tflops_sustained"])
         peak_note += "; %s spends %d tensor MAC(s) per algorithmic MAC, so frac <= %.2f by construction" % (precision, mult, 1.0 / mult)
     else:
-        peak = 2 * 128 * 148 * 1.965e9 / 1e12     # fp32 FFMA peak at clocks.max.sm
-        peak_note = "fp32 FFMA peak 128 FMA/clk/SM x 148 SMs x 1965 MHz (no measured fp32 figure in MEASURED_PEAKS.json)"
+        peak = 67.0     # H100 SXM data sheet fp32
+        peak_note = "H100 SXM data sheet fp32 peak 67 TFLOP/s (700 W card; no measured fp32 figure)"
     return {"bound": "tensor", "kernel": FAMILIES[dom], "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
             "frac": achieved / peak if peak else None, "traffic": None,
             "algorithmic_flops_per_launch": 2.0 * d_macs / max(1, d_launches), "avg_launch_ms": d_ms / max(1, d_launches),
@@ -305,26 +347,6 @@ def layer_roofline(lib, net_ptr, lm, B, steps, ms_local, precision, tf32_peak, p
                         for k in sorted(fam, key=lambda k: -fam[k][0]) if fam[k][2]],
             "top_layers_ms_per_step": [{"layer": n, "ms": t / steps, "tflops": 2.0 * m / (t / 1e3) / 1e12 if t > 0 else 0, "kernel": k}
                                        for t, n, m, k in top[:8]]}, dom
-
-
-def attach_traffic(roofline, dom):
-    """DRAM traffic of the heaviest launch of the dominant kernel, from the committed `ncu --set full` capture."""
-    for fname in ("r02_traffic.json", "r01_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", fname)
-        if not os.path.isfile(tpath):
-            continue
-        tj = json.load(open(tpath))
-        key = {2: "refine0_upconv", 1: "refine3_upconv", 3: "refine3_upconv"}.get(dom)
-        if key not in tj:
-            key = {2: "refine0_upconv", 1: "refine2_upconv", 3: "refine2_upconv"}.get(dom)
-        if key in tj:
-            roofline["traffic"] = {"bytes": tj[key], "launch": key,
-                                   "algorithmic_bytes": {"refine0_upconv": 2 * 64 * 96 * 128 * 128 * 4 + 4 * 4 * 128 * 32 * 4,
-                                                         "refine2_upconv": 64 * 24 * 32 * 256 * 4 + 64 * 48 * 64 * 64 * 4,
-                                                         # netFlow2/refine3/upconv: concat4 [64,12,16,576] in, [64,24,32,128] out, 4x4 kernel
-                                                         "refine3_upconv": 64 * 12 * 16 * 576 * 4 + 64 * 24 * 32 * 128 * 4 + 16 * 128 * 576 * 4}.get(key),
-                                   "source": "profiles/%s (one launch at batch 64, dram__bytes_read.sum + dram__bytes_write.sum of an ncu --set full capture)" % fname}
-            return
 
 
 def bench_refine(args, rank, local, world, dev, lib, precision):
@@ -353,6 +375,8 @@ def bench_refine(args, rank, local, world, dev, lib, precision):
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1)
     launches = int(lib.demon_launch_count() - l0)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"predict_depth0": out["predict_depth0"]})
     _lib.check(lib.demon_net_profile_begin(net.ptr))
     e2, e3 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e2.record()
@@ -383,9 +407,9 @@ def bench_refine(args, rank, local, world, dev, lib, precision):
             "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f32" if precision == "fp32" else ("tf32x3" if precision == "3xtf32" else "tf32"), "data": "synthetic",
             "config": {"workload": "BASELINE.json configs[4]: RefinementNet (depth_refine_block) at 1024x768, batch 8, 1 GPU", "precision": precision,
-                       "flops_per_image": flops_img, "l2": "4 rotating input batches of 75.5 MB (> 126 MB L2) and a %.2f GB activation workspace"
+                       "flops_per_image": flops_img, "l2": "4 rotating input batches of 75.5 MB (> 50 MB L2) and a %.2f GB activation workspace"
                                                           % (lib.demon_net_workspace_bytes(net.ptr) / 1e9)},
-            "gpu_launches": launches, "clocks": clocks, "roofline": roofline, "algorithmic_tflops": flops_img * value / 1e12,
+            "device": device_info(local), "gpu_launches": launches, "clocks": clocks, "roofline": roofline, "algorithmic_tflops": flops_img * value / 1e12,
             "e2e": {"value": B * n_e2e / dt, "unit": "images/s", "h2d_bytes_per_step": int(im_h.nbytes + d2_h.nbytes), "d2h_bytes_per_step": int(B * H * Wd * 4),
                     "api": "RefinementNet.eval(numpy, numpy) -> numpy: pageable host arrays, copies and synchronisation inside the call"},
             "check": {"tc_timeouts": 0, "l1_rel_vs_cpu_oracle_fp32": l1_rel(res["predict_depth0"][:1], ref), "sample": "image 0 of the last e2e step"}}
@@ -404,7 +428,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--inflight", type=int, default=None, help="batches in flight per GPU (pipelines on their own streams); default 2, 1 with --config b1")
     ap.add_argument("--no-step-graph", action="store_true", help="do not capture pipeline + all-gather in one CUDA graph per step")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32) for output-for-output comparisons")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3)
 
     rank = int(os.environ.get("RANK", "0"))
@@ -517,6 +545,10 @@ def main():
         launches += args.steps * lib.demon_net_pipeline_launches(net.ptr, ITERATIONS)
     last_k = (args.steps - 1) % NF
     last_in = inputs[((args.steps - 1) // NF) % N_INPUT_SETS]
+    if args.dump_outputs and rank == 0:
+        gl = gathers[last_k]
+        dump_outputs(args.dump_outputs, {"predict_depth0": gl.depth_all.flatten(0, 1), "predict_rotation": gl.rotation_all.flatten(0, 1),
+                                         "predict_translation": gl.translation_all.flatten(0, 1)})
     last_depth0 = gathers[last_k].depth_all[rank, 0, 0].cpu().numpy()       # sample 0 of this rank's shard, last timed step
     last_trans0 = gathers[last_k].translation_all[rank, 0].cpu().numpy()
     _lib.check_errors()
@@ -549,8 +581,6 @@ def main():
 
     tf32_peak = measure_tf32_peak(dev) if rank == 0 else None
     roofline, dom = layer_roofline(lib, net.ptr, W.layer_macs(), B, args.steps, ms_local, precision, tf32_peak, peaks())
-    if B == PER_GPU_BATCH:
-        attach_traffic(roofline, dom)
 
     # ---- end to end from pinned host buffers, copies inside the timed region -----------------------------------------
     NE = NF
@@ -658,7 +688,7 @@ def main():
                                        "(bootstrap + 3x iterative + refinement), %d GPU(s)" % ((1 if B == 1 else 2) if world == 1 else 3, B, world),
                            "global_batch": world * B, "precision": precision, "iterations": ITERATIONS,
                            "l2": "%d rotating input batches of %.1f MB%s and a %.2f GB activation workspace rewritten every step"
-                                 % (N_INPUT_SETS, B * 6 * 192 * 256 * 4 / 1e6, " (> 126 MB L2)" if B >= 32 else "",
+                                 % (N_INPUT_SETS, B * 6 * 192 * 256 * 4 / 1e6, " (> 50 MB L2)" if B >= 32 else "",
                                     lib.demon_net_workspace_bytes(net.ptr) / 1e9),
                            "parallelism": "dp%d, one NCCL all-gather (one call) of depth0+motion per step" % world if world > 1 else "single GPU",
                            "step_graph": graph_note,
@@ -668,7 +698,8 @@ def main():
                            "executed_flops_per_pair": alg_flops - 2.0 * hoisted_macs_per_pair(),
                            "flops_note": "value, algorithmic_tflops and roofline count the reference's algorithmic work; conv1/conv2 of the "
                                          "iterative nets are loop invariant and executed once per call (bit identical)"},
-                "gpu_launches": launches, "clocks": clocks, "e2e": e2e, "e2e_u8": e2e_u8, "roofline": roofline, "cpu_baseline": cpu, "check": check,
+                "device": device_info(local), "gpu_launches": launches, "clocks": clocks, "e2e": e2e, "e2e_u8": e2e_u8, "roofline": roofline,
+                "cpu_baseline": cpu, "check": check,
                 "gather_ms": gather_ms, "algorithmic_tflops": alg_flops * value / 1e12}
         print(json.dumps(line), flush=True)
     if world > 1:

@@ -1,4 +1,4 @@
-"""demon_b200 -- B200-native (sm_100a) DeMoN two-view depth+motion inference path.
+"""demon_b200 -- H100-native (sm_90a) DeMoN two-view depth+motion inference path.
 
   demon_b200.lmbspecialops       mirror of the reference op binding (warp2d, depth_to_flow, ...)
   demon_b200.networks_original   mirror of depthmotionnet.networks_original (BootstrapNet, ...)

@@ -116,7 +116,7 @@ def load():
 
 
 def check_errors():
-    """Synchronise the current device and raise if a tcgen05 kernel's bounded pipeline wait timed out since the last
+    """Synchronise the current device and raise if a tensor-core kernel's bounded pipeline wait timed out since the last
     check (its outputs are garbage) or a CUDA error is pending.  Cheap enough to call once per batch."""
     check(load().demon_check_errors())
 

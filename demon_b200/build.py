@@ -1,6 +1,6 @@
-"""Builds libdemon_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Builds libdemon_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The library and its objects (demon_b200/lib/) are build products and stay out of git.
 """
 import os
 import subprocess
@@ -11,7 +11,8 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB_DIR = os.path.join(_HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libdemon_b200.so")
 SOURCES = ["geometry_ops.cu", "metrics.cu", "training_ops.cu", "conv_simt.cu", "conv_tc.cu", "conv_tc_halo.cu", "net.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -55,14 +56,14 @@ def build(force=False, verbose=False):
         raise RuntimeError("nvcc failed")
     # the driver API (cuTensorMapEncodeTiled) is resolved at run time through cudaGetDriverEntryPoint
     tmp = LIB_PATH + ".tmp"   # link beside the target and rename: a snapshot never sees a half-written library
-    subprocess.check_call([nvcc, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+    subprocess.check_call([nvcc, "-shared", "-o", tmp] + objs + GENCODE)
     os.replace(tmp, LIB_PATH)
     return LIB_PATH
 
 
 def build_variant(name, extra_flags):
-    """Diagnostic builds (e.g. -DDEMON_TC_TIMING_FULL) next to the product library: lib/variants/<name>/libdemon_b200.so,
-    selected at run time with DEMON_B200_LIB."""
+    """Diagnostic builds (extra nvcc flags, e.g. -lineinfo -G) next to the product library:
+    lib/variants/<name>/libdemon_b200.so, selected at run time with DEMON_B200_LIB."""
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     out_dir = os.path.join(LIB_DIR, "variants", name)
     os.makedirs(out_dir, exist_ok=True)
@@ -74,7 +75,7 @@ def build_variant(name, extra_flags):
     if any(p.wait() != 0 for p in procs):
         raise RuntimeError("nvcc failed")
     path = os.path.join(out_dir, "libdemon_b200.so")
-    subprocess.check_call([nvcc, "-shared", "-o", path] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+    subprocess.check_call([nvcc, "-shared", "-o", path] + objs + GENCODE)
     return path
 
 

@@ -1,4 +1,4 @@
-// Shared helpers of the demon_b200 CUDA library (sm_100a only).
+// Shared helpers of the demon_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <atomic>
@@ -45,7 +45,7 @@ extern std::atomic<int64_t> g_launch_count;
 
 // ---- programmatic dependent launch (PDL) ------------------------------------------------------
 // The pipeline is a chain of ~270 short kernels on one stream.  A kernel launched through launch_pdl() may become
-// resident while its predecessor is still draining: its prologue (barrier init, TMEM allocation, tensor-map prefetch,
+// resident while its predecessor is still draining: its prologue (barrier init, tensor-map prefetch,
 // parameter loads, the first weight blocks) overlaps the predecessor's tail, and the launch latency disappears from the
 // chain.  Contract: such a kernel calls pdl_wait() before it reads anything an earlier kernel wrote and before its first
 // global store (buffers are reused along the chain), and every kernel calls pdl_launch_dependents() early so that its

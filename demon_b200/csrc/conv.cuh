@@ -1,5 +1,5 @@
-// Convolution problem descriptor shared by the fp32 SIMT path (conv_simt.cu), the tcgen05 path
-// (conv_tc.cu) and the network plan (net.cu).
+// Convolution problem descriptor shared by the fp32 SIMT path (conv_simt.cu), the tensor-core path
+// (conv_tc_halo.cu) and the network plan (net.cu).
 //
 // Every convolution-like layer of the DeMoN graphs -- the caffe-padded conv2d (helpers.py:70-94), the
 // separable k x 1 / 1 x k pairs (helpers.py:105-153), the k4 s2 transposed conv (blocks_original.py:54-117,

@@ -1,6 +1,6 @@
-// fp32 CUDA-core implicit-GEMM convolution (NHWC) for sm_100a.
+// fp32 CUDA-core implicit-GEMM convolution (NHWC) for sm_90a.
 //
-// Role in the design: (1) the exact-fp32 path for the layers whose shapes do not suit tcgen05 tiles
+// Role in the design: (1) the exact-fp32 path for the layers whose shapes do not suit tensor-core tiles
 // (Cin in {4,6,7,8,9,24}, Cout in {1,2,4,7}, the dense layers) and (2) the on-device fp32 reference
 // the tensor-core path is validated against in tests/.  Classic register-blocked SGEMM structure:
 // 256 threads, a BM x BN output tile (BM*BN = 4096), 4x4 outputs per thread, BK = 16, the A tile

@@ -1,314 +1,13 @@
-// tcgen05 (5th generation tensor core) implicit-GEMM convolution for sm_100a.
-//
-//   GEMM view      D[M = 128 output pixels, N = output channels] += A[M, K = 32 input channels of one tap] * W[K, N]
-//   A operand      NHWC activations.  One TMA box {32 channels, tw, 1, th, tb} of a 5-D view
-//                  {sx*C, W/sx, sy, H/sy, B} of the input slice lands in shared memory as 128 rows of 128 bytes
-//                  (K-major, 128-byte swizzle) -- exactly the canonical UMMA operand layout.  The filter tap and the
-//                  stride only change the box coordinates; pixels outside the image are zero-filled by TMA, which is
-//                  the explicit tf.pad of the reference (helpers.py:78-94).
-//   W operand      packed on the host per (n-tile, tap, 32-channel chunk) as the pre-swizzled shared-memory image,
-//                  fetched with one bulk copy (cp.async.bulk).
-//   precision      3xTF32: W is split on the host into W_hi + W_lo (both TF32-exact), A is split in shared memory by four
-//                  "splitter" warps into A_hi (= the raw fp32 bits, the tensor core ignores the low 13 mantissa bits) and
-//                  A_lo = A - trunc_tf32(A); three MMAs A*W_lo + A_lo*W_hi + A*W_hi accumulate in fp32 in TMEM.  The
-//                  dropped term A_lo*W_lo is ~2^-21 relative.  nsplit = 1 is plain single-pass TF32.
-//   accumulator    TMEM, double buffered (2 x N columns): the epilogue of tile i overlaps the main loop of tile i+1.
-//   epilogue       tcgen05.ld -> bias + leaky ReLU -> NHWC store into the channel slice of the (concat) destination.
-//   schedule       persistent: one CTA per SM loops over (m-tile, n-tile); warp 0 = TMA producer, warp 1 = MMA issuer
-//                  and TMEM owner, warps 2-5 = splitters, warps 6-9 = epilogue; mbarrier pipelines between them.
+// Tensor-core convolution path (sm_90a): the shape rules and the per-device launch state.  The kernel is
+// conv_tc_halo_kernel (conv_tc_halo.cu); layers whose problems the halo planner does not take run on it in per-tap mode.
 #include <cuda.h>
 
 #include <cstring>
 #include <mutex>
-#include <vector>
 
 #include "conv_tc.cuh"
-#include "conv_tc_ptx.cuh"
 
 namespace demon {
-
-namespace {
-
-constexpr int kThreads = 320;
-constexpr int kATileBytes = 128 * 128;   // 128 rows x 32 fp32
-
-struct TcParams {
-  // tiling of the output index space
-  int tw, th, tb;
-  int tiles_x, tiles_y, tiles_b, n_tiles, total_tiles;
-  int ntaps, k_chunks;
-  // `nclass` independent problems share the input, the tiling and the launch (the four sub-pixel classes of a
-  // transposed convolution): class c uses taps [c*ntaps, (c+1)*ntaps), its own weight block and output offset.
-  int nclass;
-  int cls_ooy[4], cls_oox[4];
-  int tap_c[kMaxTaps];   // coordinate offset in dim 0 (rx * in_pitch)
-  int tap_qx[kMaxTaps];  // offset in dim 1 (W / sx)
-  int tap_ry[kMaxTaps];  // coordinate in dim 2 (row parity)
-  int tap_qy[kMaxTaps];  // offset in dim 3 (H / sy)
-  // weights
-  const unsigned char* w;
-  int n_tile;            // UMMA N
-  int nsplit;            // 1 or 3
-  int w_stage_bytes;     // bytes of one (n-tile, tap, chunk) weight block: nsplit==3 ? 2 : 1 times n_tile*128
-  int stages;
-  int stage_bytes;       // smem bytes of one pipeline stage
-  // epilogue
-  float* out;
-  int out_pitch, B, Ho, Wo, Hfull, Wfull, osy, osx, Cout;
-  const float* bias;
-  int leaky;
-  int* err;
-};
-
-__device__ __forceinline__ void decode_tile(const TcParams& p, int tile, int& cls, int& nt, int& n0, int& y0, int& x0) {
-  nt = tile % p.n_tiles;
-  int m = tile / p.n_tiles;
-  cls = m % p.nclass;
-  m /= p.nclass;
-  const int xb = m % p.tiles_x;
-  m /= p.tiles_x;
-  const int yb = m % p.tiles_y;
-  const int bb = m / p.tiles_y;
-  n0 = bb * p.tb; y0 = yb * p.th; x0 = xb * p.tw;
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
-  extern __shared__ __align__(1024) unsigned char smem_raw[];
-  // stage layout: [A 16 KB][A_lo 16 KB][W_hi n_tile*128][W_lo n_tile*128]; every piece 1024-byte aligned
-  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ __align__(8) uint64_t bars[3 * 8 + 4];   // full[8], split[8], empty[8], accum_full[2], accum_empty[2]
-  __shared__ uint32_t tmem_base_smem;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int S = p.stages;
-  const uint32_t full0 = smem_u32(&bars[0]), split0 = smem_u32(&bars[8]), empty0 = smem_u32(&bars[16]);
-  const uint32_t afull0 = smem_u32(&bars[24]), aempty0 = smem_u32(&bars[26]);
-  // stacked 3xTF32 (N <= 128): D[:, 0:2N] (+)= A_hi * [W_hi ; W_lo] as ONE UMMA of N' = 2N, D[:, N:2N] += A_lo * W_hi, the
-  // epilogue adds the halves -- two instructions per K8 step instead of three (conv_tc_halo.cu has the measurements)
-  const bool stacked = (p.nsplit == 3) && (p.n_tile <= 128);
-  const int acc_w = stacked ? 2 * p.n_tile : p.n_tile;
-  const uint32_t tmem_cols = 2 * acc_w <= 32 ? 32 : (2 * acc_w <= 64 ? 64 : (2 * acc_w <= 128 ? 128 : (2 * acc_w <= 256 ? 256 : 512)));
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmap) : "memory");
-    for (int s = 0; s < S; ++s) {
-      mbar_init(full0 + 8 * s, 1);
-      mbar_init(split0 + 8 * s, 4);
-      mbar_init(empty0 + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(afull0 + 8 * a, 1);
-      mbar_init(aempty0 + 8 * a, 4);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(smem_u32(&tmem_base_smem), tmem_cols);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-  const int ksteps = p.ntaps * p.k_chunks;
-  const uint32_t w_half = (uint32_t)p.n_tile * 128u;
-
-  if (warp == 0) {
-    // ===== TMA producer ==============================================================================================
-    if (elect_one_sync()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint32_t tx = kATileBytes + (uint32_t)p.w_stage_bytes;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        int cls, nt, n0, y0, x0;
-        decode_tile(p, tile, cls, nt, n0, y0, x0);
-        const unsigned char* wsrc = p.w + (size_t)(cls * p.n_tiles + nt) * ksteps * p.w_stage_bytes;
-        for (int ks = 0; ks < ksteps; ++ks) {
-          const int tap = cls * p.ntaps + ks / p.k_chunks, kc = ks % p.k_chunks;
-          mbar_wait(empty0 + 8 * stage, phase ^ 1, p.err);
-          const uint32_t sbase = smem_u32(smem + (size_t)stage * p.stage_bytes);
-          mbar_expect_tx(full0 + 8 * stage, tx);
-          tma_load_5d(sbase, &tmap, full0 + 8 * stage, p.tap_c[tap] + kc * 32, x0 + p.tap_qx[tap], p.tap_ry[tap], y0 + p.tap_qy[tap], n0);
-          bulk_load(sbase + 2 * kATileBytes, wsrc + (size_t)ks * p.w_stage_bytes, (uint32_t)p.w_stage_bytes, full0 + 8 * stage);
-          if (++stage == S) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer ================================================================================================
-    if (elect_one_sync()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint32_t idesc = umma_idesc_tf32(p.n_tile), idesc2 = umma_idesc_tf32(2 * p.n_tile);
-      int it = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-        const int a = it & 1;
-        mbar_wait(aempty0 + 8 * a, ((it >> 1) & 1) ^ 1, p.err);   // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(a * acc_w);
-        for (int ks = 0; ks < ksteps; ++ks) {
-          mbar_wait(full0 + 8 * stage, phase, p.err);
-          tc_fence_after();
-          const uint32_t sbase = smem_u32(smem + (size_t)stage * p.stage_bytes);
-          const uint64_t a_hi = umma_desc_sw128(sbase), a_lo = umma_desc_sw128(sbase + kATileBytes);
-          const uint64_t w_hi = umma_desc_sw128(sbase + 2 * kATileBytes), w_lo = umma_desc_sw128(sbase + 2 * kATileBytes + w_half);
-          // the two products on the raw A image go first: they overlap the splitter warps' work on A_lo
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {   // 4 x K8 = 32 channels; +32 bytes per K8 step inside the swizzled row
-            const uint64_t adv = (uint64_t)(2 * j);
-            if (stacked) {
-              umma_tf32(d_tmem, a_hi + adv, w_hi + adv, idesc2, (ks | j) != 0);
-            } else {
-              if (p.nsplit == 3) umma_tf32(d_tmem, a_hi + adv, w_lo + adv, idesc, (ks | j) != 0);
-              umma_tf32(d_tmem, a_hi + adv, w_hi + adv, idesc, (p.nsplit == 3) ? 1u : (uint32_t)((ks | j) != 0));
-            }
-          }
-          if (p.nsplit == 3) {
-            mbar_wait(split0 + 8 * stage, phase, p.err);
-            tc_fence_after();
-            const uint32_t d_lo = stacked ? d_tmem + (uint32_t)p.n_tile : d_tmem;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) umma_tf32(d_lo, a_lo + (uint64_t)(2 * j), w_hi + (uint64_t)(2 * j), idesc, 1);
-          }
-          umma_commit(empty0 + 8 * stage);                 // frees the smem stage when these MMAs are done
-          if (ks == ksteps - 1) umma_commit(afull0 + 8 * a);   // accumulator complete
-          if (++stage == S) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp < 6) {
-    // ===== splitters: A_lo = A - trunc_tf32(A) =======================================================================
-    if (p.nsplit == 3) {
-      const int t = threadIdx.x - 64;   // 0..127
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        for (int ks = 0; ks < ksteps; ++ks) {
-          mbar_wait(full0 + 8 * stage, phase, p.err);
-          __syncwarp();
-          const uint32_t sb = smem_u32(smem + (size_t)stage * p.stage_bytes);
-          split_region(sb, sb + kATileBytes, kATileBytes / 16, t);
-          fence_proxy_async();   // generic-proxy writes -> visible to the tensor core (async proxy)
-          __syncwarp();
-          if (lane == 0) mbar_arrive(split0 + 8 * stage);
-          if (++stage == S) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    // ===== epilogue: TMEM -> registers -> bias, leaky ReLU -> NHWC slice ==============================================
-    const int q = warp & 3;                 // TMEM lane quadrant this warp may access
-    const int m = q * 32 + lane;            // GEMM row = output pixel of the tile
-    const int xl = m % p.tw, yl = (m / p.tw) % p.th, nl = m / (p.tw * p.th);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-      int cls, nt, n0, y0, x0;
-      decode_tile(p, tile, cls, nt, n0, y0, x0);
-      const int a = it & 1;
-      mbar_wait(afull0 + 8 * a, (it >> 1) & 1, p.err);
-      __syncwarp();
-      tc_fence_after();
-      const int n = n0 + nl, oy = y0 + yl, ox = x0 + xl;
-      const bool valid = n < p.B && oy < p.Ho && ox < p.Wo;
-      float* orow = p.out + ((size_t)(n * p.Hfull + oy * p.osy + p.cls_ooy[cls]) * p.Wfull + ox * p.osx + p.cls_oox[cls]) * p.out_pitch;
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * acc_w);
-      const int cbase = nt * p.n_tile;
-      for (int c0 = 0; c0 < p.n_tile; c0 += 32) {
-        uint32_t v[32];
-        const int ncol = (p.n_tile - c0) >= 32 ? 32 : 16;
-        if (ncol == 32) tmem_ld_x32(t_row + c0, v); else tmem_ld_x16(t_row + c0, v);
-        if (stacked) {   // big term + small terms
-          uint32_t u[32];
-          if (ncol == 32) tmem_ld_x32(t_row + p.n_tile + c0, u); else tmem_ld_x16(t_row + p.n_tile + c0, u);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(u[i]));
-        }
-        tmem_ld_wait();
-        if (valid) {
-#pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            const int col = cbase + c0 + 4 * g;
-            if (4 * g < ncol && col < p.Cout) {
-              const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col));
-              float4 o;
-              o.x = __uint_as_float(v[4 * g + 0]) + b.x;
-              o.y = __uint_as_float(v[4 * g + 1]) + b.y;
-              o.z = __uint_as_float(v[4 * g + 2]) + b.z;
-              o.w = __uint_as_float(v[4 * g + 3]) + b.w;
-              if (p.leaky) {
-                o.x = fmaxf(0.1f * o.x, o.x); o.y = fmaxf(0.1f * o.y, o.y);
-                o.z = fmaxf(0.1f * o.z, o.z); o.w = fmaxf(0.1f * o.w, o.w);
-              }
-              *reinterpret_cast<float4*>(orow + col) = o;
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(aempty0 + 8 * a);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
-  }
-}
-
-// ---- host side ------------------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
-
-int floor_div(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
-int pow2_ceil(int v) { int r = 1; while (r < v) r <<= 1; return r; }
-
-float tf32_round(float x) {   // round to nearest even onto 10 explicit mantissa bits
-  uint32_t u;
-  memcpy(&u, &x, 4);
-  if ((u & 0x7F800000u) == 0x7F800000u) return x;
-  u += 0x00000FFFu + ((u >> 13) & 1u);
-  u &= 0xFFFFE000u;
-  float r;
-  memcpy(&r, &u, 4);
-  return r;
-}
-
-struct Tiling { int tw, th, tb, tiles_x, tiles_y, tiles_b; };
-
-Tiling choose_tiling(int B, int Ho, int Wo) {
-  Tiling best{};
-  long best_tiles = -1;
-  const int tw = std::min(128, pow2_ceil(Wo));
-  for (int th = 1; th * tw <= 128; th <<= 1) {
-    const int tb = 128 / (tw * th);
-    const long tiles = (long)ceil_div(Wo, tw) * ceil_div(Ho, th) * ceil_div(B, tb);
-    if (best_tiles < 0 || tiles <= best_tiles) {   // ties: larger th (fewer images per tile)
-      best_tiles = tiles;
-      best = Tiling{tw, th, tb, ceil_div(Wo, tw), ceil_div(Ho, th), ceil_div(B, tb)};
-    }
-  }
-  return best;
-}
-
-int num_sms() { return tc_device_state().sms; }
-
-}  // namespace
 
 bool tc_layer_supported(const ConvProblem& p) {
   if (p.Cin < 32 || (p.Cin % 32) != 0) return false;
@@ -320,80 +19,6 @@ bool tc_layer_supported(const ConvProblem& p) {
   if (p.scale != nullptr) return false;
   if (p.Ho != p.Hi / p.sy || p.Wo != p.Wi / p.sx) return false;
   return true;
-}
-
-int tc_layer_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts, int nclass, int precision) {
-  DEMON_REQUIRE(nclass >= 1 && nclass <= 4, "tc_layer_prepare: nclass %d", nclass);
-  const ConvProblem& p = probs[0];
-  for (int c = 0; c < nclass; ++c) {
-    DEMON_REQUIRE(tc_layer_supported(probs[c]), "tc_layer_prepare: unsupported shape");
-    DEMON_REQUIRE(probs[c].ntaps == p.ntaps && probs[c].in == p.in && probs[c].Cout == p.Cout, "tc_layer_prepare: classes must share the input");
-  }
-  DEMON_REQUIRE(nclass * p.ntaps <= kMaxTaps, "tc_layer_prepare: too many taps");
-  t.nclass = nclass;
-  t.nsplit = (precision == DEMON_PREC_TF32) ? 1 : 3;
-  const Tiling tl = choose_tiling(p.B, p.Ho, p.Wo);
-  t.tw = tl.tw; t.th = tl.th; t.tb = tl.tb;
-  const int m_tiles = tl.tiles_x * tl.tiles_y * tl.tiles_b * nclass;
-  // N tile: as wide as one UMMA allows, narrowed (down to 64) while the layer would leave SMs idle
-  const int cout16 = (p.Cout + 15) / 16 * 16;
-  int n_tile = cout16 <= 256 ? cout16 : 256;
-  while (n_tile >= 128 && (n_tile % 32) == 0 && m_tiles * ceil_div(p.Cout, n_tile) < num_sms()) n_tile /= 2;
-  t.n_tile = n_tile;
-  t.n_tiles = ceil_div(p.Cout, t.n_tile);
-  t.k_chunks = p.Cin / 32;
-  const int w_block = t.n_tile * 128 * (t.nsplit == 3 ? 2 : 1);
-  const int stage_bytes = 2 * kATileBytes + 2 * t.n_tile * 128;
-  t.stages = std::min(8, (220 * 1024) / stage_bytes);
-  DEMON_REQUIRE(t.stages >= 2, "tc_layer_prepare: not enough shared memory for two stages");
-  t.smem_bytes = t.stages * stage_bytes + 1024;
-
-  // ---- weights: per (class, n-tile, tap, chunk): [W_hi | W_lo], each n_tile rows of 32 fp32, K-major, pre-swizzled ----
-  const size_t total = (size_t)nclass * t.n_tiles * p.ntaps * t.k_chunks * w_block;
-  std::vector<unsigned char> packed(total, 0);
-  for (int cls = 0; cls < nclass; ++cls)
-    for (int nt = 0; nt < t.n_tiles; ++nt)
-      for (int tap = 0; tap < p.ntaps; ++tap)
-        for (int kc = 0; kc < t.k_chunks; ++kc) {
-          unsigned char* blk = packed.data() + ((size_t)((cls * t.n_tiles + nt) * p.ntaps + tap) * t.k_chunks + kc) * w_block;
-          for (int r = 0; r < t.n_tile; ++r) {
-            const int co = nt * t.n_tile + r;
-            for (int k = 0; k < 32; ++k) {
-              float w = 0.f;
-              if (co < p.Cout) w = w_hosts[cls][((size_t)tap * p.Cin + kc * 32 + k) * p.Cout_pad + co];
-              const float hi = (t.nsplit == 3) ? tf32_round(w) : w;
-              const float lo = w - hi;
-              const size_t off = (size_t)r * 128 + (size_t)(((k >> 2) ^ (r & 7)) << 4) + (size_t)(k & 3) * 4;
-              memcpy(blk + off, &hi, 4);
-              if (t.nsplit == 3) memcpy(blk + (size_t)t.n_tile * 128 + off, &lo, 4);
-            }
-          }
-        }
-  void* dw = nullptr;
-  DEMON_CHECK_CUDA(cudaMalloc(&dw, total));
-  DEMON_CHECK_CUDA(cudaMemcpy(dw, packed.data(), total, cudaMemcpyHostToDevice));
-  t.w_packed = dw;
-
-  // ---- TMA descriptor of the input slice: {sx*C, W/sx, sy, H/sy, B} --------------------------------------------------
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) return fail(DEMON_E_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
-  const cuuint64_t cp = (cuuint64_t)p.in_pitch;
-  cuuint64_t gdim[5] = {(cuuint64_t)(p.sx - 1) * cp + (cuuint64_t)p.Cin, (cuuint64_t)(p.Wi / p.sx), (cuuint64_t)p.sy,
-                        (cuuint64_t)(p.Hi / p.sy), (cuuint64_t)p.B};
-  cuuint64_t gstr[4] = {(cuuint64_t)p.sx * cp * 4, (cuuint64_t)p.Wi * cp * 4, (cuuint64_t)p.sy * p.Wi * cp * 4,
-                        (cuuint64_t)p.Hi * p.Wi * cp * 4};
-  cuuint32_t box[5] = {32, (cuuint32_t)t.tw, 1, (cuuint32_t)t.th, (cuuint32_t)t.tb};
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUtensorMap map;
-  CUresult r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, const_cast<float*>(p.in), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    return fail(DEMON_E_CUDA, "cuTensorMapEncodeTiled failed (%d): dims {%llu,%llu,%llu,%llu,%llu} box {%u,%u,%u,%u,%u}", (int)r,
-                (unsigned long long)gdim[0], (unsigned long long)gdim[1], (unsigned long long)gdim[2], (unsigned long long)gdim[3],
-                (unsigned long long)gdim[4], box[0], box[1], box[2], box[3], box[4]);
-  static_assert(sizeof(CUtensorMap) == 128, "CUtensorMap is 128 bytes");
-  memcpy(t.tmap_host, &map, 128);
-  return DEMON_OK;
 }
 
 void tc_layer_free(TcLayer& t) {
@@ -416,56 +41,14 @@ TcDeviceState& tc_device_state() {
     s.device = dev;
     int sms = 0;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    s.sms = sms > 0 ? sms : 148;
+    s.sms = sms > 0 ? sms : 132;
     if (cudaMalloc(&s.err_dev, sizeof(int)) == cudaSuccess) cudaMemset(s.err_dev, 0, sizeof(int));
     else s.err_dev = nullptr;
   }
   return s;
 }
 
-int conv_tc_launch(const TcLayer& t, const ConvProblem* probs, cudaStream_t stream) {
-  const ConvProblem& p = probs[0];
-  TcParams prm;
-  memset(&prm, 0, sizeof(prm));
-  const Tiling tl = choose_tiling(p.B, p.Ho, p.Wo);
-  prm.tw = t.tw; prm.th = t.th; prm.tb = t.tb;
-  prm.tiles_x = tl.tiles_x; prm.tiles_y = tl.tiles_y; prm.tiles_b = tl.tiles_b;
-  prm.n_tiles = t.n_tiles;
-  prm.nclass = t.nclass;
-  prm.total_tiles = tl.tiles_x * tl.tiles_y * tl.tiles_b * t.n_tiles * t.nclass;
-  prm.ntaps = p.ntaps; prm.k_chunks = t.k_chunks;
-  for (int c = 0; c < t.nclass; ++c) {
-    const ConvProblem& q = probs[c];
-    prm.cls_ooy[c] = q.ooy; prm.cls_oox[c] = q.oox;
-    for (int i = 0; i < q.ntaps; ++i) {
-      const int qy = floor_div(q.dy[i], q.sy), qx = floor_div(q.dx[i], q.sx);
-      const int e = c * q.ntaps + i;
-      prm.tap_qy[e] = qy; prm.tap_ry[e] = q.dy[i] - qy * q.sy;
-      prm.tap_qx[e] = qx; prm.tap_c[e] = (q.dx[i] - qx * q.sx) * q.in_pitch;
-    }
-  }
-  prm.w = static_cast<const unsigned char*>(t.w_packed);
-  prm.n_tile = t.n_tile; prm.nsplit = t.nsplit;
-  prm.w_stage_bytes = t.n_tile * 128 * (t.nsplit == 3 ? 2 : 1);
-  prm.stages = t.stages;
-  prm.stage_bytes = 2 * kATileBytes + 2 * t.n_tile * 128;
-  prm.out = p.out; prm.out_pitch = p.out_pitch; prm.B = p.B; prm.Ho = p.Ho; prm.Wo = p.Wo; prm.Hfull = p.Hfull; prm.Wfull = p.Wfull;
-  prm.osy = p.osy; prm.osx = p.osx; prm.Cout = p.Cout;
-  prm.bias = p.bias; prm.leaky = p.leaky;
-  TcDeviceState& ds = tc_device_state();
-  if (!ds.err_dev) return fail(DEMON_E_CUDA, "tcgen05 path: no error flag on device %d", ds.device);
-  prm.err = ds.err_dev;
-  if (!ds.tc_attr_set) {
-    DEMON_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    ds.tc_attr_set = true;
-  }
-  CUtensorMap map;
-  memcpy(&map, t.tmap_host, 128);
-  const int grid = std::min(prm.total_tiles, num_sms());
-  conv_tc_kernel<<<grid, kThreads, t.smem_bytes, stream>>>(map, prm);
-  DEMON_LAUNCH_CHECK();
-  return DEMON_OK;
-}
+int conv_tc_launch(const TcLayer& t, const ConvProblem* probs, cudaStream_t stream) { return conv_tc_halo_launch(t, probs, stream); }
 
 int tc_read_error_flag(bool clear) {
   TcDeviceState& ds = tc_device_state();

@@ -1,4 +1,4 @@
-// tcgen05 (5th generation tensor core) implicit-GEMM convolution for sm_100a -- interface.
+// Tensor-core (wgmma) implicit-GEMM convolution for sm_90a -- interface.
 #pragma once
 #include "conv.cuh"
 
@@ -8,16 +8,14 @@ namespace demon {
 // the TMA tensor map of the input activation slice.
 struct TcLayer {
   void* w_packed = nullptr;   // device, owned
-  void* tmap_in = nullptr;    // device copy of the CUtensorMap (128 B), owned
   int nclass = 1;             // 4 for the sub-pixel classes of a transposed convolution (one launch)
-  int n_tile = 0;             // UMMA N of this layer (Cout rounded up to 16)
+  int n_tile = 0;             // wgmma N of this layer (16, 32, 64 or 128)
   int n_tiles = 0;            // grid.y
   int k_chunks = 0;           // Cin / 32
   int th = 0, tw = 0, tb = 0; // output tile: tb images x th rows x tw columns = 128 (or fewer) GEMM rows
   int nsplit = 3;             // 3 = error-compensated 3xTF32, 1 = plain TF32
   int stages = 0;
   int smem_bytes = 0;
-  unsigned char tmap_host[128];
   int per_tap = 0;            // halo kernel in per-tap mode (low-resolution layers)
   void* halo_plan = nullptr;  // non-null: the layer runs on the halo kernel (conv_tc_halo.cu); owned
   int ksplit = 1;             // halo kernel: K loop split over `ksplit` work items per tile; then the launch needs
@@ -27,7 +25,7 @@ struct TcLayer {
 bool tc_layer_supported(const ConvProblem& p);
 // `nclass` problems that share input, tiling and Cout (1 for a convolution, 4 for the sub-pixel classes of a transposed
 // convolution) are packed into one layer and run in ONE launch.  w_hosts[c]: [ntaps][Cin][Cout_pad] fp32, the same
-// packing the SIMT path uses.
+// packing the SIMT path uses.  tc_layer_prepare plans the per-tap mode of the halo kernel (one TMA box per filter tap).
 int tc_layer_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts, int nclass, int precision);
 void tc_layer_free(TcLayer& t);
 int conv_tc_launch(const TcLayer& t, const ConvProblem* probs, cudaStream_t stream);
@@ -45,13 +43,11 @@ int tc_halo_read_timing(long long* host, int nblocks);
 // the device.  tc_device_state() returns the state of the CURRENT device (cudaGetDevice), creating it on first use.
 struct TcDeviceState {
   int device = -1;
-  int sms = 148;
+  int sms = 132;
   int* err_dev = nullptr;        // device int: set to 1 by a bounded mbarrier wait that timed out
-  unsigned halo_attr_set = 0;    // bit per conv_tc_halo_kernel instantiation
-  bool tc_attr_set = false;      // conv_tc_kernel
 };
 TcDeviceState& tc_device_state();
-// 1 if an mbarrier wait of a tcgen05 kernel has timed out on the current device since the flag was last cleared
+// 1 if an mbarrier wait of the tensor-core kernel has timed out on the current device since the flag was last cleared
 // (synchronises the device); `clear` resets it.  A timed-out wait lets the kernel run to completion with garbage, so the
 // forward entry points and demon_check_errors() turn this flag into DEMON_E_STATE.
 int tc_read_error_flag(bool clear);

@@ -1,46 +1,37 @@
-// tcgen05 implicit-GEMM convolution, "halo" variant: every input pixel is fetched ONCE per output tile.
+// Tensor-core implicit-GEMM convolution for sm_90a (wgmma), "halo" variant: every input pixel is fetched ONCE per output
+// tile.
 //
-// The output tile is 16 rows x 8 columns and, per 32-channel chunk, ONE TMA box per stride-parity plane brings the tile
-// plus its halo into shared memory ((16+nqy-1) x (8+nqx-1) pixels, 128 bytes per pixel, 128-byte swizzle).  Every filter
-// tap is then just a different START ADDRESS inside the same shared-memory image:
+// The output tile is 16 rows x 8 columns (128 GEMM rows) and, per 32-channel chunk, ONE TMA box per stride-parity plane
+// brings the tile plus its halo into shared memory ((16+nqy-1) x (8+nqx-1) pixels, 128 bytes per pixel, 128-byte swizzle).
+// Every filter tap is then just a different START ADDRESS inside the same shared-memory image:
 //
 //     GEMM row m = (y, x) of the tile  ->  halo pixel (y + qy - qy_min, x + qx - qx_min)
 //
 // A STEP of the main loop is one (32-channel chunk, input shift) pair.  For a plain convolution a shift is a filter tap;
 // for a transposed convolution k4 s2 (four sub-pixel classes of 2x2 taps each) the 16 class-taps use only NINE distinct
-// input shifts, so the A operand of a shift is staged once and multiplied with the weight blocks of every class that uses
+// input shifts, so the A operand of a shift is loaded once and multiplied with the weight blocks of every class that uses
 // it (4 classes at shift (0,0), 2 on the edges, 1 in the corners): 9 steps per chunk instead of 16.
 //
 // Warp roles (persistent over tiles, mbarrier rings between them, every wait bounded):
-//     warp 0        A producer: the halo boxes (TMA)
-//     warp 1        MMA thread: TS-mode tcgen05.mma kind::tf32 (A from TMEM, B = weights from shared memory)
-//     warps 2..     stagers, G groups of four warps taking turns: shifted pixel rows of the halo image -> registers ->
-//                   A_hi (raw fp32) and A_lo = A - trunc_tf32(A) in a TMEM ring slot (tcgen05.st)
-//     next 4 warps  epilogue: tcgen05.ld -> transpose through shared memory -> bias, leaky ReLU -> coalesced NHWC stores
-//     last warp     W producer: the pre-swizzled weight blocks of the step (cp.async.bulk)
+//     warpgroup 0   producer (one elected thread): the halo boxes (TMA) and the pre-swizzled weight blocks of every step
+//                   (cp.async.bulk) into a ring of kRing slots
+//     warpgroups 1, 2  consumers, 64 GEMM rows each: wgmma.mma_async m64nNk8 kind tf32 with the A fragment in registers
+//                   (loaded from the swizzled halo image, split into A_hi = trunc_tf32(A) and A_lo = A - A_hi) and B = the
+//                   weight block in shared memory; fp32 accumulators in registers; the epilogue (bias, leaky ReLU, NHWC
+//                   store into the channel slice of the destination) runs on the same threads after the tile's last step
 //
-// ONE operand ring of kRing = 4 slots couples them: slot s = (TMEM columns of A_hi | A_lo, the weight blocks in shared
-// memory, barrier full[s], barrier free[s]).  full[s] collects the four stager warps of the step plus the weight bytes
-// (expect_tx), so the MMA thread polls ONE barrier per step; free[s] is ONE tcgen05.commit per step that releases the TMEM
-// columns to the stagers and the weight slot to the W producer at the same time.
+// K order inside a 32-channel chunk: thread (g = lane / 4, t = lane % 4) of a warp needs, for the K = 8 slice j, the
+// columns t and t + 4 of its rows g and g + 8.  Slice j column kk is mapped to input channel 8 (kk % 4) + 2 j + kk / 4,
+// so that a thread's four slices are the 8 CONSECUTIVE channels 8t .. 8t + 7 of its two pixels (two 16-byte loads per
+// pixel); the host packs the weights in the same order.
 //
-// Narrow single-n-tile layers keep their whole packed weight set (<= 96 KB) RESIDENT in shared memory instead of streaming
-// one block per step through the ring: the small bulk copies of one SM execute one after the other at ~440 cycles each, which
-// capped those layers at ~440 cycles per step (profiles/r02_ring_latency.md).  Layers with few tiles split their K loop over
-// several work items (split-K, halo_splitk_reduce_kernel).
+// Precision: 3xTF32 = A_hi * W_lo + A_lo * W_hi + A_hi * W_hi (W split on the host), three wgmma per K = 8 slice and
+// class; the dropped term A_lo * W_lo is ~2^-21 relative.  nsplit = 1 is plain single-pass TF32.
 //
-// The MMA thread is the pacemaker of the CTA (profiles/r01_wait_counters.txt: it never waits, it IS the critical path),
-// and what it pays for is its own dependent instruction stream: every value that travels from a vector register to the
-// uniform datapath (R2UR, VOTEU) in front of a UTCHMMA / UTCBAR costs tens of cycles.  The loop is therefore written so
-// that the ring slot is a COMPILE-TIME constant (switch on step & 3 into four copies of the step body): TMEM operand
-// addresses, weight descriptors and barrier addresses are loop-invariant base + immediate, and the only per-step values
-// are the accumulator base (changes per tile) and the class mask of the step.
-//
-// 3xTF32 in two instructions per K8 slice when N <= 64 ("stacked", MODE 1): the weight block holds [W_hi ; W_lo] as 2N
-// consecutive rows, D[:, 0:2N] (+)= A_hi * [W_hi ; W_lo] is ONE UMMA of N' = 2N and D[:, N:2N] += A_lo * W_hi the second;
-// the epilogue adds the halves.  MODE 2 = three instructions (64 < N <= 128, or four classes of N = 64), MODE 0 = plain
-// single-pass TF32.  Variants: PER_TAP (images that are not made of whole 16 x 8 tiles: one 128-pixel TMA box per step
-// instead of a halo) and CIN8 (8-channel inputs: four taps x 8 channels per K = 32 step).
+// Narrow single-n-tile layers keep their whole packed weight set (<= 96 KB) RESIDENT in shared memory, loaded once per CTA
+// instead of one small bulk copy per step.  Layers with few tiles split their K loop over several work items (split-K,
+// halo_splitk_reduce_kernel).  Variants: PER_TAP (images that are not made of whole 16 x 8 tiles: one 128-pixel TMA box per
+// step instead of a halo) and CIN8 (8-channel inputs: four taps x 8 channels per K = 32 step).
 #include <cuda.h>
 
 #include <algorithm>
@@ -50,22 +41,21 @@
 
 #include "conv_tc.cuh"
 #include "conv_tc_ptx.cuh"
+#include "wgmma_tf32.cuh"
 
 namespace demon {
 
 namespace {
 
-constexpr int kRing = 4;                               // operand ring slots (TMEM A slot of 64 columns + weight slot)
-#ifndef DEMON_MAX_STAGER_GROUPS
-#define DEMON_MAX_STAGER_GROUPS 2
-#endif
-constexpr int kMaxGroups = DEMON_MAX_STAGER_GROUPS;    // stager groups of four warps (3: 19 warps, 96 registers per thread)
-constexpr int kMaxThreads = 32 * (2 + 4 * kMaxGroups + 4 + 1);   // 15 warps with two stager groups
+constexpr int kRing = 4;                 // weight ring slots
+constexpr int kThreads = 384;            // producer warpgroup + two consumer warpgroups
+constexpr int kConsumerWarps = 8;
 constexpr int kMaxAStages = 4;
 constexpr int kTileH = 16, kTileW = 8;
 constexpr int kMaxPlanes = 4;
-constexpr int kEpiRowBytes = 144;                  // 32 fp32 + 16 B pad: the epilogue's transpose buffer, conflict free both ways
-constexpr int kEpiStageBytes = 32 * kEpiRowBytes;  // per epilogue warp
+constexpr int kPlanSms = 132;            // SM count the tiling model plans for (H100 SXM); the launch uses the device's count
+constexpr int kSmemBudget = 224 * 1024;  // dynamic shared memory of the plan's operand stages (+ 1 KB for alignment)
+constexpr int kMaxDynSmem = 226 * 1024;  // 227 KB per block on sm_90, minus the kernel's static shared memory
 
 struct HaloPlane {
   int c_off;      // coordinate offset in dim 0 (rx * in_pitch)
@@ -86,18 +76,17 @@ struct HaloParams {
   int ksplit, kc_split, total_items;
   uint32_t mul_ksplit;
   long long part_stride;
-  int ngroups;                                      // stager groups (2 or 3)
   // per step (one input shift of one 32-channel chunk)
   int st_plane[kMaxTaps], st_aoff[kMaxTaps];        // halo mode: plane and byte offset of the shift's first pixel
-  int st_cmask[kMaxTaps], st_fmask[kMaxTaps];       // classes multiplied in this step / classes that start their sum here (chunk 0)
+  int st_cmask[kMaxTaps];                           // classes multiplied in this step
   int st_woff[kMaxTaps], st_wbytes[kMaxTaps];       // weight blocks of the step inside a chunk's weight image
   // per-tap mode (layers whose images are not made of whole 16x8 tiles): the A stage is ONE shift's 128-pixel tile
   // (tb images x th rows x tw columns, one TMA box per step, box coordinates carry the shift)
-  int per_tap, tw, th, tb, tiles_b, aempty_count;
+  int per_tap, tw, th, tb, tiles_b;
   int tap_c[kMaxTaps], tap_qx[kMaxTaps], tap_ry[kMaxTaps], tap_qy[kMaxTaps];
   // 8-channel mode (Cin == 8, e.g. the image pair): a pixel is 32 bytes in shared memory (no swizzle), the halo is loaded
-  // once per tile, and one K = 32 step gathers FOUR taps x 8 channels into the TMEM A operand (`nsteps` then counts these
-  // groups, g_plane / g_aoff describe the real taps, -1 = missing tap -> zero columns)
+  // once per tile, and one K = 32 step gathers FOUR taps x 8 channels (`nsteps` then counts these groups, g_plane / g_aoff
+  // describe the real taps, -1 = missing tap -> zero columns)
   int cin8, ntaps_real;
   int g_plane[kMaxTaps], g_aoff[kMaxTaps];
   HaloPlane planes[kMaxPlanes];
@@ -108,10 +97,8 @@ struct HaloParams {
   int w_region_bytes;   // shared memory of the weights: kRing slots, or the whole layer when resident
   int w_resident;       // 1: ALL weight blocks of the (single) n tile live in shared memory for the whole kernel, loaded once
   int cls_bytes;        // one class block: [W_hi ; W_lo] (3xTF32) or W alone
-  int n_tile, nsplit, tmem_cols;
-  int nbuf;             // accumulator buffers (2 = epilogue overlaps the next tile; 1 when TMEM is short)
-  int mode;             // 0 single pass, 1 stacked 3xTF32, 2 three-instruction 3xTF32
-  int acc_w;            // accumulator columns per class: 2 * n_tile in stacked mode ([big | small] terms), n_tile otherwise
+  int n_tile, nsplit;
+  int mode;             // 0 single pass TF32, 2 three-instruction 3xTF32
   const unsigned char* w;
   float* out;
   int out_pitch, Ho, Wo, Hfull, Wfull, osy, osx, Cout;
@@ -126,27 +113,11 @@ struct HaloMaps {
   CUtensorMap m[kMaxPlanes];
 };
 
-__device__ __forceinline__ uint64_t umma_desc_sw128_sbo(uint32_t smem_addr, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// Bounded wait, fully inline (a call in the MMA thread's loop would force every loop-invariant operand of the UTCHMMAs back
-// through a vector register and an R2UR per step).  Fast path: one try_wait.  Slow path: spin with a cycle budget; the
-// cycles spent there go to `acc` (the wait counters of the debug timing cost nothing on the fast path).  On timeout the
-// error flag is raised and the kernel runs to completion with garbage; the host turns the flag into DEMON_E_STATE.
-__device__ __forceinline__ void wait_t(uint32_t bar, uint32_t parity, int* err, long long& acc, bool timed) {
-  // (a try_wait on a pending phase may suspend the thread in hardware and still return true: with `timed` the whole
-  // call is bracketed, otherwise only the spin path is)
-  const long long t_in = timed ? clock64() : 0;
-  if (mbar_try(bar, parity)) {
-    if (timed) acc += clock64() - t_in;
-    return;
-  }
+// Bounded wait: fast path one try_wait, slow path a spin with a cycle budget (the cycles spent there go to `acc`).  On
+// timeout the error flag is raised and the kernel runs to completion with garbage; the host turns the flag into
+// DEMON_E_STATE.
+__device__ __forceinline__ void wait_t(uint32_t bar, uint32_t parity, int* err, long long& acc) {
+  if (mbar_try(bar, parity)) return;
   const long long t0 = clock64();
   for (;;) {
     if (mbar_try(bar, parity)) break;
@@ -155,11 +126,10 @@ __device__ __forceinline__ void wait_t(uint32_t bar, uint32_t parity, int* err, 
       break;
     }
   }
-  acc += clock64() - (timed ? t_in : t0);
+  acc += clock64() - t0;
 }
 
-// x / d for small d by one multiply (mul = 2^32 / d + 1, exact while x * d < 2^32; d == 1 -> mul = 0): the tile decode
-// runs once per tile in four roles, and integer division costs ~25 instructions on a thread that has few to spare
+// x / d for small d by one multiply (mul = 2^32 / d + 1, exact while x * d < 2^32; d == 1 -> mul = 0)
 __device__ __forceinline__ int fast_div(int x, int d, uint32_t mul) { return mul ? (int)__umulhi((uint32_t)x, mul) : x; }
 
 template <bool PER_TAP>
@@ -174,171 +144,33 @@ __device__ __forceinline__ void halo_decode_tile(const HaloParams& p, int tile, 
   else { y0 = yb * kTileH; x0 = xb * kTileW; }
 }
 
-// ---- MMA thread ---------------------------------------------------------------------------------------------------------
-// loop invariants of the MMA thread (all of them end up as uniform registers or immediates)
-struct MmaCtx {
-  uint32_t full0, free0;      // barrier rings
-  uint32_t t_ring;            // TMEM address of ring slot 0 (A_hi at +0, A_lo at +32)
-  uint32_t w_ring;            // shared-memory address of weight slot 0
-  uint32_t w_stage_bytes, cls_bytes;
-  uint32_t w_resident;        // weights resident: the block of step l of a tile is at w_ring + l * w_stage_bytes
-  uint32_t n_tile, acc_w;
-  uint32_t idesc, idesc2;
-  int* err;
-#ifdef DEMON_TC_TIMING_FULL
-  mutable long long* evlog;   // CTA 0: clock64 per event of the first 64 global steps (rows of 64 behind the wait counters)
-  mutable int ev_step;
-#endif
-};
-
-// all MMAs of ONE class block of a step: K = 32 as four K8 slices
-template <int MODE>
-__device__ __forceinline__ void issue_block(const MmaCtx& c, uint32_t d, uint32_t a_hi, uint32_t wb, bool fresh) {
-  const uint64_t w_hi = umma_desc_sw128_sbo(wb, 1024);
-  const uint32_t a_lo = a_hi + 32;
-  if (MODE == 1) {
-    // D[:, 0:2N] (+)= A_hi * [W_hi ; W_lo]  (one UMMA of N' = 2N: big term | first small term);  D[:, N:2N] += A_lo * W_hi
-    if (fresh) umma_tf32_ts(d, a_hi, w_hi, c.idesc2, 0u); else umma_tf32_ts(d, a_hi, w_hi, c.idesc2, 1u);
-    umma_tf32_ts(d + c.n_tile, a_lo, w_hi, c.idesc, 1u);
+// All wgmma of ONE class block of a step: K = 32 as four K = 8 slices.  hi/lo[8 j + 0..3] = the A fragment of slice j.
+template <int N, int MODE>
+__device__ __forceinline__ void issue_block(float* acc, const uint32_t* hi, const uint32_t* lo, uint32_t wb) {
+  const uint64_t w_hi = wgmma_desc_sw128(wb);
+  const uint64_t w_lo = wgmma_desc_sw128(wb + N * 128u);
 #pragma unroll
-    for (int j = 1; j < 4; ++j) {   // + 8 TMEM columns / + 32 bytes inside the swizzled weight row per K8 slice
-      umma_tf32_ts(d, a_hi + 8 * j, w_hi + (uint64_t)(2 * j), c.idesc2, 1u);
-      umma_tf32_ts(d + c.n_tile, a_lo + 8 * j, w_hi + (uint64_t)(2 * j), c.idesc, 1u);
+  for (int j = 0; j < 4; ++j) {   // + 32 bytes inside the swizzled weight row per K = 8 slice
+    if (MODE == 2) {
+      Wgmma<N>::mma(acc, hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3], w_lo + (uint64_t)(2 * j));
+      Wgmma<N>::mma(acc, lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3], w_hi + (uint64_t)(2 * j));
     }
-  } else if (MODE == 2) {
-    const uint64_t w_lo = umma_desc_sw128_sbo(wb + c.n_tile * 128u, 1024);
-    if (fresh) umma_tf32_ts(d, a_hi, w_lo, c.idesc, 0u); else umma_tf32_ts(d, a_hi, w_lo, c.idesc, 1u);
-    umma_tf32_ts(d, a_lo, w_hi, c.idesc, 1u);
-    umma_tf32_ts(d, a_hi, w_hi, c.idesc, 1u);
-#pragma unroll
-    for (int j = 1; j < 4; ++j) {
-      umma_tf32_ts(d, a_hi + 8 * j, w_lo + (uint64_t)(2 * j), c.idesc, 1u);
-      umma_tf32_ts(d, a_lo + 8 * j, w_hi + (uint64_t)(2 * j), c.idesc, 1u);
-      umma_tf32_ts(d, a_hi + 8 * j, w_hi + (uint64_t)(2 * j), c.idesc, 1u);
-    }
-  } else {
-    if (fresh) umma_tf32_ts(d, a_hi, w_hi, c.idesc, 0u); else umma_tf32_ts(d, a_hi, w_hi, c.idesc, 1u);
-#pragma unroll
-    for (int j = 1; j < 4; ++j) umma_tf32_ts(d, a_hi + 8 * j, w_hi + (uint64_t)(2 * j), c.idesc, 1u);
+    Wgmma<N>::mma(acc, hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3], w_hi + (uint64_t)(2 * j));
   }
 }
 
-// One step with the ring slot as a compile-time constant (the main loop is unrolled by kRing, so the slot is the
-// position in the unrolled body and every operand address is a loop-invariant base plus an immediate).
-//   - wait for full[SLOT] unless the early poll issued during the previous step already saw the phase complete
-//   - poll full[SLOT + 1] (mbarrier.test_wait: never suspends the thread) BEFORE issuing, so that its latency overlaps the
-//     UTCHMMA issue
-//   - the step's MMAs: single-class layers (MULTI == false) one block, fresh only at the first step of a tile;
-//     transposed convolutions walk the class mask of the step
-//   - ONE commit: frees the TMEM columns (stagers) and the weight slot (W producer)
-template <int MODE, int SLOT, bool MULTI>
-__device__ __forceinline__ bool mma_step(const MmaCtx& c, uint32_t d_base, uint32_t par, uint32_t npar, bool rdy, bool fresh, uint32_t cm,
-                                         uint32_t fm, long long& w_full, int l) {
-#ifdef DEMON_TC_TIMING_FULL
-  // diagnostic build: every wait bracketed by clock reads, and an event log of CTA 0's first 64 steps (tools/bench_conv.py prints it)
-  if (c.evlog && c.ev_step < 64) { c.evlog[512 + c.ev_step] = clock64(); c.evlog[576 + c.ev_step] = rdy ? 1 : 0; }   // step entered, early probe result
-  if (!rdy) wait_t(c.full0 + 8 * SLOT, par, c.err, w_full, true);
-  if (c.evlog && c.ev_step < 64) c.evlog[c.ev_step] = clock64();         // full[] of the step observed
-  tc_fence_after();
-  if (c.evlog && c.ev_step < 64) c.evlog[384 + c.ev_step] = clock64();   // after tcgen05.fence::after_thread_sync
-#else
-  if (!rdy) wait_t(c.full0 + 8 * SLOT, par, c.err, w_full, false);   // (the MMA thread's waits are never bracketed: no clock reads on its fast path)
-  tc_fence_after();
-#endif
-  const bool next_rdy = mbar_test(c.full0 + 8 * ((SLOT + 1) & (kRing - 1)), npar);
-  const uint32_t a_hi = c.t_ring + (uint32_t)(SLOT * 64);
-  uint32_t wb = c.w_ring + (c.w_resident ? (uint32_t)l : (uint32_t)SLOT) * c.w_stage_bytes;
-  if (!MULTI) {
-    issue_block<MODE>(c, d_base, a_hi, wb, fresh);
-  } else {
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-      if (cm & (1u << k)) {
-        issue_block<MODE>(c, d_base + (uint32_t)k * c.acc_w, a_hi, wb, (fm & (1u << k)) != 0);
-        wb += c.cls_bytes;
-      }
-  }
-#ifdef DEMON_TC_TIMING_FULL
-  if (c.evlog && c.ev_step < 64) c.evlog[448 + c.ev_step] = clock64();   // the step's MMAs issued
-#endif
-  umma_commit(c.free0 + 8 * SLOT);
-#ifdef DEMON_TC_TIMING_FULL
-  if (c.evlog && c.ev_step < 64) c.evlog[64 + c.ev_step] = clock64();    // the step's commit issued
-  ++c.ev_step;
-#endif
-  return next_rdy;
-}
-
-// The MMA thread's whole main loop.  State per step is kept minimal: l (step inside the tile), the early-poll flag, the
-// ring parity; everything else is loop invariant.  The tile boundary is handled inline after the step that ends a tile.
-template <int MODE, bool MULTI>
-__device__ __forceinline__ void mma_main_loop(const HaloParams& p, const MmaCtx& c, uint32_t tmem_base, int acc_cols, uint32_t cfull0,
-                                              uint32_t cempty0, long long& w_cempty, long long& w_full) {
-  const int steps_per_tile = p.kc_split * p.nsteps;   // steps of one work item
-  const int nsteps = p.nsteps;
-  const int nbuf = p.nbuf;
-  uint64_t cmasks = 0, fmasks = 0;   // class / fresh masks of the steps of a chunk, four bits per step (MULTI only)
-  if (MULTI)
-    for (int t = 0; t < nsteps; ++t) { cmasks |= (uint64_t)p.st_cmask[t] << (4 * t); fmasks |= (uint64_t)p.st_fmask[t] << (4 * t); }
-  int tile = blockIdx.x;                               // (work item index)
-  if (tile >= p.total_items) return;
-  int it = 0, l = 0, t = 0;
-  uint32_t par = 0;
-  wait_t(cempty0, 1u, c.err, w_cempty, false);          // accumulator buffer 0, first use
-  uint32_t d_base = tmem_base;
-  uint32_t cfull_bar = cfull0;
-  bool rdy = mbar_test(c.full0, 0);
-
-#define DEMON_MMA_STEP(SLOT)                                                                                              \
-  {                                                                                                                       \
-    uint32_t cm = 1u, fm = 0u;                                                                                            \
-    if (MULTI) {                                                                                                          \
-      cm = (uint32_t)(cmasks >> (4 * t)) & 15u;                                                                           \
-      fm = (l < nsteps) ? ((uint32_t)(fmasks >> (4 * t)) & 15u) : 0u;                                                     \
-      if (++t == nsteps) t = 0;                                                                                           \
-    }                                                                                                                     \
-    rdy = mma_step<MODE, SLOT, MULTI>(c, d_base, par, (SLOT == kRing - 1) ? (par ^ 1u) : par, rdy, l == 0, cm, fm, w_full, l); \
-    if (++l == steps_per_tile) {                                                                                          \
-      umma_commit(cfull_bar);   /* the tile's accumulators are complete once everything issued so far has retired */      \
-      tile += gridDim.x;                                                                                                  \
-      if (tile >= p.total_items) return;                                                                                  \
-      ++it;                                                                                                               \
-      l = 0;                                                                                                              \
-      const int a = (nbuf == 2) ? (it & 1) : 0;                                                                           \
-      const uint32_t cphase = (nbuf == 2) ? ((it >> 1) & 1) : (it & 1);                                                   \
-      wait_t(cempty0 + 8 * a, cphase ^ 1u, c.err, w_cempty, false);                                                       \
-      d_base = tmem_base + (uint32_t)(a * acc_cols);                                                                      \
-      cfull_bar = cfull0 + 8 * a;                                                                                         \
-    }                                                                                                                     \
-  }
-  for (;;) {
-    DEMON_MMA_STEP(0)
-    DEMON_MMA_STEP(1)
-    DEMON_MMA_STEP(2)
-    DEMON_MMA_STEP(3)
-    par ^= 1u;
-  }
-#undef DEMON_MMA_STEP
-}
-
-template <bool PER_TAP, bool CIN8, int MODE>
-__global__ void __launch_bounds__(kMaxThreads, 1) conv_tc_halo_kernel(const __grid_constant__ HaloMaps maps, const HaloParams p) {
+template <bool PER_TAP, bool CIN8, int MODE, int N, int NCLS>
+__global__ void __launch_bounds__(kThreads, 1) conv_tc_halo_kernel(const __grid_constant__ HaloMaps maps, const HaloParams p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  // bars: A_full[4], A_empty[4], full[4], free[4], accum_full[2], accum_empty[2]
-  __shared__ __align__(8) uint64_t bars[2 * kMaxAStages + 2 * kRing + 4 + 1];   // (+ W_resident)
-  __shared__ uint32_t tmem_base_smem;
+  // bars: A_full[4], A_empty[4], W_full[4], W_empty[4], W_resident
+  __shared__ __align__(8) uint64_t bars[2 * kMaxAStages + 2 * kRing + 1];
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int n_stager_warps = 4 * p.ngroups;
-  const int epi_warp0 = 2 + n_stager_warps;
-  const int w_warp = epi_warp0 + 4;
   const uint32_t afull0 = smem_u32(&bars[0]), aempty0 = smem_u32(&bars[kMaxAStages]);
-  const uint32_t full0 = smem_u32(&bars[2 * kMaxAStages]), free0 = smem_u32(&bars[2 * kMaxAStages + kRing]);
-  const uint32_t cfull0 = smem_u32(&bars[2 * kMaxAStages + 2 * kRing]);
-  const uint32_t cempty0 = smem_u32(&bars[2 * kMaxAStages + 2 * kRing + 2]);
-  const uint32_t wres_bar = smem_u32(&bars[2 * kMaxAStages + 2 * kRing + 4]);
+  const uint32_t wfull0 = smem_u32(&bars[2 * kMaxAStages]), wempty0 = smem_u32(&bars[2 * kMaxAStages + kRing]);
+  const uint32_t wres_bar = smem_u32(&bars[2 * kMaxAStages + 2 * kRing]);
   const int a_stage_bytes = p.a_region_bytes;
   unsigned char* w_ring = smem + (size_t)p.sa * a_stage_bytes;
 
@@ -346,60 +178,47 @@ __global__ void __launch_bounds__(kMaxThreads, 1) conv_tc_halo_kernel(const __gr
     for (int i = 0; i < p.nplanes; ++i) asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.m[i]) : "memory");
     for (int s = 0; s < kMaxAStages; ++s) {
       mbar_init(afull0 + 8 * s, 1);
-      mbar_init(aempty0 + 8 * s, (uint32_t)p.aempty_count);
+      mbar_init(aempty0 + 8 * s, kConsumerWarps);
     }
     for (int s = 0; s < kRing; ++s) {
-      mbar_init(full0 + 8 * s, p.w_resident ? 4 : 4 + 1);   // the four warps of the stager group that owns the step (+ the W producer's expect_tx)
-      mbar_init(free0 + 8 * s, 1);       // the MMA thread's commit
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(cfull0 + 8 * s, 1);
-      mbar_init(cempty0 + 8 * s, 4);
+      mbar_init(wfull0 + 8 * s, 1);
+      mbar_init(wempty0 + 8 * s, kConsumerWarps);
     }
     mbar_init(wres_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(&tmem_base_smem), (uint32_t)p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-  const int acc_cols = p.nclass * p.acc_w;           // columns of one accumulator buffer
-  const uint32_t t_ring = tmem_base + (uint32_t)(p.nbuf * acc_cols);   // A-operand ring: kRing slots of 64 columns (hi | lo)
   const bool timed = p.timing != nullptr;
-  // Programmatic dependent launch: from here on the next kernel of the stream may become resident (on SMs this grid has
-  // left).  This kernel's own prologue above ran while its predecessor was still draining; the roles that read what the
-  // predecessor wrote (A producer) or write global memory (epilogue) wait for it below, the W producer does not (weights
-  // are constants) and fills the weight ring in the meantime.
+  // Programmatic dependent launch: from here on the next kernel of the stream may become resident.  The roles that read
+  // what the predecessor wrote (producer: the input) or write global memory (consumers: the output) wait for it below.
   pdl_launch_dependents();
 
-  if (warp == 0) {
-    // ===== A producer: one halo box per plane and 32-channel chunk ======================================================
-    if (elect_one_sync()) {
-      int sa = 0;
-      uint32_t pa = 0;
-      uint32_t a_bytes = 0;
-      long long w_aempty = 0;
-      const long long t_begin = clock64();
-      for (int i = 0; i < p.nplanes; ++i) a_bytes += (uint32_t)p.planes[i].bytes;
-      pdl_wait();   // the input is the previous kernel's output
-      for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
-        const int tile = fast_div(item, p.ksplit, p.mul_ksplit);
-        const int kc0 = (item - tile * p.ksplit) * p.kc_split;
-        int nt, n, y0, x0;
-        halo_decode_tile<PER_TAP>(p, tile, nt, n, y0, x0);
-        for (int kc = kc0; kc < kc0 + p.kc_split; ++kc) {
-          if (PER_TAP) {
-            for (int t = 0; t < p.nsteps; ++t) {
-              wait_t(aempty0 + 8 * sa, pa ^ 1, p.err, w_aempty, timed);
-              mbar_expect_tx(afull0 + 8 * sa, 128u * 128u);
-              tma_load_5d(smem_u32(smem + (size_t)sa * a_stage_bytes), &maps.m[0], afull0 + 8 * sa, p.tap_c[t] + kc * 32, x0 + p.tap_qx[t],
-                          p.tap_ry[t], y0 + p.tap_qy[t], n);
-              if (++sa == p.sa) { sa = 0; pa ^= 1; }
-            }
-            continue;
-          }
-          wait_t(aempty0 + 8 * sa, pa ^ 1, p.err, w_aempty, timed);
+  if (warp < 4) {
+    // ===== producer ===================================================================================================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp != 0 || !elect_one_sync()) return;
+    long long w_aempty = 0, w_wempty = 0;
+    const long long t_begin = clock64();
+    if (p.w_resident) {
+      const uint32_t total = (uint32_t)(p.k_chunks * p.w_chunk_bytes);
+      mbar_expect_tx(wres_bar, total);
+      for (int kc = 0; kc < p.k_chunks; ++kc)
+        bulk_load(smem_u32(w_ring + (size_t)kc * p.w_chunk_bytes), p.w + (size_t)kc * p.w_chunk_bytes, (uint32_t)p.w_chunk_bytes, wres_bar);
+    }
+    uint32_t a_bytes = 0;
+    for (int i = 0; i < p.nplanes; ++i) a_bytes += (uint32_t)p.planes[i].bytes;
+    int sa = 0, slot = 0;
+    uint32_t pa = 0, use = 0;
+    pdl_wait();   // the input is the previous kernel's output
+    for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
+      const int tile = fast_div(item, p.ksplit, p.mul_ksplit);
+      const int kc0 = (item - tile * p.ksplit) * p.kc_split;
+      int nt, n, y0, x0;
+      halo_decode_tile<PER_TAP>(p, tile, nt, n, y0, x0);
+      const unsigned char* wsrc = p.w + ((size_t)nt * p.k_chunks + kc0) * p.w_chunk_bytes;
+      for (int kc = kc0; kc < kc0 + p.kc_split; ++kc, wsrc += p.w_chunk_bytes) {
+        if (!PER_TAP) {
+          wait_t(aempty0 + 8 * sa, pa ^ 1, p.err, w_aempty);
           const uint32_t abase = smem_u32(smem + (size_t)sa * a_stage_bytes);
           mbar_expect_tx(afull0 + 8 * sa, a_bytes);
           for (int i = 0; i < p.nplanes; ++i) {
@@ -408,303 +227,183 @@ __global__ void __launch_bounds__(kMaxThreads, 1) conv_tc_halo_kernel(const __gr
           }
           if (++sa == p.sa) { sa = 0; pa ^= 1; }
         }
-      }
-      if (timed) { p.timing[blockIdx.x * 16 + 0] = w_aempty; p.timing[blockIdx.x * 16 + 8] = clock64() - t_begin; }
-    }
-  } else if (warp == w_warp) {
-    // ===== W producer: the weight blocks of every step into the step's ring slot ==========================================
-    // The copy's bytes complete on the step's `full` barrier (the one the stager group arrives on).  Both producers of a
-    // slot wait for free[slot] of the previous round before they arrive for the next one, so all five arrivals and the
-    // bytes of a step belong to the same barrier phase.
-    const bool w_elected = elect_one_sync();
-    if (w_elected && p.w_resident) {
-      // Resident weights (narrow single-n-tile layers: the whole layer's packed weights are 24 .. 96 KB): a few large copies
-      // at the start instead of one 4 .. 8 KB cp.async.bulk per step.  The small copies of one SM execute one after the
-      // other at ~440 cycles each (event log in profiles/r02_ring_latency.md: a copy lands ~2900 cycles after it is issued
-      // with six ahead of it), and THAT is the ~440-cycle step of the narrow layers, whatever N and whatever the ring depth.
-      const uint32_t total = (uint32_t)(p.k_chunks * p.w_chunk_bytes);
-      mbar_expect_tx(wres_bar, total);
-      for (int kc = 0; kc < p.k_chunks; ++kc)
-        bulk_load(smem_u32(w_ring + (size_t)kc * p.w_chunk_bytes), p.w + (size_t)kc * p.w_chunk_bytes, (uint32_t)p.w_chunk_bytes, wres_bar);
-    } else if (w_elected) {
-      int slot = 0;
-      uint32_t use = 0;
-      long long w_free = 0;
-      for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
-        const int tile = fast_div(item, p.ksplit, p.mul_ksplit);
-        const int kc0 = (item - tile * p.ksplit) * p.kc_split;
-        const int nt = tile - fast_div(tile, p.n_tiles, p.mul_n_tiles) * p.n_tiles;
-        const unsigned char* wsrc = p.w + ((size_t)nt * p.k_chunks + kc0) * p.w_chunk_bytes;
-        for (int kc = 0; kc < p.kc_split; ++kc, wsrc += p.w_chunk_bytes) {
-          for (int t = 0; t < p.nsteps; ++t) {
-            wait_t(free0 + 8 * slot, use ^ 1, p.err, w_free, timed);
+        for (int t = 0; t < p.nsteps; ++t) {
+          if (PER_TAP) {
+            wait_t(aempty0 + 8 * sa, pa ^ 1, p.err, w_aempty);
+            mbar_expect_tx(afull0 + 8 * sa, 128u * 128u);
+            tma_load_5d(smem_u32(smem + (size_t)sa * a_stage_bytes), &maps.m[0], afull0 + 8 * sa, p.tap_c[t] + kc * 32, x0 + p.tap_qx[t],
+                        p.tap_ry[t], y0 + p.tap_qy[t], n);
+            if (++sa == p.sa) { sa = 0; pa ^= 1; }
+          }
+          if (!p.w_resident) {
+            wait_t(wempty0 + 8 * slot, use ^ 1, p.err, w_wempty);
             const uint32_t bytes = (uint32_t)p.st_wbytes[t];
-            mbar_expect_tx(full0 + 8 * slot, bytes);
-            bulk_load(smem_u32(w_ring + (size_t)slot * p.w_stage_bytes), wsrc + p.st_woff[t], bytes, full0 + 8 * slot);
+            mbar_expect_tx(wfull0 + 8 * slot, bytes);
+            bulk_load(smem_u32(w_ring + (size_t)slot * p.w_stage_bytes), wsrc + p.st_woff[t], bytes, wfull0 + 8 * slot);
             if (++slot == kRing) { slot = 0; use ^= 1; }
           }
         }
       }
-      if (timed) p.timing[blockIdx.x * 16 + 1] = w_free;
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer: A operand from TMEM (staged by the stager warps), B operand (weights) from shared memory =========
-    if (elect_one_sync()) {
-      MmaCtx c;
-      c.full0 = full0; c.free0 = free0; c.t_ring = t_ring; c.w_ring = smem_u32(w_ring);
-      c.w_stage_bytes = (uint32_t)p.w_stage_bytes; c.cls_bytes = (uint32_t)p.cls_bytes;
-      c.n_tile = (uint32_t)p.n_tile; c.acc_w = (uint32_t)p.acc_w;
-      c.idesc = umma_idesc_tf32(p.n_tile); c.idesc2 = umma_idesc_tf32(2 * p.n_tile);
-      c.err = p.err;
-#ifdef DEMON_TC_TIMING_FULL
-      c.evlog = (timed && blockIdx.x == 0) ? p.timing + 160 * 16 : nullptr;
-      c.ev_step = 0;
-#endif
-      c.w_resident = (uint32_t)p.w_resident;
-      long long w_cempty = 0, w_full = 0;
-      const long long t_begin = clock64();
-      if (p.w_resident) wait_t(wres_bar, 0u, p.err, w_full, false);
-      if (p.nclass == 1) mma_main_loop<MODE, false>(p, c, tmem_base, acc_cols, cfull0, cempty0, w_cempty, w_full);
-      else mma_main_loop<MODE, true>(p, c, tmem_base, acc_cols, cfull0, cempty0, w_cempty, w_full);
-      if (timed) {
-        long long* tm = p.timing + blockIdx.x * 16;
-        tm[2] = w_cempty; tm[3] = w_full; tm[9] = clock64() - t_begin;
-      }
-    }
-  } else if (warp < epi_warp0) {
-    // ===== stagers: halo image (shared memory) -> A operand of one shift in TMEM ========================================
-    // Thread (quadrant q, lane l) owns GEMM row m = 32q + l = tile pixel (m / 8, m % 8).  For every step it reads its
-    // (shifted) 128-byte pixel out of the swizzled halo image -- conflict free: the 8 lanes of a quarter warp hit 8
-    // different 16-byte columns -- and writes the raw fp32 values (A_hi: the tensor core ignores the low 13 mantissa bits)
-    // and A_lo = A - trunc_tf32(A) to its TMEM lane.  The groups of four warps take the steps in turns.
-    const int q = warp & 3;
-    const int grp = (warp - 2) >> 2;
-    const int m = q * 32 + lane;
-    const int g8 = m >> 3, r = m & 7;
-    const int ngroups = p.ngroups;
-    long long w_safull = 0, w_free = 0;
-#ifdef DEMON_TC_TIMING_FULL
-    long long d_load = 0, d_store = 0, d_arrive = 0;
-#endif
-    const long long t_begin = clock64();
-    // The group visits only its OWN steps: global step gs = grp, grp + G, grp + 2G, ...; t_own is that step's index
-    // inside the current chunk.  Ring slot and parity follow from gs; in per-tap mode so does the A stage (one per step).
-    uint32_t gs = (uint32_t)grp;
-    int t_own = grp;
-    int sa = PER_TAP ? (grp % p.sa) : 0;          // halo mode: stage of the current chunk; per-tap: stage of step gs
-    uint32_t pa = PER_TAP ? (uint32_t)((grp / p.sa) & 1) : 0u;
-    const int nsteps = p.nsteps;
-    for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
-      for (int kc = 0; kc < p.kc_split; ++kc) {
-        uint32_t abase = 0;
-        if (!PER_TAP) {
-          wait_t(afull0 + 8 * sa, pa, p.err, w_safull, timed);
-          __syncwarp();
-          abase = smem_u32(smem + (size_t)sa * a_stage_bytes);
-        }
-        for (; t_own < nsteps; t_own += ngroups, gs += (uint32_t)ngroups) {
-          const int t = t_own;
-          const int slot_cur = (int)(gs & (kRing - 1));
-          const uint32_t use_cur = (gs >> 2) & 1u;
-          const int sa_cur = sa;
-          uint32_t row;
-#ifdef DEMON_TC_TIMING_FULL
-          const long long c0 = clock64();
-#endif
-          if (PER_TAP) {
-            wait_t(afull0 + 8 * sa_cur, pa, p.err, w_safull, timed);
-            __syncwarp();
-            row = smem_u32(smem + (size_t)sa_cur * a_stage_bytes) + (uint32_t)(g8 * 1024 + r * 128);
-            sa += ngroups;                                  // the A stage of this group's next step
-            while (sa >= p.sa) { sa -= p.sa; pa ^= 1u; }
-          } else if (!CIN8) {
-            const HaloPlane& pl = p.planes[p.st_plane[t]];
-            row = abase + (uint32_t)(pl.smem_off + p.st_aoff[t] + g8 * pl.cols * 128 + r * 128);
-          } else {
-            row = 0;
-          }
-          uint32_t hi[32], lo[32];   // the shared-memory loads are in flight while the slot's barrier is polled
-          if (CIN8) {
-            // four taps x 8 channels -> the 32 columns of this K step; a pixel is 32 contiguous bytes
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const int rt = 4 * t + j;
-              const int pi = (rt < p.ntaps_real) ? p.g_plane[rt] : -1;
-              float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
-              if (pi >= 0) {
-                const HaloPlane& pl = p.planes[pi];
-                const uint32_t px = abase + (uint32_t)(pl.smem_off + p.g_aoff[rt] + (g8 * pl.cols + r) * 32);
-                v0 = lds128(px); v1 = lds128(px + 16);
-              }
-              hi[8 * j + 0] = __float_as_uint(v0.x); hi[8 * j + 1] = __float_as_uint(v0.y);
-              hi[8 * j + 2] = __float_as_uint(v0.z); hi[8 * j + 3] = __float_as_uint(v0.w);
-              hi[8 * j + 4] = __float_as_uint(v1.x); hi[8 * j + 5] = __float_as_uint(v1.y);
-              hi[8 * j + 6] = __float_as_uint(v1.z); hi[8 * j + 7] = __float_as_uint(v1.w);
-            }
-          } else {
-            const uint32_t phase = (row >> 7) & 7u;
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-              const float4 v = lds128(row + ((c ^ phase) << 4));
-              hi[4 * c + 0] = __float_as_uint(v.x); hi[4 * c + 1] = __float_as_uint(v.y);
-              hi[4 * c + 2] = __float_as_uint(v.z); hi[4 * c + 3] = __float_as_uint(v.w);
-            }
-          }
-#ifdef DEMON_TC_TIMING_FULL
-          const long long c1 = clock64();
-#endif
-          wait_t(free0 + 8 * slot_cur, use_cur ^ 1, p.err, w_free, timed);
-          __syncwarp();
-          tc_fence_after();
-#ifdef DEMON_TC_TIMING_FULL
-          const long long c2 = clock64();
-          if (timed && blockIdx.x == 0 && q == 0 && lane == 0 && gs < 64) p.timing[160 * 16 + 128 + gs] = c2;   // free[] observed
-#endif
-          const uint32_t taddr = t_ring + ((uint32_t)(q * 32) << 16) + (uint32_t)(slot_cur * 64);
-          tmem_st_x32(taddr, hi);
-          if (MODE != 0) {
-#pragma unroll
-            for (int c = 0; c < 32; c += 2) tf32_lo2(hi[c], hi[c + 1], lo[c], lo[c + 1]);
-            tmem_st_x32(taddr + 32, lo);
-          }
-          tmem_st_wait();
-#ifdef DEMON_TC_TIMING_FULL
-          const long long c3 = clock64();
-#endif
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(full0 + 8 * slot_cur);
-            if (PER_TAP) mbar_arrive(aempty0 + 8 * sa_cur);   // the shift's tile has been consumed: stage back to the producer
-          }
-#ifdef DEMON_TC_TIMING_FULL
-          d_load += c1 - c0; d_store += c3 - c2; d_arrive += clock64() - c3;
-          if (timed && blockIdx.x == 0 && q == 0 && lane == 0 && gs < 64) {
-            p.timing[160 * 16 + 192 + gs] = clock64();   // arrived on full[]
-            p.timing[160 * 16 + 256 + gs] = c0;          // started on the step (address math, shared loads)
-            p.timing[160 * 16 + 320 + gs] = c3;          // tcgen05.wait::st returned
-          }
-#endif
-        }
-        t_own -= nsteps;   // index of the next own step inside the NEXT chunk
-        if (!PER_TAP) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(aempty0 + 8 * sa);   // this warp is done reading the halo stage
-          if (++sa == p.sa) { sa = 0; pa ^= 1; }
-        }
-      }
-    }
-    if (timed && lane == 0 && q == 0) {
-      if (grp == 0) { p.timing[blockIdx.x * 16 + 6] = w_safull; p.timing[blockIdx.x * 16 + 4] = w_free; p.timing[blockIdx.x * 16 + 10] = clock64() - t_begin; }
-      else if (grp == 1) p.timing[blockIdx.x * 16 + 12] = w_free;
-#ifdef DEMON_TC_TIMING_FULL
-      if (grp == 0) { p.timing[blockIdx.x * 16 + 13] = d_load; p.timing[blockIdx.x * 16 + 14] = d_store; p.timing[blockIdx.x * 16 + 15] = d_arrive; }
-#endif
-    }
-  } else if (warp < w_warp) {
-    // ===== epilogue ======================================================================================================
-    // After the TMEM load a thread holds one output pixel (GEMM row) x 32 channels, and consecutive pixels are a whole
-    // pixel pitch apart in global memory: storing rows directly costs 32 memory wavefronts per store instruction.  Each
-    // warp therefore transposes its 32 x 32 block through shared memory (row pitch 144 B: conflict free both ways) and
-    // stores with lane = (row % 4, 16-byte chunk), i.e. four pixels x 128 contiguous bytes per instruction; the bias is
-    // then one float4 per lane and chunk.
-    const int q = warp & 3;
-    const int sub = lane >> 3, chunk = lane & 7;
-    const uint32_t stg = smem_u32(w_ring + (size_t)p.w_region_bytes) + (uint32_t)(q * kEpiStageBytes);
-    int rowoff[8];          // element offset of row 4 i + sub of this warp's block inside the output tile
-    uint32_t rowpos[8];     // its (yl, xl, nl) for the bounds test
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int m = q * 32 + 4 * i + sub;
-      const int xl = PER_TAP ? (m % p.tw) : (m & 7);
-      const int yl = PER_TAP ? ((m / p.tw) % p.th) : (m >> 3);
-      const int nl = PER_TAP ? (m / (p.tw * p.th)) : 0;
-      rowoff[i] = ((nl * p.Hfull + yl * p.osy) * p.Wfull + xl * p.osx) * p.out_pitch;
-      rowpos[i] = (uint32_t)yl | ((uint32_t)xl << 10) | ((uint32_t)nl << 20);
-    }
-    const float slope = p.leaky ? 0.1f : 1.0f;
-    long long w_cfull = 0;
-    const long long t_begin = clock64();
-    int it = 0;
-    pdl_wait();   // the output buffer may still be read (or written) by the previous kernel
-    for (int item = blockIdx.x; item < p.total_items; item += gridDim.x, ++it) {
-      const int tile = fast_div(item, p.ksplit, p.mul_ksplit);
-      const int z = item - tile * p.ksplit;
-      int nt, n, y0, x0;
-      halo_decode_tile<PER_TAP>(p, tile, nt, n, y0, x0);
-      const int a = (p.nbuf == 2) ? (it & 1) : 0;
-      wait_t(cfull0 + 8 * a, (p.nbuf == 2) ? ((it >> 1) & 1) : (it & 1), p.err, w_cfull, timed);
-      __syncwarp();
-      tc_fence_after();
-      uint32_t rowmask = 0xFFu;
-      const bool whole = PER_TAP ? (y0 + p.th <= p.Ho && x0 + p.tw <= p.Wo && n + p.tb <= p.B) : (y0 + kTileH <= p.Ho && x0 + kTileW <= p.Wo);
-      if (!whole) {
-        rowmask = 0;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int yl = (int)(rowpos[i] & 1023u), xl = (int)((rowpos[i] >> 10) & 1023u), nl = (int)(rowpos[i] >> 20);
-          if (y0 + yl < p.Ho && x0 + xl < p.Wo && n + nl < p.B) rowmask |= 1u << i;
-        }
-      }
-      float* tile_out = p.out + (size_t)z * p.part_stride + ((size_t)(n * p.Hfull + y0 * p.osy) * p.Wfull + x0 * p.osx) * p.out_pitch;
-      const int cbase = nt * p.n_tile;
-      for (int cls = 0; cls < p.nclass; ++cls) {
-        float* cls_out = tile_out + (size_t)(p.cls_ooy[cls] * p.Wfull + p.cls_oox[cls]) * p.out_pitch;
-        const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * acc_cols + cls * p.acc_w);
-        for (int c0 = 0; c0 < p.n_tile; c0 += 32) {
-          uint32_t v[32];
-          const int ncol = (p.n_tile - c0) >= 32 ? 32 : 16;
-          if (ncol == 32) tmem_ld_x32(t_row + c0, v); else tmem_ld_x16(t_row + c0, v);
-          if (MODE == 1) {   // big term + small terms
-            uint32_t u[32];
-            if (ncol == 32) tmem_ld_x32(t_row + p.n_tile + c0, u); else tmem_ld_x16(t_row + p.n_tile + c0, u);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(u[i]));
-          }
-          tmem_ld_wait();
-          if (cls == p.nclass - 1 && c0 + 32 >= p.n_tile) {   // last TMEM read of the tile: hand the accumulators back now
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(cempty0 + 8 * a);
-          }
-          __syncwarp();   // the previous block has been read back
-#pragma unroll
-          for (int c = 0; c < 8; ++c)
-            if (4 * c < ncol)
-              sts128(stg + (uint32_t)(lane * kEpiRowBytes + c * 16),
-                     make_float4(__uint_as_float(v[4 * c + 0]), __uint_as_float(v[4 * c + 1]), __uint_as_float(v[4 * c + 2]),
-                                 __uint_as_float(v[4 * c + 3])));
-          __syncwarp();
-          const int col = cbase + c0 + 4 * chunk;
-          if (4 * chunk < ncol && col < p.Cout) {
-            const float4 b = p.bias ? __ldg(reinterpret_cast<const float4*>(p.bias + col)) : make_float4(0.f, 0.f, 0.f, 0.f);   // (null: split-K partial sums)
-            float* colp = cls_out + col;
-            const uint32_t sbase = stg + (uint32_t)(sub * kEpiRowBytes + chunk * 16);
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              if (!((rowmask >> i) & 1u)) continue;
-              const float4 x = lds128(sbase + (uint32_t)(4 * i * kEpiRowBytes));
-              float4 o;
-              o.x = x.x + b.x; o.y = x.y + b.y; o.z = x.z + b.z; o.w = x.w + b.w;
-              // max(slope * x, x) with slope 0.1 (leaky ReLU, helpers.py:36-38) or 1 (identity, exact)
-              o.x = fmaxf(slope * o.x, o.x); o.y = fmaxf(slope * o.y, o.y);
-              o.z = fmaxf(slope * o.z, o.z); o.w = fmaxf(slope * o.w, o.w);
-              *reinterpret_cast<float4*>(colp + rowoff[i]) = o;
-            }
-          }
-        }
-      }
-    }
-    if (timed && q == 0 && lane == 0) { p.timing[blockIdx.x * 16 + 7] = w_cfull; p.timing[blockIdx.x * 16 + 11] = clock64() - t_begin; }
+    if (timed) { p.timing[blockIdx.x * 16 + 0] = w_aempty; p.timing[blockIdx.x * 16 + 1] = w_wempty; p.timing[blockIdx.x * 16 + 8] = clock64() - t_begin; }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
+  // ===== consumers ======================================================================================================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int wg = (warp >> 2) - 1;            // 0, 1: GEMM rows 64 wg .. 64 wg + 63
+  const int wq = warp & 3;                   // warp inside the warpgroup: rows + 16 wq
+  const int g = lane >> 2, tq = lane & 3;
+  const int m0 = 64 * wg + 16 * wq + g;      // this thread's GEMM rows m0 and m0 + 8
+  // tile-relative position of the two rows
+  int pos_y[2], pos_x[2], pos_n[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = m0 + 8 * h;
+    pos_x[h] = PER_TAP ? (m % p.tw) : (m & 7);
+    pos_y[h] = PER_TAP ? ((m / p.tw) % p.th) : (m >> 3);
+    pos_n[h] = PER_TAP ? (m / (p.tw * p.th)) : 0;
   }
+  const float slope = p.leaky ? 0.1f : 1.0f;
+  const uint32_t w_ring_u = smem_u32(w_ring);
+  long long w_afull = 0, w_wfull = 0;
+  const long long t_begin = clock64();
+  int sa = 0, slot = 0, l_res = 0;
+  uint32_t pa = 0, use = 0;
+  if (p.w_resident) wait_t(wres_bar, 0u, p.err, w_wfull);
+  pdl_wait();   // the output buffer may still be read (or written) by the previous kernel
+  float acc[NCLS][N / 2];
+  for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
+    const int tile = fast_div(item, p.ksplit, p.mul_ksplit);
+    const int z = item - tile * p.ksplit;
+    int nt, n, y0, x0;
+    halo_decode_tile<PER_TAP>(p, tile, nt, n, y0, x0);
+#pragma unroll
+    for (int k = 0; k < NCLS; ++k)
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) acc[k][i] = 0.f;
+    l_res = 0;
+    for (int kc = 0; kc < p.kc_split; ++kc) {
+      uint32_t abase = 0;
+      if (!PER_TAP) {
+        wait_t(afull0 + 8 * sa, pa, p.err, w_afull);
+        abase = smem_u32(smem + (size_t)sa * a_stage_bytes);
+      }
+      for (int t = 0; t < p.nsteps; ++t) {
+        if (PER_TAP) {
+          wait_t(afull0 + 8 * sa, pa, p.err, w_afull);
+          abase = smem_u32(smem + (size_t)sa * a_stage_bytes);
+        }
+        // the A fragment: channels 8 tq .. 8 tq + 7 of the two pixels (rows m0, m0 + 8)
+        float v[2][8];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (CIN8) {
+            const int rt = 4 * t + tq;   // this thread's tap of the group of four
+            const int pi = (rt < p.ntaps_real) ? p.g_plane[rt] : -1;
+            float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
+            if (pi >= 0) {
+              const HaloPlane& pl = p.planes[pi];
+              const uint32_t px = abase + (uint32_t)(pl.smem_off + p.g_aoff[rt] + (pos_y[h] * pl.cols + pos_x[h]) * 32);
+              a = lds128(px); b = lds128(px + 16);
+            }
+            v[h][0] = a.x; v[h][1] = a.y; v[h][2] = a.z; v[h][3] = a.w; v[h][4] = b.x; v[h][5] = b.y; v[h][6] = b.z; v[h][7] = b.w;
+          } else {
+            uint32_t row;
+            if (PER_TAP) {
+              row = abase + (uint32_t)((m0 + 8 * h) * 128);
+            } else {
+              const HaloPlane& pl = p.planes[p.st_plane[t]];
+              row = abase + (uint32_t)(pl.smem_off + p.st_aoff[t] + (pos_y[h] * pl.cols + pos_x[h]) * 128);
+            }
+            const uint32_t phase = (row >> 7) & 7u;   // 128-byte swizzle: 16-byte chunk c of the pixel lives at chunk c ^ phase
+            const float4 a = lds128(row + (((uint32_t)(2 * tq) ^ phase) << 4));
+            const float4 b = lds128(row + (((uint32_t)(2 * tq + 1) ^ phase) << 4));
+            v[h][0] = a.x; v[h][1] = a.y; v[h][2] = a.z; v[h][3] = a.w; v[h][4] = b.x; v[h][5] = b.y; v[h][6] = b.z; v[h][7] = b.w;
+          }
+        }
+        // slice j: a0 = (row g, col tq) = v[0][2j], a1 = (row g + 8, col tq), a2 = (row g, col tq + 4) = v[0][2j + 1], a3
+        uint32_t hi[16], lo[16];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float f[4] = {v[0][2 * j], v[1][2 * j], v[0][2 * j + 1], v[1][2 * j + 1]};
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const uint32_t u = __float_as_uint(f[e]);
+            hi[4 * j + e] = (MODE == 2) ? (u & 0xFFFFE000u) : u;
+            lo[4 * j + e] = __float_as_uint(f[e] - __uint_as_float(u & 0xFFFFE000u));
+          }
+        }
+        uint32_t wb;
+        if (p.w_resident) {
+          wb = w_ring_u + (uint32_t)(l_res++) * (uint32_t)p.w_stage_bytes;
+        } else {
+          wait_t(wfull0 + 8 * slot, use, p.err, w_wfull);
+          wb = w_ring_u + (uint32_t)slot * (uint32_t)p.w_stage_bytes;
+        }
+#pragma unroll
+        for (int k = 0; k < NCLS; ++k)
+#pragma unroll
+          for (int i = 0; i < N / 2; ++i) reg_fence(acc[k][i]);
+        wgmma_fence();
+        if (NCLS == 1) {
+          issue_block<N, MODE>(acc[0], hi, lo, wb);
+        } else {
+          const uint32_t cm = (uint32_t)p.st_cmask[t];
+#pragma unroll
+          for (int k = 0; k < NCLS; ++k)
+            if (cm & (1u << k)) {
+              issue_block<N, MODE>(acc[k], hi, lo, wb);
+              wb += (uint32_t)p.cls_bytes;
+            }
+        }
+        wgmma_commit();
+        wgmma_wait0();
+#pragma unroll
+        for (int k = 0; k < NCLS; ++k)
+#pragma unroll
+          for (int i = 0; i < N / 2; ++i) reg_fence(acc[k][i]);
+        __syncwarp();
+        if (lane == 0) {
+          if (!p.w_resident) mbar_arrive(wempty0 + 8 * slot);
+          if (PER_TAP) mbar_arrive(aempty0 + 8 * sa);
+        }
+        if (!p.w_resident && ++slot == kRing) { slot = 0; use ^= 1; }
+        if (PER_TAP && ++sa == p.sa) { sa = 0; pa ^= 1; }
+      }
+      if (!PER_TAP) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(aempty0 + 8 * sa);   // this warp is done reading the halo stage
+        if (++sa == p.sa) { sa = 0; pa ^= 1; }
+      }
+    }
+    // ---- epilogue: accumulator (row, col 8 i + 2 tq .. + 1) -> bias, leaky ReLU -> NHWC slice ------------------------
+    float* tile_out = p.out + (size_t)z * p.part_stride + ((size_t)(n * p.Hfull + y0 * p.osy) * p.Wfull + x0 * p.osx) * p.out_pitch;
+    const int cbase = nt * N;
+#pragma unroll
+    for (int k = 0; k < NCLS; ++k) {
+      if (k >= p.nclass) break;
+      float* cls_out = tile_out + (size_t)(p.cls_ooy[k] * p.Wfull + p.cls_oox[k]) * p.out_pitch;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (y0 + pos_y[h] >= p.Ho || x0 + pos_x[h] >= p.Wo || n + pos_n[h] >= p.B) continue;
+        float* orow = cls_out + ((size_t)(pos_n[h] * p.Hfull + pos_y[h] * p.osy) * p.Wfull + pos_x[h] * p.osx) * p.out_pitch;
+#pragma unroll
+        for (int i = 0; i < N / 8; ++i) {
+          const int col = cbase + 8 * i + 2 * tq;
+          if (col >= p.Cout) continue;
+          const float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col)) : make_float2(0.f, 0.f);   // (null: split-K partial sums)
+          float2 o;
+          o.x = acc[k][4 * i + 2 * h] + b.x;
+          o.y = acc[k][4 * i + 2 * h + 1] + b.y;
+          // max(slope * x, x) with slope 0.1 (leaky ReLU, helpers.py:36-38) or 1 (identity, exact)
+          o.x = fmaxf(slope * o.x, o.x); o.y = fmaxf(slope * o.y, o.y);
+          *reinterpret_cast<float2*>(orow + col) = o;
+        }
+      }
+    }
+  }
+  if (timed && threadIdx.x == 128) { p.timing[blockIdx.x * 16 + 6] = w_afull; p.timing[blockIdx.x * 16 + 3] = w_wfull; p.timing[blockIdx.x * 16 + 9] = clock64() - t_begin; }
 }
 
 // Split-K second pass: out[pix][c] = act(bias[c] + sum_z part[z][pix][c]); the partial buffers have the geometry of the
@@ -748,15 +447,6 @@ struct HaloPlan {
 static int pow2_ceil_h(int v) { int r = 1; while (r < v) r <<= 1; return r; }
 static int popcount4(int m) { return (m & 1) + ((m >> 1) & 1) + ((m >> 2) & 1) + ((m >> 3) & 1); }
 
-static int stager_groups() {
-  static const int g = []() {
-    const char* e = getenv("DEMON_STAGER_GROUPS");
-    int v = e ? atoi(e) : 2;
-    return (v < 1 || v > kMaxGroups) ? 2 : v;
-  }();
-  return g;
-}
-
 static bool w_resident_enabled() {   // DEMON_W_RESIDENT=0: weights always through the 4-slot ring (A/B measurements)
   static const bool v = []() { const char* e = getenv("DEMON_W_RESIDENT"); return !(e && e[0] == '0'); }();
   return v;
@@ -767,19 +457,14 @@ static bool splitk_enabled() {   // DEMON_TC_SPLITK=0: never split the K loop of
   return v;
 }
 
-static bool wave_model_enabled() {   // DEMON_WAVE_MODEL=0: N tile by width alone (A/B measurements)
-  static const bool v = []() { const char* e = getenv("DEMON_WAVE_MODEL"); return !(e && e[0] == '0'); }();
-  return v;
-}
-
 // Steps of one chunk: the distinct input shifts of all classes, each with the mask of the classes that use it.
 // max_cls: at most this many classes per step (a wide step needs a wide weight slot; a shift is repeated if necessary).
 struct ShiftStep { int ry, rx, qy, qx, cmask, tap[4]; };
 
-static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPlan& plan, bool encode) {
+static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPlan& plan, bool encode, bool force_per_tap) {
   const ConvProblem& p = probs[0];
   HaloParams& prm = plan.prm;
-  const int budget = 224 * 1024 - 4 * kEpiStageBytes;   // dynamic shared memory minus the epilogue's transpose buffers
+  const int budget = kSmemBudget;
   // candidates, widest first: classes per step (a wide step needs a wide weight slot), then the N tile cap
   struct Cand { int max_cls, n_cap; };
   std::vector<Cand> cands;
@@ -793,10 +478,9 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
     memset(plan.st_tap, -1, sizeof(plan.st_tap));
     prm.nclass = nclass;
     prm.nsplit = nsplit;
-    prm.ngroups = stager_groups();
     prm.cin8 = (p.Cin == 8) ? 1 : 0;
     const int px_bytes = prm.cin8 ? 32 : 128;   // bytes of one pixel of a halo plane in shared memory
-    prm.per_tap = ((p.Ho % kTileH) != 0 || (p.Wo % kTileW) != 0) ? 1 : 0;
+    prm.per_tap = (force_per_tap || (p.Ho % kTileH) != 0 || (p.Wo % kTileW) != 0) ? 1 : 0;
     if (prm.cin8 && (prm.per_tap || nclass != 1)) return false;
     // ---- steps ---------------------------------------------------------------------------------------------------
     std::vector<ShiftStep> steps;
@@ -835,10 +519,8 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
       }
       prm.planes[0].cols = prm.tw; prm.planes[0].rows = prm.th; prm.planes[0].bytes = 128 * 128;
       prm.a_region_bytes = 128 * 128;
-      prm.aempty_count = 4;     // the four stager warps of the group that consumed the shift release its shared-memory stage
       m_tiles = prm.tiles_x * prm.tiles_y * prm.tiles_b;
     } else {
-      prm.aempty_count = 4 * prm.ngroups;
       // planes: shifts grouped by stride parity
       struct PInfo { int ry, rx, qy_min, qy_max, qx_min, qx_max; };
       std::vector<PInfo> pinfo;
@@ -876,12 +558,9 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
       prm.tiles_x = ceil_div(p.Wo, kTileW); prm.tiles_y = ceil_div(p.Ho, kTileH); prm.tiles_b = p.B;
       m_tiles = prm.tiles_x * prm.tiles_y * p.B;
     }
-    // class / fresh masks, weight source of every (step, class)
-    int seen = 0;
+    // class masks, weight source of every (step, class)
     for (int t = 0; t < nreal; ++t) {
       prm.st_cmask[t] = steps[t].cmask;
-      prm.st_fmask[t] = steps[t].cmask & ~seen;
-      seen |= steps[t].cmask;
       for (int c = 0; c < 4; ++c) plan.st_tap[t][c] = steps[t].tap[c];
     }
     prm.nsteps = nreal;
@@ -889,44 +568,17 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
       prm.ntaps_real = nreal;
       for (int t = 0; t < nreal; ++t) { prm.g_plane[t] = prm.st_plane[t]; prm.g_aoff[t] = prm.st_aoff[t]; }
       prm.nsteps = (nreal + 3) / 4;
-      for (int t = 0; t < prm.nsteps; ++t) { prm.st_plane[t] = 0; prm.st_aoff[t] = 0; prm.st_cmask[t] = 1; prm.st_fmask[t] = (t == 0) ? 1 : 0; }
+      for (int t = 0; t < prm.nsteps; ++t) { prm.st_plane[t] = 0; prm.st_aoff[t] = 0; prm.st_cmask[t] = 1; }
     }
-    // ---- TMEM budget (512 columns): nbuf accumulator buffers x nclass x acc_w  +  the A-operand ring, kRing slots of 64
-    // columns (A_hi | A_lo of one shift).  acc_w = 2N in stacked 3xTF32 mode (big | small terms side by side), N otherwise.
-    const int ring_cols = kRing * 64;
+    // ---- N tile: one of the kernel's instantiations (16, 32, 64, 128), at most 64 per class when several classes share
+    // a step: the accumulators live in registers, N / 2 floats per thread and class (<= 128 of the consumers' 232).
     const int cout16 = (p.Cout + 15) / 16 * 16;
-    int n_tile = std::min(std::min(cout16, nsplit == 1 ? 256 : 128), cand.n_cap);
-    while (n_tile > 16 && nclass * n_tile + ring_cols > 512) n_tile = (n_tile > 32) ? (n_tile / 2 + 15) / 16 * 16 : n_tile - 16;
+    int n_tile = std::min(pow2_ceil_h(std::max(cout16, 16)), std::min(nclass > 1 ? 64 : 128, cand.n_cap));
     // narrow the N tile (down to 64) while the layer would leave SMs idle
-    while (n_tile >= 128 && (n_tile % 32) == 0 && (long)m_tiles * ceil_div(p.Cout, n_tile) < 148) n_tile /= 2;
-    // wave quantisation: a persistent grid of 148 CTAs needs ceil(tiles / 148) rounds.  A step costs ~800 cycles at N = 128
-    // (three-instruction 3xTF32) and ~470 at N = 64 (stacked): e.g. 192 tiles of N = 128 take 2 rounds x 800, the same layer
-    // as 384 tiles of N = 64 takes 3 x 470.  Pick the cheaper (single-class 3xTF32 layers; measured per-step costs).
-    if (wave_model_enabled() && nsplit == 3 && nclass == 1 && n_tile == 128 && p.Cout % 64 == 0) {
-      const long t128 = (long)m_tiles * ceil_div(p.Cout, 128), t64 = (long)m_tiles * ceil_div(p.Cout, 64);
-      const long c128 = ((t128 + 147) / 148) * 800, c64 = ((t64 + 147) / 148) * 470;
-      if (c64 * 100 < c128 * 95) n_tile = 64;
-    }
-    if (n_tile < 16 || nclass * n_tile + ring_cols > 512) return false;
+    while (n_tile >= 128 && (long)m_tiles * ceil_div(p.Cout, n_tile) < kPlanSms) n_tile /= 2;
     prm.mode = (nsplit == 1) ? 0 : 2;
-    if (nsplit == 3 && n_tile <= 64 && nclass * 2 * n_tile + ring_cols <= 512) prm.mode = 1;
-    // Three-instruction mode instead of the stacked one where the stacked accumulators would cost the double buffering (four
-    // classes of N = 32, netRefine/refine0: 0.626 -> 0.585 ms, the epilogue of tile i overlaps tile i + 1 again) and where the
-    // epilogue is the bound (8-channel layers: half the TMEM reads and no add per tile, conv1y 0.124 -> 0.119 ms).
-    // DEMON_TC_MODE2=0 switches both off (A/B), bit 0 = multi-class, bit 1 = 8-channel.
-    {
-      static const int mode2 = []() { const char* e = getenv("DEMON_TC_MODE2"); return e ? atoi(e) : 3; }();
-      if (prm.mode == 1 && (((mode2 & 1) && nclass == 4 && 2 * nclass * 2 * n_tile + ring_cols > 512 && 2 * nclass * n_tile + ring_cols <= 512) ||
-                            ((mode2 & 2) && prm.cin8)))
-        prm.mode = 2;
-    }
     prm.n_tile = n_tile;
-    prm.acc_w = (prm.mode == 1 ? 2 : 1) * n_tile;
-    prm.nbuf = (2 * nclass * prm.acc_w + ring_cols <= 512) ? 2 : 1;
     prm.n_tiles = ceil_div(p.Cout, n_tile);
-    int cols = 32;
-    while (cols < prm.nbuf * nclass * prm.acc_w + ring_cols) cols <<= 1;
-    prm.tmem_cols = cols;
     prm.k_chunks = prm.cin8 ? 1 : p.Cin / 32;
     // ---- weights: one class block = [W_hi ; W_lo] (3xTF32) or W alone, 1024-byte aligned; a step holds the blocks of its
     // classes in ascending class order; the ring slot is as large as the widest step
@@ -945,7 +597,7 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
     const int w_total = prm.k_chunks * prm.w_chunk_bytes;
     prm.w_resident = 0;
     prm.w_region_bytes = kRing * wmax;
-    if (w_resident_enabled() && nclass == 1 && prm.n_tiles == 1 && w_total <= 96 * 1024 && wmax * prm.nsteps == prm.w_chunk_bytes &&
+    if (w_resident_enabled() && !force_per_tap && nclass == 1 && prm.n_tiles == 1 && w_total <= 96 * 1024 && wmax * prm.nsteps == prm.w_chunk_bytes &&
         budget - w_total >= 2 * prm.a_region_bytes) {
       prm.w_resident = 1;
       prm.w_region_bytes = w_total;
@@ -953,7 +605,7 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
     const int rest = budget - prm.w_region_bytes;
     if (rest < 2 * prm.a_region_bytes) continue;   // next candidate: narrower steps / narrower N tile
     prm.sa = std::min(kMaxAStages, rest / prm.a_region_bytes);
-    plan.smem_bytes = prm.sa * prm.a_region_bytes + prm.w_region_bytes + 4 * kEpiStageBytes + 1024;
+    plan.smem_bytes = prm.sa * prm.a_region_bytes + prm.w_region_bytes + 1024;
     found = true;
     break;
   }
@@ -962,16 +614,15 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
   const int m_tiles = prm.tiles_x * prm.tiles_y * prm.tiles_b;
   prm.total_tiles = m_tiles * prm.n_tiles;
   // ---- split-K: layers with few tiles and a long K loop (the 6x8 / 12x16 levels; everything at batch 1) leave most SMs
-  // idle and run their K loop serially.  Cost model in cycles: rounds of 148 items x (steps of an item x ~600 + ~3000 of
-  // prologue / epilogue), + ~12000 for the second pass + the partial sums' trip through L2; a split has to win 10 %.
+  // idle and run their K loop serially.  Cost model in cycles: rounds of kPlanSms items x (steps of an item x ~600 + ~3000
+  // of prologue / epilogue), + ~12000 for the second pass + the partial sums' trip through L2; a split has to win 10 %.
   prm.ksplit = 1;
   if (splitk_enabled() && !prm.cin8 && !prm.w_resident && prm.k_chunks >= 4) {
-    // the partial sums travel to the second pass through L2 (~4000 B per cycle for write + read back): measured on
-    // netFlow2/refine3/upconv at batch 64 (25 MB of output), three slices win 8 %, not the 24 % the rounds alone promise
+    // the partial sums travel to the second pass through L2 (~4000 B per cycle for write + read back)
     const long out_bytes = (long)p.B * p.Hfull * p.Wfull * ((p.Cout + 3) / 4 * 4) * 4;
     auto cost = [&](int ks) {
       const long items = (long)prm.total_tiles * ks;
-      return ((items + 147) / 148) * ((long)(prm.k_chunks / ks) * prm.nsteps * 600 + 3000) + (ks > 1 ? 12000 + ks * out_bytes * 2 / 4000 : 0);
+      return ((items + kPlanSms - 1) / kPlanSms) * ((long)(prm.k_chunks / ks) * prm.nsteps * 600 + 3000) + (ks > 1 ? 12000 + ks * out_bytes * 2 / 4000 : 0);
     };
     long best = cost(1);
     for (int ks = 2; ks <= 8; ++ks) {
@@ -1028,19 +679,19 @@ bool tc_halo_supported(const ConvProblem* probs, int nclass) {
     if (probs[c].in != probs[0].in || probs[c].Cout != probs[0].Cout || probs[c].sy != probs[0].sy || probs[c].sx != probs[0].sx) return false;
   }
   HaloPlan plan;
-  return halo_build(probs, nclass, 3, plan, false);
+  return halo_build(probs, nclass, 3, plan, false, false);
 }
 
 // debug: the plan halo_build chooses for a layer, as text (no device needed)
 int tc_halo_describe(const ConvProblem* probs, int nclass, int nsplit, char* buf, int buflen) {
   HaloPlan plan;
-  if (!halo_build(probs, nclass, nsplit, plan, false)) return snprintf(buf, buflen, "halo: unsupported");
+  if (!halo_build(probs, nclass, nsplit, plan, false, false)) return snprintf(buf, buflen, "halo: unsupported");
   const HaloParams& q = plan.prm;
-  int n = snprintf(buf, buflen, "halo %s mode %d n_tile %d x%d nbuf %d tmem %d steps %d x %d chunks sa %d a_stage %d w_slot %d smem %d tiles %d groups %d ksplit %d wres %d |",
-                   q.per_tap ? "per-tap" : (q.cin8 ? "cin8" : "halo"), q.mode, q.n_tile, q.n_tiles, q.nbuf, q.tmem_cols, q.nsteps, q.k_chunks, q.sa,
-                   q.a_region_bytes, q.w_stage_bytes, plan.smem_bytes, q.total_tiles, q.ngroups, q.ksplit, q.w_resident);
+  int n = snprintf(buf, buflen, "halo %s mode %d n_tile %d x%d steps %d x %d chunks sa %d a_stage %d w_slot %d smem %d tiles %d ksplit %d wres %d |",
+                   q.per_tap ? "per-tap" : (q.cin8 ? "cin8" : "halo"), q.mode, q.n_tile, q.n_tiles, q.nsteps, q.k_chunks, q.sa,
+                   q.a_region_bytes, q.w_stage_bytes, plan.smem_bytes, q.total_tiles, q.ksplit, q.w_resident);
   for (int t = 0; t < q.nsteps && n < buflen - 32; ++t)
-    n += snprintf(buf + n, buflen - n, " [c%x f%x w%d+%d]", q.st_cmask[t], q.st_fmask[t], q.st_woff[t], q.st_wbytes[t]);
+    n += snprintf(buf + n, buflen - n, " [c%x w%d+%d]", q.st_cmask[t], q.st_woff[t], q.st_wbytes[t]);
   return n;
 }
 
@@ -1055,16 +706,17 @@ static float tf32_round_h(float x) {
   return r;
 }
 
-int tc_halo_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts, int nclass, int precision) {
+static int prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts, int nclass, int precision, bool per_tap) {
   const ConvProblem& p = probs[0];
   const int nsplit = (precision == DEMON_PREC_TF32) ? 1 : 3;
   HaloPlan* plan = new HaloPlan();
-  if (!halo_build(probs, nclass, nsplit, *plan, true)) {
+  if (!halo_build(probs, nclass, nsplit, *plan, true, per_tap)) {
     delete plan;
     return fail(DEMON_E_CUDA, "tc_halo_prepare: could not build the plan (tensor map encode failed?)");
   }
   const HaloParams& prm = plan->prm;
-  // weights: [n tile][chunk][step][class of the step] blocks of [W_hi | W_lo], n_tile rows x 32 fp32, K-major, pre-swizzled
+  // weights: [n tile][chunk][step][class of the step] blocks of [W_hi | W_lo], n_tile rows x 32 fp32, K-major, pre-swizzled;
+  // K position k of a row holds input channel kphys (the K order of the kernel's A fragment, see the top of this file)
   const size_t total = (size_t)prm.n_tiles * prm.k_chunks * prm.w_chunk_bytes;
   std::vector<unsigned char> packed(total, 0);
   for (int nt = 0; nt < prm.n_tiles; ++nt)
@@ -1079,12 +731,13 @@ int tc_halo_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_
           for (int r = 0; r < prm.n_tile; ++r) {
             const int co = nt * prm.n_tile + r;
             for (int k = 0; k < 32; ++k) {
+              const int kk = k & 7, kphys = 8 * (kk & 3) + 2 * (k >> 3) + (kk >> 2);
               float w = 0.f;
-              if (prm.cin8) {   // K index = (tap within the group of four, channel)
-                const int rt = 4 * tt + k / 8;
-                if (co < p.Cout && rt < prm.ntaps_real) w = w_hosts[0][((size_t)plan->st_tap[rt][0] * 8 + (k & 7)) * p.Cout_pad + co];
+              if (prm.cin8) {   // channel index = (tap within the group of four, channel)
+                const int rt = 4 * tt + kphys / 8;
+                if (co < p.Cout && rt < prm.ntaps_real) w = w_hosts[0][((size_t)plan->st_tap[rt][0] * 8 + (kphys & 7)) * p.Cout_pad + co];
               } else if (co < p.Cout) {
-                w = w_hosts[cls][((size_t)tap * p.Cin + kc * 32 + k) * p.Cout_pad + co];
+                w = w_hosts[cls][((size_t)tap * p.Cin + kc * 32 + kphys) * p.Cout_pad + co];
               }
               const float hi = (nsplit == 3) ? tf32_round_h(w) : w;
               const float lo = w - hi;
@@ -1111,6 +764,16 @@ int tc_halo_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_
   return DEMON_OK;
 }
 
+int tc_halo_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts, int nclass, int precision) {
+  return prepare(t, probs, w_hosts, nclass, precision, false);
+}
+
+int tc_layer_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts, int nclass, int precision) {
+  DEMON_REQUIRE(nclass >= 1 && nclass <= 4, "tc_layer_prepare: nclass %d", nclass);
+  for (int c = 0; c < nclass; ++c) DEMON_REQUIRE(tc_layer_supported(probs[c]), "tc_layer_prepare: unsupported shape");
+  return prepare(t, probs, w_hosts, nclass, precision, true);
+}
+
 void tc_halo_free(TcLayer& t) {
   if (t.halo_plan) delete static_cast<HaloPlan*>(t.halo_plan);
   t.halo_plan = nullptr;
@@ -1128,18 +791,35 @@ int tc_halo_read_timing(long long* host, int nblocks) {
   return 0;
 }
 
-template <bool PER_TAP, bool CIN8, int MODE>
-static int launch_variant(const HaloPlan* plan, const HaloParams& prm, int grid, int threads, cudaStream_t stream) {
+template <bool PER_TAP, bool CIN8, int MODE, int N, int NCLS>
+static int launch_variant(const HaloPlan* plan, const HaloParams& prm, int grid, cudaStream_t stream) {
   TcDeviceState& ds = tc_device_state();
-  const int slot = (PER_TAP ? 1 : 0) + (CIN8 ? 2 : 0) + 3 * MODE;
-  if (!(ds.halo_attr_set & (1u << slot))) {
-    DEMON_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_halo_kernel<PER_TAP, CIN8, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    ds.halo_attr_set |= 1u << slot;
+  static int attr_device = -1;   // per instantiation: the device whose shared-memory limit was raised last
+  if (attr_device != ds.device) {
+    DEMON_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_halo_kernel<PER_TAP, CIN8, MODE, N, NCLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+    attr_device = ds.device;
   }
-  cudaError_t le = launch_pdl(conv_tc_halo_kernel<PER_TAP, CIN8, MODE>, dim3(grid), dim3(threads), (size_t)plan->smem_bytes, stream, plan->maps, prm);
+  cudaError_t le = launch_pdl(conv_tc_halo_kernel<PER_TAP, CIN8, MODE, N, NCLS>, dim3(grid), dim3(kThreads), (size_t)plan->smem_bytes, stream, plan->maps, prm);
   if (le != cudaSuccess) return fail(DEMON_E_CUDA, "conv_tc_halo launch: %s", cudaGetErrorString(le));
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
+}
+
+template <bool PER_TAP, bool CIN8, int MODE, int NCLS>
+static int launch_n(const HaloPlan* plan, const HaloParams& prm, int grid, cudaStream_t stream) {
+  switch (prm.n_tile) {
+    case 16: return launch_variant<PER_TAP, CIN8, MODE, 16, NCLS>(plan, prm, grid, stream);
+    case 32: return launch_variant<PER_TAP, CIN8, MODE, 32, NCLS>(plan, prm, grid, stream);
+    case 64: return launch_variant<PER_TAP, CIN8, MODE, 64, NCLS>(plan, prm, grid, stream);
+    default: break;
+  }
+  if (NCLS == 1 && prm.n_tile == 128) return launch_variant<PER_TAP, CIN8, MODE, (NCLS == 1 ? 128 : 64), NCLS>(plan, prm, grid, stream);
+  return fail(DEMON_E_STATE, "conv_tc_halo: no kernel for N tile %d with %d classes", prm.n_tile, prm.nclass);
+}
+
+template <bool PER_TAP, bool CIN8, int NCLS>
+static int launch_mode(const HaloPlan* plan, const HaloParams& prm, int grid, cudaStream_t stream) {
+  return prm.mode == 0 ? launch_n<PER_TAP, CIN8, 0, NCLS>(plan, prm, grid, stream) : launch_n<PER_TAP, CIN8, 2, NCLS>(plan, prm, grid, stream);
 }
 
 int conv_tc_halo_launch(const TcLayer& t, const ConvProblem* probs, cudaStream_t stream) {
@@ -1148,7 +828,7 @@ int conv_tc_halo_launch(const TcLayer& t, const ConvProblem* probs, cudaStream_t
   prm.out = probs[0].out;          // the output slice may be re-pointed between calls (caller-owned result buffers)
   prm.out_pitch = probs[0].out_pitch;
   TcDeviceState& ds = tc_device_state();
-  if (!ds.err_dev) return fail(DEMON_E_CUDA, "tcgen05 path: no error flag on device %d", ds.device);
+  if (!ds.err_dev) return fail(DEMON_E_CUDA, "tensor-core path: no error flag on device %d", ds.device);
   prm.err = ds.err_dev;
   prm.timing = g_timing_dev;
   const int cpitch = (prm.Cout + 3) / 4 * 4;
@@ -1164,21 +844,10 @@ int conv_tc_halo_launch(const TcLayer& t, const ConvProblem* probs, cudaStream_t
     prm.leaky = 0;
   }
   const int grid = std::min(prm.total_items, ds.sms);
-  const int threads = 32 * (2 + 4 * prm.ngroups + 4 + 1);
   int rc;
-  if (prm.per_tap) {
-    if (prm.mode == 0) rc = launch_variant<true, false, 0>(plan, prm, grid, threads, stream);
-    else if (prm.mode == 1) rc = launch_variant<true, false, 1>(plan, prm, grid, threads, stream);
-    else rc = launch_variant<true, false, 2>(plan, prm, grid, threads, stream);
-  } else if (prm.cin8) {
-    if (prm.mode == 0) rc = launch_variant<false, true, 0>(plan, prm, grid, threads, stream);
-    else if (prm.mode == 1) rc = launch_variant<false, true, 1>(plan, prm, grid, threads, stream);
-    else rc = launch_variant<false, true, 2>(plan, prm, grid, threads, stream);
-  } else {
-    if (prm.mode == 0) rc = launch_variant<false, false, 0>(plan, prm, grid, threads, stream);
-    else if (prm.mode == 1) rc = launch_variant<false, false, 1>(plan, prm, grid, threads, stream);
-    else rc = launch_variant<false, false, 2>(plan, prm, grid, threads, stream);
-  }
+  if (prm.cin8) rc = launch_mode<false, true, 1>(plan, prm, grid, stream);
+  else if (prm.per_tap) rc = prm.nclass == 1 ? launch_mode<true, false, 1>(plan, prm, grid, stream) : launch_mode<true, false, 4>(plan, prm, grid, stream);
+  else rc = prm.nclass == 1 ? launch_mode<false, false, 1>(plan, prm, grid, stream) : launch_mode<false, false, 4>(plan, prm, grid, stream);
   if (rc != DEMON_OK || prm.ksplit == 1) return rc;
   const long long total = npix * (cpitch / 4);
   const int blocks = (int)std::min<long long>((total + 255) / 256, (long long)ds.sms * 8);

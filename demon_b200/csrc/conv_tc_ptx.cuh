@@ -1,4 +1,4 @@
-// PTX wrappers shared by the tcgen05 convolution kernels (sm_100a): mbarrier, TMA / bulk copies, TMEM, UMMA.
+// PTX wrappers of the tensor-core convolution kernel (sm_90a): mbarrier, TMA / bulk copies, wgmma.
 #pragma once
 #include <cuda.h>
 #include <cstdint>
@@ -63,9 +63,6 @@ __device__ __forceinline__ bool mbar_wait(uint32_t bar, uint32_t parity, int* er
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3, int c4) {
   asm volatile(
       "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
@@ -77,89 +74,27 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_
                "r"(bytes), "r"(bar)
                : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], kind::tf32, issued by one thread
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]: A = 128 lanes x 8 columns (one tf32 per 32-bit column, lane = GEMM row)
-__device__ __forceinline__ void umma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives on the mbarrier once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-        "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-        "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_x32(uint32_t taddr, const uint32_t* v) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]),
-        "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]),
-        "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous wgmma region
+__device__ __forceinline__ void reg_fence(float& x) { asm volatile("" : "+f"(x)::"memory"); }
 
-// Shared-memory matrix descriptor, K-major operand with 128-byte swizzle: rows of 128 bytes, 8-row groups 1024 bytes
-// apart (SBO), descriptor version 1 (Blackwell), layout type 2 = SWIZZLE_128B.  (cute/arch/mma_sm100_desc.hpp)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// Shared-memory matrix descriptor (sm_90 wgmma), K-major operand with 128-byte swizzle: rows of 128 bytes, 8-row groups
+// 1024 bytes apart (stride byte offset), layout type 1 = SWIZZLE_128B.  Advancing the start address by 32 bytes selects
+// the next K = 8 slice inside the swizzled rows.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);   // start address, bits [0,14)
-  d |= (uint64_t)0 << 16;                        // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)1 << 16;                        // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                        // version
-  d |= (uint64_t)2 << 61;                        // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                        // SWIZZLE_128B
   return d;
 }
 
-// Instruction descriptor for kind::tf32, fp32 accumulate, A and B K-major, M = 128 (cute/arch/mma_sm100_desc.hpp)
-__device__ __forceinline__ uint32_t umma_idesc_tf32(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-
-
 // elect.sync: exactly one lane of the (converged) warp gets `true`.  Unlike `lane == 0`, the compiler then KNOWS the
-// region runs with a single active thread and emits the uniform-datapath instructions (UTCHMMA, UTMALDG, UBLKCP, ...)
-// directly instead of wrapping each one in a per-thread serialisation loop (measured: ~90 cycles per MMA issue).
+// region runs with a single active thread and emits the uniform-datapath instructions (UTMALDG, UBLKCP, ...)
+// directly instead of wrapping each one in a per-thread serialisation loop.
 __device__ __forceinline__ bool elect_one_sync() {
   uint32_t pred;
   asm volatile("{\n.reg .b32 rx;\n.reg .pred px;\nelect.sync rx|px, 0xffffffff;\nselp.b32 %0, 1, 0, px;\n}" : "=r"(pred));
@@ -171,36 +106,5 @@ __device__ __forceinline__ float4 lds128(uint32_t addr) {
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
   return v;
 }
-__device__ __forceinline__ void sts128(uint32_t addr, const float4& v) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
-__device__ __forceinline__ float tf32_lo(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
-// two at a time with the packed fp32 pipe (sub.f32x2: one instruction for two subtractions; the result is exact either
-// way, x - trunc(x) only has bits below the truncation point)
-__device__ __forceinline__ void tf32_lo2(uint32_t x0, uint32_t x1, uint32_t& l0, uint32_t& l1) {
-  const uint32_t h0 = x0 & 0xFFFFE000u, h1 = x1 & 0xFFFFE000u;
-  asm("{\n.reg .b64 a, b, d;\nmov.b64 a, {%2, %3};\nmov.b64 b, {%4, %5};\nsub.f32x2 d, a, b;\nmov.b64 {%0, %1}, d;\n}"
-      : "=r"(l0), "=r"(l1)
-      : "r"(x0), "r"(x1), "r"(h0), "r"(h1));
-}
-
-// lo image = A - trunc_tf32(A) for `nvec` 16-byte vectors, 128 cooperating threads (t = 0..127); elementwise on the
-// swizzled bytes, so layout agnostic.  Four independent loads in flight per thread.
-__device__ __forceinline__ void split_region(uint32_t src, uint32_t dst, int nvec, int t) {
-  int i = t;
-  for (; i + 384 < nvec; i += 512) {
-    const float4 v0 = lds128(src + (uint32_t)i * 16u), v1 = lds128(src + (uint32_t)(i + 128) * 16u);
-    const float4 v2 = lds128(src + (uint32_t)(i + 256) * 16u), v3 = lds128(src + (uint32_t)(i + 384) * 16u);
-    sts128(dst + (uint32_t)i * 16u, make_float4(tf32_lo(v0.x), tf32_lo(v0.y), tf32_lo(v0.z), tf32_lo(v0.w)));
-    sts128(dst + (uint32_t)(i + 128) * 16u, make_float4(tf32_lo(v1.x), tf32_lo(v1.y), tf32_lo(v1.z), tf32_lo(v1.w)));
-    sts128(dst + (uint32_t)(i + 256) * 16u, make_float4(tf32_lo(v2.x), tf32_lo(v2.y), tf32_lo(v2.z), tf32_lo(v2.w)));
-    sts128(dst + (uint32_t)(i + 384) * 16u, make_float4(tf32_lo(v3.x), tf32_lo(v3.y), tf32_lo(v3.z), tf32_lo(v3.w)));
-  }
-  for (; i < nvec; i += 128) {
-    const float4 v = lds128(src + (uint32_t)i * 16u);
-    sts128(dst + (uint32_t)i * 16u, make_float4(tf32_lo(v.x), tf32_lo(v.y), tf32_lo(v.z), tf32_lo(v.w)));
-  }
-}
-
 }  // namespace
 }  // namespace demon

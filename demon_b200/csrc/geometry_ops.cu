@@ -1,8 +1,8 @@
 // Standalone geometry ops of the DeMoN hot path (the lmbspecialops ops the network threads between
-// its blocks) as HBM-roofline kernels for sm_100a.  All of them move a few bytes per pixel and do
+// its blocks) as HBM-roofline kernels for sm_90a.  All of them move a few bytes per pixel and do
 // almost no arithmetic, so the design rules are: one thread per (vector of) output pixel(s), the W
 // dimension on threadIdx.x so every warp reads and writes whole 128-byte lines, grids sized from the
-// tensor (they are far larger than 148 SMs at the benchmark sizes), no shared memory except the
+// tensor (they are far larger than 132 SMs at the benchmark sizes), no shared memory except the
 // per-sample camera.
 #include <cstdlib>
 #include "geometry.cuh"
@@ -372,7 +372,7 @@ static int leaky_relu_launch(const T* in, T* out, int64_t size, T leak, void* st
   if (size == 0) return DEMON_OK;
   DEMON_REQUIRE(in && out, "leaky_relu: null pointer");
   int64_t blocks = ceil_div64(ceil_div64(size, 16 / sizeof(T)), 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;   // 16 resident CTAs of 256 threads per SM, grid-stride beyond
+  if (blocks > 132 * 16) blocks = 132 * 16;   // 16 resident CTAs of 256 threads per SM, grid-stride beyond
   leaky_relu_kernel<T><<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(in, out, size, leak);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
@@ -535,7 +535,7 @@ __global__ void __launch_bounds__(128) sig_kernel(const T* __restrict__ in, T* _
 // float fast path: FOUR consecutive pixels per thread (W a multiple of 4, 16-byte aligned pointers, fewer than 2^31
 // elements).  The centre row and the row y + d are read as float4; the x neighbours x + d .. x + d + 3 come from the one or
 // two aligned groups that hold them.  Per pixel and delta the SAME sequence of IEEE operations as sig_kernel
-// (scaleinvariantgradient.cc:148-195): the ten divisions per pixel are what bounds the op (profiles/r02_ncu_ops.md).
+// (scaleinvariantgradient.cc:148-195): the ten divisions per pixel are what bounds the op.
 __global__ void __launch_bounds__(128) sig_v4_kernel(const float* __restrict__ in, float* __restrict__ out, int H, int W, int zbase,
                                                     SigParams<float> prm) {
   const int x = (blockIdx.x * 128 + threadIdx.x) * 4;
@@ -623,7 +623,7 @@ using namespace demon;
 extern "C" {
 
 const char* demon_last_error(void) { return last_error_ref().c_str(); }
-const char* demon_version(void) { return "demon_b200 0.1 sm_100a"; }
+const char* demon_version(void) { return "demon_b200 0.1 sm_90a"; }
 int64_t demon_launch_count(void) { return g_launch_count.load(); }
 
 int demon_warp2d_f32(const float* i, const float* d, float* o, int n, int c, int h, int w, int nm, int bm, float bv, void* s) {

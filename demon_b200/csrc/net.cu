@@ -153,7 +153,7 @@ void build_trunk(demon_net* n, const std::string& s, bool flow, bool iterative) 
     const int extra = flow ? 9 : (iterative ? 8 : 7);
     n->add_sep(s + "conv2_extra_inputs", 3, 1, n->extra_in, 0, extra, n->exy, 32, cat2, 32, 32);
     // the 7 / 8 / 9 real channels sit in a 32-channel (128-byte) pixel whose other channels are zero and carry zero weights:
-    // one K = 32 chunk of the tcgen05 halo kernel (3 steps per tile) instead of the fp32 SIMT kernel (0.10 -> 0.02 ms per launch)
+    // one K = 32 chunk of the tensor-core halo kernel (3 steps per tile) instead of the fp32 SIMT kernel
     n->by_name[s + "conv2_extra_inputsy"]->cin_buf = 32;
   }
   n->add_sep(s + "conv2_1", 3, 1, cat2, 0, 64, n->c21y, 64, n->concat2, 64, 64);
@@ -235,7 +235,7 @@ void build_plan(demon_net* n) {
   n->c4y = n->add_buf(12, 32, 256);
   n->c4 = n->add_buf(12, 16, 256);
   n->c41y = n->add_buf(12, 16, 256);
-  n->concat4 = n->add_buf(12, 16, 576);   // 512 + 2 (upsampled flow) padded to 18 chunks of 32 channels for the tcgen05 path (18 = 2 x 3 x 3: split-K)
+  n->concat4 = n->add_buf(12, 16, 576);   // 512 + 2 (upsampled flow) padded to 18 chunks of 32 channels for the tensor-core path (18 = 2 x 3 x 3: split-K)
   n->c5y = n->add_buf(6, 16, 512);
   n->c5 = n->add_buf(6, 8, 512);
   n->c51y = n->add_buf(6, 8, 512);
@@ -465,7 +465,7 @@ int strided_copy(const float* src, float* dst, int N, int P, int C, long sn, lon
   const long total = (long)N * P * C;
   if (total == 0) return DEMON_OK;
   long blocks = (total + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   (void)launch_pdl(strided_copy_kernel, dim3((int)blocks), dim3(256), 0, stream, src, dst, N, P, C, sn, sp, sc, dn, dp, dc);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
@@ -714,7 +714,7 @@ int run_refine_block(demon_net* n, const float* image1, long img_sn, long img_sp
                      int dh, int dw, float* depth0, cudaStream_t s) {
   const long total = (long)n->B * n->RH * n->RW;
   long blocks = (total + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   (void)launch_pdl(refine_input_kernel, dim3((int)blocks), dim3(256), 0, s, image1, img_sn, img_sp, img_sc, depth, d_sn, d_sp, n->rin->p, n->B, n->RH, n->RW, dh, dw);
   DEMON_LAUNCH_CHECK();
   // the last layer writes straight into the caller's output (C = 1: NHWC == NCHW)
@@ -869,7 +869,7 @@ int demon_check_errors(void) {
   cudaError_t e = cudaDeviceSynchronize();
   if (e != cudaSuccess) return fail(DEMON_E_CUDA, "demon_check_errors: %s", cudaGetErrorString(e));
   if (tc_read_error_flag(true))
-    return fail(DEMON_E_STATE, "a pipeline wait inside a tcgen05 convolution kernel timed out: results since the last check are invalid");
+    return fail(DEMON_E_STATE, "a pipeline wait inside a tensor-core convolution kernel timed out: results since the last check are invalid");
   return DEMON_OK;
 }
 int demon_debug_tc_timing(int enable, int64_t* host_out, int nblocks) {
@@ -926,7 +926,7 @@ int demon_net_layer_profile(const demon_net* n, int i, double* ms, int64_t* call
   if (ms) *ms = i < (int)n->prof_ms.size() ? n->prof_ms[i] : 0.0;
   if (calls) *calls = i < (int)n->prof_calls.size() ? n->prof_calls[i] : 0;
   if (launches_per_call) *launches_per_call = n->layers[i]->use_tc ? 1 : (n->layers[i]->kind == L_DECONV ? 4 : (n->layers[i]->ksplit > 1 ? 2 : 1));
-  // kernel family: 0 conv_simt_kernel, 1 conv_tc_kernel, 2 conv_tc_halo_kernel<false> (halo), 3 conv_tc_halo_kernel<true> (per tap)
+  // kernel family: 0 conv_simt_kernel, 2 conv_tc_halo_kernel (halo), 3 conv_tc_halo_kernel (per tap)
   if (uses_tc) *uses_tc = !n->layers[i]->use_tc ? 0 : (!n->layers[i]->tc.halo_plan ? 1 : (n->layers[i]->tc.per_tap ? 3 : 2));
   return DEMON_OK;
 }
@@ -1009,7 +1009,7 @@ static int pipeline_body(demon_net* n, const PipelineInput& in, int iterations, 
     // img8 straight from the bytes; image 2's planes go to c1y (free until conv1y runs) for the median pair
     float* planes2 = in.image2_2_u8 ? nullptr : n->c1y->p;
     long blocks = ((long)n->B * P + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;
     (void)launch_pdl(u8_import_kernel, dim3((int)blocks), dim3(256), 0, s, in.images_u8, n->img8->p, planes2, n->B, (int)P);
     DEMON_LAUNCH_CHECK();
     if (in.image2_2_u8) {
@@ -1167,7 +1167,7 @@ static int pipeline_host(demon_net* n, const void* images_host, const void* imag
   if (sync) {
     DEMON_CHECK_CUDA(cudaStreamSynchronize(s));
     if (tc_read_error_flag(true))
-      return fail(DEMON_E_STATE, "a pipeline wait inside a tcgen05 convolution kernel timed out: the outputs are invalid");
+      return fail(DEMON_E_STATE, "a pipeline wait inside a tensor-core convolution kernel timed out: the outputs are invalid");
   }
   return DEMON_OK;
 }
@@ -1255,7 +1255,7 @@ static int standalone_conv(const float* in, float* out, int B, int H, int W, int
     const bool halo = use_halo_kernel() && tc_halo_supported(probs, nclass);
     if (!all && !halo) {
       for (void* q : tmp.dev_allocs) cudaFree(q);
-      return fail(DEMON_E_INVALID, "conv test entry: shape not supported by the tcgen05 path");
+      return fail(DEMON_E_INVALID, "conv test entry: shape not supported by the tensor-core path");
     }
     if (halo) rc = tc_halo_prepare(l.tc, probs, ptrs, nclass, precision);
     else rc = tc_layer_prepare(l.tc, probs, ptrs, nclass, precision);

@@ -118,7 +118,7 @@ int elementwise_launch(const T* a, const T* b, T* out, int64_t size, T param, vo
   if (size == 0) return DEMON_OK;
   DEMON_REQUIRE(a && out && (OP == 1 || b), "%s: null pointer", what);
   int64_t blocks = ceil_div64(size, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   elementwise_kernel<T, OP><<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(a, b, out, size, param);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;

@@ -1,6 +1,6 @@
 """Mirror of the reference's op binding `lmbspecialops`
 (lmbspecialops/python/lmbspecialops/__init__.py:45-58,296-308; signatures documented in
-lmbspecialops/doc/lmbspecialops_doc.md) over the sm_100a kernels of libdemon_b200.so.
+lmbspecialops/doc/lmbspecialops_doc.md) over the sm_90a kernels of libdemon_b200.so.
 
 Same function names, keyword arguments, shape rules and error behaviour as the TensorFlow ops:
 

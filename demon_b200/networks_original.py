@@ -343,7 +343,7 @@ class DemonPipeline:
             return x.data_ptr() if isinstance(x, torch.Tensor) else x.ctypes.data
         _lib.check(_lib.load().demon_pipeline_forward_host(
             self.net.ptr, hp(image_pair), hp(image2_2), self.iterations, hp(depth0), hp(rotation), hp(translation), _stream()))
-        # (the C call synchronises and returns DEMON_E_STATE itself if a tcgen05 pipeline wait timed out)
+        # (the C call synchronises and returns DEMON_E_STATE itself if a tensor-core pipeline wait timed out)
 
     def forward_host_async(self, image_pair, image2_2, depth0, rotation, translation, stream=None):
         """forward_host without the final synchronisation, on `stream` (a torch.cuda.Stream; default: current).  The host

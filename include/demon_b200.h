@@ -1,5 +1,5 @@
 /*
- * demon_b200 -- C ABI of the B200-native DeMoN two-view inference path.
+ * demon_b200 -- C ABI of the H100-native (sm_90a) DeMoN two-view inference path.
  *
  * This is the drop-in boundary: every entry point replaces one TensorFlow
  * custom-op kernel (or one `session.run` of a network graph) of the reference
@@ -40,7 +40,7 @@ extern "C" {
 #define DEMON_ROT_ANGLEAXIS3 2
 
 const char* demon_last_error(void);
-/* "demon_b200 <version> sm_100a" */
+/* "demon_b200 <version> sm_90a" */
 const char* demon_version(void);
 /* number of kernels this library has launched in this process (bench.py's gpu_launches) */
 int64_t demon_launch_count(void);
@@ -151,8 +151,8 @@ typedef struct demon_net demon_net;
 
 /* precision of the tensor-core convolution path */
 #define DEMON_PREC_FP32_SIMT  0   /* CUDA-core fp32 FFMA for every layer                           */
-#define DEMON_PREC_3XTF32     1   /* tcgen05 kind::tf32 with error compensation (fp32-grade)       */
-#define DEMON_PREC_TF32       2   /* single-pass tcgen05 kind::tf32 (fast mode, ~1e-3 relative)    */
+#define DEMON_PREC_3XTF32     1   /* wgmma kind tf32 with error compensation (fp32-grade)         */
+#define DEMON_PREC_TF32       2   /* single-pass wgmma kind tf32 (fast mode, ~1e-3 relative)      */
 
 /* replaces BootstrapNet/IterativeNet/RefinementNet.__init__ (networks_original.py:22-57,92-152,202-234).
  * refine_h/refine_w: input size of the refinement block (192, 256 for the standard pipeline). */
@@ -227,7 +227,7 @@ int demon_net_batch(const demon_net* net);
 int64_t demon_net_workspace_bytes(const demon_net* net);
 /* number of kernel launches of one demon_pipeline_forward with `iterations` */
 int demon_net_pipeline_launches(const demon_net* net, int iterations);
-/* 1 if layer `tf_name` (e.g. "netRefine/conv1_1") runs on the tcgen05 path */
+/* 1 if layer `tf_name` (e.g. "netRefine/conv1_1") runs on the tensor-core path */
 int demon_net_layer_uses_tensor_cores(const demon_net* net, const char* tf_name);
 
 /* Per-layer device timing with CUDA events recorded on the launching stream around every layer of the
@@ -237,15 +237,15 @@ int demon_net_profile_begin(demon_net* net);
 int demon_net_profile_end(demon_net* net);
 int demon_net_num_layers(const demon_net* net);
 const char* demon_net_layer_name(const demon_net* net, int i);
-/* uses_tc: kernel family of the layer -- 0 conv_simt_kernel (fp32 CUDA cores), 1 conv_tc_kernel (tcgen05, operands in
- * shared memory), 2 conv_tc_halo_kernel<false> (tcgen05, halo tile, A operand in TMEM), 3 conv_tc_halo_kernel<true> (per tap) */
+/* uses_tc: kernel family of the layer -- 0 conv_simt_kernel (fp32 CUDA cores), 2 conv_tc_halo_kernel (wgmma, halo tile),
+ * 3 conv_tc_halo_kernel in per-tap mode (one TMA box per filter tap); 1 is not produced by this version */
 int demon_net_layer_profile(const demon_net* net, int i, double* ms, int64_t* calls, int* launches_per_call,
                             int* uses_tc);
 
-/* 1 if a pipeline wait inside a tcgen05 kernel has timed out on the current device since the flag was last
+/* 1 if a pipeline wait inside a tensor-core kernel has timed out on the current device since the flag was last
  * cleared (synchronises the device; does not clear). */
 int demon_debug_tc_timeouts(void);
-/* Synchronises the current device and returns DEMON_E_STATE if a bounded pipeline wait inside a tcgen05 convolution
+/* Synchronises the current device and returns DEMON_E_STATE if a bounded pipeline wait inside a tensor-core convolution
  * kernel timed out since the last check (such a kernel runs to completion with garbage instead of hanging the GPU),
  * DEMON_E_CUDA for a pending CUDA error, DEMON_OK otherwise.  Clears the flag.  The `_host` entry points that
  * synchronise call it themselves; callers of the asynchronous / device-pointer entry points call it after their own
@@ -267,7 +267,7 @@ int demon_debug_describe_conv(int B, int H, int W, int Cin, int in_pitch, int Co
  * demon_deconv4x4s2_nhwc call, in milliseconds (weight packing and uploads excluded); < 0 if none was timed */
 double demon_debug_last_conv_ms(void);
 
-/* Standalone convolution entry used by tests to compare the tcgen05 path with the fp32 SIMT path on
+/* Standalone convolution entry used by tests to compare the tensor-core path with the fp32 SIMT path on
  * the same NHWC tensors.  in [B,H,W,Cin], kernel TF layout [kh,kw,cin,cout] (host), bias [cout] (host)
  * -> out [B,ceil(H/sy),ceil(W/sx),Cout]; caffe padding (helpers.py:70-94). */
 int demon_conv2d_nhwc(const float* in, float* out, int B, int H, int W, int Cin, int Cout,

@@ -26,15 +26,15 @@ def test_header_symbols_are_exported_and_bound(lib):
     for name in declared:
         assert hasattr(lib, name), "library does not export %s" % name
     assert declared == set(_lib.PROTOTYPES), declared ^ set(_lib.PROTOTYPES)
-    assert lib.demon_version().decode().endswith("sm_100a")
+    assert lib.demon_version().decode().endswith("sm_90a")
 
 
-def test_library_is_sm100a_only():
-    """cuobjdump lists exactly one cubin architecture: sm_100a."""
+def test_library_is_sm90a_only():
+    """cuobjdump lists exactly one cubin architecture: sm_90a."""
     import subprocess
     out = subprocess.run(["cuobjdump", "--list-elf", _lib.lib_path()], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_no_cpu_fallback():

@@ -1,5 +1,5 @@
 """GPU: the convolution kernels through the C-ABI test entries, against torch-CPU float64 convolutions
-of the same tensors (the definitionally correct result).  fp32 SIMT path: fp32 rounding only.  tcgen05
+of the same tensors (the definitionally correct result).  fp32 SIMT path: fp32 rounding only.  tensor-core
 path: 3xTF32 must be fp32-grade, single-pass TF32 is the flagged fast mode (~1e-3)."""
 import ctypes
 
@@ -114,7 +114,7 @@ def test_simt_deconv_matches_float64(case):
     assert got.shape == ref.shape and rel_err(got, ref) < 5e-6
 
 
-# shapes the tcgen05 path takes (Cin % 32 == 0, Cout >= 16)
+# shapes the tensor-core path takes (Cin % 32 == 0, Cout >= 16)
 TC_CASES = [
     (2, 32, 16, 8, 32, 9, 1, 2, 1),      # conv1y: 8-channel mode (4 taps per K step)
     (1, 32, 24, 8, 32, 3, 3, 1, 1),      # netRefine/conv0 (4 -> 8 padded channels)
@@ -144,7 +144,7 @@ def test_tc_conv_3xtf32_is_fp32_grade(case):
     try:
         got = run_conv(x, k, b, sy, sx, True, X3TF32)
     except ValueError as e:
-        pytest.skip("shape not on the tcgen05 path: %s" % e)
+        pytest.skip("shape not on the tensor-core path: %s" % e)
     ref = ref_conv(x, k, b, sy, sx, True)
     simt = run_conv(x, k, b, sy, sx, True, FP32)
     assert got.shape == ref.shape
@@ -192,7 +192,7 @@ def test_tc_deconv_3xtf32_is_fp32_grade(case):
     try:
         got = run_deconv(x, k, b, True, X3TF32)
     except ValueError as e:
-        pytest.skip("shape not on the tcgen05 path: %s" % e)
+        pytest.skip("shape not on the tensor-core path: %s" % e)
     ref = ref_deconv(x, k, b, True)
     assert got.shape == ref.shape and not np.isnan(got).any()
     assert rel_err(got, ref) < 2e-5, rel_err(got, ref)

@@ -1,4 +1,4 @@
-"""GPU: the sm_100a geometry-op kernels against the CPU oracle, through the C ABI (via the
+"""GPU: the sm_90a geometry-op kernels against the CPU oracle, through the C ABI (via the
 lmbspecialops mirror).  Bit exact where the arithmetic is comparison / IEEE only, a few ulp where libm
 (sin/cos) or a different least-squares solver is involved; tolerances are written at each assert."""
 import os

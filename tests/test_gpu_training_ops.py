@@ -9,7 +9,7 @@ pytestmark = pytest.mark.gpu
 
 from oracle import ref
 
-needs_ref = pytest.mark.skipif(not ref.available(), reason="oracle/_ref is not built and /root/reference is absent")
+needs_ref = pytest.mark.skipif(not ref.available(), reason="neither oracle/_ref nor the stored reference results are present")
 TYPES = (np.float32, np.float64)
 
 
@@ -21,6 +21,8 @@ def ops():
 
 
 def bits_equal(a, b):
+    if isinstance(b, ref.Recorded):                # the stored digest of the reference kernel's output
+        return b.matches(a)
     a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
     if a.shape != b.shape or a.dtype != b.dtype:
         return False
@@ -92,7 +94,7 @@ def test_depth_to_normals_equals_reference_source(ops, dtype, inverse_depth):
     want = ref.depth_to_normals(d, K, inverse_depth)
     assert got.shape == (3, 3, 37, 141) and bits_equal(got, want)
     one = ops.depth_to_normals(d[0, 0], K[0], inverse_depth)                      # rank 2 depth, [4] intrinsics
-    assert one.shape == (1, 3, 37, 141) and bits_equal(one, want[:1])
+    assert one.shape == (1, 3, 37, 141) and bits_equal(one, got[:1])                 # got == want bit for bit (above)
     with pytest.raises(ValueError):
         ops.depth_to_normals(np.ones(5, dtype), K[0])
     with pytest.raises(ValueError):

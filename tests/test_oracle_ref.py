@@ -8,12 +8,14 @@ import pytest
 from oracle import ops as oops
 from oracle import ref
 
-pytestmark = pytest.mark.skipif(not ref.available(), reason="oracle/_ref is not built and /root/reference is absent")
+pytestmark = pytest.mark.skipif(not ref.available(), reason="neither oracle/_ref nor the stored reference results are present")
 
 TYPES = (np.float32, np.float64)
 
 
 def bits_equal(a, b):
+    if isinstance(b, ref.Recorded):                # the stored digest of the reference kernel's output
+        return b.matches(a)
     a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
     if a.shape != b.shape or a.dtype != b.dtype:
         return False

@@ -1,7 +1,7 @@
 """CPU: the tiling plans the halo planner picks for the DeMoN layers (demon_debug_describe_conv needs no device).
 
-These are the decisions DESIGN.md section 3.1 describes -- resident weights, split-K, the wave-aware N tile, the
-three-instruction mode for the epilogue-bound layers -- pinned here so that a planner change shows up as a test diff."""
+These are the decisions DESIGN.md section 3.1 describes -- resident weights, split-K, the N tile, the 3xTF32 mode --
+pinned here so that a planner change shows up as a test diff."""
 import ctypes
 import re
 
@@ -28,7 +28,7 @@ def plan():
 
 def test_resident_weights_for_the_narrow_single_n_tile_layers(plan):
     pd0 = plan(64, 192, 256, 64, 16, 3, 3, 1, 1)                 # netRefine/predict_depth0/conv1: 2 x 9 x 4 KB
-    assert (pd0["n_tile"], pd0["mode"], pd0["wres"], pd0["ksplit"]) == (16, 1, 1, 1)
+    assert (pd0["n_tile"], pd0["mode"], pd0["wres"], pd0["ksplit"]) == (16, 2, 1, 1)
     conv1x = plan(64, 96, 256, 32, 32, 1, 9, 1, 2)               # 9 x 8 KB
     assert conv1x["wres"] == 1 and conv1x["sa"] >= 2
     p2 = plan(64, 48, 64, 128, 24, 3, 3, 1, 1)                   # predict_flow2/conv1: 4 x 9 x 8 KB = 288 KB -> ring
@@ -37,9 +37,11 @@ def test_resident_weights_for_the_narrow_single_n_tile_layers(plan):
     assert (wide["n_tile"], wide["mode"], wide["wres"]) == (128, 2, 0)
 
 
-def test_wave_model_and_split_k(plan):
-    assert plan(64, 12, 32, 256, 256, 1, 5, 1, 2)["n_tile"] == 64       # conv4x: 384 tiles of N = 64 (3 rounds x 470) beat 192 of N = 128 (2 x 800)
-    assert plan(64, 24, 64, 128, 128, 1, 5, 1, 2)["n_tile"] == 128      # conv3x: 384 tiles of N = 128 stay
+def test_n_tile_and_split_k(plan):
+    conv4x = plan(64, 12, 32, 256, 256, 1, 5, 1, 2)              # 96 pixel tiles x 2 N tiles of 128 fill the 132 SMs
+    assert (conv4x["n_tile"], conv4x["tiles"]) == (128, 192)
+    assert plan(64, 24, 64, 128, 128, 1, 5, 1, 2)["n_tile"] == 128      # conv3x
+    assert plan(64, 6, 8, 128, 128, 3, 3, 1, 1)["n_tile"] == 64         # 24 pixel tiles: narrower N tiles for more CTAs
     pf5 = plan(64, 6, 8, 512, 24, 3, 3, 1, 1)                          # predict_flow5/conv1: 24 tiles, 144 steps each
     assert pf5["tiles"] == 24 and pf5["ksplit"] >= 2
     assert plan(64, 12, 16, 576, 128, 4, 4, 2, 2, deconv=1)["ksplit"] == 1   # refine3 at batch 64: the partial sums would cost more than the rounds save
@@ -47,10 +49,13 @@ def test_wave_model_and_split_k(plan):
     assert plan(1, 12, 16, 544, 128, 4, 4, 2, 2, deconv=1)["ksplit"] == 1    # 17 chunks: prime
 
 
-def test_three_instruction_mode_where_the_epilogue_or_the_double_buffer_matters(plan):
+def test_three_instruction_mode_and_register_accumulators(plan):
     conv1y = plan(64, 192, 256, 8, 32, 9, 1, 2, 1)                     # 8-channel input
     assert "cin8" in conv1y["text"] and conv1y["mode"] == 2
-    refine0 = plan(64, 96, 128, 128, 32, 4, 4, 2, 2, deconv=1)         # four classes of N = 32
-    assert (refine0["mode"], refine0["nbuf"]) == (2, 2)
-    refine1 = plan(64, 48, 64, 128, 64, 4, 4, 2, 2, deconv=1)          # four classes of N = 64: one buffer
-    assert (refine1["mode"], refine1["nbuf"]) == (2, 1)
+    # transposed convolutions: four classes of accumulators in registers, so at most N = 64 per class
+    refine0 = plan(64, 96, 128, 128, 32, 4, 4, 2, 2, deconv=1)
+    assert (refine0["mode"], refine0["n_tile"]) == (2, 32)
+    refine1 = plan(64, 48, 64, 128, 64, 4, 4, 2, 2, deconv=1)
+    assert (refine1["mode"], refine1["n_tile"]) == (2, 64)
+    refine3 = plan(64, 12, 16, 576, 128, 4, 4, 2, 2, deconv=1)
+    assert refine3["n_tile"] == 64 and "n_tile 64 x2" in refine3["text"]

@@ -64,21 +64,12 @@ def main():
     if timing:
         full = np.zeros((256, 16), np.int64)
         if lib.demon_debug_tc_timing(0, full.ctypes.data, 256) == 0:
-            buf = full[:148]
-            names = ["A-producer wait A_empty", "W-producer wait W_empty", "MMA wait accum_empty", "MMA wait T_full", "stager0 wait T_empty",
-                     "MMA wait W_full", "stager0 wait A_full", "epilogue wait accum_full", "A-producer total", "MMA total", "stager0 total",
-                     "epilogue total", "stager1 wait T_empty", "stager0: address math + shared loads issued", "stager0: tcgen05.st x2 + split + wait::st", "stager0: fence + arrive"]
+            buf = full[:132]
+            names = {0: "producer wait A_empty", 1: "producer wait W_empty", 3: "consumer wait W_full", 6: "consumer wait A_full",
+                     8: "producer total", 9: "consumer total"}
             m = buf.mean(axis=0)
-            for i, nm in enumerate(names):
+            for i, nm in names.items():
                 print("  %-44s %12.0f cycles (avg per CTA)" % (nm, m[i]))
-            ev = full.reshape(-1)[160 * 16:160 * 16 + 640].reshape(10, 64)
-            if ev.any():   # diagnostic build: event times of CTA 0, first 64 global steps of the LAST launch
-                t0 = ev[:9][ev[:9] > 0].min()
-                print("  step | stager: start  free[] seen  wait::st done  arrived | MMA: step entered  rdy  full[] seen  fenced  MMAs issued  commit issued   (cycles since the first event)")
-                for sidx in range(24, 48):
-                    obs, com, fre, arr, st0, stw, fen, iss, ent = (int(ev[k][sidx] - t0) if ev[k][sidx] else -1 for k in range(9))
-                    print("  %4d | %13d %12d %14d %8d | %17d %4d %12d %7d %12d %14d" % (sidx, st0, fre, stw, arr, ent, int(ev[9][sidx]), obs, fen, iss, com))
-
 
 if __name__ == "__main__":
     main()
