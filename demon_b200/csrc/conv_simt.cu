@@ -6,8 +6,6 @@
 // 256 threads, a BM x BN output tile (BM*BN = 4096), 4x4 outputs per thread, BK = 16, the A tile
 // gathered on the fly from the NHWC input (zero for padding taps), global loads of tile k+1 in flight
 // while tile k is multiplied out of shared memory.
-#include <cstdlib>
-
 #include "conv.cuh"
 
 namespace demon {
@@ -320,21 +318,16 @@ int conv_simt_launch(const ConvProblem& p, cudaStream_t stream) {
   DEMON_REQUIRE(M < (1ll << 31), "conv: too many output pixels");
   if (M == 0 || p.Cout == 0) return DEMON_OK;
   if (p.Cout <= 4 && p.Cin <= 32 && p.ntaps > 1 && p.partial == nullptr && p.Ho <= 65535 && p.B <= 65535) {
-    static const int pixel_mode = []() { const char* e = getenv("DEMON_SMALL_COUT_PIXEL"); return e ? atoi(e) : 2; }();   // 0: lane sharing everywhere, 1: pixel kernel everywhere, 2 (default, measured): lane sharing for Cout == 1 only
-    if (pixel_mode == 1 || (pixel_mode == 2 && p.Cout > 1)) {
-      dim3 g1(ceil_div(p.Wo, 128), p.Ho, p.B);
-      if (p.Cout == 1) SIMT_LAUNCH((conv_small_cout_pixel_kernel<1>), g1, 128, p);
-      else SIMT_LAUNCH((conv_small_cout_pixel_kernel<4>), g1, 128, p);
+    if (p.Cout > 1) {   // measured: one thread per pixel for Cout 2..4, lane sharing for Cout == 1 (see the kernels)
+      SIMT_LAUNCH((conv_small_cout_pixel_kernel<4>), dim3(ceil_div(p.Wo, 128), p.Ho, p.B), 128, p);
       DEMON_LAUNCH_CHECK();
       return DEMON_OK;
     }
     const int lpp = (p.Cin <= 16) ? 4 : 8;   // lanes per output pixel, one float4 of channels each
     dim3 grid(ceil_div(p.Wo, (128 / lpp) * kSmallCoutGroups), p.Ho, p.B);
     const bool nine = p.ntaps == 9;
-    if (p.Cout == 1 && lpp == 4) { if (nine) SIMT_LAUNCH((conv_small_cout_kernel<1, 4, 9>), grid, 128, p); else SIMT_LAUNCH((conv_small_cout_kernel<1, 4, 0>), grid, 128, p); }
-    else if (p.Cout == 1) { if (nine) SIMT_LAUNCH((conv_small_cout_kernel<1, 8, 9>), grid, 128, p); else SIMT_LAUNCH((conv_small_cout_kernel<1, 8, 0>), grid, 128, p); }
-    else if (lpp == 4) { if (nine) SIMT_LAUNCH((conv_small_cout_kernel<4, 4, 9>), grid, 128, p); else SIMT_LAUNCH((conv_small_cout_kernel<4, 4, 0>), grid, 128, p); }
-    else { if (nine) SIMT_LAUNCH((conv_small_cout_kernel<4, 8, 9>), grid, 128, p); else SIMT_LAUNCH((conv_small_cout_kernel<4, 8, 0>), grid, 128, p); }
+    if (lpp == 4) { if (nine) SIMT_LAUNCH((conv_small_cout_kernel<1, 4, 9>), grid, 128, p); else SIMT_LAUNCH((conv_small_cout_kernel<1, 4, 0>), grid, 128, p); }
+    else { if (nine) SIMT_LAUNCH((conv_small_cout_kernel<1, 8, 9>), grid, 128, p); else SIMT_LAUNCH((conv_small_cout_kernel<1, 8, 0>), grid, 128, p); }
     DEMON_LAUNCH_CHECK();
     return DEMON_OK;
   }

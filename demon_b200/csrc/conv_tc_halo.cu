@@ -32,11 +32,15 @@
 // instead of one small bulk copy per step.  Layers with few tiles split their K loop over several work items (split-K,
 // halo_splitk_reduce_kernel).  Variants: PER_TAP (images that are not made of whole 16 x 8 tiles: one 128-pixel TMA box per
 // step instead of a halo) and CIN8 (8-channel inputs: four taps x 8 channels per K = 32 step).
+//
+// Host side: tc_plan is the only place that decides whether a layer runs on this kernel and in which mode; tc_prepare
+// plans and packs a layer, conv_tc_launch launches it, and the per-device launch state and timeout flag live here too.
 #include <cuda.h>
 
 #include <algorithm>
-#include <cstdlib>
 #include <cstring>
+#include <memory>
+#include <mutex>
 #include <vector>
 
 #include "conv_tc.cuh"
@@ -447,21 +451,13 @@ struct HaloPlan {
 static int pow2_ceil_h(int v) { int r = 1; while (r < v) r <<= 1; return r; }
 static int popcount4(int m) { return (m & 1) + ((m >> 1) & 1) + ((m >> 2) & 1) + ((m >> 3) & 1); }
 
-static bool w_resident_enabled() {   // DEMON_W_RESIDENT=0: weights always through the 4-slot ring (A/B measurements)
-  static const bool v = []() { const char* e = getenv("DEMON_W_RESIDENT"); return !(e && e[0] == '0'); }();
-  return v;
-}
-
-static bool splitk_enabled() {   // DEMON_TC_SPLITK=0: never split the K loop of a tensor-core layer (A/B measurements)
-  static const bool v = []() { const char* e = getenv("DEMON_TC_SPLITK"); return !(e && e[0] == '0'); }();
-  return v;
-}
-
 // Steps of one chunk: the distinct input shifts of all classes, each with the mask of the classes that use it.
 // max_cls: at most this many classes per step (a wide step needs a wide weight slot; a shift is repeated if necessary).
 struct ShiftStep { int ry, rx, qy, qx, cmask, tap[4]; };
 
-static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPlan& plan, bool encode, bool force_per_tap) {
+// The tiling of one layer (no tensor maps, no weights).  force_per_tap: per-tap mode even for images made of whole
+// 16 x 8 tiles (the fallback for shapes the halo mode refuses).
+static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPlan& plan, bool force_per_tap) {
   const ConvProblem& p = probs[0];
   HaloParams& prm = plan.prm;
   const int budget = kSmemBudget;
@@ -597,7 +593,7 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
     const int w_total = prm.k_chunks * prm.w_chunk_bytes;
     prm.w_resident = 0;
     prm.w_region_bytes = kRing * wmax;
-    if (w_resident_enabled() && !force_per_tap && nclass == 1 && prm.n_tiles == 1 && w_total <= 96 * 1024 && wmax * prm.nsteps == prm.w_chunk_bytes &&
+    if (!force_per_tap && nclass == 1 && prm.n_tiles == 1 && w_total <= 96 * 1024 && wmax * prm.nsteps == prm.w_chunk_bytes &&
         budget - w_total >= 2 * prm.a_region_bytes) {
       prm.w_resident = 1;
       prm.w_region_bytes = w_total;
@@ -617,7 +613,7 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
   // idle and run their K loop serially.  Cost model in cycles: rounds of kPlanSms items x (steps of an item x ~600 + ~3000
   // of prologue / epilogue), + ~12000 for the second pass + the partial sums' trip through L2; a split has to win 10 %.
   prm.ksplit = 1;
-  if (splitk_enabled() && !prm.cin8 && !prm.w_resident && prm.k_chunks >= 4) {
+  if (!prm.cin8 && !prm.w_resident && prm.k_chunks >= 4) {
     // the partial sums travel to the second pass through L2 (~4000 B per cycle for write + read back)
     const long out_bytes = (long)p.B * p.Hfull * p.Wfull * ((p.Cout + 3) / 4 * 4) * 4;
     auto cost = [&](int ks) {
@@ -642,8 +638,40 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
   prm.out = p.out; prm.out_pitch = p.out_pitch; prm.Ho = p.Ho; prm.Wo = p.Wo; prm.Hfull = p.Hfull; prm.Wfull = p.Wfull;
   prm.osy = p.osy; prm.osx = p.osx; prm.Cout = p.Cout; prm.bias = p.bias; prm.leaky = p.leaky;
   for (int c = 0; c < nclass; ++c) { prm.cls_ooy[c] = probs[c].ooy; prm.cls_oox[c] = probs[c].oox; }
-  if (!encode) return true;
-  // TMA descriptors: 5-D view {sx*C, W/sx, sy, H/sy, B} of the input slice, one box shape per plane
+  return true;
+}
+
+// The shape rules of the kernel, for one problem
+static bool tc_shape_supported(const ConvProblem& p) {
+  const bool cin8 = p.Cin == 8 && p.in_pitch == 8;   // 8-channel mode: four taps x 8 channels per K = 32 step
+  if (!cin8 && (p.Cin < 32 || (p.Cin % 32) != 0)) return false;
+  if (p.Cout < 16 || (p.Cout % 4) != 0) return false;
+  if ((p.in_pitch % 4) != 0 || (p.out_pitch % 4) != 0) return false;
+  if ((reinterpret_cast<uintptr_t>(p.in) & 15) != 0 || (reinterpret_cast<uintptr_t>(p.out) & 15) != 0) return false;
+  if (p.sy < 1 || p.sx < 1 || (p.Hi % p.sy) != 0 || (p.Wi % p.sx) != 0) return false;
+  if (p.ntaps < 1 || p.ntaps > kMaxTaps) return false;
+  if (p.scale != nullptr) return false;
+  if (p.Ho != p.Hi / p.sy || p.Wo != p.Wi / p.sx) return false;
+  return true;
+}
+
+// The one decision of the tensor-core path: whether a layer gets a plan, and in which mode.  The halo plan picks the
+// per-tap mode itself for images not made of whole 16 x 8 tiles; shapes it refuses (e.g. more than kMaxPlanes stride-parity
+// planes) get the per-tap mode forced, which takes every 32-channel multiple but no 8-channel input.
+static bool tc_plan(const ConvProblem* probs, int nclass, int nsplit, HaloPlan& plan) {
+  if (nclass < 1 || nclass > 4) return false;
+  for (int c = 0; c < nclass; ++c) {
+    if (!tc_shape_supported(probs[c])) return false;
+    if (probs[c].in != probs[0].in || probs[c].Cout != probs[0].Cout || probs[c].sy != probs[0].sy || probs[c].sx != probs[0].sx) return false;
+  }
+  return halo_build(probs, nclass, nsplit, plan, false) || halo_build(probs, nclass, nsplit, plan, true);
+}
+
+static int nsplit_of(int precision) { return (precision == DEMON_PREC_TF32) ? 1 : 3; }
+
+// TMA descriptors: 5-D view {sx*C, W/sx, sy, H/sy, B} of the input slice, one box shape per plane
+static bool encode_maps(const ConvProblem& p, HaloPlan& plan) {
+  const HaloParams& prm = plan.prm;
   typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -670,22 +698,9 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
   return true;
 }
 
-bool tc_halo_supported(const ConvProblem* probs, int nclass) {
-  if (nclass < 1 || nclass > 4) return false;
-  for (int c = 0; c < nclass; ++c) {
-    ConvProblem q = probs[c];
-    if (q.Cin == 8 && q.in_pitch == 8) q.Cin = 32;   // 8-channel mode: everything but the channel rule must hold
-    if (!tc_layer_supported(q)) return false;
-    if (probs[c].in != probs[0].in || probs[c].Cout != probs[0].Cout || probs[c].sy != probs[0].sy || probs[c].sx != probs[0].sx) return false;
-  }
+int tc_describe(const ConvProblem* probs, int nclass, int precision, char* buf, int buflen) {
   HaloPlan plan;
-  return halo_build(probs, nclass, 3, plan, false, false);
-}
-
-// debug: the plan halo_build chooses for a layer, as text (no device needed)
-int tc_halo_describe(const ConvProblem* probs, int nclass, int nsplit, char* buf, int buflen) {
-  HaloPlan plan;
-  if (!halo_build(probs, nclass, nsplit, plan, false, false)) return snprintf(buf, buflen, "halo: unsupported");
+  if (!tc_plan(probs, nclass, nsplit_of(precision), plan)) return 0;
   const HaloParams& q = plan.prm;
   int n = snprintf(buf, buflen, "halo %s mode %d n_tile %d x%d steps %d x %d chunks sa %d a_stage %d w_slot %d smem %d tiles %d ksplit %d wres %d |",
                    q.per_tap ? "per-tap" : (q.cin8 ? "cin8" : "halo"), q.mode, q.n_tile, q.n_tiles, q.nsteps, q.k_chunks, q.sa,
@@ -706,14 +721,12 @@ static float tf32_round_h(float x) {
   return r;
 }
 
-static int prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts, int nclass, int precision, bool per_tap) {
+int tc_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts, int nclass, int precision) {
   const ConvProblem& p = probs[0];
-  const int nsplit = (precision == DEMON_PREC_TF32) ? 1 : 3;
-  HaloPlan* plan = new HaloPlan();
-  if (!halo_build(probs, nclass, nsplit, *plan, true, per_tap)) {
-    delete plan;
-    return fail(DEMON_E_CUDA, "tc_halo_prepare: could not build the plan (tensor map encode failed?)");
-  }
+  const int nsplit = nsplit_of(precision);
+  std::unique_ptr<HaloPlan> plan(new HaloPlan());
+  if (!tc_plan(probs, nclass, nsplit, *plan)) return kTcNoPlan;
+  if (!encode_maps(p, *plan)) return fail(DEMON_E_CUDA, "tc_prepare: tensor map encode failed");
   const HaloParams& prm = plan->prm;
   // weights: [n tile][chunk][step][class of the step] blocks of [W_hi | W_lo], n_tile rows x 32 fp32, K-major, pre-swizzled;
   // K position k of a row holds input channel kphys (the K order of the kernel's A fragment, see the top of this file)
@@ -750,33 +763,63 @@ static int prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_h
       }
   void* dw = nullptr;
   cudaError_t e = cudaMalloc(&dw, total);
-  if (e == cudaSuccess) e = cudaMemcpy(dw, packed.data(), total, cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) { delete plan; return fail(DEMON_E_CUDA, "tc_halo_prepare: %s", cudaGetErrorString(e)); }
+  if (e == cudaSuccess) {
+    e = cudaMemcpy(dw, packed.data(), total, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) cudaFree(dw);
+  }
+  if (e != cudaSuccess) return fail(DEMON_E_CUDA, "tc_prepare: %s", cudaGetErrorString(e));
   plan->prm.w = static_cast<const unsigned char*>(dw);
-  t.w_packed = dw;
-  t.halo_plan = plan;
-  t.per_tap = prm.per_tap;
-  t.nclass = nclass;
-  t.n_tile = prm.n_tile; t.n_tiles = prm.n_tiles; t.k_chunks = prm.k_chunks; t.nsplit = nsplit;
-  t.th = kTileH; t.tw = kTileW; t.tb = 1; t.stages = prm.sa; t.smem_bytes = plan->smem_bytes;
-  t.ksplit = prm.ksplit;
+  t.per_tap = prm.per_tap != 0;
   t.splitk_bytes = (prm.ksplit > 1) ? (size_t)prm.ksplit * p.B * p.Hfull * p.Wfull * ((p.Cout + 3) / 4 * 4) * sizeof(float) : 0;
+  t.plan = plan.release();
   return DEMON_OK;
 }
 
-int tc_halo_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts, int nclass, int precision) {
-  return prepare(t, probs, w_hosts, nclass, precision, false);
+void tc_layer_free(TcLayer& t) {
+  if (t.plan) {
+    cudaFree(const_cast<unsigned char*>(t.plan->prm.w));
+    delete t.plan;
+  }
+  t.plan = nullptr;
 }
 
-int tc_layer_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts, int nclass, int precision) {
-  DEMON_REQUIRE(nclass >= 1 && nclass <= 4, "tc_layer_prepare: nclass %d", nclass);
-  for (int c = 0; c < nclass; ++c) DEMON_REQUIRE(tc_layer_supported(probs[c]), "tc_layer_prepare: unsupported shape");
-  return prepare(t, probs, w_hosts, nclass, precision, true);
+// Per-DEVICE launch state (one process may drive several GPUs): the dynamic shared-memory attribute has to be set on
+// every device a kernel is launched on, the SM count and the pipeline-timeout flag live on the device.
+// tc_device_state() returns the state of the CURRENT device (cudaGetDevice), creating it on first use.
+struct TcDeviceState {
+  int device = -1;
+  int sms = 132;
+  int* err_dev = nullptr;   // device int: set to 1 by a bounded mbarrier wait that timed out
+};
+
+static TcDeviceState& tc_device_state() {
+  constexpr int kMaxDevices = 64;
+  static TcDeviceState states[kMaxDevices];
+  static std::mutex mu;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= kMaxDevices) dev = 0;
+  std::lock_guard<std::mutex> lock(mu);
+  TcDeviceState& s = states[dev];
+  if (s.device != dev) {
+    s = TcDeviceState();
+    s.device = dev;
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    s.sms = sms > 0 ? sms : 132;
+    if (cudaMalloc(&s.err_dev, sizeof(int)) == cudaSuccess) cudaMemset(s.err_dev, 0, sizeof(int));
+    else s.err_dev = nullptr;
+  }
+  return s;
 }
 
-void tc_halo_free(TcLayer& t) {
-  if (t.halo_plan) delete static_cast<HaloPlan*>(t.halo_plan);
-  t.halo_plan = nullptr;
+int tc_read_error_flag(bool clear) {
+  TcDeviceState& ds = tc_device_state();
+  if (!ds.err_dev) return 0;
+  int v = 0;
+  cudaMemcpy(&v, ds.err_dev, sizeof(int), cudaMemcpyDeviceToHost);
+  if (v && clear) cudaMemset(ds.err_dev, 0, sizeof(int));
+  return v;
 }
 
 static long long* g_timing_dev = nullptr;
@@ -822,8 +865,8 @@ static int launch_mode(const HaloPlan* plan, const HaloParams& prm, int grid, cu
   return prm.mode == 0 ? launch_n<PER_TAP, CIN8, 0, NCLS>(plan, prm, grid, stream) : launch_n<PER_TAP, CIN8, 2, NCLS>(plan, prm, grid, stream);
 }
 
-int conv_tc_halo_launch(const TcLayer& t, const ConvProblem* probs, cudaStream_t stream) {
-  HaloPlan* plan = static_cast<HaloPlan*>(t.halo_plan);
+int conv_tc_launch(const TcLayer& t, const ConvProblem* probs, cudaStream_t stream) {
+  const HaloPlan* plan = t.plan;
   HaloParams prm = plan->prm;
   prm.out = probs[0].out;          // the output slice may be re-pointed between calls (caller-owned result buffers)
   prm.out_pitch = probs[0].out_pitch;

@@ -20,8 +20,7 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("{\n.reg .b64 st;\nmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n}" ::"r"(bar), "r"(bytes) : "memory");
 }
-// Bounded wait: a pipeline bug must not hang the GPU; on timeout the error flag is raised and the kernel runs to
-// completion with garbage (the host checks the flag in tests).
+// One try_wait on the phase `parity` (the bounded wait around it, wait_t, is in conv_tc_halo.cu).
 __device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
   uint32_t done;
   asm volatile(
@@ -33,36 +32,7 @@ __device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
       : "memory");
   return done != 0;
 }
-// non-blocking probe (try_wait may suspend the thread for a hardware time-out when the phase is still pending)
-__device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  asm volatile(
-      "{\n.reg .pred p;\n"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n}"
-      : "=r"(done)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return done != 0;
-}
-__device__ __noinline__ bool mbar_wait_slow(uint32_t bar, uint32_t parity, int* err) {
-  const long long t0 = clock64();
-  for (;;) {
-    for (int i = 0; i < 64; ++i)
-      if (mbar_try(bar, parity)) return true;
-    if (*reinterpret_cast<volatile int*>(err) != 0) return false;   // somebody already timed out: drain quickly
-    if (clock64() - t0 > kTimeoutCycles) {
-      atomicExch(err, 1);
-      return false;
-    }
-  }
-}
-__device__ __forceinline__ bool mbar_wait(uint32_t bar, uint32_t parity, int* err) {
-  if (mbar_try(bar, parity)) return true;
-  return mbar_wait_slow(bar, parity, err);
-}
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3, int c4) {
   asm volatile(
       "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"

@@ -6,6 +6,7 @@
 // geometry ops between the blocks (blocks_original.py:155-187,336-366) run as two fused glue kernels
 // that produce the `conv2_extra_inputs` tensor directly, and nothing on the forward path allocates,
 // synchronises or touches the host.
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <map>
@@ -56,8 +57,8 @@ struct Layer {
   float* w_dev[4] = {nullptr, nullptr, nullptr, nullptr};  // 1 (conv/dense) or 4 (deconv parity classes)
   float* bias_dev = nullptr;
   // tensor-core path
-  bool use_tc = false;
   TcLayer tc;
+  bool use_tc() const { return tc.plan != nullptr; }
   // split-K for dense layers (SIMT path)
   int ksplit = 1;
 };
@@ -338,12 +339,6 @@ void fill_problem(const Layer& l, int B, ConvProblem& p) {
   p.osy = p.osx = 1;
 }
 
-// DEMON_TC_HALO=0 keeps every tensor-core layer on the per-tap kernel (A/B measurements)
-bool use_halo_kernel() {
-  const char* e = getenv("DEMON_TC_HALO");
-  return !(e && e[0] == '0');
-}
-
 // The convolution problem(s) of a layer: 1 for conv / dense, 4 sub-pixel classes for a transposed conv.
 int build_problems(const Layer& l, int B, ConvProblem* out) {
   ConvProblem p;
@@ -390,9 +385,9 @@ int build_problems(const Layer& l, int B, ConvProblem* out) {
 int run_layer(const Layer& l, int B, cudaStream_t stream, float* splitk_ws = nullptr, float* tc_ws = nullptr) {
   ConvProblem probs[4];
   const int nclass = build_problems(l, B, probs);
-  if (l.use_tc) {
+  if (l.use_tc()) {
     probs[0].partial = tc_ws;   // scratch of the split-K tensor-core layers (the net's, so two nets in flight do not share it)
-    return l.tc.halo_plan ? conv_tc_halo_launch(l.tc, probs, stream) : conv_tc_launch(l.tc, probs, stream);
+    return conv_tc_launch(l.tc, probs, stream);
   }
   for (int c = 0; c < nclass; ++c) {
     if (l.kind == L_DENSE && l.ksplit > 1 && splitk_ws) { probs[c].partial = splitk_ws; probs[c].ksplit = l.ksplit; }
@@ -401,6 +396,57 @@ int run_layer(const Layer& l, int B, cudaStream_t stream, float* splitk_ws = nul
   }
   return DEMON_OK;
 }
+
+// Uploads a layer's bias and its kernel (TF layout) packed for the SIMT path; at a tensor-core precision the planner
+// (tc_prepare) then decides whether the layer runs on the tensor cores and packs the kernel for them.
+int upload_layer(demon_net* n, Layer& l, const HostVar& k, const float* bias_host) {
+  std::vector<float> bias(l.cout_pad, 0.f);
+  std::copy(bias_host, bias_host + l.cout, bias.begin());
+  int rc;
+  if ((rc = upload(n, bias, &l.bias_dev))) return rc;
+  std::vector<float> w[4];
+  const float* w_hosts[4] = {nullptr, nullptr, nullptr, nullptr};
+  const int nw = (l.kind == L_DECONV) ? 4 : 1;
+  for (int c = 0; c < nw; ++c) {
+    if (l.kind == L_CONV) pack_conv(l, k, w[c]);
+    else if (l.kind == L_DENSE) pack_dense(l, k, w[c]);
+    else pack_deconv_class(l, k, c / 2, c % 2, w[c]);
+    if ((rc = upload(n, w[c], &l.w_dev[c]))) return rc;
+    w_hosts[c] = w[c].data();
+  }
+  if (n->precision == DEMON_PREC_FP32_SIMT || l.kind == L_DENSE) return DEMON_OK;
+  ConvProblem probs[4];
+  const int nclass = build_problems(l, n->B, probs);
+  rc = tc_prepare(l.tc, probs, w_hosts, nclass, n->precision);
+  return (rc == kTcNoPlan) ? DEMON_OK : rc;
+}
+
+// The plan line of a layer: the tensor-core planner's, or "simt" for a layer it does not take.
+int describe_layer(const Layer& l, int B, int precision, char* buf, int buflen) {
+  if (l.kind == L_DENSE) return snprintf(buf, buflen, "dense simt");
+  ConvProblem probs[4];
+  const int nclass = build_problems(l, B, probs);
+  const int len = (precision != DEMON_PREC_FP32_SIMT) ? tc_describe(probs, nclass, precision, buf, buflen) : 0;
+  return (len > 0) ? len : snprintf(buf, buflen, "simt");
+}
+
+// A layer outside any net (the standalone entries): a convolution, or with `deconv` a k4 s2 transposed convolution, of
+// an NHWC [B,H,W,in_pitch] input into an NHWC output of channel pitch out_pitch.
+struct StandaloneLayer {
+  Buf in, out;
+  Layer layer;
+  StandaloneLayer(const float* in_p, float* out_p, int H, int W, int Cin, int in_pitch, int Cout, int out_pitch, int kh, int kw, int sy,
+                  int sx, bool deconv, bool leaky) {
+    in.p = const_cast<float*>(in_p); in.H = H; in.W = W; in.C = in_pitch;
+    out.p = out_p; out.C = out_pitch;
+    if (deconv) { out.H = 2 * H; out.W = 2 * W; } else { out.H = ceil_div(H, sy); out.W = ceil_div(W, sx); }
+    Layer& l = layer;
+    l.name = "standalone"; l.kind = deconv ? L_DECONV : L_CONV; l.in = &in; l.cin = Cin; l.cin_buf = (Cin + 3) / 4 * 4; l.out = &out;
+    l.cout = Cout; l.cout_pad = (Cout + 3) / 4 * 4; l.kh = kh; l.kw = kw; l.sy = sy; l.sx = sx; l.leaky = leaky;
+  }
+  StandaloneLayer(const StandaloneLayer&) = delete;             // `layer` points at `in` and `out`
+  StandaloneLayer& operator=(const StandaloneLayer&) = delete;
+};
 
 int run_layer_profiled(demon_net* n, int idx, cudaStream_t stream) {
   const Layer& l = *n->layers[idx];
@@ -806,53 +852,14 @@ int demon_net_finalize(demon_net* n) {
   if (n->finalized) return DEMON_OK;
   for (auto& nm : n->var_names)
     if (!n->host_vars.count(nm)) return fail(DEMON_E_STATE, "demon_net_finalize: variable %s was not set", nm.c_str());
-  std::vector<float> packed, bias;
   for (auto& lp : n->layers) {
     Layer& l = *lp;
-    const HostVar& k = n->host_vars[l.name + "/kernel"];
-    const HostVar& b = n->host_vars[l.name + "/bias"];
-    bias.assign(l.cout_pad, 0.f);
-    for (int i = 0; i < l.cout; ++i) bias[i] = b.data[i];
-    int rc;
-    if ((rc = upload(n, bias, &l.bias_dev))) return rc;
-    if (l.kind == L_CONV) {
-      pack_conv(l, k, packed);
-      if ((rc = upload(n, packed, &l.w_dev[0]))) return rc;
-    } else if (l.kind == L_DENSE) {
-      pack_dense(l, k, packed);
-      if ((rc = upload(n, packed, &l.w_dev[0]))) return rc;
-    } else {
-      for (int py = 0; py < 2; ++py)
-        for (int px = 0; px < 2; ++px) {
-          pack_deconv_class(l, k, py, px, packed);
-          if ((rc = upload(n, packed, &l.w_dev[py * 2 + px]))) return rc;
-        }
-    }
-    // tensor-core eligibility and packing
-    if (n->precision != DEMON_PREC_FP32_SIMT && l.kind != L_DENSE) {
-      ConvProblem probs[4];
-      const int nclass = build_problems(l, n->B, probs);
-      bool all = true;
-      for (int c = 0; c < nclass; ++c) all = all && tc_layer_supported(probs[c]);
-      const bool halo = use_halo_kernel() && tc_halo_supported(probs, nclass);   // also takes the 8-channel layers
-      if (all || halo) {
-        std::vector<float> cls_w[4];
-        const float* ptrs[4] = {nullptr, nullptr, nullptr, nullptr};
-        for (int c = 0; c < nclass; ++c) {
-          if (l.kind == L_CONV) pack_conv(l, k, cls_w[c]); else pack_deconv_class(l, k, c / 2, c % 2, cls_w[c]);
-          ptrs[c] = cls_w[c].data();
-        }
-        if (halo) rc = tc_halo_prepare(l.tc, probs, ptrs, nclass, n->precision);
-        else rc = tc_layer_prepare(l.tc, probs, ptrs, nclass, n->precision);
-        if (rc) return rc;
-        l.use_tc = true;
-      }
-    }
+    const int rc = upload_layer(n, l, n->host_vars[l.name + "/kernel"], n->host_vars[l.name + "/bias"].data.data());
+    if (rc) return rc;
   }
   // scratch of the split-K tensor-core layers: the largest need, owned by the net
   size_t need = 0;
-  for (auto& lp : n->layers)
-    if (lp->use_tc) need = std::max(need, lp->tc.splitk_bytes);
+  for (auto& lp : n->layers) need = std::max(need, lp->tc.splitk_bytes);
   if (need) {
     void* q = nullptr;
     DEMON_CHECK_CUDA(cudaMalloc(&q, need));
@@ -887,7 +894,7 @@ int demon_net_pipeline_launches(const demon_net* n, int iterations) {
 int demon_net_layer_uses_tensor_cores(const demon_net* n, const char* name) {
   if (!n || !name) return 0;
   auto it = n->by_name.find(name);
-  return (it != n->by_name.end() && it->second->use_tc) ? 1 : 0;
+  return (it != n->by_name.end() && it->second->use_tc()) ? 1 : 0;
 }
 
 int demon_net_profile_begin(demon_net* n) {
@@ -925,9 +932,10 @@ int demon_net_layer_profile(const demon_net* n, int i, double* ms, int64_t* call
   DEMON_REQUIRE(n && i >= 0 && i < (int)n->layers.size(), "layer index");
   if (ms) *ms = i < (int)n->prof_ms.size() ? n->prof_ms[i] : 0.0;
   if (calls) *calls = i < (int)n->prof_calls.size() ? n->prof_calls[i] : 0;
-  if (launches_per_call) *launches_per_call = n->layers[i]->use_tc ? 1 : (n->layers[i]->kind == L_DECONV ? 4 : (n->layers[i]->ksplit > 1 ? 2 : 1));
+  const Layer& l = *n->layers[i];
+  if (launches_per_call) *launches_per_call = l.use_tc() ? 1 : (l.kind == L_DECONV ? 4 : (l.ksplit > 1 ? 2 : 1));
   // kernel family: 0 conv_simt_kernel, 2 conv_tc_halo_kernel (halo), 3 conv_tc_halo_kernel (per tap)
-  if (uses_tc) *uses_tc = !n->layers[i]->use_tc ? 0 : (!n->layers[i]->tc.halo_plan ? 1 : (n->layers[i]->tc.per_tap ? 3 : 2));
+  if (uses_tc) *uses_tc = !l.use_tc() ? 0 : (l.tc.per_tap ? 3 : 2);
   return DEMON_OK;
 }
 
@@ -1177,20 +1185,9 @@ int demon_debug_describe_layers(const demon_net* n, char* buf, int buflen) {
   DEMON_REQUIRE(n && buf && buflen > 0, "describe: null");
   int off = 0;
   for (auto& lp : n->layers) {
-    const Layer& l = *lp;
     if (off >= buflen - 256) break;
-    off += snprintf(buf + off, buflen - off, "%-40s ", l.name.c_str());
-    if (l.kind == L_DENSE) { off += snprintf(buf + off, buflen - off, "dense simt\n"); continue; }
-    ConvProblem probs[4];
-    const int nclass = build_problems(l, n->B, probs);
-    for (int c = 0; c < nclass; ++c) { probs[c].in = (const float*)0x1000; probs[c].out = (float*)0x1000; }
-    if (n->precision != DEMON_PREC_FP32_SIMT && use_halo_kernel() && tc_halo_supported(probs, nclass))
-      off += tc_halo_describe(probs, nclass, n->precision == DEMON_PREC_TF32 ? 1 : 3, buf + off, buflen - off);
-    else {
-      bool all = n->precision != DEMON_PREC_FP32_SIMT;
-      for (int c = 0; c < nclass; ++c) all = all && tc_layer_supported(probs[c]);
-      off += snprintf(buf + off, buflen - off, all ? "conv_tc_kernel" : "simt");
-    }
+    off += snprintf(buf + off, buflen - off, "%-40s ", lp->name.c_str());
+    off += describe_layer(*lp, n->B, n->precision, buf + off, buflen - off);
     off += snprintf(buf + off, buflen - off, "\n");
   }
   return off;
@@ -1200,20 +1197,8 @@ int demon_debug_describe_layers(const demon_net* n, char* buf, int buflen) {
 int demon_debug_describe_conv(int B, int H, int W, int Cin, int in_pitch, int Cout, int out_pitch, int kh, int kw, int sy, int sx, int deconv,
                               int precision, char* buf, int buflen) {
   DEMON_REQUIRE(buf && buflen > 0, "describe: null");
-  Buf bi, bo;
-  bi.p = (float*)0x10000; bi.H = H; bi.W = W; bi.C = in_pitch;
-  Layer l;
-  l.name = "shape"; l.kind = deconv ? L_DECONV : L_CONV; l.in = &bi; l.cin = Cin; l.cin_buf = (Cin + 3) / 4 * 4; l.out = &bo; l.cout = Cout;
-  l.cout_pad = (Cout + 3) / 4 * 4; l.kh = kh; l.kw = kw; l.sy = sy; l.sx = sx;
-  bo.p = (float*)0x10000; bo.C = out_pitch;
-  if (deconv) { bo.H = 2 * H; bo.W = 2 * W; } else { bo.H = ceil_div(H, sy); bo.W = ceil_div(W, sx); }
-  ConvProblem probs[4];
-  const int nclass = build_problems(l, B, probs);
-  if (precision != DEMON_PREC_FP32_SIMT && use_halo_kernel() && tc_halo_supported(probs, nclass))
-    return tc_halo_describe(probs, nclass, precision == DEMON_PREC_TF32 ? 1 : 3, buf, buflen);
-  bool all = precision != DEMON_PREC_FP32_SIMT;
-  for (int c = 0; c < nclass; ++c) all = all && tc_layer_supported(probs[c]);
-  return snprintf(buf, buflen, all ? "conv_tc_kernel" : "simt");
+  StandaloneLayer s(nullptr, nullptr, H, W, Cin, in_pitch, Cout, out_pitch, kh, kw, sy, sx, deconv != 0, false);
+  return describe_layer(s.layer, B, precision, buf, buflen);
 }
 
 // ---- standalone convolution entries (tests) ---------------------------------------------------
@@ -1226,58 +1211,36 @@ static int standalone_conv(const float* in, float* out, int B, int H, int W, int
   DEMON_REQUIRE(Cin % 4 == 0, "conv test entry: Cin must be a multiple of 4");
   demon_net tmp;
   tmp.B = B;
-  Buf bi, bo;
-  bi.p = const_cast<float*>(in); bi.H = H; bi.W = W; bi.C = Cin;
-  Layer l;
-  l.name = "standalone"; l.kind = deconv ? L_DECONV : L_CONV; l.in = &bi; l.cin = Cin; l.cin_buf = Cin; l.out = &bo; l.cout = Cout;
-  l.cout_pad = (Cout + 3) / 4 * 4; l.kh = kh; l.kw = kw; l.sy = sy; l.sx = sx; l.leaky = leaky != 0;
-  bo.p = out; bo.C = Cout;
-  if (deconv) { bo.H = 2 * H; bo.W = 2 * W; } else { bo.H = ceil_div(H, sy); bo.W = ceil_div(W, sx); }
+  tmp.precision = precision;
+  StandaloneLayer s(in, out, H, W, Cin, Cin, Cout, Cout, kh, kw, sy, sx, deconv, leaky != 0);
+  Layer& l = s.layer;
   HostVar k;
   k.data.assign(kernel_host, kernel_host + (size_t)kh * kw * Cin * Cout);
-  std::vector<float> packed, bias(l.cout_pad, 0.f);
-  for (int i = 0; i < Cout; ++i) bias[i] = bias_host[i];
-  int rc;
-  if ((rc = upload(&tmp, bias, &l.bias_dev))) return rc;
-  const int nclass = deconv ? 4 : 1;
-  std::vector<float> cls_w[4];
-  const float* ptrs[4] = {nullptr, nullptr, nullptr, nullptr};
-  for (int c = 0; c < nclass; ++c) {
-    if (deconv) pack_deconv_class(l, k, c / 2, c % 2, cls_w[c]); else pack_conv(l, k, cls_w[c]);
-    ptrs[c] = cls_w[c].data();
-    if ((rc = upload(&tmp, cls_w[c], &l.w_dev[c]))) return rc;
-  }
-  if (precision != DEMON_PREC_FP32_SIMT) {
-    ConvProblem probs[4];
-    build_problems(l, B, probs);
-    bool all = true;
-    for (int c = 0; c < nclass; ++c) all = all && tc_layer_supported(probs[c]);
-    const bool halo = use_halo_kernel() && tc_halo_supported(probs, nclass);
-    if (!all && !halo) {
-      for (void* q : tmp.dev_allocs) cudaFree(q);
-      return fail(DEMON_E_INVALID, "conv test entry: shape not supported by the tensor-core path");
-    }
-    if (halo) rc = tc_halo_prepare(l.tc, probs, ptrs, nclass, precision);
-    else rc = tc_layer_prepare(l.tc, probs, ptrs, nclass, precision);
-    if (rc) return rc;
-    l.use_tc = true;
-  }
+  int rc = upload_layer(&tmp, l, k, bias_host);
+  if (rc == DEMON_OK && precision != DEMON_PREC_FP32_SIMT && !l.use_tc())
+    rc = fail(DEMON_E_INVALID, "conv test entry: shape not supported by the tensor-core path");
   float* tc_ws = nullptr;
-  if (l.use_tc && l.tc.splitk_bytes) {
+  if (rc == DEMON_OK && l.tc.splitk_bytes) {
     void* q = nullptr;
-    if (cudaMalloc(&q, l.tc.splitk_bytes) != cudaSuccess) return fail(DEMON_E_CUDA, "conv test entry: scratch allocation failed");
-    tmp.dev_allocs.push_back(q);
-    tc_ws = static_cast<float*>(q);
+    if (cudaMalloc(&q, l.tc.splitk_bytes) == cudaSuccess) {
+      tmp.dev_allocs.push_back(q);
+      tc_ws = static_cast<float*>(q);
+    } else {
+      rc = fail(DEMON_E_CUDA, "conv test entry: scratch allocation failed");
+    }
   }
-  cudaEvent_t ev0, ev1;
-  cudaEventCreate(&ev0); cudaEventCreate(&ev1);
-  cudaEventRecord(ev0, (cudaStream_t)stream);
-  rc = run_layer(l, B, (cudaStream_t)stream, nullptr, tc_ws);
-  cudaEventRecord(ev1, (cudaStream_t)stream);
-  cudaError_t e = cudaStreamSynchronize((cudaStream_t)stream);
-  float ms = -1.f;
-  if (e == cudaSuccess && cudaEventElapsedTime(&ms, ev0, ev1) == cudaSuccess) g_last_conv_ms = ms;
-  cudaEventDestroy(ev0); cudaEventDestroy(ev1);
+  cudaError_t e = cudaSuccess;
+  if (rc == DEMON_OK) {
+    cudaEvent_t ev0, ev1;
+    cudaEventCreate(&ev0); cudaEventCreate(&ev1);
+    cudaEventRecord(ev0, (cudaStream_t)stream);
+    rc = run_layer(l, B, (cudaStream_t)stream, nullptr, tc_ws);
+    cudaEventRecord(ev1, (cudaStream_t)stream);
+    e = cudaStreamSynchronize((cudaStream_t)stream);
+    float ms = -1.f;
+    if (e == cudaSuccess && cudaEventElapsedTime(&ms, ev0, ev1) == cudaSuccess) g_last_conv_ms = ms;
+    cudaEventDestroy(ev0); cudaEventDestroy(ev1);
+  }
   for (void* q : tmp.dev_allocs) cudaFree(q);
   tc_layer_free(l.tc);
   if (rc) return rc;

@@ -238,7 +238,7 @@ int demon_net_profile_end(demon_net* net);
 int demon_net_num_layers(const demon_net* net);
 const char* demon_net_layer_name(const demon_net* net, int i);
 /* uses_tc: kernel family of the layer -- 0 conv_simt_kernel (fp32 CUDA cores), 2 conv_tc_halo_kernel (wgmma, halo tile),
- * 3 conv_tc_halo_kernel in per-tap mode (one TMA box per filter tap); 1 is not produced by this version */
+ * 3 conv_tc_halo_kernel in per-tap mode (one TMA box per filter tap) */
 int demon_net_layer_profile(const demon_net* net, int i, double* ms, int64_t* calls, int* launches_per_call,
                             int* uses_tc);
 

@@ -3,6 +3,8 @@
 These are the decisions DESIGN.md section 3.1 describes -- resident weights, split-K, the N tile, the 3xTF32 mode --
 pinned here so that a planner change shows up as a test diff."""
 import ctypes
+import importlib.util
+import os
 import re
 
 import pytest
@@ -10,6 +12,7 @@ import pytest
 from demon_b200 import _lib
 
 X3TF32 = 1
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -59,3 +62,32 @@ def test_three_instruction_mode_and_register_accumulators(plan):
     assert (refine1["mode"], refine1["n_tile"]) == (2, 64)
     refine3 = plan(64, 12, 16, 576, 128, 4, 4, 2, 2, deconv=1)
     assert refine3["n_tile"] == 64 and "n_tile 64 x2" in refine3["text"]
+
+
+# the mode of conv_tc_halo_kernel every shape of tools/describe_plan.py gets: halo on whole 16x8 tiles, per-tap on the
+# 24x32 ... 6x8 levels, cin8 for the 8-channel inputs
+MODES = {
+    "conv1y": "cin8", "conv1x": "halo", "conv2y(32)": "halo", "conv2x(32)": "halo", "conv2y(64)": "halo", "conv2x(64)": "halo",
+    "extra_y": "halo", "extra_x": "halo", "conv2_1y": "halo", "conv2_1x": "halo",
+    "conv3y": "per-tap", "conv3x": "per-tap", "conv3_1y": "per-tap", "conv3_1x": "per-tap", "conv4y": "per-tap", "conv4x": "per-tap",
+    "conv4_1y": "per-tap", "conv4_1x": "per-tap", "conv5y(k5)": "per-tap", "conv5x(k5)": "per-tap", "conv5y(k3)": "per-tap",
+    "conv5x(k3)": "per-tap", "conv5_1y": "per-tap", "conv5_1x": "per-tap", "predict_flow5/conv1": "per-tap", "motion_conv1": "per-tap",
+    "refine4": "per-tap", "refine3": "per-tap", "refine2": "per-tap", "predict2/conv1": "halo",
+    "R conv0": "cin8", "R conv1": "halo", "R conv1_1": "halo", "R conv2": "halo", "R conv2_1": "halo", "R refine1": "halo",
+    "R refine0": "halo", "R pd0/conv1": "halo",
+}
+
+
+@pytest.mark.parametrize("B", [1, 64])
+def test_every_network_shape_keeps_its_kernel_mode(B):
+    spec = importlib.util.spec_from_file_location("describe_plan", os.path.join(ROOT, "tools", "describe_plan.py"))
+    tool = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(tool)
+    lib = _lib.load()
+    buf = ctypes.create_string_buffer(8192)
+    modes = {}
+    for name, dec, H, W, Cin, ipitch, Cout, opitch, kh, kw, sy, sx in tool.SHAPES:
+        lib.demon_debug_describe_conv(B, H, W, Cin, ipitch, Cout, opitch, kh, kw, sy, sx, dec, X3TF32, buf, 8192)
+        m = re.match(r"halo (\S+) mode ", buf.value.decode())
+        modes[name] = m.group(1) if m else buf.value.decode()
+    assert modes == MODES
