@@ -46,7 +46,8 @@ struct Layer {
   int cout = 0;
   int kh = 1, kw = 1, sy = 1, sx = 1;
   bool leaky = false;
-  const float* scale = nullptr;
+  Buf* scale = nullptr;  // optional: channel 0 of the output is multiplied by scale[scale_coff + n*scale_stride]
+  int scale_coff = 0;
   int scale_stride = 0;
   bool dense_nchw_flatten = false;  // motion_fc1: TF flattens NCHW (blocks_original.py:388-392)
   int dense_c = 0, dense_hw = 0;
@@ -63,10 +64,10 @@ struct Layer {
   int ksplit = 1;
 };
 
-struct HostVar {
-  std::vector<float> data;
-  std::vector<int64_t> shape;
-};
+// A block's layers, in the order they run: [begin, head_end) is conv1 / conv2 of the trunk (the pipeline hoists it out of
+// its iteration loop), [head_end, end) the rest, which starts with the conv2_extra_inputs pair when the block has one.
+// The refinement block has no head (head_end == begin).
+struct Block { int begin = 0, head_end = 0, end = 0; };
 
 }  // namespace
 }  // namespace demon
@@ -84,7 +85,7 @@ struct demon_net {
   std::vector<std::unique_ptr<Layer>> layers;
   std::map<std::string, Layer*> by_name;
   std::vector<std::string> var_names;
-  std::map<std::string, HostVar> host_vars;
+  std::map<std::string, std::vector<float>> host_vars;   // the weights set so far, TF layout; uploaded at finalize
   std::vector<void*> dev_allocs;
   int pipeline_launches[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   // CUDA graphs of demon_pipeline_forward, keyed by the pointer arguments (launch-bound at small batch: ~270 launches)
@@ -105,6 +106,8 @@ struct demon_net {
   Buf *img8, *i22, *i22_half, *c1y, *c1, *c2y, *cat2, *extra_in, *exy, *c21y, *concat2, *c3y, *c3, *c31y, *concat3, *c4y, *c4,
       *c41y, *concat4, *c5y, *c5, *c51y, *c51, *pf5a, *pf5, *p2a, *flowconf2, *dn2, *mc1, *fc1, *fc2, *motion;
   Buf *rin, *concat0, *rc1, *concat1, *rc2, *rc21, *pd0a, *rdepth0, *splitk;
+  // the five blocks' layer ranges
+  Block flow1, dm1, flow2, dm2, refine;
 
   Buf* add_buf(int H, int W, int C) {
     bufs.emplace_back(new Buf());
@@ -129,11 +132,12 @@ struct demon_net {
     var_names.push_back(name + "/bias");
     return l;
   }
-  // convrelu2_caffe_padding (helpers.py:105-153): y conv into `mid`, x conv into `out`
-  void add_sep(const std::string& name, int k, int stride, Buf* in, int in_coff, int cin, Buf* mid, int cmid, Buf* out,
-               int out_coff, int cout) {
-    add_layer(name + "y", L_CONV, in, in_coff, cin, mid, 0, cmid, k, 1, stride, 1, true);
+  // convrelu2_caffe_padding (helpers.py:105-153): y conv into `mid`, x conv into `out`; returns the y conv
+  Layer* add_sep(const std::string& name, int k, int stride, Buf* in, int in_coff, int cin, Buf* mid, int cmid, Buf* out,
+                 int out_coff, int cout) {
+    Layer* y = add_layer(name + "y", L_CONV, in, in_coff, cin, mid, 0, cmid, k, 1, stride, 1, true);
     add_layer(name + "x", L_CONV, mid, 0, cmid, out, out_coff, cout, 1, k, 1, stride, true);
+    return y;
   }
 };
 
@@ -143,19 +147,21 @@ namespace {
 // ---------------------------------------------------------------------------------------------
 // plan construction
 // ---------------------------------------------------------------------------------------------
-void build_trunk(demon_net* n, const std::string& s, bool flow, bool iterative) {
+// returns the index of the first layer after conv2
+int build_trunk(demon_net* n, const std::string& s, bool flow, bool iterative) {
   const int conv2_out = (flow && !iterative) ? 64 : 32;
   // conv1 and conv2 of the iterative nets depend only on the image pair (blocks_original.py:141,147 / :331,333), so the
   // pipeline computes them once per call: they get a concat buffer of their own that survives the other blocks
   Buf* cat2 = iterative ? (flow ? n->cat2_f2 : n->cat2_d2) : n->cat2;
   n->add_sep(s + "conv1", 9, 2, n->img8, 0, 6, n->c1y, 32, n->c1, 0, 32);
   n->add_sep(s + "conv2", 7, 2, n->c1, 0, 32, n->c2y, conv2_out, cat2, 0, conv2_out);
+  const int head_end = (int)n->layers.size();
   if (!(flow && !iterative)) {
     const int extra = flow ? 9 : (iterative ? 8 : 7);
-    n->add_sep(s + "conv2_extra_inputs", 3, 1, n->extra_in, 0, extra, n->exy, 32, cat2, 32, 32);
+    Layer* ey = n->add_sep(s + "conv2_extra_inputs", 3, 1, n->extra_in, 0, extra, n->exy, 32, cat2, 32, 32);
     // the 7 / 8 / 9 real channels sit in a 32-channel (128-byte) pixel whose other channels are zero and carry zero weights:
     // one K = 32 chunk of the tensor-core halo kernel (3 steps per tile) instead of the fp32 SIMT kernel
-    n->by_name[s + "conv2_extra_inputsy"]->cin_buf = 32;
+    ey->cin_buf = 32;
   }
   n->add_sep(s + "conv2_1", 3, 1, cat2, 0, 64, n->c21y, 64, n->concat2, 64, 64);
   n->add_sep(s + "conv3", 5, 2, n->concat2, 64, 64, n->c3y, 128, n->c3, 0, 128);
@@ -164,11 +170,13 @@ void build_trunk(demon_net* n, const std::string& s, bool flow, bool iterative) 
   n->add_sep(s + "conv4_1", 3, 1, n->c4, 0, 256, n->c41y, 256, n->concat4, 256, 256);
   n->add_sep(s + "conv5", flow ? 5 : 3, 2, n->concat4, 256, 256, n->c5y, 512, n->c5, 0, 512);
   n->add_sep(s + "conv5_1", 3, 1, n->c5, 0, 512, n->c51y, 512, n->c51, 0, 512);
+  return head_end;
 }
 
-void build_flow_block(demon_net* n, const std::string& scope, bool iterative) {
+Block build_flow_block(demon_net* n, const std::string& scope, bool iterative) {
   const std::string s = scope + "/";
-  build_trunk(n, s, true, iterative);
+  const int begin = (int)n->layers.size();
+  const int head_end = build_trunk(n, s, true, iterative);
   n->add_layer(s + "predict_flow5/conv1", L_CONV, n->c51, 0, 512, n->pf5a, 0, 24, 3, 3, 1, 1, true);
   n->add_layer(s + "predict_flow5/conv2", L_CONV, n->pf5a, 0, 24, n->pf5, 0, 4, 3, 3, 1, 1, false);
   // _upsample_prediction: no activation (blocks_original.py:70); lands in concat4[512:514]
@@ -179,11 +187,13 @@ void build_flow_block(demon_net* n, const std::string& scope, bool iterative) {
   n->add_layer(s + "refine2/upconv", L_DECONV, n->concat3, 0, 256, n->concat2, 0, 64, 4, 4, 2, 2, true);
   n->add_layer(s + "predict_flow2/conv1", L_CONV, n->concat2, 0, 128, n->p2a, 0, 24, 3, 3, 1, 1, true);
   n->add_layer(s + "predict_flow2/conv2", L_CONV, n->p2a, 0, 24, n->flowconf2, 0, 4, 3, 3, 1, 1, false);
+  return {begin, head_end, (int)n->layers.size()};
 }
 
-void build_dm_block(demon_net* n, const std::string& scope, bool iterative) {
+Block build_dm_block(demon_net* n, const std::string& scope, bool iterative) {
   const std::string s = scope + "/";
-  build_trunk(n, s, false, iterative);
+  const int begin = (int)n->layers.size();
+  const int head_end = build_trunk(n, s, false, iterative);
   n->add_layer(s + "motion_conv1", L_CONV, n->c51, 0, 512, n->mc1, 0, 128, 3, 3, 1, 1, true);
   Layer* f1 = n->add_layer(s + "motion_fc1", L_DENSE, n->mc1, 0, 6144, n->fc1, 0, 1024, 1, 1, 1, 1, true);
   f1->dense_nchw_flatten = true; f1->dense_c = 128; f1->dense_hw = 48;
@@ -196,12 +206,13 @@ void build_dm_block(demon_net* n, const std::string& scope, bool iterative) {
   n->add_layer(s + "refine2/upconv", L_DECONV, n->concat3, 0, 256, n->concat2, 0, 64, 4, 4, 2, 2, true);
   n->add_layer(s + "predict_depthnormal2/conv1", L_CONV, n->concat2, 0, 128, n->p2a, 0, 24, 3, 3, 1, 1, true);
   Layer* dn = n->add_layer(s + "predict_depthnormal2/conv2", L_CONV, n->p2a, 0, 24, n->dn2, 0, 4, 3, 3, 1, 1, false);
-  dn->scale = nullptr;  // bound to motion[:,6] at finalize (buffer addresses are not known yet)
-  dn->scale_stride = 8;
+  dn->scale = n->motion; dn->scale_coff = 6; dn->scale_stride = 8;   // depth = motion[:,6] (the scale) * channel 0
+  return {begin, head_end, (int)n->layers.size()};
 }
 
-void build_refine_block(demon_net* n, const std::string& scope) {
+Block build_refine_block(demon_net* n, const std::string& scope) {
   const std::string s = scope + "/";
+  const int begin = (int)n->layers.size();
   Layer* c0 = n->add_layer(s + "conv0", L_CONV, n->rin, 0, 4, n->concat0, 32, 32, 3, 3, 1, 1, true);
   c0->cin_buf = 8;
   n->add_layer(s + "conv1", L_CONV, n->concat0, 32, 32, n->rc1, 0, 64, 3, 3, 2, 2, true);
@@ -212,6 +223,7 @@ void build_refine_block(demon_net* n, const std::string& scope) {
   n->add_layer(s + "refine0/upconv", L_DECONV, n->concat1, 0, 128, n->concat0, 0, 32, 4, 4, 2, 2, true);
   n->add_layer(s + "predict_depth0/conv1", L_CONV, n->concat0, 0, 64, n->pd0a, 0, 16, 3, 3, 1, 1, true);
   n->add_layer(s + "predict_depth0/conv2", L_CONV, n->pd0a, 0, 16, n->rdepth0, 0, 1, 3, 3, 1, 1, false);
+  return {begin, begin, (int)n->layers.size()};
 }
 
 void build_plan(demon_net* n) {
@@ -261,11 +273,11 @@ void build_plan(demon_net* n) {
   n->pd0a = n->add_buf(RH, RW, 16);
   n->rdepth0 = n->add_buf(RH, RW, 1);
 
-  build_flow_block(n, "netFlow1", false);
-  build_dm_block(n, "netDM1", false);
-  build_flow_block(n, "netFlow2", true);
-  build_dm_block(n, "netDM2", true);
-  build_refine_block(n, "netRefine");
+  n->flow1 = build_flow_block(n, "netFlow1", false);
+  n->dm1 = build_dm_block(n, "netDM1", false);
+  n->flow2 = build_flow_block(n, "netFlow2", true);
+  n->dm2 = build_dm_block(n, "netDM2", true);
+  n->refine = build_refine_block(n, "netRefine");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -277,16 +289,16 @@ void build_plan(demon_net* n) {
 const int kDeconvK[2][2] = {{1, 3}, {0, 2}};
 const int kDeconvD[2][2] = {{0, -1}, {1, 0}};
 
-void pack_conv(const Layer& l, const HostVar& k, std::vector<float>& out) {
+void pack_conv(const Layer& l, const float* k, std::vector<float>& out) {
   const int taps = l.kh * l.kw;
   out.assign((size_t)taps * l.cin_buf * l.cout_pad, 0.f);
   for (int t = 0; t < taps; ++t)
     for (int ci = 0; ci < l.cin; ++ci)
       for (int co = 0; co < l.cout; ++co)
-        out[((size_t)t * l.cin_buf + ci) * l.cout_pad + co] = k.data[((size_t)t * l.cin + ci) * l.cout + co];
+        out[((size_t)t * l.cin_buf + ci) * l.cout_pad + co] = k[((size_t)t * l.cin + ci) * l.cout + co];
 }
 
-void pack_deconv_class(const Layer& l, const HostVar& k, int py, int px, std::vector<float>& out) {
+void pack_deconv_class(const Layer& l, const float* k, int py, int px, std::vector<float>& out) {
   out.assign((size_t)4 * l.cin_buf * l.cout_pad, 0.f);
   for (int a = 0; a < 2; ++a)
     for (int b = 0; b < 2; ++b) {
@@ -294,11 +306,11 @@ void pack_deconv_class(const Layer& l, const HostVar& k, int py, int px, std::ve
       const int t = a * 2 + b;
       for (int ci = 0; ci < l.cin; ++ci)
         for (int co = 0; co < l.cout; ++co)
-          out[((size_t)t * l.cin_buf + ci) * l.cout_pad + co] = k.data[(((size_t)ky * 4 + kx) * l.cout + co) * l.cin + ci];
+          out[((size_t)t * l.cin_buf + ci) * l.cout_pad + co] = k[(((size_t)ky * 4 + kx) * l.cout + co) * l.cin + ci];
     }
 }
 
-void pack_dense(const Layer& l, const HostVar& k, std::vector<float>& out) {
+void pack_dense(const Layer& l, const float* k, std::vector<float>& out) {
   out.assign((size_t)l.cin_buf * l.cout_pad, 0.f);
   for (int i = 0; i < l.cin; ++i) {
     int src = i;
@@ -306,14 +318,14 @@ void pack_dense(const Layer& l, const HostVar& k, std::vector<float>& out) {
       const int hw = i / l.dense_c, c = i % l.dense_c;
       src = c * l.dense_hw + hw;
     }
-    for (int co = 0; co < l.cout; ++co) out[(size_t)i * l.cout_pad + co] = k.data[(size_t)src * l.cout + co];
+    for (int co = 0; co < l.cout; ++co) out[(size_t)i * l.cout_pad + co] = k[(size_t)src * l.cout + co];
   }
 }
 
-int upload(demon_net* n, const std::vector<float>& host, float** dev) {
+int upload(std::vector<void*>& allocs, const std::vector<float>& host, float** dev) {
   void* p = nullptr;
   DEMON_CHECK_CUDA(cudaMalloc(&p, host.size() * sizeof(float) + 256));
-  n->dev_allocs.push_back(p);
+  allocs.push_back(p);
   DEMON_CHECK_CUDA(cudaMemcpy(p, host.data(), host.size() * sizeof(float), cudaMemcpyHostToDevice));
   *dev = (float*)p;
   return DEMON_OK;
@@ -322,31 +334,27 @@ int upload(demon_net* n, const std::vector<float>& host, float** dev) {
 // ---------------------------------------------------------------------------------------------
 // layer execution
 // ---------------------------------------------------------------------------------------------
-void fill_problem(const Layer& l, int B, ConvProblem& p) {
+// The convolution problem(s) of a layer: 1 for conv / dense, 4 sub-pixel classes for a transposed conv.
+// `dst`, if given, replaces the base of the layer's output buffer (same shape and channel pitch).
+int build_problems(const Layer& l, int B, ConvProblem* out, float* dst = nullptr) {
+  ConvProblem p;
   memset(&p, 0, sizeof(p));
   p.in = l.in->p + l.in_coff;
   p.in_pitch = l.in->C;
   p.B = B;
   p.Cin = l.cin_buf;
-  p.out = l.out->p + l.out_coff;
+  p.out = (dst ? dst : l.out->p) + l.out_coff;
   p.out_pitch = l.out->C;
   p.Cout = l.cout;
   p.Cout_pad = l.cout_pad;
   p.bias = l.bias_dev;
   p.leaky = l.leaky ? 1 : 0;
-  p.scale = l.scale;
+  p.scale = l.scale ? l.scale->p + l.scale_coff : nullptr;
   p.scale_stride = l.scale_stride;
   p.osy = p.osx = 1;
-}
-
-// The convolution problem(s) of a layer: 1 for conv / dense, 4 sub-pixel classes for a transposed conv.
-int build_problems(const Layer& l, int B, ConvProblem* out) {
-  ConvProblem p;
-  fill_problem(l, B, p);
   if (l.kind == L_DENSE) {
     p.Hi = p.Wi = p.Ho = p.Wo = p.Hfull = p.Wfull = 1;
     p.in_pitch = l.cin_buf;
-    p.out_pitch = l.out->C;
     p.sy = p.sx = 1;
     p.ntaps = 1;
     p.w = l.w_dev[0];
@@ -382,9 +390,9 @@ int build_problems(const Layer& l, int B, ConvProblem* out) {
   return 4;
 }
 
-int run_layer(const Layer& l, int B, cudaStream_t stream, float* splitk_ws = nullptr, float* tc_ws = nullptr) {
+int run_layer(const Layer& l, int B, cudaStream_t stream, float* splitk_ws, float* tc_ws, float* dst = nullptr) {
   ConvProblem probs[4];
-  const int nclass = build_problems(l, B, probs);
+  const int nclass = build_problems(l, B, probs, dst);
   if (l.use_tc()) {
     probs[0].partial = tc_ws;   // scratch of the split-K tensor-core layers (the net's, so two nets in flight do not share it)
     return conv_tc_launch(l.tc, probs, stream);
@@ -397,13 +405,14 @@ int run_layer(const Layer& l, int B, cudaStream_t stream, float* splitk_ws = nul
   return DEMON_OK;
 }
 
-// Uploads a layer's bias and its kernel (TF layout) packed for the SIMT path; at a tensor-core precision the planner
-// (tc_prepare) then decides whether the layer runs on the tensor cores and packs the kernel for them.
-int upload_layer(demon_net* n, Layer& l, const HostVar& k, const float* bias_host) {
+// Uploads a layer's bias and its kernel (TF layout) packed for the path that runs it: at a tensor-core precision the planner
+// (tc_prepare) may take a conv / transposed conv and pack the kernel for the tensor cores; any other layer gets the SIMT
+// packing [tap][cin_buf][cout_pad].  Device allocations other than the plan's (tc_layer_free) are appended to `allocs`.
+int upload_layer(Layer& l, const float* k, const float* bias_host, int B, int precision, std::vector<void*>& allocs) {
   std::vector<float> bias(l.cout_pad, 0.f);
   std::copy(bias_host, bias_host + l.cout, bias.begin());
   int rc;
-  if ((rc = upload(n, bias, &l.bias_dev))) return rc;
+  if ((rc = upload(allocs, bias, &l.bias_dev))) return rc;
   std::vector<float> w[4];
   const float* w_hosts[4] = {nullptr, nullptr, nullptr, nullptr};
   const int nw = (l.kind == L_DECONV) ? 4 : 1;
@@ -411,14 +420,17 @@ int upload_layer(demon_net* n, Layer& l, const HostVar& k, const float* bias_hos
     if (l.kind == L_CONV) pack_conv(l, k, w[c]);
     else if (l.kind == L_DENSE) pack_dense(l, k, w[c]);
     else pack_deconv_class(l, k, c / 2, c % 2, w[c]);
-    if ((rc = upload(n, w[c], &l.w_dev[c]))) return rc;
     w_hosts[c] = w[c].data();
   }
-  if (n->precision == DEMON_PREC_FP32_SIMT || l.kind == L_DENSE) return DEMON_OK;
-  ConvProblem probs[4];
-  const int nclass = build_problems(l, n->B, probs);
-  rc = tc_prepare(l.tc, probs, w_hosts, nclass, n->precision);
-  return (rc == kTcNoPlan) ? DEMON_OK : rc;
+  if (precision != DEMON_PREC_FP32_SIMT && l.kind != L_DENSE) {
+    ConvProblem probs[4];
+    const int nclass = build_problems(l, B, probs);
+    rc = tc_prepare(l.tc, probs, w_hosts, nclass, precision);
+    if (rc != kTcNoPlan) return rc;   // on the tensor cores, or an error
+  }
+  for (int c = 0; c < nw; ++c)
+    if ((rc = upload(allocs, w[c], &l.w_dev[c]))) return rc;
+  return DEMON_OK;
 }
 
 // The plan line of a layer: the tensor-core planner's, or "simt" for a layer it does not take.
@@ -448,44 +460,37 @@ struct StandaloneLayer {
   StandaloneLayer& operator=(const StandaloneLayer&) = delete;
 };
 
-int run_layer_profiled(demon_net* n, int idx, cudaStream_t stream) {
+// `dst`: see build_problems
+int run_layer_profiled(demon_net* n, int idx, cudaStream_t stream, float* dst = nullptr) {
   const Layer& l = *n->layers[idx];
   static const bool sync_layers = getenv("DEMON_SYNC_LAYERS") && atoi(getenv("DEMON_SYNC_LAYERS")) != 0;   // debugging aid
   if (sync_layers) {
-    int rc = run_layer(l, n->B, stream, n->splitk->p, n->tc_scratch);
+    int rc = run_layer(l, n->B, stream, n->splitk->p, n->tc_scratch, dst);
     cudaError_t e = cudaStreamSynchronize(stream);
     if (rc == DEMON_OK && e != cudaSuccess) return fail(DEMON_E_CUDA, "layer %s: %s", l.name.c_str(), cudaGetErrorString(e));
     return rc;
   }
-  if (!n->profiling) return run_layer(l, n->B, stream, n->splitk->p, n->tc_scratch);
+  if (!n->profiling) return run_layer(l, n->B, stream, n->splitk->p, n->tc_scratch, dst);
   if (n->prof_used + 2 > n->prof_events.size()) {
     const size_t old = n->prof_events.size();
     n->prof_events.resize(old + 1024);
     for (size_t i = old; i < n->prof_events.size(); ++i) DEMON_CHECK_CUDA(cudaEventCreate(&n->prof_events[i]));
   }
   DEMON_CHECK_CUDA(cudaEventRecord(n->prof_events[n->prof_used], stream));
-  int rc = run_layer(l, n->B, stream, n->splitk->p, n->tc_scratch);
+  int rc = run_layer(l, n->B, stream, n->splitk->p, n->tc_scratch, dst);
   DEMON_CHECK_CUDA(cudaEventRecord(n->prof_events[n->prof_used + 1], stream));
   n->prof_layer.push_back(idx);
   n->prof_used += 2;
   return rc;
 }
 
-int run_range(demon_net* n, const std::string& first, const std::string& last, cudaStream_t stream) {
-  bool on = false;
-  for (size_t li = 0; li < n->layers.size(); ++li) {
-    auto& l = n->layers[li];
-    if (l->name == first) on = true;
-    if (on) {
-      int rc = run_layer_profiled(n, (int)li, stream);
-      if (rc != DEMON_OK) return rc;
-    }
-    if (l->name == last) {
-      if (!on) break;
-      return DEMON_OK;
-    }
+// layers [begin, end) in order
+int run_layers(demon_net* n, int begin, int end, cudaStream_t stream) {
+  for (int i = begin; i < end; ++i) {
+    int rc = run_layer_profiled(n, i, stream);
+    if (rc != DEMON_OK) return rc;
   }
-  return fail(DEMON_E_STATE, "run_range: layers %s .. %s not found in order", first.c_str(), last.c_str());
+  return DEMON_OK;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -506,13 +511,23 @@ __global__ void __launch_bounds__(256) strided_copy_kernel(const float* __restri
   }
 }
 
-int strided_copy(const float* src, float* dst, int N, int P, int C, long sn, long sp, long sc, long dn, long dp, long dc,
-                 cudaStream_t stream) {
+// strides in floats between samples, pixels and channels
+struct Strides { long n, p, c; };
+
+// an API tensor of C channels over P pixels: [B,C,H,W] (data_format 0) or [B,H,W,C] (data_format 1)
+Strides api_strides(int data_format, long P, int C) {
+  return data_format == 0 ? Strides{C * P, 1, P} : Strides{C * P, C, 1};
+}
+
+// a workspace buffer (NHWC)
+Strides buf_strides(const Buf* b) { return Strides{(long)b->H * b->W * b->C, b->C, 1}; }
+
+int strided_copy(const float* src, float* dst, int N, int P, int C, Strides s, Strides d, cudaStream_t stream) {
   const long total = (long)N * P * C;
   if (total == 0) return DEMON_OK;
   long blocks = (total + 255) / 256;
   if (blocks > 132 * 32) blocks = 132 * 32;
-  (void)launch_pdl(strided_copy_kernel, dim3((int)blocks), dim3(256), 0, stream, src, dst, N, P, C, sn, sp, sc, dn, dp, dc);
+  (void)launch_pdl(strided_copy_kernel, dim3((int)blocks), dim3(256), 0, stream, src, dst, N, P, C, s.n, s.p, s.c, d.n, d.p, d.c);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
 }
@@ -688,17 +703,17 @@ __global__ void __launch_bounds__(256) u8_planes_kernel(const unsigned char* __r
 // ---------------------------------------------------------------------------------------------
 int import_image_pair(demon_net* n, const float* image_pair, int data_format, cudaStream_t s) {
   const int P = 192 * 256;
-  if (data_format == 0) return strided_copy(image_pair, n->img8->p, n->B, P, 6, 6L * P, 1, P, 8L * P, 8, 1, s);
-  return strided_copy(image_pair, n->img8->p, n->B, P, 6, 6L * P, 6, 1, 8L * P, 8, 1, s);
+  return strided_copy(image_pair, n->img8->p, n->B, P, 6, api_strides(data_format, P, 6), buf_strides(n->img8), s);
 }
 
+// i22 holds NCHW planes: an NCHW image2_2 is a plain copy
 int import_image2_2(demon_net* n, const float* image2_2, int data_format, cudaStream_t s) {
   const int P = 48 * 64;
   if (data_format == 0) {
     DEMON_CHECK_CUDA(cudaMemcpyAsync(n->i22->p, image2_2, (size_t)n->B * 3 * P * sizeof(float), cudaMemcpyDeviceToDevice, s));
     return DEMON_OK;
   }
-  return strided_copy(image2_2, n->i22->p, n->B, P, 3, 3L * P, 3, 1, 3L * P, 1, P, s);
+  return strided_copy(image2_2, n->i22->p, n->B, P, 3, api_strides(data_format, P, 3), api_strides(0, P, 3), s);
 }
 
 // planes: image 2 as NCHW fp32 planes, `sn` floats between samples (6*P inside an image pair, 3*P for a packed copy)
@@ -715,8 +730,7 @@ int median_image2_2(demon_net* n, const float* planes, long sn, cudaStream_t s) 
 int export_slice(demon_net* n, const Buf* b, int coff, int C, float* dst, int data_format, cudaStream_t s) {
   if (!dst) return DEMON_OK;
   const int P = b->H * b->W;
-  if (data_format == 0) return strided_copy(b->p + coff, dst, n->B, P, C, (long)P * b->C, b->C, 1, (long)C * P, 1, P, s);
-  return strided_copy(b->p + coff, dst, n->B, P, C, (long)P * b->C, b->C, 1, (long)C * P, C, 1, s);
+  return strided_copy(b->p + coff, dst, n->B, P, C, buf_strides(b), api_strides(data_format, P, C), s);
 }
 
 int export_predictions(demon_net* n, float* flow5, float* flow2, float* depth2, float* normal2, float* rotation, float* translation,
@@ -726,52 +740,46 @@ int export_predictions(demon_net* n, float* flow5, float* flow2, float* depth2, 
   if ((rc = export_slice(n, n->flowconf2, 0, 2, flow2, data_format, s))) return rc;
   if ((rc = export_slice(n, n->dn2, 0, 1, depth2, data_format, s))) return rc;
   if ((rc = export_slice(n, n->dn2, 1, 3, normal2, data_format, s))) return rc;
-  if (rotation && (rc = strided_copy(n->motion->p, rotation, n->B, 1, 3, 8, 0, 1, 3, 0, 1, s))) return rc;
-  if (translation && (rc = strided_copy(n->motion->p + 3, translation, n->B, 1, 3, 8, 0, 1, 3, 0, 1, s))) return rc;
+  if (rotation && (rc = strided_copy(n->motion->p, rotation, n->B, 1, 3, {8, 0, 1}, {3, 0, 1}, s))) return rc;
+  if (translation && (rc = strided_copy(n->motion->p + 3, translation, n->B, 1, 3, {8, 0, 1}, {3, 0, 1}, s))) return rc;
   return DEMON_OK;
 }
 
-// flow block, everything after the trunk's conv2 (blocks_original.py:190-235)
-// `head`: run conv1 / conv2 (false when the pipeline has hoisted them out of the iteration loop)
-int run_flow_block(demon_net* n, const std::string& scope, bool iterative, cudaStream_t s, bool head = true) {
-  const std::string p = scope + "/";
+// flow block (blocks_original.py:190-235); `head`: run conv1 / conv2 (false when the pipeline has hoisted them out of the
+// iteration loop)
+int run_flow_block(demon_net* n, const Block& b, bool iterative, cudaStream_t s, bool head = true) {
   int rc;
-  if (head && (rc = run_range(n, p + "conv1y", p + "conv2x", s))) return rc;
+  if (head && (rc = run_layers(n, b.begin, b.head_end, s))) return rc;
   if (iterative) {
     (void)launch_pdl(flow_extra_kernel, dim3(dim3(ceil_div(48 * 64, 256), n->B)), dim3(256), 0, s, n->dn2->p, n->motion->p, n->i22->p, n->extra_in->p, 48, 64, n->extra_in->C);
     DEMON_LAUNCH_CHECK();
-    if ((rc = run_range(n, p + "conv2_extra_inputsy", p + "conv2_extra_inputsx", s))) return rc;
   }
-  return run_range(n, p + "conv2_1y", p + "predict_flow2/conv2", s);
+  return run_layers(n, b.head_end, b.end, s);
 }
 
-int run_dm_block(demon_net* n, const std::string& scope, bool iterative, cudaStream_t s, bool head = true) {
-  const std::string p = scope + "/";
+int run_dm_block(demon_net* n, const Block& b, bool iterative, cudaStream_t s, bool head = true) {
   int rc;
-  if (head && (rc = run_range(n, p + "conv1y", p + "conv2x", s))) return rc;
+  if (head && (rc = run_layers(n, b.begin, b.head_end, s))) return rc;
   // the previous motion is still in n->motion here: this block's motion_fc3 overwrites it later
   (void)launch_pdl(dm_extra_kernel, dim3(dim3(ceil_div(48 * 64, 128), n->B)), dim3(128), 0, s, n->flowconf2->p, n->motion->p, n->i22->p, n->extra_in->p, 48, 64,
                                                                    n->extra_in->C, iterative);
   DEMON_LAUNCH_CHECK();
-  return run_range(n, p + "conv2_extra_inputsy", p + "predict_depthnormal2/conv2", s);
+  return run_layers(n, b.head_end, b.end, s);
 }
 
-int run_refine_block(demon_net* n, const float* image1, long img_sn, long img_sp, long img_sc, const float* depth, long d_sn, long d_sp,
-                     int dh, int dw, float* depth0, cudaStream_t s) {
+// `depth`: channel 0 of (sample, pixel) strided depth planes; `depth0`: the output, or null for rdepth0
+int run_refine_block(demon_net* n, const float* image1, Strides img, const float* depth, Strides dep, int dh, int dw, float* depth0,
+                     cudaStream_t s) {
   const long total = (long)n->B * n->RH * n->RW;
   long blocks = (total + 255) / 256;
   if (blocks > 132 * 32) blocks = 132 * 32;
-  (void)launch_pdl(refine_input_kernel, dim3((int)blocks), dim3(256), 0, s, image1, img_sn, img_sp, img_sc, depth, d_sn, d_sp, n->rin->p, n->B, n->RH, n->RW, dh, dw);
+  (void)launch_pdl(refine_input_kernel, dim3((int)blocks), dim3(256), 0, s, image1, img.n, img.p, img.c, depth, dep.n, dep.p, n->rin->p, n->B, n->RH, n->RW, dh, dw);
   DEMON_LAUNCH_CHECK();
+  const Block& b = n->refine;
+  int rc;
+  if ((rc = run_layers(n, b.begin, b.end - 1, s))) return rc;
   // the last layer writes straight into the caller's output (C = 1: NHWC == NCHW)
-  Layer* last = n->by_name["netRefine/predict_depth0/conv2"];
-  Buf out = *n->rdepth0;
-  if (depth0) out.p = depth0;
-  Buf* saved = last->out;
-  last->out = &out;
-  int rc = run_range(n, "netRefine/conv0", "netRefine/predict_depth0/conv2", s);
-  last->out = saved;
-  return rc;
+  return run_layer_profiled(n, b.end - 1, s, depth0);
 }
 
 }  // namespace
@@ -796,8 +804,6 @@ int demon_net_create(demon_net** out, int batch, int refine_h, int refine_w, int
   n->ws = (float*)p;
   DEMON_CHECK_CUDA(cudaMemset(p, 0, n->ws_floats * sizeof(float)));
   for (auto& b : n->bufs) b->p = n->ws + b->offset;
-  n->by_name["netDM1/predict_depthnormal2/conv2"]->scale = n->motion->p + 6;
-  n->by_name["netDM2/predict_depthnormal2/conv2"]->scale = n->motion->p + 6;
   *out = n.release();
   return DEMON_OK;
 }
@@ -841,9 +847,7 @@ int demon_net_set_weight(demon_net* n, const char* name, const float* data, cons
   }
   int64_t numel = 1;
   for (int i = 0; i < rank; ++i) numel *= shape[i];
-  HostVar& hv = n->host_vars[nm];
-  hv.data.assign(data, data + numel);
-  hv.shape.assign(shape, shape + rank);
+  n->host_vars[nm].assign(data, data + numel);
   return DEMON_OK;
 }
 
@@ -854,7 +858,8 @@ int demon_net_finalize(demon_net* n) {
     if (!n->host_vars.count(nm)) return fail(DEMON_E_STATE, "demon_net_finalize: variable %s was not set", nm.c_str());
   for (auto& lp : n->layers) {
     Layer& l = *lp;
-    const int rc = upload_layer(n, l, n->host_vars[l.name + "/kernel"], n->host_vars[l.name + "/bias"].data.data());
+    const int rc = upload_layer(l, n->host_vars[l.name + "/kernel"].data(), n->host_vars[l.name + "/bias"].data(), n->B, n->precision,
+                                n->dev_allocs);
     if (rc) return rc;
   }
   // scratch of the split-K tensor-core layers: the largest need, owned by the net
@@ -958,8 +963,8 @@ int demon_bootstrap_forward(demon_net* n, const float* image_pair, const float* 
   int rc;
   if ((rc = import_image_pair(n, image_pair, data_format, s))) return rc;
   if ((rc = import_image2_2(n, image2_2, data_format, s))) return rc;
-  if ((rc = run_flow_block(n, "netFlow1", false, s))) return rc;
-  if ((rc = run_dm_block(n, "netDM1", false, s))) return rc;
+  if ((rc = run_flow_block(n, n->flow1, false, s))) return rc;
+  if ((rc = run_dm_block(n, n->dm1, false, s))) return rc;
   return export_predictions(n, flow5, flow2, depth2, normal2, rotation, translation, data_format, s);
 }
 
@@ -975,17 +980,12 @@ int demon_iterative_forward(demon_net* n, const float* image_pair, const float* 
   if ((rc = import_image_pair(n, image_pair, data_format, s))) return rc;
   if ((rc = import_image2_2(n, image2_2, data_format, s))) return rc;
   // previous predictions -> dn2 (NHWC4) and motion
-  if (data_format == 0) {
-    if ((rc = strided_copy(depth2_in, n->dn2->p, n->B, P, 1, P, 1, 0, 4L * P, 4, 1, s))) return rc;
-    if ((rc = strided_copy(normal2_in, n->dn2->p + 1, n->B, P, 3, 3L * P, 1, P, 4L * P, 4, 1, s))) return rc;
-  } else {
-    if ((rc = strided_copy(depth2_in, n->dn2->p, n->B, P, 1, P, 1, 0, 4L * P, 4, 1, s))) return rc;
-    if ((rc = strided_copy(normal2_in, n->dn2->p + 1, n->B, P, 3, 3L * P, 3, 1, 4L * P, 4, 1, s))) return rc;
-  }
-  if ((rc = strided_copy(rotation_in, n->motion->p, n->B, 1, 3, 3, 0, 1, 8, 0, 1, s))) return rc;
-  if ((rc = strided_copy(translation_in, n->motion->p + 3, n->B, 1, 3, 3, 0, 1, 8, 0, 1, s))) return rc;
-  if ((rc = run_flow_block(n, "netFlow2", true, s))) return rc;
-  if ((rc = run_dm_block(n, "netDM2", true, s))) return rc;
+  if ((rc = strided_copy(depth2_in, n->dn2->p, n->B, P, 1, api_strides(data_format, P, 1), buf_strides(n->dn2), s))) return rc;
+  if ((rc = strided_copy(normal2_in, n->dn2->p + 1, n->B, P, 3, api_strides(data_format, P, 3), buf_strides(n->dn2), s))) return rc;
+  if ((rc = strided_copy(rotation_in, n->motion->p, n->B, 1, 3, {3, 0, 1}, {8, 0, 1}, s))) return rc;
+  if ((rc = strided_copy(translation_in, n->motion->p + 3, n->B, 1, 3, {3, 0, 1}, {8, 0, 1}, s))) return rc;
+  if ((rc = run_flow_block(n, n->flow2, true, s))) return rc;
+  if ((rc = run_dm_block(n, n->dm2, true, s))) return rc;
   return export_predictions(n, flow5, flow2, depth2, normal2, rotation, translation, data_format, s);
 }
 
@@ -995,9 +995,8 @@ int demon_refine_forward(demon_net* n, const float* image1, const float* depth2,
   DEMON_REQUIRE(data_format == 0 || data_format == 1, "refine: data_format %d", data_format);
   const long P = (long)n->RH * n->RW;
   const int dh = n->RH / 4, dw = n->RW / 4;
-  if (data_format == 0)
-    return run_refine_block(n, image1, 3 * P, 1, P, depth2, (long)dh * dw, 1, dh, dw, depth0, (cudaStream_t)stream);
-  return run_refine_block(n, image1, 3 * P, 3, 1, depth2, (long)dh * dw, 1, dh, dw, depth0, (cudaStream_t)stream);
+  return run_refine_block(n, image1, api_strides(data_format, P, 3), depth2, api_strides(data_format, (long)dh * dw, 1), dh, dw, depth0,
+                          (cudaStream_t)stream);
 }
 
 // Input of the fused pipeline: fp32 NCHW (image_pair [B,6,192,256], image2_2 [B,3,48,64] or null) or uint8
@@ -1035,21 +1034,21 @@ static int pipeline_body(demon_net* n, const PipelineInput& in, int iterations, 
       if ((rc = median_image2_2(n, in.image_pair + 3 * P, 6 * P, s))) return rc;
     }
   }
-  if ((rc = run_flow_block(n, "netFlow1", false, s))) return rc;
-  if ((rc = run_dm_block(n, "netDM1", false, s))) return rc;
+  if ((rc = run_flow_block(n, n->flow1, false, s))) return rc;
+  if ((rc = run_dm_block(n, n->dm1, false, s))) return rc;
   // conv1 / conv2 of netFlow2 and netDM2 read only the image pair and fixed weights: once per call instead of once per
   // iteration (bit identical; 2 x 2 x 221.7 MMAC per pair less to execute at three iterations)
   if (iterations > 0) {
-    if ((rc = run_range(n, "netFlow2/conv1y", "netFlow2/conv2x", s))) return rc;
-    if ((rc = run_range(n, "netDM2/conv1y", "netDM2/conv2x", s))) return rc;
+    if ((rc = run_layers(n, n->flow2.begin, n->flow2.head_end, s))) return rc;
+    if ((rc = run_layers(n, n->dm2.begin, n->dm2.head_end, s))) return rc;
   }
   for (int it = 0; it < iterations; ++it) {
-    if ((rc = run_flow_block(n, "netFlow2", true, s, false))) return rc;
-    if ((rc = run_dm_block(n, "netDM2", true, s, false))) return rc;
+    if ((rc = run_flow_block(n, n->flow2, true, s, false))) return rc;
+    if ((rc = run_dm_block(n, n->dm2, true, s, false))) return rc;
   }
   if ((rc = export_predictions(n, nullptr, flow2, depth2, normal2, rotation, translation, 0, s))) return rc;
   // image1 for the refinement block is read back from img8 (NHWC8: the first three channels), whatever the input kind
-  return run_refine_block(n, n->img8->p, 8 * P, 8, 1, n->dn2->p, 4L * 48 * 64, 4, 48, 64, depth0, s);
+  return run_refine_block(n, n->img8->p, buf_strides(n->img8), n->dn2->p, buf_strides(n->dn2), 48, 64, depth0, s);
 }
 
 static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iterations, float* depth0, float* rotation, float* translation,
@@ -1209,21 +1208,17 @@ static int standalone_conv(const float* in, float* out, int B, int H, int W, int
                            const float* kernel_host, const float* bias_host, int leaky, int precision, bool deconv, void* stream) {
   DEMON_REQUIRE(in && out && kernel_host && bias_host, "conv: null pointer");
   DEMON_REQUIRE(Cin % 4 == 0, "conv test entry: Cin must be a multiple of 4");
-  demon_net tmp;
-  tmp.B = B;
-  tmp.precision = precision;
+  std::vector<void*> allocs;
   StandaloneLayer s(in, out, H, W, Cin, Cin, Cout, Cout, kh, kw, sy, sx, deconv, leaky != 0);
   Layer& l = s.layer;
-  HostVar k;
-  k.data.assign(kernel_host, kernel_host + (size_t)kh * kw * Cin * Cout);
-  int rc = upload_layer(&tmp, l, k, bias_host);
+  int rc = upload_layer(l, kernel_host, bias_host, B, precision, allocs);
   if (rc == DEMON_OK && precision != DEMON_PREC_FP32_SIMT && !l.use_tc())
     rc = fail(DEMON_E_INVALID, "conv test entry: shape not supported by the tensor-core path");
   float* tc_ws = nullptr;
   if (rc == DEMON_OK && l.tc.splitk_bytes) {
     void* q = nullptr;
     if (cudaMalloc(&q, l.tc.splitk_bytes) == cudaSuccess) {
-      tmp.dev_allocs.push_back(q);
+      allocs.push_back(q);
       tc_ws = static_cast<float*>(q);
     } else {
       rc = fail(DEMON_E_CUDA, "conv test entry: scratch allocation failed");
@@ -1241,7 +1236,7 @@ static int standalone_conv(const float* in, float* out, int B, int H, int W, int
     if (e == cudaSuccess && cudaEventElapsedTime(&ms, ev0, ev1) == cudaSuccess) g_last_conv_ms = ms;
     cudaEventDestroy(ev0); cudaEventDestroy(ev1);
   }
-  for (void* q : tmp.dev_allocs) cudaFree(q);
+  for (void* q : allocs) cudaFree(q);
   tc_layer_free(l.tc);
   if (rc) return rc;
   if (e != cudaSuccess) return fail(DEMON_E_CUDA, "conv test entry: %s", cudaGetErrorString(e));
