@@ -17,6 +17,7 @@
 #include "conv.cuh"
 #include "conv_tc.cuh"
 #include "geometry.cuh"
+#include "images.cuh"
 
 namespace demon {
 
@@ -999,19 +1000,38 @@ int demon_refine_forward(demon_net* n, const float* image1, const float* depth2,
                           (cudaStream_t)stream);
 }
 
-// Input of the fused pipeline: fp32 NCHW (image_pair [B,6,192,256], image2_2 [B,3,48,64] or null) or uint8
-// (images [B,2,192,256,3], image2_2 [B,48,64,3] or null).
+// Input of the fused pipeline: fp32 NCHW (image_pair [B,6,192,256], image2_2 [B,3,48,64] or null), uint8
+// (images [B,2,192,256,3], image2_2 [B,48,64,3] or null) or uint8 pairs of any size to resize first (src, see
+// demon_pipeline_forward_images_u8).
 struct PipelineInput {
   const float* image_pair = nullptr;
   const float* image2_2 = nullptr;
   const unsigned char* images_u8 = nullptr;
   const unsigned char* image2_2_u8 = nullptr;
+  const unsigned char* src = nullptr;
+  int64_t src_sn = 0, src_si = 0, src_sy = 0;
+  int src_h = 0, src_w = 0, resample = 0, image2_2_mode = 0;
 };
 
-static int pipeline_body(demon_net* n, const PipelineInput& in, int iterations, float* depth0, float* rotation,
+static int pipeline_body(demon_net* n, const PipelineInput& arg, int iterations, float* depth0, float* rotation,
                          float* translation, float* flow2, float* depth2, float* normal2, cudaStream_t s) {
   int rc;
   const long P = 192L * 256;
+  PipelineInput in = arg;
+  if (in.src) {
+    // resized pair -> concat0 as uint8 [B,2,192,256,3] and the 64x48 image2_2 -> pd0a as uint8 [B,48,64,3]: both buffers are
+    // free until the refinement block (the same staging as pipeline_host), and the uint8 path below reads them first
+    unsigned char* pair = reinterpret_cast<unsigned char*>(n->concat0->p);
+    if ((rc = resize_u8_launch(in.src, in.src_sn, in.src_si, 2, in.src_sy, 2 * n->B, in.src_h, in.src_w, pair, 192, 256, in.resample, s)))
+      return rc;
+    in.images_u8 = pair;
+    in.image2_2_u8 = nullptr;
+    if (in.image2_2_mode == 1) {
+      unsigned char* i22 = reinterpret_cast<unsigned char*>(n->pd0a->p);
+      if ((rc = resize_u8_launch(pair + P * 3, 2 * P * 3, 0, 1, 256 * 3, n->B, 192, 256, i22, 48, 64, in.resample, s))) return rc;
+      in.image2_2_u8 = i22;
+    }
+  }
   if (in.images_u8) {
     // img8 straight from the bytes; image 2's planes go to c1y (free until conv1y runs) for the median pair
     float* planes2 = in.image2_2_u8 ? nullptr : n->c1y->p;
@@ -1072,6 +1092,22 @@ int demon_pipeline_forward_u8(demon_net* n, const uint8_t* images, const uint8_t
   return pipeline_forward_impl(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, stream);
 }
 
+int demon_pipeline_forward_images_u8(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, int resample,
+                                     int image2_2_mode, int iterations, float* depth0, float* rotation, float* translation, float* flow2,
+                                     float* depth2, float* normal2, void* stream) {
+  REQUIRE_READY(n);
+  DEMON_REQUIRE(images, "pipeline_images_u8: null images");
+  DEMON_REQUIRE(sn >= 0 && si >= 0 && sy >= 0, "pipeline_images_u8: negative stride");
+  DEMON_REQUIRE(image2_2_mode == 0 || image2_2_mode == 1, "pipeline_images_u8: image2_2_mode %d is not 0 (median) or 1 (resize)",
+                image2_2_mode);
+  int rc = resize_u8_check(h, w, 192, 256, resample, "pipeline_images_u8");
+  if (rc) return rc;
+  PipelineInput in;
+  in.src = images; in.src_sn = sn; in.src_si = si; in.src_sy = sy; in.src_h = h; in.src_w = w; in.resample = resample;
+  in.image2_2_mode = image2_2_mode;
+  return pipeline_forward_impl(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, stream);
+}
+
 static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iterations, float* depth0, float* rotation, float* translation,
                                  float* flow2, float* depth2, float* normal2, void* stream) {
   DEMON_REQUIRE(iterations >= 0 && iterations <= 7, "pipeline: iterations %d", iterations);
@@ -1084,8 +1120,10 @@ static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iter
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(s, &cap);
   if (graphs_on && !n->profiling && cap == cudaStreamCaptureStatusNone) {
+    const auto val = [](int64_t v) { return reinterpret_cast<const void*>((intptr_t)v); };
     const std::vector<const void*> key = {in.image_pair, in.image2_2, in.images_u8, in.image2_2_u8, depth0, rotation, translation, flow2, depth2,
-                                          normal2, reinterpret_cast<const void*>((intptr_t)iterations)};
+                                          normal2, val(iterations), in.src, val(in.src_sn), val(in.src_si), val(in.src_sy), val(in.src_h),
+                                          val(in.src_w), val(in.resample), val(in.image2_2_mode)};
     for (auto& g : n->graphs)
       if (g.key == key) {
         if (g.exec == nullptr) {   // second call: capture

@@ -323,6 +323,32 @@ class DemonPipeline:
             ptr("predict_flow2"), ptr("predict_depth2"), ptr("predict_normal2"), _stream()))
         return outputs
 
+    def forward_images(self, images, resample="bicubic", image2_2="resize", outputs=None):
+        """The pipeline on image pairs of any size (examples/example.py:15-42 and :87-99 in one call): images CUDA uint8
+        [B,2,h,w,3] (HWC RGB, pixel stride 3 and channel stride 1; a cropped view is read in place).  Both images are resized
+        to 256x192 on the device exactly like PIL.Image.resize with `resample` ('nearest', 'bilinear', 'bicubic' or Pillow's
+        enum value); image2_2 is 'resize' (the resized second image resized to 64x48 with the same filter, example.py:22) or
+        'median' (median3x3_downsample twice, examples/evaluation.py:170-173).  Same outputs as forward_u8 on the resized
+        bytes, bit for bit."""
+        from .images import check_images, resample_code
+        b = self.batch_size
+        code = resample_code(resample)
+        if image2_2 not in ("resize", "median"):
+            raise ValueError("image2_2 must be 'resize' or 'median', got %r" % (image2_2,))
+        check_images(images, "images", 5)
+        if tuple(images.shape[:2]) != (b, 2):
+            raise ValueError("images: expected shape (%d, 2, h, w, 3), got %s" % (b, tuple(images.shape)))
+        h, w = images.shape[2], images.shape[3]
+        if outputs is None:
+            outputs = self.own_outputs()
+        ptr = lambda k: outputs[k].data_ptr() if outputs.get(k) is not None else None
+        _lib.check(_lib.load().demon_pipeline_forward_images_u8(
+            self.net.ptr, images.data_ptr(), images.stride(0), images.stride(1), images.stride(2), h, w, code,
+            1 if image2_2 == "resize" else 0, self.iterations,
+            ptr("predict_depth0"), ptr("predict_rotation"), ptr("predict_translation"),
+            ptr("predict_flow2"), ptr("predict_depth2"), ptr("predict_normal2"), _stream()))
+        return outputs
+
     def forward_host_u8(self, images, image2_2, depth0, rotation, translation, stream=None, sync=True):
         """End to end from HOST uint8 images [B,2,192,256,3] (numpy or pinned torch CPU uint8): H2D of the bytes, the
         pipeline, D2H of depth0 / rotation / translation.  sync=False: asynchronous on `stream` like forward_host_async."""

@@ -141,6 +141,19 @@ int demon_depth_scale_factor(const double* sums, int n, int mode, float* scale, 
 int demon_flow_epe_sums_f32(const float* flow1, const float* flow2, int n, int64_t hw, double* sums, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------
+ * Image input (examples/example.py:15-42 resizes every image with PIL.Image.resize).
+ * ---------------------------------------------------------------------- */
+/* resample filters, with Pillow's enum values (PIL.Image.Resampling) */
+#define DEMON_RESAMPLE_NEAREST   0
+#define DEMON_RESAMPLE_BILINEAR  2
+#define DEMON_RESAMPLE_BICUBIC   3
+/* PIL.Image.resize((ow, oh), resample) of n RGB uint8 images, bit for bit: src [n,h,w,3] with `src_sn` bytes between
+ * images and `src_sy` between rows (pixel stride 3, channel stride 1) -> dst [n,oh,ow,3] contiguous.  Sides 1..8192,
+ * n 0..65535.  Other filters (LANCZOS, BOX, HAMMING) are DEMON_E_INVALID. */
+int demon_resize_u8(const uint8_t* src, int64_t src_sn, int64_t src_sy, int n, int h, int w, uint8_t* dst, int oh, int ow,
+                    int resample, void* stream);
+
+/* ------------------------------------------------------------------------
  * Network graphs (python/depthmotionnet/networks_original.py).
  * One handle = the five blocks netFlow1, netDM1, netFlow2, netDM2, netRefine for a
  * fixed batch size at 256x192 (networks_original.py:38-42), plus a refinement block that
@@ -221,6 +234,17 @@ int demon_pipeline_forward_host_u8(demon_net* net, const uint8_t* images_host, c
                                    float* depth0_host, float* rotation_host, float* translation_host, void* stream);
 int demon_pipeline_forward_host_u8_async(demon_net* net, const uint8_t* images_host, const uint8_t* image2_2_host, int iterations,
                                          float* depth0_host, float* rotation_host, float* translation_host, void* stream);
+
+/* The same pipeline on image pairs of any size, resized on the device first, the whole of examples/example.py:15-42:
+ * images [B,2,h,w,3] uint8 RGB with `sn`, `si`, `sy` bytes between samples, between the two images of a pair and between
+ * rows (pixel stride 3, channel stride 1, so a cropped view is read in place), 1 <= h, w <= 8192.  Both images are resized
+ * to 256x192 with `resample` exactly like PIL.Image.resize (demon_resize_u8), then image2_2 is
+ *   image2_2_mode 0: median3x3_downsample twice of the resized second image (examples/evaluation.py:170-173), or
+ *   image2_2_mode 1: the resized second image resized to 64x48 with the same filter (examples/example.py:22).
+ * The outputs equal demon_pipeline_forward_u8 on the resized bytes, bit for bit. */
+int demon_pipeline_forward_images_u8(demon_net* net, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w,
+                                     int resample, int image2_2_mode, int iterations, float* depth0, float* rotation,
+                                     float* translation, float* flow2, float* depth2, float* normal2, void* stream);
 
 /* introspection for tests and bench */
 int demon_net_batch(const demon_net* net);
