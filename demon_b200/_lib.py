@@ -42,6 +42,11 @@ PROTOTYPES = {
     "demon_depth_error_sums_f32": [_P, _P, c_int, c_int64, c_int, c_int, _P, _P, _P, _P, _P],
     "demon_depth_scale_factor": [_P, c_int, c_int, _P, _P],
     "demon_flow_epe_sums_f32": [_P, _P, c_int, c_int64, _P, _P, _P],
+    "demon_depth_error_sums_resampled_f32": [_P, c_int, c_int, _P, _P] + [c_int] * 7 + [_P, _P, c_int, c_int] + [_P] * 5,
+    "demon_flow_epe_sums_resampled_f32": [_P, c_int, c_int, _P] + [c_int] * 7 + [_P] * 5,
+    "demon_motion_errors": [_P, _P, _P, c_int, _P, _P, _P],
+    "demon_visible_points_mask_f32": [_P] * 5 + [c_int] * 7 + [_P, _P],
+    "demon_visible_points_mask_inverse_f32": [_P] * 5 + [c_int] * 7 + [_P, _P],
     "demon_net_create": [ctypes.POINTER(c_void_p), c_int, c_int, c_int, c_int],
     "demon_net_destroy": [_P],
     "demon_net_set_weight": [_P, c_char_p, _P, _P, c_int],
@@ -52,6 +57,7 @@ PROTOTYPES = {
     "demon_iterative_forward": [_P] + [_P] * 12 + [c_int, _P],
     "demon_refine_forward": [_P, _P, _P, _P, c_int, _P],
     "demon_pipeline_forward": [_P, _P, _P, c_int] + [_P] * 6 + [_P],
+    "demon_pipeline_forward_snapshots": [_P, _P, _P, c_int] + [_P] * 6 + [_P],
     "demon_pipeline_forward_host": [_P, _P, _P, c_int, _P, _P, _P, _P],
     "demon_pipeline_forward_host_async": [_P, _P, _P, c_int, _P, _P, _P, _P],
     "demon_pipeline_forward_u8": [_P, _P, _P, c_int] + [_P] * 6 + [_P],
@@ -62,6 +68,7 @@ PROTOTYPES = {
     "demon_net_batch": [_P],
     "demon_net_workspace_bytes": [_P],
     "demon_net_pipeline_launches": [_P, c_int],
+    "demon_net_snapshot_launches": [_P, c_int],
     "demon_net_layer_uses_tensor_cores": [_P, c_char_p],
     "demon_net_profile_begin": [_P],
     "demon_net_profile_end": [_P],

@@ -89,6 +89,7 @@ struct demon_net {
   std::map<std::string, std::vector<float>> host_vars;   // the weights set so far, TF layout; uploaded at finalize
   std::vector<void*> dev_allocs;
   int pipeline_launches[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  int snapshot_launches[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // the same for demon_pipeline_forward_snapshots (kept apart: bench.py reads the above)
   // CUDA graphs of demon_pipeline_forward, keyed by the pointer arguments (launch-bound at small batch: ~270 launches)
   struct GraphEntry { std::vector<const void*> key; cudaGraphExec_t exec; int launches; };
   std::vector<GraphEntry> graphs;
@@ -897,6 +898,10 @@ int demon_net_pipeline_launches(const demon_net* n, int iterations) {
   if (!n || iterations < 0 || iterations > 7) return 0;
   return n->pipeline_launches[iterations];
 }
+int demon_net_snapshot_launches(const demon_net* n, int iterations) {
+  if (!n || iterations < 0 || iterations > 7) return 0;
+  return n->snapshot_launches[iterations];
+}
 int demon_net_layer_uses_tensor_cores(const demon_net* n, const char* name) {
   if (!n || !name) return 0;
   auto it = n->by_name.find(name);
@@ -1013,8 +1018,37 @@ struct PipelineInput {
   int src_h = 0, src_w = 0, resample = 0, image2_2_mode = 0;
 };
 
+// Outputs of demon_pipeline_forward_snapshots: snapshot k (0 = bootstrap, k = after iteration k) of every array is the
+// k-th [B, ...] slice; any pointer may be null.  `depth0` set: the refinement block also runs on every snapshot's depth2
+// (examples/evaluation.py:225-255 refines all four).
+struct SnapshotOutputs {
+  float* flow2 = nullptr;
+  float* depth2 = nullptr;
+  float* normal2 = nullptr;
+  float* rotation = nullptr;
+  float* translation = nullptr;
+  float* depth0 = nullptr;
+};
+
+// Snapshot k of the predictions.  Running the refinement block here, between two iterations, is safe because it shares
+// no buffer with the iteration state (build_plan): it writes rin, concat0, rc1, concat1, rc2, rc21, pd0a, rdepth0 (or the
+// caller's depth0) and the split-K scratch, which holds partial sums only inside one layer; the iterations carry dn2,
+// flowconf2, motion, i22, img8, cat2_f2, cat2_d2 and extra_in from one block to the next, and the refinement block only
+// reads img8 and dn2.  concat0 / pd0a double as staging of a uint8 or resized input, which is consumed into img8 / i22
+// before the first block runs.
+static int export_snapshot(demon_net* n, const SnapshotOutputs& o, int k, cudaStream_t s) {
+  const long B = n->B, P2 = 48L * 64, P0 = 192L * 256;
+  const auto at = [k](float* p, long per_snapshot) { return p ? p + k * per_snapshot : nullptr; };
+  int rc = export_predictions(n, nullptr, at(o.flow2, B * 2 * P2), at(o.depth2, B * P2), at(o.normal2, B * 3 * P2), at(o.rotation, B * 3),
+                              at(o.translation, B * 3), 0, s);
+  if (rc || !o.depth0) return rc;
+  return run_refine_block(n, n->img8->p, buf_strides(n->img8), n->dn2->p, buf_strides(n->dn2), 48, 64, at(o.depth0, B * P0), s);
+}
+
+// `snap` null: the plain pipeline (last iteration's outputs); otherwise every snapshot goes to `snap` and the other outputs
+// are unused
 static int pipeline_body(demon_net* n, const PipelineInput& arg, int iterations, float* depth0, float* rotation,
-                         float* translation, float* flow2, float* depth2, float* normal2, cudaStream_t s) {
+                         float* translation, float* flow2, float* depth2, float* normal2, const SnapshotOutputs* snap, cudaStream_t s) {
   int rc;
   const long P = 192L * 256;
   PipelineInput in = arg;
@@ -1056,6 +1090,7 @@ static int pipeline_body(demon_net* n, const PipelineInput& arg, int iterations,
   }
   if ((rc = run_flow_block(n, n->flow1, false, s))) return rc;
   if ((rc = run_dm_block(n, n->dm1, false, s))) return rc;
+  if (snap && (rc = export_snapshot(n, *snap, 0, s))) return rc;
   // conv1 / conv2 of netFlow2 and netDM2 read only the image pair and fixed weights: once per call instead of once per
   // iteration (bit identical; 2 x 2 x 221.7 MMAC per pair less to execute at three iterations)
   if (iterations > 0) {
@@ -1065,14 +1100,16 @@ static int pipeline_body(demon_net* n, const PipelineInput& arg, int iterations,
   for (int it = 0; it < iterations; ++it) {
     if ((rc = run_flow_block(n, n->flow2, true, s, false))) return rc;
     if ((rc = run_dm_block(n, n->dm2, true, s, false))) return rc;
+    if (snap && (rc = export_snapshot(n, *snap, it + 1, s))) return rc;
   }
+  if (snap) return DEMON_OK;
   if ((rc = export_predictions(n, nullptr, flow2, depth2, normal2, rotation, translation, 0, s))) return rc;
   // image1 for the refinement block is read back from img8 (NHWC8: the first three channels), whatever the input kind
   return run_refine_block(n, n->img8->p, buf_strides(n->img8), n->dn2->p, buf_strides(n->dn2), 48, 64, depth0, s);
 }
 
 static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iterations, float* depth0, float* rotation, float* translation,
-                                 float* flow2, float* depth2, float* normal2, void* stream);
+                                 float* flow2, float* depth2, float* normal2, void* stream, const SnapshotOutputs* snap = nullptr);
 
 int demon_pipeline_forward(demon_net* n, const float* image_pair, const float* image2_2, int iterations, float* depth0, float* rotation,
                            float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
@@ -1081,6 +1118,18 @@ int demon_pipeline_forward(demon_net* n, const float* image_pair, const float* i
   PipelineInput in;
   in.image_pair = image_pair; in.image2_2 = image2_2;
   return pipeline_forward_impl(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, stream);
+}
+
+int demon_pipeline_forward_snapshots(demon_net* n, const float* image_pair, const float* image2_2, int iterations, float* flow2,
+                                     float* depth2, float* normal2, float* rotation, float* translation, float* depth0, void* stream) {
+  REQUIRE_READY(n);
+  DEMON_REQUIRE(image_pair, "pipeline_snapshots: null image_pair");
+  PipelineInput in;
+  in.image_pair = image_pair; in.image2_2 = image2_2;
+  SnapshotOutputs snap;
+  snap.flow2 = flow2; snap.depth2 = depth2; snap.normal2 = normal2; snap.rotation = rotation; snap.translation = translation;
+  snap.depth0 = depth0;
+  return pipeline_forward_impl(n, in, iterations, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, stream, &snap);
 }
 
 int demon_pipeline_forward_u8(demon_net* n, const uint8_t* images, const uint8_t* image2_2, int iterations, float* depth0, float* rotation,
@@ -1109,8 +1158,9 @@ int demon_pipeline_forward_images_u8(demon_net* n, const uint8_t* images, int64_
 }
 
 static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iterations, float* depth0, float* rotation, float* translation,
-                                 float* flow2, float* depth2, float* normal2, void* stream) {
+                                 float* flow2, float* depth2, float* normal2, void* stream, const SnapshotOutputs* snap) {
   DEMON_REQUIRE(iterations >= 0 && iterations <= 7, "pipeline: iterations %d", iterations);
+  int* launch_record = snap ? n->snapshot_launches : n->pipeline_launches;
   DEMON_REQUIRE(n->RH == 192 && n->RW == 256, "pipeline: net was created with a %dx%d refinement block", n->RH, n->RW);
   cudaStream_t s = (cudaStream_t)stream;
   // The call is one CUDA graph per distinct set of pointer arguments (DEMON_GRAPH=0 disables): the first call with a new
@@ -1121,9 +1171,14 @@ static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iter
   cudaStreamIsCapturing(s, &cap);
   if (graphs_on && !n->profiling && cap == cudaStreamCaptureStatusNone) {
     const auto val = [](int64_t v) { return reinterpret_cast<const void*>((intptr_t)v); };
+    // snapshot calls: mode 1, or 2 with the per-snapshot refinement; their output pointers are part of the key as well
+    const SnapshotOutputs none;
+    const SnapshotOutputs& so = snap ? *snap : none;
+    const int mode = snap ? (snap->depth0 ? 2 : 1) : 0;
     const std::vector<const void*> key = {in.image_pair, in.image2_2, in.images_u8, in.image2_2_u8, depth0, rotation, translation, flow2, depth2,
                                           normal2, val(iterations), in.src, val(in.src_sn), val(in.src_si), val(in.src_sy), val(in.src_h),
-                                          val(in.src_w), val(in.resample), val(in.image2_2_mode)};
+                                          val(in.src_w), val(in.resample), val(in.image2_2_mode), val(mode), so.flow2, so.depth2, so.normal2,
+                                          so.rotation, so.translation, so.depth0};
     for (auto& g : n->graphs)
       if (g.key == key) {
         if (g.exec == nullptr) {   // second call: capture
@@ -1131,7 +1186,7 @@ static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iter
           const int64_t l0 = g_launch_count.load();
           if (!n->cap_stream) DEMON_CHECK_CUDA(cudaStreamCreateWithFlags(&n->cap_stream, cudaStreamNonBlocking));
           DEMON_CHECK_CUDA(cudaStreamBeginCapture(n->cap_stream, cudaStreamCaptureModeThreadLocal));
-          int rc = pipeline_body(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, n->cap_stream);
+          int rc = pipeline_body(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, snap, n->cap_stream);
           cudaError_t e = cudaStreamEndCapture(n->cap_stream, &graph);
           if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
           if (e != cudaSuccess) return fail(DEMON_E_CUDA, "pipeline: stream capture failed: %s", cudaGetErrorString(e));
@@ -1143,7 +1198,7 @@ static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iter
         }
         DEMON_CHECK_CUDA(cudaGraphLaunch(g.exec, s));
         g_launch_count.fetch_add(g.launches);
-        n->pipeline_launches[iterations] = g.launches;
+        launch_record[iterations] = g.launches;
         return DEMON_OK;
       }
     if (n->graphs.size() >= 32) {   // evict the oldest entry
@@ -1153,9 +1208,9 @@ static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iter
     n->graphs.push_back({key, nullptr, 0});
   }
   const int64_t launches0 = g_launch_count.load();
-  int rc = pipeline_body(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, s);
+  int rc = pipeline_body(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, snap, s);
   if (rc) return rc;
-  n->pipeline_launches[iterations] = (int)(g_launch_count.load() - launches0);
+  launch_record[iterations] = (int)(g_launch_count.load() - launches0);
   return DEMON_OK;
 }
 

@@ -240,6 +240,7 @@ class DemonPipeline:
         # The C call replays ONE CUDA graph per set of pointer arguments, so the pipeline owns persistent input staging
         # and output buffers: the graph key is then the same for every call, whatever tensors the caller passes.
         self._ip = self._i22 = self._out = None
+        self._snap = self._snap_refined = None
 
     def stage(self, image_pair, image2_2=None):
         """Copies the inputs into the pipeline's own device buffers (asynchronous, current stream) and returns them."""
@@ -300,6 +301,40 @@ class DemonPipeline:
             ptr("predict_depth0"), ptr("predict_rotation"), ptr("predict_translation"),
             ptr("predict_flow2"), ptr("predict_depth2"), ptr("predict_normal2"), _stream()))
         return outputs
+
+    def own_snapshot_outputs(self, refine=True):
+        """The persistent output buffers of forward_snapshots (S = iterations + 1 snapshots); one set per `refine`."""
+        key = "_snap_refined" if refine else "_snap"
+        if getattr(self, key, None) is None:
+            b, s = self.batch_size, self.iterations + 1
+            dev = self._ip.device if self._ip is not None else torch.device("cuda", torch.cuda.current_device())
+            mk = lambda *sh: torch.empty(sh, dtype=torch.float32, device=dev)
+            out = {"predict_flow2": mk(s, b, 2, 48, 64), "predict_depth2": mk(s, b, 1, 48, 64), "predict_normal2": mk(s, b, 3, 48, 64),
+                   "predict_rotation": mk(s, b, 3), "predict_translation": mk(s, b, 3)}
+            if refine:
+                out["predict_depth0"] = mk(s, b, 1, 192, 256)
+            setattr(self, key, out)
+        return getattr(self, key)
+
+    def forward_snapshots(self, image_pair, image2_2=None, refine=True, outputs=None):
+        """The pipeline keeping every intermediate prediction, as examples/evaluation.py:225-255 stores them: snapshot 0
+        is the bootstrap net's output, snapshot k the output after iteration k.  Returns a dict of torch CUDA tensors
+        [S, B, ...] with S = iterations + 1: predict_flow2 [S,B,2,48,64], predict_depth2 [S,B,1,48,64], predict_normal2
+        [S,B,3,48,64], predict_rotation / predict_translation [S,B,3], and with `refine` predict_depth0 [S,B,1,192,256]
+        (the refinement net on every snapshot's depth, evaluation.py:249).  Inputs are staged like forward(); with
+        `outputs=None` the results are the pipeline's own buffers, overwritten by the next call."""
+        ip, i2 = self.stage(image_pair, image2_2)
+        if outputs is None:
+            outputs = self.own_snapshot_outputs(refine)
+        ptr = lambda k: outputs[k].data_ptr() if outputs.get(k) is not None else None
+        _lib.check(_lib.load().demon_pipeline_forward_snapshots(
+            self.net.ptr, ip.data_ptr(), None if i2 is None else i2.data_ptr(), self.iterations,
+            ptr("predict_flow2"), ptr("predict_depth2"), ptr("predict_normal2"), ptr("predict_rotation"),
+            ptr("predict_translation"), ptr("predict_depth0") if refine else None, _stream()))
+        return outputs
+
+    def snapshot_launches(self):
+        return _lib.load().demon_net_snapshot_launches(self.net.ptr, self.iterations)
 
     def forward_u8(self, images, image2_2=None, outputs=None):
         """The pipeline on uint8 images (torch CUDA uint8): images [B,2,192,256,3] = image 1 and image 2 of every pair as

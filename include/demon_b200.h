@@ -140,6 +140,39 @@ int demon_depth_scale_factor(const double* sums, int n, int mode, float* scale, 
 /* compute_flow_epe (metrics.py:377-387): flow1, flow2 [n,2,hw] -> sums[n][2] = {sum of the valid end point errors, count} */
 int demon_flow_epe_sums_f32(const float* flow1, const float* flow2, int n, int64_t hw, double* sums, void* workspace, void* stream);
 
+/* The two sums above with the prediction at its own size, resized to the ground truth's by nearest neighbour and cropped,
+ * without materialising either (evaluate_to_xarray.py:200-211).  pred [n,ph,pw] (flow [n,2,ph,pw]), gt [n,gh,gw] (flow
+ * [n,2,gh,gw]); the output window is gt rows y0..y0+oh-1, columns x0..x0+ow-1; window row r reads prediction row
+ * row_idx[r], column c reads column col_idx[c] (int32 device tables, see evaluation.nearest_index); an index of -1 reads
+ * 0 (skimage's cval).  gt_valid [n,gh,gw] uint8 or NULL: 0 marks a gt pixel as invalid, as a NaN there would
+ * (invalidate_points_not_visible_in_second_image).  Pixel order and CTA slots are those of the entries above over oh*ow
+ * pixels, so the sums equal theirs on the materialised arrays bit for bit.  Workspace: demon_metric_workspace_bytes(n, oh*ow). */
+int demon_depth_error_sums_resampled_f32(const float* pred, int ph, int pw, const float* gt, const uint8_t* gt_valid, int gh, int gw,
+                                         int n, int y0, int x0, int oh, int ow, const int* row_idx, const int* col_idx,
+                                         int inverse_pred, int inverse_gt, const float* gt_div, const float* pred_scale,
+                                         double* sums, void* workspace, void* stream);
+int demon_flow_epe_sums_resampled_f32(const float* pred, int ph, int pw, const float* gt, int gh, int gw, int n, int y0, int x0,
+                                      int oh, int ow, const int* row_idx, const int* col_idx, double* sums, void* workspace,
+                                      void* stream);
+
+/* compute_motion_errors (metrics.py:390-445, normalize_translations) for n samples, one thread each, in double:
+ * pred_rotation / pred_translation [n,3], gt_motion [n,6] (angle axis | translation), float32 ->
+ * out[n][4] = rot_err (degrees), tran_err, tran_angle_err (degrees), camera_baseline = |t_gt| (NaN if gt_motion has a NaN)
+ * and gt_div[n] (float32; may be NULL): the translation norm evaluate_depth divides the gt depth by, 1 where it is
+ * numpy.isclose to 1, with t_gt = (1, 0, 0) for a motion with a NaN (evaluate_to_xarray.py:290-294). */
+int demon_motion_errors(const float* pred_rotation, const float* pred_translation, const float* gt_motion, int n, double* out,
+                        float* gt_div, void* stream);
+
+/* compute_visible_points_mask (dataset_tools/view_tools_cython.pyx:9-58) for n views, bit for bit: depth [n,h,w] camera z,
+ * per sample K1 [3,3], R1 [3,3], t1 [3], P2 [3,4] (float32) -> mask [n,h,w] = 1 where the pixel's point projects into the
+ * second image strictly inside the border (borderx, bordery) of a width2 x height2 image and in front of the camera. */
+int demon_visible_points_mask_f32(const float* depth, const float* K1, const float* R1, const float* t1, const float* P2, int n, int h,
+                                  int w, int width2, int height2, int borderx, int bordery, uint8_t* mask, void* stream);
+/* the same on INVERSE depth: the kernel takes 1/depth in float32 first (evaluate_to_xarray.py:110) */
+int demon_visible_points_mask_inverse_f32(const float* inverse_depth, const float* K1, const float* R1, const float* t1, const float* P2,
+                                          int n, int h, int w, int width2, int height2, int borderx, int bordery, uint8_t* mask,
+                                          void* stream);
+
 /* ------------------------------------------------------------------------
  * Image input (examples/example.py:15-42 resizes every image with PIL.Image.resize).
  * ---------------------------------------------------------------------- */
@@ -212,6 +245,16 @@ int demon_pipeline_forward(demon_net* net, const float* image_pair, const float*
                            float* depth0, float* rotation, float* translation,
                            float* flow2, float* depth2, float* normal2, void* stream);
 
+/* The pipeline as examples/evaluation.py:225-255 runs it for an accuracy table: every intermediate prediction is kept.
+ * Snapshot k = 0 is the bootstrap block's output, snapshot k = 1..iterations the output after iteration k; the arrays hold
+ * S = iterations + 1 snapshots of the batch: flow2 [S,B,2,48,64], depth2 [S,B,1,48,64], normal2 [S,B,3,48,64],
+ * rotation / translation [S,B,3].  depth0 [S,B,1,192,256], if not NULL, is the refinement block run on every snapshot's
+ * depth2 (evaluation.py:249).  Inputs, image2_2 = NULL and the CUDA graph cache as demon_pipeline_forward; snapshot k
+ * equals the stage-wise entries after k iterations bit for bit.  Any output pointer may be NULL. */
+int demon_pipeline_forward_snapshots(demon_net* net, const float* image_pair, const float* image2_2, int iterations,
+                                     float* flow2, float* depth2, float* normal2, float* rotation, float* translation,
+                                     float* depth0, void* stream);
+
 /* Same, HOST buffers in and out (pinned or pageable): H2D copies, the pipeline, D2H copies and a
  * stream synchronisation, all inside the call.  This is the end-to-end path bench.py times. */
 int demon_pipeline_forward_host(demon_net* net, const float* image_pair_host, const float* image2_2_host,
@@ -251,6 +294,9 @@ int demon_net_batch(const demon_net* net);
 int64_t demon_net_workspace_bytes(const demon_net* net);
 /* number of kernel launches of one demon_pipeline_forward with `iterations` */
 int demon_net_pipeline_launches(const demon_net* net, int iterations);
+/* the same for the last demon_pipeline_forward_snapshots with `iterations` (counted apart: snapshot calls leave the value
+ * above untouched) */
+int demon_net_snapshot_launches(const demon_net* net, int iterations);
 /* 1 if layer `tf_name` (e.g. "netRefine/conv1_1") runs on the tensor-core path */
 int demon_net_layer_uses_tensor_cores(const demon_net* net, const char* tf_name);
 
