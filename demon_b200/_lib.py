@@ -47,6 +47,9 @@ PROTOTYPES = {
     "demon_motion_errors": [_P, _P, _P, c_int, _P, _P, _P],
     "demon_visible_points_mask_f32": [_P] * 5 + [c_int] * 7 + [_P, _P],
     "demon_visible_points_mask_inverse_f32": [_P] * 5 + [c_int] * 7 + [_P, _P],
+    "demon_point_cloud_scratch_bytes": [c_int, c_int, c_int],
+    "demon_point_cloud_f32": [_P] * 7 + [c_int] * 3 + [_P] * 6,
+    "demon_point_cloud_inverse_f32": [_P] * 7 + [c_int] * 3 + [_P] * 6,
     "demon_net_create": [ctypes.POINTER(c_void_p), c_int, c_int, c_int, c_int],
     "demon_net_destroy": [_P],
     "demon_net_set_weight": [_P, c_char_p, _P, _P, c_int],
@@ -93,6 +96,7 @@ _RESTYPES = {
     "demon_net_layer_name": c_char_p,
     "demon_net_workspace_bytes": c_int64,
     "demon_metric_workspace_bytes": c_int64,
+    "demon_point_cloud_scratch_bytes": c_int64,
     "demon_last_error": c_char_p,
     "demon_version": c_char_p,
     "demon_launch_count": c_int64,

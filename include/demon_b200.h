@@ -174,6 +174,30 @@ int demon_visible_points_mask_inverse_f32(const float* inverse_depth, const floa
                                           void* stream);
 
 /* ------------------------------------------------------------------------
+ * Point clouds of depth maps (python/depthmotionnet/vis.py:223-401 over vis_cython.pyx:24-173).
+ * ---------------------------------------------------------------------- */
+/* bytes of device scratch the two point-cloud entries need for n views of h x w (0 for an empty batch) */
+int64_t demon_point_cloud_scratch_bytes(int n, int h, int w);
+/* compute_point_cloud_from_depthmap (vis_cython.pyx:24-173) for n views, bit for bit: depth [n,h,w] camera z; per view K [3,3],
+ * R [3,3], t [3] (float32 device arrays, so a captured graph replays with new cameras).  The valid pixels (finite and > 0) in
+ * row-major order give rows 0..counts[i]-1 of view i:
+ *   points [n,h*w,3]   R^T ((d*((x+0.5)-cx)/fx, d*((y+0.5)-cy)/fy, d) - t), with the .pyx's float32 operations and reciprocals
+ *   normals_out        R^T normal of normals [n,3,h,w] (both NULL to skip)
+ *   colors_out [n,h*w,3] uint8: colors [n,3,h,w] uint8 as is, or image [n,3,h,w] float32 as ((image+0.5)*255).astype(uint8)
+ *                      of vis.py:276 (numpy's x86 cast: the low byte of the truncation, 0 for NaN and out-of-range values);
+ *                      at most one of colors and image, colors_out NULL with neither
+ *   counts [n] int32
+ * Rows at and past counts[i] are not written.  Scratch: demon_point_cloud_scratch_bytes(n, h, w) bytes.  Sides 1..8192,
+ * n up to 65535.  Output rows do not depend on scheduling; nothing synchronises, so the call can be captured in a graph. */
+int demon_point_cloud_f32(const float* depth, const float* K, const float* R, const float* t, const float* normals,
+                          const uint8_t* colors, const float* image, int n, int h, int w, void* scratch, float* points,
+                          float* normals_out, uint8_t* colors_out, int* counts, void* stream);
+/* the same on INVERSE depth: the kernels take d = 1/inverse_depth in float32 first (visualize_prediction, vis.py:246) */
+int demon_point_cloud_inverse_f32(const float* inverse_depth, const float* K, const float* R, const float* t, const float* normals,
+                                  const uint8_t* colors, const float* image, int n, int h, int w, void* scratch, float* points,
+                                  float* normals_out, uint8_t* colors_out, int* counts, void* stream);
+
+/* ------------------------------------------------------------------------
  * Image input (examples/example.py:15-42 resizes every image with PIL.Image.resize).
  * ---------------------------------------------------------------------- */
 /* resample filters, with Pillow's enum values (PIL.Image.Resampling) */
