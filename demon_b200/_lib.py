@@ -68,6 +68,8 @@ PROTOTYPES = {
     "demon_pipeline_forward_host_u8_async": [_P, _P, _P, c_int, _P, _P, _P, _P],
     "demon_resize_u8": [_P, c_int64, c_int64, c_int, c_int, c_int, _P, c_int, c_int, c_int, _P],
     "demon_pipeline_forward_images_u8": [_P, _P, c_int64, c_int64, c_int64] + [c_int] * 5 + [_P] * 6 + [_P],
+    "demon_adjust_intrinsics_u8": [_P, c_int64, c_int64, c_int, c_int, c_int, _P] + [c_double] * 4 + [_P, c_int, c_int, _P, _P],
+    "demon_pipeline_forward_views_u8": [_P, _P, c_int64, c_int64, c_int64, c_int, c_int, _P, _P] + [c_int] * 3 + [_P] * 6 + [_P],
     "demon_net_batch": [_P],
     "demon_net_workspace_bytes": [_P],
     "demon_net_pipeline_launches": [_P, c_int],

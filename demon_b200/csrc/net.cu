@@ -1007,7 +1007,8 @@ int demon_refine_forward(demon_net* n, const float* image1, const float* depth2,
 
 // Input of the fused pipeline: fp32 NCHW (image_pair [B,6,192,256], image2_2 [B,3,48,64] or null), uint8
 // (images [B,2,192,256,3], image2_2 [B,48,64,3] or null) or uint8 pairs of any size to resize first (src, see
-// demon_pipeline_forward_images_u8).
+// demon_pipeline_forward_images_u8), or with K [B,2,4] to adapt to the network's intrinsics first (see
+// demon_pipeline_forward_views_u8).
 struct PipelineInput {
   const float* image_pair = nullptr;
   const float* image2_2 = nullptr;
@@ -1016,7 +1017,12 @@ struct PipelineInput {
   const unsigned char* src = nullptr;
   int64_t src_sn = 0, src_si = 0, src_sy = 0;
   int src_h = 0, src_w = 0, resample = 0, image2_2_mode = 0;
+  const double* K = nullptr;
+  unsigned char* status = nullptr;
 };
+
+// The intrinsics DeMoN was trained for (examples/example.py:51-61), in pixels of the 256x192 input
+static const double kNetIntrinsics[4] = {0.89115971 * 256, 1.18821287 * 192, 0.5 * 256, 0.5 * 192};
 
 // Outputs of demon_pipeline_forward_snapshots: snapshot k (0 = bootstrap, k = after iteration k) of every array is the
 // k-th [B, ...] slice; any pointer may be null.  `depth0` set: the refinement block also runs on every snapshot's depth2
@@ -1056,8 +1062,12 @@ static int pipeline_body(demon_net* n, const PipelineInput& arg, int iterations,
     // resized pair -> concat0 as uint8 [B,2,192,256,3] and the 64x48 image2_2 -> pd0a as uint8 [B,48,64,3]: both buffers are
     // free until the refinement block (the same staging as pipeline_host), and the uint8 path below reads them first
     unsigned char* pair = reinterpret_cast<unsigned char*>(n->concat0->p);
-    if ((rc = resize_u8_launch(in.src, in.src_sn, in.src_si, 2, in.src_sy, 2 * n->B, in.src_h, in.src_w, pair, 192, 256, in.resample, s)))
-      return rc;
+    if (in.K)
+      rc = adjust_intrinsics_launch(in.src, in.src_sn, in.src_si, 2, in.src_sy, 2 * n->B, in.src_h, in.src_w, in.K, kNetIntrinsics, pair,
+                                    192, 256, in.status, s);
+    else
+      rc = resize_u8_launch(in.src, in.src_sn, in.src_si, 2, in.src_sy, 2 * n->B, in.src_h, in.src_w, pair, 192, 256, in.resample, s);
+    if (rc) return rc;
     in.images_u8 = pair;
     in.image2_2_u8 = nullptr;
     if (in.image2_2_mode == 1) {
@@ -1157,6 +1167,23 @@ int demon_pipeline_forward_images_u8(demon_net* n, const uint8_t* images, int64_
   return pipeline_forward_impl(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, stream);
 }
 
+int demon_pipeline_forward_views_u8(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, const double* K,
+                                    uint8_t* status, int resample, int image2_2_mode, int iterations, float* depth0, float* rotation,
+                                    float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
+  REQUIRE_READY(n);
+  DEMON_REQUIRE(images && K && status, "pipeline_views_u8: null images, K or status");
+  DEMON_REQUIRE(sn >= 0 && si >= 0 && sy >= 0, "pipeline_views_u8: negative stride");
+  DEMON_REQUIRE(image2_2_mode == 0 || image2_2_mode == 1, "pipeline_views_u8: image2_2_mode %d is not 0 (median) or 1 (resize)",
+                image2_2_mode);
+  int rc = adjust_intrinsics_check(h, w, kNetIntrinsics, 192, 256, "pipeline_views_u8");
+  if (rc) return rc;
+  if ((rc = resize_u8_check(192, 256, 48, 64, resample, "pipeline_views_u8"))) return rc;
+  PipelineInput in;
+  in.src = images; in.src_sn = sn; in.src_si = si; in.src_sy = sy; in.src_h = h; in.src_w = w; in.resample = resample;
+  in.image2_2_mode = image2_2_mode; in.K = K; in.status = status;
+  return pipeline_forward_impl(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, stream);
+}
+
 static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iterations, float* depth0, float* rotation, float* translation,
                                  float* flow2, float* depth2, float* normal2, void* stream, const SnapshotOutputs* snap) {
   DEMON_REQUIRE(iterations >= 0 && iterations <= 7, "pipeline: iterations %d", iterations);
@@ -1178,7 +1205,7 @@ static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iter
     const std::vector<const void*> key = {in.image_pair, in.image2_2, in.images_u8, in.image2_2_u8, depth0, rotation, translation, flow2, depth2,
                                           normal2, val(iterations), in.src, val(in.src_sn), val(in.src_si), val(in.src_sy), val(in.src_h),
                                           val(in.src_w), val(in.resample), val(in.image2_2_mode), val(mode), so.flow2, so.depth2, so.normal2,
-                                          so.rotation, so.translation, so.depth0};
+                                          so.rotation, so.translation, so.depth0, in.K, in.status};
     for (auto& g : n->graphs)
       if (g.key == key) {
         if (g.exec == nullptr) {   // second call: capture

@@ -1,8 +1,10 @@
-"""Input preparation on the device: `PIL.Image.resize` and `prepare_input_data` of examples/example.py:15-42.
+"""Input preparation on the device: `PIL.Image.resize` and `prepare_input_data` of examples/example.py:15-42, and the image
+part of `adjust_intrinsics` (dataset_tools/view_tools.py:97-172) for photos from other cameras.
 
     from demon_b200 import images
     small = images.resize(frames, (256, 192))                    # CUDA uint8 [N,h,w,3] -> [N,192,256,3]
     input_data = images.prepare_input_data(img1, img2)           # the dict examples/example.py builds, as CUDA tensors
+    adapted, K_new, status = images.adjust_intrinsics(frames, K) # to the intrinsics DeMoN was trained for, 256x192
 
 `resize` returns Pillow's bytes exactly for NEAREST, BILINEAR and BICUBIC (the kernel is resize_u8_kernel in
 csrc/images.cu).  Inputs are CUDA uint8 RGB tensors in HWC order, as `torch.from_numpy(np.array(pil_image)).cuda()` gives
@@ -10,6 +12,7 @@ them; a cropped view such as `x[..., y0:y1, x0:x1, :]` is read in place.
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -17,6 +20,9 @@ from . import _lib
 NEAREST, BILINEAR, BICUBIC = 0, 2, 3   # PIL.Image.Resampling values
 RESAMPLE = {"nearest": NEAREST, "bilinear": BILINEAR, "bicubic": BICUBIC}
 MAX_SIDE = 8192
+# The intrinsics DeMoN was trained for, normalised (fx, fy, cx, cy); examples/example.py:51-61 asks for images adapted to them
+NETWORK_INTRINSICS = (0.89115971, 1.18821287, 0.5, 0.5)
+MAX_OFFSET = 2 ** 24   # largest crop offset adjust_intrinsics accepts
 
 
 def resample_code(resample):
@@ -114,3 +120,98 @@ def prepare_input_data(img1, img2, data_format="channels_first", resample="bicub
     else:
         pair = torch.cat((i1, i2), dim=-1)
     return {"image_pair": pair.contiguous(), "image1": i1.contiguous(), "image2_2": i22.contiguous()}
+
+
+def demon_intrinsics(width=256, height=192):
+    """The intrinsics DeMoN was trained for in pixels of a width x height image: numpy float64 K [3,3]."""
+    fx, fy, cx, cy = NETWORK_INTRINSICS
+    return np.array([[fx * width, 0.0, cx * width], [0.0, fy * height, cy * height], [0.0, 0.0, 1.0]])
+
+
+def intrinsics4(K, lead, name):
+    """K as [*lead,3,3] (the skew K[0,1] is ignored, as in the reference), [*lead,4] (fx, fy, cx, cy) or one [3,3] for all,
+    from numpy, a CPU or a CUDA tensor -> float64 [*lead,4]: a numpy array for host input, a CUDA tensor for CUDA input."""
+    cuda = isinstance(K, torch.Tensor) and K.is_cuda
+    try:
+        k = K.to(torch.float64) if cuda else np.asarray(K.cpu() if isinstance(K, torch.Tensor) else K, dtype=np.float64)
+    except (TypeError, ValueError):
+        raise ValueError("%s: expected a numpy array or a tensor of intrinsics, got %s" % (name, type(K).__name__))
+    shape = tuple(k.shape)
+    if shape == (3, 3) or shape == tuple(lead) + (3, 3):
+        k = k[..., [0, 1, 0, 1], [0, 1, 2, 2]]
+    elif shape != tuple(lead) + (4,):
+        raise ValueError("%s: expected shape %s, %s or (3, 3), got %s" % (name, tuple(lead) + (3, 3), tuple(lead) + (4,), shape))
+    if cuda:
+        return k.expand(tuple(lead) + (4,)).contiguous()
+    return np.ascontiguousarray(np.broadcast_to(k, tuple(lead) + (4,)))
+
+
+def intrinsics_window(K, K_new, w, h, width_new, height_new):
+    """What csrc/images.cu (window_of) computes for every image, on the host: K [...,4] and K_new [4] float64 numpy
+    (fx, fy, cx, cy), a w x h source, a width_new x height_new output -> dict of int64 arrays rw, rh (size of the resize),
+    x0, y0 (window offset in it), bilinear (1: BILINEAR, 0: LANCZOS) and status (0 ok, 1 fill added, 2 invalid)."""
+    K = np.asarray(K, dtype=np.float64)
+    fx, fy, cx, cy = (K[..., i] for i in range(4))
+    with np.errstate(all="ignore"):
+        sx, sy = K_new[0] / fx, K_new[1] / fy
+        rw, rh = w * sx, h * sy
+        x0, y0 = np.rint(cx * sx - K_new[2]), np.rint(cy * sy - K_new[3])
+        ok = (np.isfinite(fx) & (fx > 0) & np.isfinite(fy) & (fy > 0) & np.isfinite(cx) & np.isfinite(cy) & (rw >= 1) & (rw < MAX_SIDE + 1)
+              & (rh >= 1) & (rh < MAX_SIDE + 1) & (np.abs(x0) <= MAX_OFFSET) & (np.abs(y0) <= MAX_OFFSET))
+        z = lambda a: np.where(ok, a, 0).astype(np.int64)
+        rw, rh, x0, y0 = z(rw), z(rh), z(x0), z(y0)
+        leaves = (x0 < 0) | (y0 < 0) | (x0 + width_new > rw) | (y0 + height_new > rh)
+    return {"rw": rw, "rh": rh, "x0": x0, "y0": y0, "bilinear": z(sx > 1), "status": np.where(ok, leaves.astype(np.int64), 2)}
+
+
+def _check_adjust_source(h, w, name):
+    if h > 100 * w:
+        raise ValueError("%s: a source more than 100 times taller than wide (%dx%d, width x height) is not supported" % (name, w, h))
+
+
+def _device_intrinsics(K, lead, name, w, h, knew, width_new, height_new, device):
+    """intrinsics4 on `device`; host K is checked first (ValueError for what the kernel would mark invalid, status 2)."""
+    k = intrinsics4(K, lead, name)
+    if isinstance(k, np.ndarray):
+        bad = np.flatnonzero(intrinsics_window(k, knew, w, h, width_new, height_new)["status"].reshape(-1) == 2)
+        if bad.size:
+            raise ValueError("%s: the intrinsics %s of image %d give no valid resize of a %dx%d image: the focal lengths must be "
+                             "finite and positive, the principal point finite, the resized size within 1..%d and the offset within "
+                             "+-2^24" % (name, k.reshape(-1, 4)[bad[0]].tolist(), bad[0], w, h, MAX_SIDE))
+        k = torch.from_numpy(k).to(device)
+    return k
+
+
+def adjust_intrinsics(images, K, K_new=None, width_new=256, height_new=192):
+    """The image part of the reference's `adjust_intrinsics(view, K_new, width_new, height_new)` on the device: every image
+    (CUDA uint8 [N,h,w,3], or one [h,w,3]) with intrinsics K ([N,3,3], [3,3] or [N,4] = fx, fy, cx, cy in pixels; numpy,
+    CPU or CUDA) is resized so that its focal lengths become K_new's (BILINEAR if fx_new / fx > 1, else LANCZOS, bit for bit
+    with Pillow) and cropped so that its principal point and size become K_new's and width_new x height_new, with
+    (127, 127, 127) where the crop leaves the resized image.  K_new (host [3,3] or [4]) defaults to demon_intrinsics(width_new,
+    height_new).  Returns (images [N,height_new,width_new,3], K_new numpy [3,3], status CUDA uint8 [N]): 0 ok, 1 fill was
+    added (where the reference prints a warning), 2 invalid K (only for CUDA K; host K is checked here: ValueError).
+    Asynchronous on the current stream.  Unlike the reference's safe_crop_image, the crop is also right when the box leaves
+    the image with a positive offset (DESIGN.md section 7)."""
+    ow, oh = _check_size((width_new, height_new))
+    single = isinstance(images, torch.Tensor) and images.dim() == 3
+    x = images.unsqueeze(0) if single else images
+    check_images(x, "images", 4)
+    n, h, w = x.shape[0], x.shape[1], x.shape[2]
+    if n > 65535:
+        raise ValueError("images: at most 65535 images per call, got %d" % n)
+    _check_adjust_source(h, w, "images")
+    knew = intrinsics4(demon_intrinsics(ow, oh) if K_new is None else K_new, (), "K_new")
+    if not isinstance(knew, np.ndarray):
+        knew = knew.cpu().numpy()
+    if not (np.all(np.isfinite(knew)) and knew[0] > 0 and knew[1] > 0):
+        raise ValueError("K_new: the focal lengths must be finite and positive and the principal point finite, got %s" % knew.tolist())
+    k = _device_intrinsics(K, (n,), "K", w, h, knew, ow, oh, x.device)
+    out = torch.empty((n, oh, ow, 3), dtype=torch.uint8, device=x.device)
+    status = torch.empty((n,), dtype=torch.uint8, device=x.device)
+    if n:
+        with torch.cuda.device(x.device):
+            _lib.check(_lib.load().demon_adjust_intrinsics_u8(
+                x.data_ptr(), x.stride(0), x.stride(1), n, h, w, k.data_ptr(), *(float(v) for v in knew), out.data_ptr(), oh, ow,
+                status.data_ptr(), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
+    K_out = np.array([[knew[0], 0.0, knew[2]], [0.0, knew[1], knew[3]], [0.0, 0.0, 1.0]])
+    return (out[0], K_out, status[0]) if single else (out, K_out, status)

@@ -241,6 +241,7 @@ class DemonPipeline:
         # and output buffers: the graph key is then the same for every call, whatever tensors the caller passes.
         self._ip = self._i22 = self._out = None
         self._snap = self._snap_refined = None
+        self._K = self._status = None   # forward_views: intrinsics staging [B,2,4] float64 and status [B,2] uint8
 
     def stage(self, image_pair, image2_2=None):
         """Copies the inputs into the pipeline's own device buffers (asynchronous, current stream) and returns them."""
@@ -383,6 +384,40 @@ class DemonPipeline:
             ptr("predict_depth0"), ptr("predict_rotation"), ptr("predict_translation"),
             ptr("predict_flow2"), ptr("predict_depth2"), ptr("predict_normal2"), _stream()))
         return outputs
+
+    def forward_views(self, images, intrinsics, resample="bicubic", image2_2="resize", outputs=None):
+        """The pipeline on photos from any calibrated camera: images CUDA uint8 [B,2,h,w,3] as in forward_images, intrinsics
+        [B,2,3,3] or [B,2,4] (fx, fy, cx, cy in pixels) or one [3,3] for all, from numpy, CPU or CUDA.  Every image is first
+        adapted to the intrinsics DeMoN was trained for at 256x192 (images.adjust_intrinsics with its defaults, the step
+        examples/example.py:51-61 asks for); image2_2 is then made from the adapted second image as in forward_images.  The
+        intrinsics are copied into a buffer of the pipeline, so the call replays one CUDA graph for new values.  Returns the
+        outputs of forward_u8 on the adapted bytes, bit for bit, plus 'status' CUDA uint8 [B,2] (adjust_intrinsics' status;
+        host intrinsics are checked here instead: ValueError)."""
+        from .images import _check_adjust_source, _device_intrinsics, check_images, demon_intrinsics, intrinsics4, resample_code
+        b = self.batch_size
+        code = resample_code(resample)
+        if image2_2 not in ("resize", "median"):
+            raise ValueError("image2_2 must be 'resize' or 'median', got %r" % (image2_2,))
+        check_images(images, "images", 5)
+        if tuple(images.shape[:2]) != (b, 2):
+            raise ValueError("images: expected shape (%d, 2, h, w, 3), got %s" % (b, tuple(images.shape)))
+        h, w = images.shape[2], images.shape[3]
+        _check_adjust_source(h, w, "images")
+        k = _device_intrinsics(intrinsics, (b, 2), "intrinsics", w, h, intrinsics4(demon_intrinsics(), (), "K_new"), 256, 192,
+                               images.device)
+        if self._K is None:
+            self._K = torch.empty((b, 2, 4), dtype=torch.float64, device=images.device)
+            self._status = torch.empty((b, 2), dtype=torch.uint8, device=images.device)
+        self._K.copy_(k, non_blocking=True)
+        if outputs is None:
+            outputs = self.own_outputs()
+        ptr = lambda k: outputs[k].data_ptr() if outputs.get(k) is not None else None
+        _lib.check(_lib.load().demon_pipeline_forward_views_u8(
+            self.net.ptr, images.data_ptr(), images.stride(0), images.stride(1), images.stride(2), h, w, self._K.data_ptr(),
+            self._status.data_ptr(), code, 1 if image2_2 == "resize" else 0, self.iterations,
+            ptr("predict_depth0"), ptr("predict_rotation"), ptr("predict_translation"),
+            ptr("predict_flow2"), ptr("predict_depth2"), ptr("predict_normal2"), _stream()))
+        return dict(outputs, status=self._status)
 
     def forward_host_u8(self, images, image2_2, depth0, rotation, translation, stream=None, sync=True):
         """End to end from HOST uint8 images [B,2,192,256,3] (numpy or pinned torch CPU uint8): H2D of the bytes, the

@@ -209,6 +209,18 @@ int demon_point_cloud_inverse_f32(const float* inverse_depth, const float* K, co
  * n 0..65535.  Other filters (LANCZOS, BOX, HAMMING) are DEMON_E_INVALID. */
 int demon_resize_u8(const uint8_t* src, int64_t src_sn, int64_t src_sy, int n, int h, int w, uint8_t* dst, int oh, int ow,
                     int resample, void* stream);
+/* adjust_intrinsics (dataset_tools/view_tools.py:97-172) of n RGB uint8 images, the image part, bit for bit with Pillow:
+ * image i of src (addressed as in demon_resize_u8) with intrinsics K[i] = (fx, fy, cx, cy) in pixels (DEVICE doubles [n,4],
+ * so a captured graph replays with new values in the same buffer; the skew is ignored) is resized to
+ * rw = trunc(w fx_new/fx) x rh = trunc(h fy_new/fy) with BILINEAR if fx_new/fx > 1, else LANCZOS, and cropped to
+ * dst [n,oh,ow,3] from x0 = rint(cx fx_new/fx - cx_new), y0 = rint(cy fy_new/fy - cy_new), filling with 127 outside the
+ * resized image.  status [n] (device): 0 ok, 1 fill was added (the reference's printed warning), 2 invalid K (non-finite or
+ * non-positive focal length, non-finite principal point, rw or rh outside 1..8192, an offset beyond +-2^24): all fill.
+ * The crop is the correct one where the reference's safe_crop_image is not (a box leaving the image with x0 > 0 or y0 > 0,
+ * DESIGN.md section 7).  Sides 1..8192 and h <= 100 w (Pillow reorders its passes beyond), n 0..65535. */
+int demon_adjust_intrinsics_u8(const uint8_t* src, int64_t src_sn, int64_t src_sy, int n, int h, int w, const double* K, double fx_new,
+                               double fy_new, double cx_new, double cy_new, uint8_t* dst, int oh, int ow, uint8_t* status,
+                               void* stream);
 
 /* ------------------------------------------------------------------------
  * Network graphs (python/depthmotionnet/networks_original.py).
@@ -312,6 +324,16 @@ int demon_pipeline_forward_host_u8_async(demon_net* net, const uint8_t* images_h
 int demon_pipeline_forward_images_u8(demon_net* net, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w,
                                      int resample, int image2_2_mode, int iterations, float* depth0, float* rotation,
                                      float* translation, float* flow2, float* depth2, float* normal2, void* stream);
+
+/* The same pipeline on photos from any calibrated camera: images as in demon_pipeline_forward_images_u8 with their
+ * intrinsics K [B,2,4] (fx, fy, cx, cy in pixels, DEVICE doubles).  Every image is adapted to the network's intrinsics,
+ * K_new = (0.89115971 * 256, 1.18821287 * 192, 0.5 * 256, 0.5 * 192) at 256x192, exactly like demon_adjust_intrinsics_u8
+ * (status [B,2] as there); image2_2 is made from the adapted second image as image2_2_mode says.  The outputs equal
+ * demon_pipeline_forward_u8 on the adapted bytes, bit for bit.  K and status are part of the CUDA-graph key: a replay
+ * reads the K buffer's current values. */
+int demon_pipeline_forward_views_u8(demon_net* net, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w,
+                                    const double* K, uint8_t* status, int resample, int image2_2_mode, int iterations, float* depth0,
+                                    float* rotation, float* translation, float* flow2, float* depth2, float* normal2, void* stream);
 
 /* introspection for tests and bench */
 int demon_net_batch(const demon_net* net);
