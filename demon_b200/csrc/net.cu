@@ -12,6 +12,7 @@
 #include <map>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "conv.cuh"
@@ -70,6 +71,32 @@ struct Layer {
 // The refinement block has no head (head_end == begin).
 struct Block { int begin = 0, head_end = 0, end = 0; };
 
+// The outputs of a fused-pipeline call, in the C ABI's order; any pointer may be null
+struct PipelineOutputs { float *depth0, *rotation, *translation, *flow2, *depth2, *normal2; };
+
+enum PipelineInput : int64_t { IN_FP32, IN_U8, IN_RESIZE, IN_VIEWS };
+// NO_SNAPSHOTS: the last iteration's predictions and the refinement block; otherwise snapshot k (0 = bootstrap, k = after
+// iteration k) of every output is its k-th [B, ...] slice, and SNAPSHOTS_REFINED runs the refinement block on every snapshot
+// (examples/evaluation.py:225-255 refines all four)
+enum SnapshotMode : int64_t { NO_SNAPSHOTS, SNAPSHOTS, SNAPSHOTS_REFINED };
+
+// Everything one demon_pipeline_forward* call depends on, and so also the key of its CUDA graph: every field is 64 bits
+// wide, so the struct has no padding and equal calls are equal bytes.  Entries value-initialise it (unused fields are 0).
+struct PipelineCall {
+  PipelineInput input;
+  const float* image_pair;        // IN_FP32: [B,6,192,256]
+  const float* image2_2;          // IN_FP32: [B,3,48,64] or null (median3x3_downsample twice)
+  const uint8_t* images;          // IN_U8: [B,2,192,256,3]; IN_RESIZE / IN_VIEWS: [B,2,h,w,3] with strides sn, si, sy
+  const uint8_t* image2_2_u8;     // IN_U8: [B,48,64,3] or null
+  int64_t sn, si, sy, h, w, resample, image2_2_mode;
+  const double* K;                // IN_VIEWS: [B,2,4], adapted to the network's intrinsics with status [B,2]
+  uint8_t* status;
+  int64_t iterations;
+  PipelineOutputs out;
+  SnapshotMode snapshots;
+};
+static_assert(std::has_unique_object_representations<PipelineCall>::value, "PipelineCall is compared with memcmp");
+
 }  // namespace
 }  // namespace demon
 
@@ -90,8 +117,8 @@ struct demon_net {
   std::vector<void*> dev_allocs;
   int pipeline_launches[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   int snapshot_launches[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // the same for demon_pipeline_forward_snapshots (kept apart: bench.py reads the above)
-  // CUDA graphs of demon_pipeline_forward, keyed by the pointer arguments (launch-bound at small batch: ~270 launches)
-  struct GraphEntry { std::vector<const void*> key; cudaGraphExec_t exec; int launches; };
+  // CUDA graphs of the fused pipeline, one per distinct call (launch-bound at small batch: ~270 launches)
+  struct GraphEntry { PipelineCall call; cudaGraphExec_t exec; int launches; };
   std::vector<GraphEntry> graphs;
   cudaStream_t cap_stream = nullptr;   // capture happens on this private stream (the caller's may be the legacy default stream)
   // optional per-layer timing with CUDA events on the launching stream (bench.py's roofline leg)
@@ -108,6 +135,8 @@ struct demon_net {
   Buf *img8, *i22, *i22_half, *c1y, *c1, *c2y, *cat2, *extra_in, *exy, *c21y, *concat2, *c3y, *c3, *c31y, *concat3, *c4y, *c4,
       *c41y, *concat4, *c5y, *c5, *c51y, *c51, *pf5a, *pf5, *p2a, *flowconf2, *dn2, *mc1, *fc1, *fc2, *motion;
   Buf *rin, *concat0, *rc1, *concat1, *rc2, *rc21, *pd0a, *rdepth0, *splitk;
+  // staging roles of the buffers above (see build_plan)
+  Buf *pair_bytes, *i22_bytes, *planes2, *host_depth0, *host_motion;
   // the five blocks' layer ranges
   Block flow1, dm1, flow2, dm2, refine;
 
@@ -274,6 +303,19 @@ void build_plan(demon_net* n) {
   n->rc21 = n->add_buf(RH / 4, RW / 4, 128);
   n->pd0a = n->add_buf(RH, RW, 16);
   n->rdepth0 = n->add_buf(RH, RW, 1);
+  // The fused pipeline stages its inputs and the host entries' outputs in buffers that hold nothing live at the time:
+  n->pair_bytes = n->concat0;    // the image pair as uint8 [B,2,192,256,3] (resized / adapted), or a host entry's image pair
+  n->i22_bytes = n->pd0a;        // image2_2 as uint8 [B,48,64,3] (resized), or a host entry's image2_2
+  n->planes2 = n->c1y;           // image 2 as NCHW fp32 planes, input of the median pair of a uint8 call without image2_2
+  n->host_depth0 = n->rdepth0;   // a host entry's depth0 before its copy to the host
+  n->host_motion = n->fc1;       // a host entry's rotation and translation ([B,3] each) before their copy to the host
+  // The first three are consumed into img8 / i22 before the first block runs; then c1y is next written by conv1y, and
+  // concat0 and pd0a only by the refinement block.  That block shares no buffer with the iteration state, so it may also
+  // run between two iterations (snapshots): it writes rin, concat0, rc1, concat1, rc2, rc21, pd0a, rdepth0 (or the
+  // caller's depth0) and the split-K scratch, which holds partial sums only inside one layer; the iterations carry dn2,
+  // flowconf2, motion, i22, img8, cat2_f2, cat2_d2 and extra_in from one block to the next, and the refinement block only
+  // reads img8 (image 1, whatever the input kind) and dn2.  rdepth0 is that block's own output, and fc1 is free after the
+  // last DM block, which a host entry's one export follows.
 
   n->flow1 = build_flow_block(n, "netFlow1", false);
   n->dm1 = build_dm_block(n, "netDM1", false);
@@ -1005,215 +1047,100 @@ int demon_refine_forward(demon_net* n, const float* image1, const float* depth2,
                           (cudaStream_t)stream);
 }
 
-// Input of the fused pipeline: fp32 NCHW (image_pair [B,6,192,256], image2_2 [B,3,48,64] or null), uint8
-// (images [B,2,192,256,3], image2_2 [B,48,64,3] or null) or uint8 pairs of any size to resize first (src, see
-// demon_pipeline_forward_images_u8), or with K [B,2,4] to adapt to the network's intrinsics first (see
-// demon_pipeline_forward_views_u8).
-struct PipelineInput {
-  const float* image_pair = nullptr;
-  const float* image2_2 = nullptr;
-  const unsigned char* images_u8 = nullptr;
-  const unsigned char* image2_2_u8 = nullptr;
-  const unsigned char* src = nullptr;
-  int64_t src_sn = 0, src_si = 0, src_sy = 0;
-  int src_h = 0, src_w = 0, resample = 0, image2_2_mode = 0;
-  const double* K = nullptr;
-  unsigned char* status = nullptr;
-};
-
 // The intrinsics DeMoN was trained for (examples/example.py:51-61), in pixels of the 256x192 input
 static const double kNetIntrinsics[4] = {0.89115971 * 256, 1.18821287 * 192, 0.5 * 256, 0.5 * 192};
 
-// Outputs of demon_pipeline_forward_snapshots: snapshot k (0 = bootstrap, k = after iteration k) of every array is the
-// k-th [B, ...] slice; any pointer may be null.  `depth0` set: the refinement block also runs on every snapshot's depth2
-// (examples/evaluation.py:225-255 refines all four).
-struct SnapshotOutputs {
-  float* flow2 = nullptr;
-  float* depth2 = nullptr;
-  float* normal2 = nullptr;
-  float* rotation = nullptr;
-  float* translation = nullptr;
-  float* depth0 = nullptr;
-};
-
-// Snapshot k of the predictions.  Running the refinement block here, between two iterations, is safe because it shares
-// no buffer with the iteration state (build_plan): it writes rin, concat0, rc1, concat1, rc2, rc21, pd0a, rdepth0 (or the
-// caller's depth0) and the split-K scratch, which holds partial sums only inside one layer; the iterations carry dn2,
-// flowconf2, motion, i22, img8, cat2_f2, cat2_d2 and extra_in from one block to the next, and the refinement block only
-// reads img8 and dn2.  concat0 / pd0a double as staging of a uint8 or resized input, which is consumed into img8 / i22
-// before the first block runs.
-static int export_snapshot(demon_net* n, const SnapshotOutputs& o, int k, cudaStream_t s) {
+// The predictions at snapshot point k (0 = bootstrap, k = after iteration k) into the call's outputs, at slice k with
+// snapshots, then the refinement block on them unless the call takes snapshots without it
+static int export_outputs(demon_net* n, const PipelineCall& c, int k, cudaStream_t s) {
   const long B = n->B, P2 = 48L * 64, P0 = 192L * 256;
-  const auto at = [k](float* p, long per_snapshot) { return p ? p + k * per_snapshot : nullptr; };
+  const long slice = c.snapshots == NO_SNAPSHOTS ? 0 : k;
+  const auto at = [slice](float* p, long per_snapshot) { return p ? p + slice * per_snapshot : nullptr; };
+  const PipelineOutputs& o = c.out;
   int rc = export_predictions(n, nullptr, at(o.flow2, B * 2 * P2), at(o.depth2, B * P2), at(o.normal2, B * 3 * P2), at(o.rotation, B * 3),
                               at(o.translation, B * 3), 0, s);
-  if (rc || !o.depth0) return rc;
+  if (rc || c.snapshots == SNAPSHOTS) return rc;
+  // image1 is read back from img8 (NHWC8: the first three channels), whatever the input kind; no depth0: into rdepth0
   return run_refine_block(n, n->img8->p, buf_strides(n->img8), n->dn2->p, buf_strides(n->dn2), 48, 64, at(o.depth0, B * P0), s);
 }
 
-// `snap` null: the plain pipeline (last iteration's outputs); otherwise every snapshot goes to `snap` and the other outputs
-// are unused
-static int pipeline_body(demon_net* n, const PipelineInput& arg, int iterations, float* depth0, float* rotation,
-                         float* translation, float* flow2, float* depth2, float* normal2, const SnapshotOutputs* snap, cudaStream_t s) {
+static int pipeline_body(demon_net* n, const PipelineCall& c, cudaStream_t s) {
   int rc;
   const long P = 192L * 256;
-  PipelineInput in = arg;
-  if (in.src) {
-    // resized pair -> concat0 as uint8 [B,2,192,256,3] and the 64x48 image2_2 -> pd0a as uint8 [B,48,64,3]: both buffers are
-    // free until the refinement block (the same staging as pipeline_host), and the uint8 path below reads them first
-    unsigned char* pair = reinterpret_cast<unsigned char*>(n->concat0->p);
-    if (in.K)
-      rc = adjust_intrinsics_launch(in.src, in.src_sn, in.src_si, 2, in.src_sy, 2 * n->B, in.src_h, in.src_w, in.K, kNetIntrinsics, pair,
-                                    192, 256, in.status, s);
+  const uint8_t* images = c.images;
+  const uint8_t* image2_2_u8 = c.image2_2_u8;
+  if (c.input == IN_RESIZE || c.input == IN_VIEWS) {
+    uint8_t* pair = reinterpret_cast<uint8_t*>(n->pair_bytes->p);
+    if (c.input == IN_VIEWS)
+      rc = adjust_intrinsics_launch(c.images, c.sn, c.si, 2, c.sy, 2 * n->B, (int)c.h, (int)c.w, c.K, kNetIntrinsics, pair, 192, 256,
+                                    c.status, s);
     else
-      rc = resize_u8_launch(in.src, in.src_sn, in.src_si, 2, in.src_sy, 2 * n->B, in.src_h, in.src_w, pair, 192, 256, in.resample, s);
+      rc = resize_u8_launch(c.images, c.sn, c.si, 2, c.sy, 2 * n->B, (int)c.h, (int)c.w, pair, 192, 256, (int)c.resample, s);
     if (rc) return rc;
-    in.images_u8 = pair;
-    in.image2_2_u8 = nullptr;
-    if (in.image2_2_mode == 1) {
-      unsigned char* i22 = reinterpret_cast<unsigned char*>(n->pd0a->p);
-      if ((rc = resize_u8_launch(pair + P * 3, 2 * P * 3, 0, 1, 256 * 3, n->B, 192, 256, i22, 48, 64, in.resample, s))) return rc;
-      in.image2_2_u8 = i22;
+    images = pair;
+    if (c.image2_2_mode == 1) {
+      uint8_t* i22 = reinterpret_cast<uint8_t*>(n->i22_bytes->p);
+      if ((rc = resize_u8_launch(pair + P * 3, 2 * P * 3, 0, 1, 256 * 3, n->B, 192, 256, i22, 48, 64, (int)c.resample, s))) return rc;
+      image2_2_u8 = i22;
     }
   }
-  if (in.images_u8) {
-    // img8 straight from the bytes; image 2's planes go to c1y (free until conv1y runs) for the median pair
-    float* planes2 = in.image2_2_u8 ? nullptr : n->c1y->p;
+  if (c.input != IN_FP32) {
+    // img8 straight from the bytes; without image2_2, image 2's planes for the median pair
+    float* planes2 = image2_2_u8 ? nullptr : n->planes2->p;
     long blocks = ((long)n->B * P + 255) / 256;
     if (blocks > 132 * 32) blocks = 132 * 32;
-    (void)launch_pdl(u8_import_kernel, dim3((int)blocks), dim3(256), 0, s, in.images_u8, n->img8->p, planes2, n->B, (int)P);
+    (void)launch_pdl(u8_import_kernel, dim3((int)blocks), dim3(256), 0, s, images, n->img8->p, planes2, n->B, (int)P);
     DEMON_LAUNCH_CHECK();
-    if (in.image2_2_u8) {
+    if (image2_2_u8) {
       long b2 = ((long)n->B * 48 * 64 + 255) / 256;
-      (void)launch_pdl(u8_planes_kernel, dim3((int)b2), dim3(256), 0, s, in.image2_2_u8, n->i22->p, n->B, 48 * 64);
+      (void)launch_pdl(u8_planes_kernel, dim3((int)b2), dim3(256), 0, s, image2_2_u8, n->i22->p, n->B, 48 * 64);
       DEMON_LAUNCH_CHECK();
     } else if ((rc = median_image2_2(n, planes2, 3 * P, s))) {
       return rc;
     }
   } else {
-    if ((rc = import_image_pair(n, in.image_pair, 0, s))) return rc;
-    if (in.image2_2) {
-      if ((rc = import_image2_2(n, in.image2_2, 0, s))) return rc;
+    if ((rc = import_image_pair(n, c.image_pair, 0, s))) return rc;
+    if (c.image2_2) {
+      if ((rc = import_image2_2(n, c.image2_2, 0, s))) return rc;
     } else {
-      if ((rc = median_image2_2(n, in.image_pair + 3 * P, 6 * P, s))) return rc;
+      if ((rc = median_image2_2(n, c.image_pair + 3 * P, 6 * P, s))) return rc;
     }
   }
-  if ((rc = run_flow_block(n, n->flow1, false, s))) return rc;
-  if ((rc = run_dm_block(n, n->dm1, false, s))) return rc;
-  if (snap && (rc = export_snapshot(n, *snap, 0, s))) return rc;
-  // conv1 / conv2 of netFlow2 and netDM2 read only the image pair and fixed weights: once per call instead of once per
-  // iteration (bit identical; 2 x 2 x 221.7 MMAC per pair less to execute at three iterations)
-  if (iterations > 0) {
-    if ((rc = run_layers(n, n->flow2.begin, n->flow2.head_end, s))) return rc;
-    if ((rc = run_layers(n, n->dm2.begin, n->dm2.head_end, s))) return rc;
+  // k = 0: the bootstrap blocks; k > 0: iteration k
+  for (int k = 0; k <= c.iterations; ++k) {
+    if ((rc = run_flow_block(n, k ? n->flow2 : n->flow1, k > 0, s, k == 0))) return rc;
+    if ((rc = run_dm_block(n, k ? n->dm2 : n->dm1, k > 0, s, k == 0))) return rc;
+    if ((c.snapshots != NO_SNAPSHOTS || k == c.iterations) && (rc = export_outputs(n, c, k, s))) return rc;
+    // conv1 / conv2 of netFlow2 and netDM2 read only the image pair and fixed weights: once per call instead of once per
+    // iteration (bit identical; 2 x 2 x 221.7 MMAC per pair less to execute at three iterations)
+    if (k == 0 && c.iterations > 0) {
+      if ((rc = run_layers(n, n->flow2.begin, n->flow2.head_end, s))) return rc;
+      if ((rc = run_layers(n, n->dm2.begin, n->dm2.head_end, s))) return rc;
+    }
   }
-  for (int it = 0; it < iterations; ++it) {
-    if ((rc = run_flow_block(n, n->flow2, true, s, false))) return rc;
-    if ((rc = run_dm_block(n, n->dm2, true, s, false))) return rc;
-    if (snap && (rc = export_snapshot(n, *snap, it + 1, s))) return rc;
-  }
-  if (snap) return DEMON_OK;
-  if ((rc = export_predictions(n, nullptr, flow2, depth2, normal2, rotation, translation, 0, s))) return rc;
-  // image1 for the refinement block is read back from img8 (NHWC8: the first three channels), whatever the input kind
-  return run_refine_block(n, n->img8->p, buf_strides(n->img8), n->dn2->p, buf_strides(n->dn2), 48, 64, depth0, s);
+  return DEMON_OK;
 }
 
-static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iterations, float* depth0, float* rotation, float* translation,
-                                 float* flow2, float* depth2, float* normal2, void* stream, const SnapshotOutputs* snap = nullptr);
-
-int demon_pipeline_forward(demon_net* n, const float* image_pair, const float* image2_2, int iterations, float* depth0, float* rotation,
-                           float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
-  REQUIRE_READY(n);
-  DEMON_REQUIRE(image_pair, "pipeline: null image_pair");
-  PipelineInput in;
-  in.image_pair = image_pair; in.image2_2 = image2_2;
-  return pipeline_forward_impl(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, stream);
-}
-
-int demon_pipeline_forward_snapshots(demon_net* n, const float* image_pair, const float* image2_2, int iterations, float* flow2,
-                                     float* depth2, float* normal2, float* rotation, float* translation, float* depth0, void* stream) {
-  REQUIRE_READY(n);
-  DEMON_REQUIRE(image_pair, "pipeline_snapshots: null image_pair");
-  PipelineInput in;
-  in.image_pair = image_pair; in.image2_2 = image2_2;
-  SnapshotOutputs snap;
-  snap.flow2 = flow2; snap.depth2 = depth2; snap.normal2 = normal2; snap.rotation = rotation; snap.translation = translation;
-  snap.depth0 = depth0;
-  return pipeline_forward_impl(n, in, iterations, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, stream, &snap);
-}
-
-int demon_pipeline_forward_u8(demon_net* n, const uint8_t* images, const uint8_t* image2_2, int iterations, float* depth0, float* rotation,
-                              float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
-  REQUIRE_READY(n);
-  DEMON_REQUIRE(images, "pipeline_u8: null images");
-  PipelineInput in;
-  in.images_u8 = images; in.image2_2_u8 = image2_2;
-  return pipeline_forward_impl(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, stream);
-}
-
-int demon_pipeline_forward_images_u8(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, int resample,
-                                     int image2_2_mode, int iterations, float* depth0, float* rotation, float* translation, float* flow2,
-                                     float* depth2, float* normal2, void* stream) {
-  REQUIRE_READY(n);
-  DEMON_REQUIRE(images, "pipeline_images_u8: null images");
-  DEMON_REQUIRE(sn >= 0 && si >= 0 && sy >= 0, "pipeline_images_u8: negative stride");
-  DEMON_REQUIRE(image2_2_mode == 0 || image2_2_mode == 1, "pipeline_images_u8: image2_2_mode %d is not 0 (median) or 1 (resize)",
-                image2_2_mode);
-  int rc = resize_u8_check(h, w, 192, 256, resample, "pipeline_images_u8");
-  if (rc) return rc;
-  PipelineInput in;
-  in.src = images; in.src_sn = sn; in.src_si = si; in.src_sy = sy; in.src_h = h; in.src_w = w; in.resample = resample;
-  in.image2_2_mode = image2_2_mode;
-  return pipeline_forward_impl(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, stream);
-}
-
-int demon_pipeline_forward_views_u8(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, const double* K,
-                                    uint8_t* status, int resample, int image2_2_mode, int iterations, float* depth0, float* rotation,
-                                    float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
-  REQUIRE_READY(n);
-  DEMON_REQUIRE(images && K && status, "pipeline_views_u8: null images, K or status");
-  DEMON_REQUIRE(sn >= 0 && si >= 0 && sy >= 0, "pipeline_views_u8: negative stride");
-  DEMON_REQUIRE(image2_2_mode == 0 || image2_2_mode == 1, "pipeline_views_u8: image2_2_mode %d is not 0 (median) or 1 (resize)",
-                image2_2_mode);
-  int rc = adjust_intrinsics_check(h, w, kNetIntrinsics, 192, 256, "pipeline_views_u8");
-  if (rc) return rc;
-  if ((rc = resize_u8_check(192, 256, 48, 64, resample, "pipeline_views_u8"))) return rc;
-  PipelineInput in;
-  in.src = images; in.src_sn = sn; in.src_si = si; in.src_sy = sy; in.src_h = h; in.src_w = w; in.resample = resample;
-  in.image2_2_mode = image2_2_mode; in.K = K; in.status = status;
-  return pipeline_forward_impl(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, stream);
-}
-
-static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iterations, float* depth0, float* rotation, float* translation,
-                                 float* flow2, float* depth2, float* normal2, void* stream, const SnapshotOutputs* snap) {
-  DEMON_REQUIRE(iterations >= 0 && iterations <= 7, "pipeline: iterations %d", iterations);
-  int* launch_record = snap ? n->snapshot_launches : n->pipeline_launches;
+static int pipeline_forward_impl(demon_net* n, const PipelineCall& c, void* stream) {
+  DEMON_REQUIRE(c.iterations >= 0 && c.iterations <= 7, "pipeline: iterations %d", (int)c.iterations);
+  int* launch_record = c.snapshots != NO_SNAPSHOTS ? n->snapshot_launches : n->pipeline_launches;
   DEMON_REQUIRE(n->RH == 192 && n->RW == 256, "pipeline: net was created with a %dx%d refinement block", n->RH, n->RW);
   cudaStream_t s = (cudaStream_t)stream;
-  // The call is one CUDA graph per distinct set of pointer arguments (DEMON_GRAPH=0 disables): the first call with a new
-  // set runs eagerly, the second captures, later ones replay.  Not used while per-layer profiling is on or when the
-  // caller is itself capturing this stream.
+  // The call is one CUDA graph per distinct PipelineCall (DEMON_GRAPH=0 disables): the first call with a new one runs
+  // eagerly, the second captures, later ones replay.  Not used while per-layer profiling is on or when the caller is itself
+  // capturing this stream.
   static const bool graphs_on = []() { const char* e = getenv("DEMON_GRAPH"); return !(e && e[0] == '0'); }();
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(s, &cap);
   if (graphs_on && !n->profiling && cap == cudaStreamCaptureStatusNone) {
-    const auto val = [](int64_t v) { return reinterpret_cast<const void*>((intptr_t)v); };
-    // snapshot calls: mode 1, or 2 with the per-snapshot refinement; their output pointers are part of the key as well
-    const SnapshotOutputs none;
-    const SnapshotOutputs& so = snap ? *snap : none;
-    const int mode = snap ? (snap->depth0 ? 2 : 1) : 0;
-    const std::vector<const void*> key = {in.image_pair, in.image2_2, in.images_u8, in.image2_2_u8, depth0, rotation, translation, flow2, depth2,
-                                          normal2, val(iterations), in.src, val(in.src_sn), val(in.src_si), val(in.src_sy), val(in.src_h),
-                                          val(in.src_w), val(in.resample), val(in.image2_2_mode), val(mode), so.flow2, so.depth2, so.normal2,
-                                          so.rotation, so.translation, so.depth0, in.K, in.status};
     for (auto& g : n->graphs)
-      if (g.key == key) {
+      if (memcmp(&g.call, &c, sizeof(c)) == 0) {
         if (g.exec == nullptr) {   // second call: capture
           cudaGraph_t graph = nullptr;
           const int64_t l0 = g_launch_count.load();
           if (!n->cap_stream) DEMON_CHECK_CUDA(cudaStreamCreateWithFlags(&n->cap_stream, cudaStreamNonBlocking));
           DEMON_CHECK_CUDA(cudaStreamBeginCapture(n->cap_stream, cudaStreamCaptureModeThreadLocal));
-          int rc = pipeline_body(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, snap, n->cap_stream);
+          int rc = pipeline_body(n, c, n->cap_stream);
           cudaError_t e = cudaStreamEndCapture(n->cap_stream, &graph);
           if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
           if (e != cudaSuccess) return fail(DEMON_E_CUDA, "pipeline: stream capture failed: %s", cudaGetErrorString(e));
@@ -1225,24 +1152,124 @@ static int pipeline_forward_impl(demon_net* n, const PipelineInput& in, int iter
         }
         DEMON_CHECK_CUDA(cudaGraphLaunch(g.exec, s));
         g_launch_count.fetch_add(g.launches);
-        launch_record[iterations] = g.launches;
+        launch_record[c.iterations] = g.launches;
         return DEMON_OK;
       }
     if (n->graphs.size() >= 32) {   // evict the oldest entry
       if (n->graphs.front().exec) cudaGraphExecDestroy(n->graphs.front().exec);
       n->graphs.erase(n->graphs.begin());
     }
-    n->graphs.push_back({key, nullptr, 0});
+    n->graphs.push_back({c, nullptr, 0});
   }
   const int64_t launches0 = g_launch_count.load();
-  int rc = pipeline_body(n, in, iterations, depth0, rotation, translation, flow2, depth2, normal2, snap, s);
+  int rc = pipeline_body(n, c, s);
   if (rc) return rc;
-  launch_record[iterations] = (int)(g_launch_count.load() - launches0);
+  launch_record[c.iterations] = (int)(g_launch_count.load() - launches0);
   return DEMON_OK;
 }
 
+int demon_pipeline_forward(demon_net* n, const float* image_pair, const float* image2_2, int iterations, float* depth0, float* rotation,
+                           float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
+  REQUIRE_READY(n);
+  DEMON_REQUIRE(image_pair, "pipeline: null image_pair");
+  PipelineCall c{};
+  c.input = IN_FP32; c.image_pair = image_pair; c.image2_2 = image2_2; c.iterations = iterations;
+  c.out = {depth0, rotation, translation, flow2, depth2, normal2};
+  return pipeline_forward_impl(n, c, stream);
+}
+
+int demon_pipeline_forward_snapshots(demon_net* n, const float* image_pair, const float* image2_2, int iterations, float* flow2,
+                                     float* depth2, float* normal2, float* rotation, float* translation, float* depth0, void* stream) {
+  REQUIRE_READY(n);
+  DEMON_REQUIRE(image_pair, "pipeline_snapshots: null image_pair");
+  PipelineCall c{};
+  c.input = IN_FP32; c.image_pair = image_pair; c.image2_2 = image2_2; c.iterations = iterations;
+  c.out = {depth0, rotation, translation, flow2, depth2, normal2};
+  c.snapshots = depth0 ? SNAPSHOTS_REFINED : SNAPSHOTS;
+  return pipeline_forward_impl(n, c, stream);
+}
+
+int demon_pipeline_forward_u8(demon_net* n, const uint8_t* images, const uint8_t* image2_2, int iterations, float* depth0, float* rotation,
+                              float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
+  REQUIRE_READY(n);
+  DEMON_REQUIRE(images, "pipeline_u8: null images");
+  PipelineCall c{};
+  c.input = IN_U8; c.images = images; c.image2_2_u8 = image2_2; c.iterations = iterations;
+  c.out = {depth0, rotation, translation, flow2, depth2, normal2};
+  return pipeline_forward_impl(n, c, stream);
+}
+
+// The argument checks shared by the entries that take uint8 pairs of any size, which then fill the source fields of `c`
+static int set_source(PipelineCall& c, PipelineInput input, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w,
+                      int resample, int image2_2_mode, const char* who) {
+  DEMON_REQUIRE(sn >= 0 && si >= 0 && sy >= 0, "%s: negative stride", who);
+  DEMON_REQUIRE(image2_2_mode == 0 || image2_2_mode == 1, "%s: image2_2_mode %d is not 0 (median) or 1 (resize)", who, image2_2_mode);
+  c.input = input; c.images = images; c.sn = sn; c.si = si; c.sy = sy; c.h = h; c.w = w; c.resample = resample;
+  c.image2_2_mode = image2_2_mode;
+  return DEMON_OK;
+}
+
+int demon_pipeline_forward_images_u8(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, int resample,
+                                     int image2_2_mode, int iterations, float* depth0, float* rotation, float* translation, float* flow2,
+                                     float* depth2, float* normal2, void* stream) {
+  REQUIRE_READY(n);
+  DEMON_REQUIRE(images, "pipeline_images_u8: null images");
+  PipelineCall c{};
+  int rc = set_source(c, IN_RESIZE, images, sn, si, sy, h, w, resample, image2_2_mode, "pipeline_images_u8");
+  if (rc || (rc = resize_u8_check(h, w, 192, 256, resample, "pipeline_images_u8"))) return rc;
+  c.iterations = iterations;
+  c.out = {depth0, rotation, translation, flow2, depth2, normal2};
+  return pipeline_forward_impl(n, c, stream);
+}
+
+int demon_pipeline_forward_views_u8(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, const double* K,
+                                    uint8_t* status, int resample, int image2_2_mode, int iterations, float* depth0, float* rotation,
+                                    float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
+  REQUIRE_READY(n);
+  DEMON_REQUIRE(images && K && status, "pipeline_views_u8: null images, K or status");
+  PipelineCall c{};
+  int rc = set_source(c, IN_VIEWS, images, sn, si, sy, h, w, resample, image2_2_mode, "pipeline_views_u8");
+  if (rc || (rc = adjust_intrinsics_check(h, w, kNetIntrinsics, 192, 256, "pipeline_views_u8"))) return rc;
+  if ((rc = resize_u8_check(192, 256, 48, 64, resample, "pipeline_views_u8"))) return rc;
+  c.K = K; c.status = status; c.iterations = iterations;
+  c.out = {depth0, rotation, translation, flow2, depth2, normal2};
+  return pipeline_forward_impl(n, c, stream);
+}
+
+// H2D of the inputs into the staging buffers (build_plan), the pipeline, D2H of depth0 / rotation / translation
 static int pipeline_host(demon_net* n, const void* images_host, const void* image2_2_host, bool u8, int iterations, float* depth0_host,
-                         float* rotation_host, float* translation_host, void* stream, bool sync);
+                         float* rotation_host, float* translation_host, void* stream, bool sync) {
+  REQUIRE_READY(n);
+  DEMON_REQUIRE(images_host && depth0_host, "pipeline_host: null pointer");
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t px = (size_t)n->B * 192 * 256;
+  const size_t ip_bytes = u8 ? px * 6 : px * 6 * sizeof(float);
+  const size_t i22_bytes = (size_t)n->B * 3 * 48 * 64 * (u8 ? 1 : sizeof(float));
+  void* ip_dev = n->pair_bytes->p;
+  void* i22_dev = image2_2_host ? n->i22_bytes->p : nullptr;
+  DEMON_CHECK_CUDA(cudaMemcpyAsync(ip_dev, images_host, ip_bytes, cudaMemcpyHostToDevice, s));
+  if (i22_dev) DEMON_CHECK_CUDA(cudaMemcpyAsync(i22_dev, image2_2_host, i22_bytes, cudaMemcpyHostToDevice, s));
+  float* rt_dev = n->host_motion->p;
+  PipelineCall c{};
+  if (u8) { c.input = IN_U8; c.images = static_cast<const uint8_t*>(ip_dev); c.image2_2_u8 = static_cast<const uint8_t*>(i22_dev); }
+  else { c.input = IN_FP32; c.image_pair = static_cast<const float*>(ip_dev); c.image2_2 = static_cast<const float*>(i22_dev); }
+  c.iterations = iterations;
+  c.out.depth0 = n->host_depth0->p;
+  c.out.rotation = rotation_host ? rt_dev : nullptr;
+  c.out.translation = translation_host ? rt_dev + 3 * n->B : nullptr;
+  int rc = pipeline_forward_impl(n, c, stream);
+  if (rc) return rc;
+  DEMON_CHECK_CUDA(cudaMemcpyAsync(depth0_host, c.out.depth0, px * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if (rotation_host) DEMON_CHECK_CUDA(cudaMemcpyAsync(rotation_host, rt_dev, (size_t)n->B * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if (translation_host)
+    DEMON_CHECK_CUDA(cudaMemcpyAsync(translation_host, rt_dev + 3 * n->B, (size_t)n->B * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if (sync) {
+    DEMON_CHECK_CUDA(cudaStreamSynchronize(s));
+    if (tc_read_error_flag(true))
+      return fail(DEMON_E_STATE, "a pipeline wait inside a tensor-core convolution kernel timed out: the outputs are invalid");
+  }
+  return DEMON_OK;
+}
 
 int demon_pipeline_forward_host(demon_net* n, const float* image_pair_host, const float* image2_2_host, int iterations, float* depth0_host,
                                 float* rotation_host, float* translation_host, void* stream) {
@@ -1262,41 +1289,6 @@ int demon_pipeline_forward_host_u8(demon_net* n, const uint8_t* images_host, con
 int demon_pipeline_forward_host_u8_async(demon_net* n, const uint8_t* images_host, const uint8_t* image2_2_host, int iterations,
                                          float* depth0_host, float* rotation_host, float* translation_host, void* stream) {
   return pipeline_host(n, images_host, image2_2_host, true, iterations, depth0_host, rotation_host, translation_host, stream, false);
-}
-
-static int pipeline_host(demon_net* n, const void* images_host, const void* image2_2_host, bool u8, int iterations, float* depth0_host,
-                         float* rotation_host, float* translation_host, void* stream, bool sync) {
-  REQUIRE_READY(n);
-  DEMON_REQUIRE(images_host && depth0_host, "pipeline_host: null pointer");
-  cudaStream_t s = (cudaStream_t)stream;
-  // staging lives in buffers that are free at the respective moments:
-  //   images     -> concat0 ([B,192,256,64]; only written by the refinement block, which reads image1 back from img8)
-  //   image2_2   -> pd0a    (only written by netRefine/predict_depth0/conv1)
-  const size_t px = (size_t)n->B * 192 * 256;
-  const size_t ip_bytes = u8 ? px * 6 : px * 6 * sizeof(float);
-  const size_t i22_bytes = (size_t)n->B * 3 * 48 * 64 * (u8 ? 1 : sizeof(float));
-  void* ip_dev = n->concat0->p;
-  void* i22_dev = n->pd0a->p;
-  DEMON_CHECK_CUDA(cudaMemcpyAsync(ip_dev, images_host, ip_bytes, cudaMemcpyHostToDevice, s));
-  if (image2_2_host) DEMON_CHECK_CUDA(cudaMemcpyAsync(i22_dev, image2_2_host, i22_bytes, cudaMemcpyHostToDevice, s));
-  float* out_dev = n->rdepth0->p;
-  float* rt_dev = n->fc1->p;                 // 6 floats per sample, fc1 is free after the last DM block
-  PipelineInput in;
-  if (u8) { in.images_u8 = static_cast<const unsigned char*>(ip_dev); in.image2_2_u8 = image2_2_host ? static_cast<const unsigned char*>(i22_dev) : nullptr; }
-  else { in.image_pair = static_cast<const float*>(ip_dev); in.image2_2 = image2_2_host ? static_cast<const float*>(i22_dev) : nullptr; }
-  int rc = pipeline_forward_impl(n, in, iterations, out_dev, rotation_host ? rt_dev : nullptr, translation_host ? rt_dev + 3 * n->B : nullptr,
-                                 nullptr, nullptr, nullptr, stream);
-  if (rc) return rc;
-  DEMON_CHECK_CUDA(cudaMemcpyAsync(depth0_host, out_dev, (size_t)n->B * 192 * 256 * sizeof(float), cudaMemcpyDeviceToHost, s));
-  if (rotation_host) DEMON_CHECK_CUDA(cudaMemcpyAsync(rotation_host, rt_dev, (size_t)n->B * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
-  if (translation_host)
-    DEMON_CHECK_CUDA(cudaMemcpyAsync(translation_host, rt_dev + 3 * n->B, (size_t)n->B * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
-  if (sync) {
-    DEMON_CHECK_CUDA(cudaStreamSynchronize(s));
-    if (tc_read_error_flag(true))
-      return fail(DEMON_E_STATE, "a pipeline wait inside a tensor-core convolution kernel timed out: the outputs are invalid");
-  }
-  return DEMON_OK;
 }
 
 // debug: which kernel family / plan every layer of the net got (one line per layer)

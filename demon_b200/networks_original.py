@@ -138,6 +138,18 @@ def _shape(fmt, b, c, h, w):
     return (b, c, h, w) if fmt == 0 else (b, h, w, c)
 
 
+def _ptr(x):
+    """The address of a torch tensor (host or device) or of a numpy array; None for None."""
+    if x is None:
+        return None
+    return x.data_ptr() if isinstance(x, torch.Tensor) else x.ctypes.data
+
+
+# the output pointers of the fused-pipeline entries, in C ABI order
+_OUTPUTS = ("predict_depth0", "predict_rotation", "predict_translation", "predict_flow2", "predict_depth2", "predict_normal2")
+_SNAPSHOT_OUTPUTS = ("predict_flow2", "predict_depth2", "predict_normal2", "predict_rotation", "predict_translation", "predict_depth0")
+
+
 class _NetBase:
     def __init__(self, session, data_format="channels_first", batch_size=1):
         self.session = session if session is not None else default_session()
@@ -260,14 +272,26 @@ class DemonPipeline:
             i2 = self._i22
         return self._ip, i2
 
-    def own_outputs(self):
-        if self._out is None:
-            b = self.batch_size
+    def _own(self, attr, shapes):
+        """The persistent float32 buffers `attr` of the pipeline (name -> shape), made on the first call."""
+        if getattr(self, attr) is None:
             dev = self._ip.device if self._ip is not None else torch.device("cuda", torch.cuda.current_device())
-            mk = lambda *s: torch.empty(s, dtype=torch.float32, device=dev)
-            self._out = {"predict_depth0": mk(b, 1, 192, 256), "predict_rotation": mk(b, 3), "predict_translation": mk(b, 3),
-                         "predict_flow2": mk(b, 2, 48, 64), "predict_depth2": mk(b, 1, 48, 64), "predict_normal2": mk(b, 3, 48, 64)}
-        return self._out
+            setattr(self, attr, {k: torch.empty(s, dtype=torch.float32, device=dev) for k, s in shapes.items()})
+        return getattr(self, attr)
+
+    def own_outputs(self):
+        b = self.batch_size
+        return self._own("_out", {"predict_depth0": (b, 1, 192, 256), "predict_rotation": (b, 3), "predict_translation": (b, 3),
+                                  "predict_flow2": (b, 2, 48, 64), "predict_depth2": (b, 1, 48, 64), "predict_normal2": (b, 3, 48, 64)})
+
+    def _run(self, entry, args, outputs=None, keys=_OUTPUTS):
+        """Calls the C entry `entry` on the net with `args`, the iteration count, the pointers of `outputs` (default: the
+        pipeline's own) in the order of `keys` (null for a missing one) and the current stream; raises on an error code."""
+        if outputs is None:
+            outputs = self.own_outputs()
+        fn = getattr(_lib.load(), entry)
+        _lib.check(fn(self.net.ptr, *args, self.iterations, *(_ptr(outputs.get(k)) for k in keys), _stream()))
+        return outputs
 
     def forward(self, image_pair, image2_2=None, outputs=None, stage_inputs=True):
         """image_pair: torch CUDA [B,6,192,256]; image2_2: torch CUDA [B,3,48,64] or None (then it is
@@ -294,28 +318,16 @@ class DemonPipeline:
             if self._ip is None:
                 raise RuntimeError("forward_staged() before stage()")
             ip, i2 = self._ip, (self._i22 if use_image2_2 else None)
-        if outputs is None:
-            outputs = self.own_outputs()
-        ptr = lambda k: outputs[k].data_ptr() if outputs.get(k) is not None else None
-        _lib.check(_lib.load().demon_pipeline_forward(
-            self.net.ptr, ip.data_ptr(), None if i2 is None else i2.data_ptr(), self.iterations,
-            ptr("predict_depth0"), ptr("predict_rotation"), ptr("predict_translation"),
-            ptr("predict_flow2"), ptr("predict_depth2"), ptr("predict_normal2"), _stream()))
-        return outputs
+        return self._run("demon_pipeline_forward", (ip.data_ptr(), _ptr(i2)), outputs)
 
     def own_snapshot_outputs(self, refine=True):
         """The persistent output buffers of forward_snapshots (S = iterations + 1 snapshots); one set per `refine`."""
-        key = "_snap_refined" if refine else "_snap"
-        if getattr(self, key, None) is None:
-            b, s = self.batch_size, self.iterations + 1
-            dev = self._ip.device if self._ip is not None else torch.device("cuda", torch.cuda.current_device())
-            mk = lambda *sh: torch.empty(sh, dtype=torch.float32, device=dev)
-            out = {"predict_flow2": mk(s, b, 2, 48, 64), "predict_depth2": mk(s, b, 1, 48, 64), "predict_normal2": mk(s, b, 3, 48, 64),
-                   "predict_rotation": mk(s, b, 3), "predict_translation": mk(s, b, 3)}
-            if refine:
-                out["predict_depth0"] = mk(s, b, 1, 192, 256)
-            setattr(self, key, out)
-        return getattr(self, key)
+        b, s = self.batch_size, self.iterations + 1
+        shapes = {"predict_flow2": (s, b, 2, 48, 64), "predict_depth2": (s, b, 1, 48, 64), "predict_normal2": (s, b, 3, 48, 64),
+                  "predict_rotation": (s, b, 3), "predict_translation": (s, b, 3)}
+        if refine:
+            shapes["predict_depth0"] = (s, b, 1, 192, 256)
+        return self._own("_snap_refined" if refine else "_snap", shapes)
 
     def forward_snapshots(self, image_pair, image2_2=None, refine=True, outputs=None):
         """The pipeline keeping every intermediate prediction, as examples/evaluation.py:225-255 stores them: snapshot 0
@@ -327,11 +339,9 @@ class DemonPipeline:
         ip, i2 = self.stage(image_pair, image2_2)
         if outputs is None:
             outputs = self.own_snapshot_outputs(refine)
-        ptr = lambda k: outputs[k].data_ptr() if outputs.get(k) is not None else None
-        _lib.check(_lib.load().demon_pipeline_forward_snapshots(
-            self.net.ptr, ip.data_ptr(), None if i2 is None else i2.data_ptr(), self.iterations,
-            ptr("predict_flow2"), ptr("predict_depth2"), ptr("predict_normal2"), ptr("predict_rotation"),
-            ptr("predict_translation"), ptr("predict_depth0") if refine else None, _stream()))
+        # without `refine` no depth0 pointer, which is what skips the refinement
+        self._run("demon_pipeline_forward_snapshots", (ip.data_ptr(), _ptr(i2)),
+                  outputs if refine else dict(outputs, predict_depth0=None), _SNAPSHOT_OUTPUTS)
         return outputs
 
     def snapshot_launches(self):
@@ -350,14 +360,18 @@ class DemonPipeline:
         images = images.contiguous()
         if image2_2 is not None:
             image2_2 = image2_2.contiguous()
-        if outputs is None:
-            outputs = self.own_outputs()
-        ptr = lambda k: outputs[k].data_ptr() if outputs.get(k) is not None else None
-        _lib.check(_lib.load().demon_pipeline_forward_u8(
-            self.net.ptr, images.data_ptr(), None if image2_2 is None else image2_2.data_ptr(), self.iterations,
-            ptr("predict_depth0"), ptr("predict_rotation"), ptr("predict_translation"),
-            ptr("predict_flow2"), ptr("predict_depth2"), ptr("predict_normal2"), _stream()))
-        return outputs
+        return self._run("demon_pipeline_forward_u8", (images.data_ptr(), _ptr(image2_2)), outputs)
+
+    def _check_pairs(self, images, resample, image2_2):
+        """The checks of forward_images / forward_views; returns h, w, the resample code and the image2_2 mode."""
+        from .images import check_images, resample_code
+        code = resample_code(resample)
+        if image2_2 not in ("resize", "median"):
+            raise ValueError("image2_2 must be 'resize' or 'median', got %r" % (image2_2,))
+        check_images(images, "images", 5)
+        if tuple(images.shape[:2]) != (self.batch_size, 2):
+            raise ValueError("images: expected shape (%d, 2, h, w, 3), got %s" % (self.batch_size, tuple(images.shape)))
+        return images.shape[2], images.shape[3], code, 1 if image2_2 == "resize" else 0
 
     def forward_images(self, images, resample="bicubic", image2_2="resize", outputs=None):
         """The pipeline on image pairs of any size (examples/example.py:15-42 and :87-99 in one call): images CUDA uint8
@@ -366,24 +380,8 @@ class DemonPipeline:
         enum value); image2_2 is 'resize' (the resized second image resized to 64x48 with the same filter, example.py:22) or
         'median' (median3x3_downsample twice, examples/evaluation.py:170-173).  Same outputs as forward_u8 on the resized
         bytes, bit for bit."""
-        from .images import check_images, resample_code
-        b = self.batch_size
-        code = resample_code(resample)
-        if image2_2 not in ("resize", "median"):
-            raise ValueError("image2_2 must be 'resize' or 'median', got %r" % (image2_2,))
-        check_images(images, "images", 5)
-        if tuple(images.shape[:2]) != (b, 2):
-            raise ValueError("images: expected shape (%d, 2, h, w, 3), got %s" % (b, tuple(images.shape)))
-        h, w = images.shape[2], images.shape[3]
-        if outputs is None:
-            outputs = self.own_outputs()
-        ptr = lambda k: outputs[k].data_ptr() if outputs.get(k) is not None else None
-        _lib.check(_lib.load().demon_pipeline_forward_images_u8(
-            self.net.ptr, images.data_ptr(), images.stride(0), images.stride(1), images.stride(2), h, w, code,
-            1 if image2_2 == "resize" else 0, self.iterations,
-            ptr("predict_depth0"), ptr("predict_rotation"), ptr("predict_translation"),
-            ptr("predict_flow2"), ptr("predict_depth2"), ptr("predict_normal2"), _stream()))
-        return outputs
+        h, w, code, mode = self._check_pairs(images, resample, image2_2)
+        return self._run("demon_pipeline_forward_images_u8", (images.data_ptr(), *images.stride()[:3], h, w, code, mode), outputs)
 
     def forward_views(self, images, intrinsics, resample="bicubic", image2_2="resize", outputs=None):
         """The pipeline on photos from any calibrated camera: images CUDA uint8 [B,2,h,w,3] as in forward_images, intrinsics
@@ -393,15 +391,9 @@ class DemonPipeline:
         intrinsics are copied into a buffer of the pipeline, so the call replays one CUDA graph for new values.  Returns the
         outputs of forward_u8 on the adapted bytes, bit for bit, plus 'status' CUDA uint8 [B,2] (adjust_intrinsics' status;
         host intrinsics are checked here instead: ValueError)."""
-        from .images import _check_adjust_source, _device_intrinsics, check_images, demon_intrinsics, intrinsics4, resample_code
+        from .images import _check_adjust_source, _device_intrinsics, demon_intrinsics, intrinsics4
         b = self.batch_size
-        code = resample_code(resample)
-        if image2_2 not in ("resize", "median"):
-            raise ValueError("image2_2 must be 'resize' or 'median', got %r" % (image2_2,))
-        check_images(images, "images", 5)
-        if tuple(images.shape[:2]) != (b, 2):
-            raise ValueError("images: expected shape (%d, 2, h, w, 3), got %s" % (b, tuple(images.shape)))
-        h, w = images.shape[2], images.shape[3]
+        h, w, code, mode = self._check_pairs(images, resample, image2_2)
         _check_adjust_source(h, w, "images")
         k = _device_intrinsics(intrinsics, (b, 2), "intrinsics", w, h, intrinsics4(demon_intrinsics(), (), "K_new"), 256, 192,
                                images.device)
@@ -409,49 +401,31 @@ class DemonPipeline:
             self._K = torch.empty((b, 2, 4), dtype=torch.float64, device=images.device)
             self._status = torch.empty((b, 2), dtype=torch.uint8, device=images.device)
         self._K.copy_(k, non_blocking=True)
-        if outputs is None:
-            outputs = self.own_outputs()
-        ptr = lambda k: outputs[k].data_ptr() if outputs.get(k) is not None else None
-        _lib.check(_lib.load().demon_pipeline_forward_views_u8(
-            self.net.ptr, images.data_ptr(), images.stride(0), images.stride(1), images.stride(2), h, w, self._K.data_ptr(),
-            self._status.data_ptr(), code, 1 if image2_2 == "resize" else 0, self.iterations,
-            ptr("predict_depth0"), ptr("predict_rotation"), ptr("predict_translation"),
-            ptr("predict_flow2"), ptr("predict_depth2"), ptr("predict_normal2"), _stream()))
-        return dict(outputs, status=self._status)
+        out = self._run("demon_pipeline_forward_views_u8",
+                        (images.data_ptr(), *images.stride()[:3], h, w, self._K.data_ptr(), self._status.data_ptr(), code, mode), outputs)
+        return dict(out, status=self._status)
 
     def forward_host_u8(self, images, image2_2, depth0, rotation, translation, stream=None, sync=True):
         """End to end from HOST uint8 images [B,2,192,256,3] (numpy or pinned torch CPU uint8): H2D of the bytes, the
         pipeline, D2H of depth0 / rotation / translation.  sync=False: asynchronous on `stream` like forward_host_async."""
-        def hp(x):
-            if x is None:
-                return None
-            return x.data_ptr() if isinstance(x, torch.Tensor) else x.ctypes.data
         s = ctypes.c_void_p((stream or torch.cuda.current_stream()).cuda_stream)
         fn = _lib.load().demon_pipeline_forward_host_u8 if sync else _lib.load().demon_pipeline_forward_host_u8_async
-        _lib.check(fn(self.net.ptr, hp(images), hp(image2_2), self.iterations, hp(depth0), hp(rotation), hp(translation), s))
+        _lib.check(fn(self.net.ptr, _ptr(images), _ptr(image2_2), self.iterations, _ptr(depth0), _ptr(rotation), _ptr(translation), s))
 
     def forward_host(self, image_pair, image2_2, depth0, rotation, translation):
         """End-to-end call on HOST buffers (pinned torch CPU tensors or numpy arrays): H2D, pipeline, D2H and a
         stream synchronise inside the C call."""
-        def hp(x):
-            if x is None:
-                return None
-            return x.data_ptr() if isinstance(x, torch.Tensor) else x.ctypes.data
         _lib.check(_lib.load().demon_pipeline_forward_host(
-            self.net.ptr, hp(image_pair), hp(image2_2), self.iterations, hp(depth0), hp(rotation), hp(translation), _stream()))
+            self.net.ptr, _ptr(image_pair), _ptr(image2_2), self.iterations, _ptr(depth0), _ptr(rotation), _ptr(translation), _stream()))
         # (the C call synchronises and returns DEMON_E_STATE itself if a tensor-core pipeline wait timed out)
 
     def forward_host_async(self, image_pair, image2_2, depth0, rotation, translation, stream=None):
         """forward_host without the final synchronisation, on `stream` (a torch.cuda.Stream; default: current).  The host
         buffers must be pinned and are valid after `stream.synchronize()`.  Two DemonPipeline objects on two Sessions'
         nets and two streams overlap one batch's copies with the other's compute."""
-        def hp(x):
-            if x is None:
-                return None
-            return x.data_ptr() if isinstance(x, torch.Tensor) else x.ctypes.data
         s = ctypes.c_void_p((stream or torch.cuda.current_stream()).cuda_stream)
         _lib.check(_lib.load().demon_pipeline_forward_host_async(
-            self.net.ptr, hp(image_pair), hp(image2_2), self.iterations, hp(depth0), hp(rotation), hp(translation), s))
+            self.net.ptr, _ptr(image_pair), _ptr(image2_2), self.iterations, _ptr(depth0), _ptr(rotation), _ptr(translation), s))
 
     def launches(self):
         return _lib.load().demon_net_pipeline_launches(self.net.ptr, self.iterations)
