@@ -86,6 +86,7 @@ PROTOTYPES = {
     "demon_debug_describe_conv": [c_int] * 13 + [_P, c_int],
     "demon_debug_last_conv_ms": [],
     "demon_debug_tc_timing": [c_int, _P, c_int],
+    "demon_conv_slice_nhwc": [_P, c_int, _P] + [c_int] * 11 + [_P, _P, c_int, c_int, _P],
     "demon_conv2d_nhwc": [_P, _P] + [c_int] * 9 + [_P, _P, c_int, c_int, _P],
     "demon_deconv4x4s2_nhwc": [_P, _P] + [c_int] * 5 + [_P, _P, c_int, c_int, _P],
     "demon_last_error": [],

@@ -702,9 +702,12 @@ int tc_describe(const ConvProblem* probs, int nclass, int precision, char* buf, 
   HaloPlan plan;
   if (!tc_plan(probs, nclass, nsplit_of(precision), plan)) return 0;
   const HaloParams& q = plan.prm;
-  int n = snprintf(buf, buflen, "halo %s mode %d n_tile %d x%d steps %d x %d chunks sa %d a_stage %d w_slot %d smem %d tiles %d ksplit %d wres %d |",
+  // per-tap mode: a pixel tile is tb images x th rows x tw columns (halo mode: 1 x 16 x 8)
+  int n = snprintf(buf, buflen,
+                   "halo %s mode %d n_tile %d x%d steps %d x %d chunks sa %d a_stage %d w_slot %d smem %d tiles %d ksplit %d wres %d tb %d th %d tw %d |",
                    q.per_tap ? "per-tap" : (q.cin8 ? "cin8" : "halo"), q.mode, q.n_tile, q.n_tiles, q.nsteps, q.k_chunks, q.sa,
-                   q.a_region_bytes, q.w_stage_bytes, plan.smem_bytes, q.total_tiles, q.ksplit, q.w_resident);
+                   q.a_region_bytes, q.w_stage_bytes, plan.smem_bytes, q.total_tiles, q.ksplit, q.w_resident, q.per_tap ? q.tb : 1,
+                   q.per_tap ? q.th : kTileH, q.per_tap ? q.tw : kTileW);
   for (int t = 0; t < q.nsteps && n < buflen - 32; ++t)
     n += snprintf(buf + n, buflen - n, " [c%x w%d+%d]", q.st_cmask[t], q.st_woff[t], q.st_wbytes[t]);
   return n;

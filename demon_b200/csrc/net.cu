@@ -1291,14 +1291,19 @@ int demon_pipeline_forward_host_u8_async(demon_net* n, const uint8_t* images_hos
   return pipeline_host(n, images_host, image2_2_host, true, iterations, depth0_host, rotation_host, translation_host, stream, false);
 }
 
-// debug: which kernel family / plan every layer of the net got (one line per layer)
+// debug: the geometry of every layer of the net and which kernel family / plan it got (one line per layer)
 int demon_debug_describe_layers(const demon_net* n, char* buf, int buflen) {
   DEMON_REQUIRE(n && buf && buflen > 0, "describe: null");
+  static const char* const kKind[] = {"conv", "deconv", "dense"};
   int off = 0;
   for (auto& lp : n->layers) {
-    if (off >= buflen - 256) break;
-    off += snprintf(buf + off, buflen - off, "%-40s ", lp->name.c_str());
-    off += describe_layer(*lp, n->B, n->precision, buf + off, buflen - off);
+    if (off >= buflen - 512) break;
+    const Layer& l = *lp;
+    off += snprintf(buf + off, buflen - off,
+                    "%-40s %s H %d W %d cin %d cin_buf %d in_pitch %d in_off %d cout %d out_pitch %d out_off %d kh %d kw %d sy %d sx %d leaky %d scale %d : ",
+                    l.name.c_str(), kKind[l.kind], l.in->H, l.in->W, l.cin, l.cin_buf, l.in->C, l.in_coff, l.cout, l.out->C, l.out_coff,
+                    l.kh, l.kw, l.sy, l.sx, l.leaky ? 1 : 0, l.scale ? 1 : 0);
+    off += describe_layer(l, n->B, n->precision, buf + off, buflen - off);
     off += snprintf(buf + off, buflen - off, "\n");
   }
   return off;
@@ -1316,12 +1321,16 @@ int demon_debug_describe_conv(int B, int H, int W, int Cin, int in_pitch, int Co
 static double g_last_conv_ms = -1.0;
 double demon_debug_last_conv_ms(void) { return g_last_conv_ms; }
 
-static int standalone_conv(const float* in, float* out, int B, int H, int W, int Cin, int Cout, int kh, int kw, int sy, int sx,
-                           const float* kernel_host, const float* bias_host, int leaky, int precision, bool deconv, void* stream) {
+static int standalone_conv(const float* in, int in_pitch, float* out, int out_pitch, int B, int H, int W, int Cin, int Cout, int kh, int kw,
+                           int sy, int sx, const float* kernel_host, const float* bias_host, int leaky, int precision, bool deconv, void* stream) {
   DEMON_REQUIRE(in && out && kernel_host && bias_host, "conv: null pointer");
   DEMON_REQUIRE(Cin % 4 == 0, "conv test entry: Cin must be a multiple of 4");
+  DEMON_REQUIRE(B >= 1 && H >= 1 && W >= 1 && Cout >= 1 && in_pitch >= Cin && out_pitch >= Cout, "conv test entry: shape or pitch");
+  if (deconv) DEMON_REQUIRE(kh == 4 && kw == 4 && sy == 2 && sx == 2, "deconv: only k4 s2");
+  else DEMON_REQUIRE(kh >= 1 && kw >= 1 && kh * kw <= kMaxTaps && (kh & 1) && (kw & 1), "conv: kernel %dx%d", kh, kw);
+  DEMON_REQUIRE(sy >= 1 && sx >= 1, "conv: stride");
   std::vector<void*> allocs;
-  StandaloneLayer s(in, out, H, W, Cin, Cin, Cout, Cout, kh, kw, sy, sx, deconv, leaky != 0);
+  StandaloneLayer s(in, out, H, W, Cin, in_pitch, Cout, out_pitch, kh, kw, sy, sx, deconv, leaky != 0);
   Layer& l = s.layer;
   int rc = upload_layer(l, kernel_host, bias_host, B, precision, allocs);
   if (rc == DEMON_OK && precision != DEMON_PREC_FP32_SIMT && !l.use_tc())
@@ -1355,16 +1364,20 @@ static int standalone_conv(const float* in, float* out, int B, int H, int W, int
   return DEMON_OK;
 }
 
+int demon_conv_slice_nhwc(const float* in, int in_pitch, float* out, int out_pitch, int B, int H, int W, int Cin, int Cout, int kh, int kw,
+                          int sy, int sx, int deconv, const float* kernel_host, const float* bias_host, int leaky, int precision, void* stream) {
+  return standalone_conv(in, in_pitch, out, out_pitch, B, H, W, Cin, Cout, kh, kw, sy, sx, kernel_host, bias_host, leaky, precision,
+                         deconv != 0, stream);
+}
+
 int demon_conv2d_nhwc(const float* in, float* out, int B, int H, int W, int Cin, int Cout, int kh, int kw, int sy, int sx,
                       const float* kernel_host, const float* bias_host, int leaky, int precision, void* stream) {
-  DEMON_REQUIRE(kh >= 1 && kw >= 1 && kh * kw <= kMaxTaps && (kh & 1) && (kw & 1), "conv: kernel %dx%d", kh, kw);
-  DEMON_REQUIRE(sy >= 1 && sx >= 1, "conv: stride");
-  return standalone_conv(in, out, B, H, W, Cin, Cout, kh, kw, sy, sx, kernel_host, bias_host, leaky, precision, false, stream);
+  return demon_conv_slice_nhwc(in, Cin, out, Cout, B, H, W, Cin, Cout, kh, kw, sy, sx, 0, kernel_host, bias_host, leaky, precision, stream);
 }
 
 int demon_deconv4x4s2_nhwc(const float* in, float* out, int B, int H, int W, int Cin, int Cout, const float* kernel_host,
                            const float* bias_host, int leaky, int precision, void* stream) {
-  return standalone_conv(in, out, B, H, W, Cin, Cout, 4, 4, 2, 2, kernel_host, bias_host, leaky, precision, true, stream);
+  return demon_conv_slice_nhwc(in, Cin, out, Cout, B, H, W, Cin, Cout, 4, 4, 2, 2, 1, kernel_host, bias_host, leaky, precision, stream);
 }
 
 }  // extern "C"

@@ -371,17 +371,32 @@ int demon_check_errors(void);
  * counters of the last launch to host_out. */
 int demon_debug_tc_timing(int enable, int64_t* host_out, int nblocks);
 
-/* debug: one text line per layer with the kernel family and tiling plan it gets (works without a device as long as the
- * net was created -- creation needs one; see tools/describe_plan.py for the offline variant). Returns bytes written. */
+/* debug: one text line per layer: its name, then its geometry as fixed key-value pairs
+ *     <kind> H <h> W <w> cin <c> cin_buf <c> in_pitch <p> in_off <o> cout <c> out_pitch <p> out_off <o> kh <k> kw <k> sy <s> sx <s> leaky <0|1>
+ *     scale <0|1> :
+ * (kind conv / deconv / dense; H, W of the input; cin_buf = channels read, the ones past cin carry zero weights; scale 1:
+ * channel 0 of the output is multiplied by a per-image scale), then the
+ * kernel family and tiling plan it gets (works without a device as long as the net was created -- creation needs one;
+ * see tools/describe_plan.py for the offline variant). Returns bytes written. */
 int demon_debug_describe_layers(const demon_net* net, char* buf, int buflen);
 
 /* debug, no device needed: the kernel family and tiling plan one convolution shape would get */
 int demon_debug_describe_conv(int B, int H, int W, int Cin, int in_pitch, int Cout, int out_pitch, int kh, int kw, int sy, int sx,
                               int deconv, int precision, char* buf, int buflen);
 
-/* debug: device time (CUDA events on the launching stream) of the kernel launches of the last demon_conv2d_nhwc /
- * demon_deconv4x4s2_nhwc call, in milliseconds (weight packing and uploads excluded); < 0 if none was timed */
+/* debug: device time (CUDA events on the launching stream) of the kernel launches of the last standalone convolution
+ * call (demon_conv_slice_nhwc and the two entries below), in milliseconds (weight packing and uploads excluded); < 0 if
+ * none was timed */
 double demon_debug_last_conv_ms(void);
+
+/* Standalone convolution on channel SLICES, the way the network's layers read and write their concat buffers: `in`
+ * points at the first channel of a [B,H,W,*] slice of channel pitch in_pitch, `out` at the first channel of an output
+ * slice of pitch out_pitch; only those Cin input and Cout output channels are read or written.  Kernel TF layout
+ * [kh,kw,cin,cout] (host), or with `deconv` the k4 s2 transposed convolution (kh = kw = 4, sy = sx = 2) with kernel
+ * [4,4,cout,cin].  At a tensor-core precision a shape the tensor-core path gets no plan for is refused (DEMON_E_INVALID). */
+int demon_conv_slice_nhwc(const float* in, int in_pitch, float* out, int out_pitch, int B, int H, int W, int Cin, int Cout,
+                          int kh, int kw, int sy, int sx, int deconv, const float* kernel_host, const float* bias_host,
+                          int leaky, int precision, void* stream);
 
 /* Standalone convolution entry used by tests to compare the tensor-core path with the fp32 SIMT path on
  * the same NHWC tensors.  in [B,H,W,Cin], kernel TF layout [kh,kw,cin,cout] (host), bias [cout] (host)
