@@ -83,6 +83,7 @@ PROTOTYPES = {
     "demon_debug_tc_timeouts": [],
     "demon_check_errors": [],
     "demon_debug_describe_layers": [_P, _P, c_int],
+    "demon_debug_trace_layers": [_P, _P, _P],
     "demon_debug_describe_conv": [c_int] * 13 + [_P, c_int],
     "demon_debug_last_conv_ms": [],
     "demon_debug_tc_timing": [c_int, _P, c_int],

@@ -128,6 +128,9 @@ struct demon_net {
   size_t prof_used = 0;
   std::vector<double> prof_ms;               // accumulated per layer
   std::vector<int64_t> prof_calls;
+  // optional per-layer copies of every layer's input and output slice (demon_debug_trace_layers); one per layer, null skips
+  bool tracing = false;
+  std::vector<float*> trace_in, trace_out;
 
   // named buffers
   float* tc_scratch = nullptr;   // partial sums of the split-K tensor-core layers (conv_tc_halo.cu), sized at finalize
@@ -479,7 +482,7 @@ int upload_layer(Layer& l, const float* k, const float* bias_host, int B, int pr
 
 // The plan line of a layer: the tensor-core planner's, or "simt" for a layer it does not take.
 int describe_layer(const Layer& l, int B, int precision, char* buf, int buflen) {
-  if (l.kind == L_DENSE) return snprintf(buf, buflen, "dense simt");
+  if (l.kind == L_DENSE) return snprintf(buf, buflen, "dense simt ksplit %d", l.ksplit);
   ConvProblem probs[4];
   const int nclass = build_problems(l, B, probs);
   const int len = (precision != DEMON_PREC_FP32_SIMT) ? tc_describe(probs, nclass, precision, buf, buflen) : 0;
@@ -505,7 +508,7 @@ struct StandaloneLayer {
 };
 
 // `dst`: see build_problems
-int run_layer_profiled(demon_net* n, int idx, cudaStream_t stream, float* dst = nullptr) {
+int run_layer_timed(demon_net* n, int idx, cudaStream_t stream, float* dst) {
   const Layer& l = *n->layers[idx];
   static const bool sync_layers = getenv("DEMON_SYNC_LAYERS") && atoi(getenv("DEMON_SYNC_LAYERS")) != 0;   // debugging aid
   if (sync_layers) {
@@ -525,6 +528,29 @@ int run_layer_profiled(demon_net* n, int idx, cudaStream_t stream, float* dst = 
   DEMON_CHECK_CUDA(cudaEventRecord(n->prof_events[n->prof_used + 1], stream));
   n->prof_layer.push_back(idx);
   n->prof_used += 2;
+  return rc;
+}
+
+// A dense copy of layer l's input slice (cin_buf channels) or output slice (cout channels) to `to`: float32 [B,H,W,C], or
+// [B,C] for a dense layer, which reads rows of cin_buf floats (build_problems) and writes one pixel per image.
+int trace_copy(const demon_net* n, const Layer& l, bool input, float* dst, float* to, cudaStream_t stream) {
+  const Buf* b = input ? l.in : l.out;
+  const float* src = input ? l.in->p + l.in_coff : (dst ? dst : l.out->p) + l.out_coff;
+  const size_t width = (input ? l.cin_buf : l.cout) * sizeof(float);
+  const size_t pitch = (input && l.kind == L_DENSE ? l.cin_buf : b->C) * sizeof(float);
+  const size_t rows = (size_t)n->B * (l.kind == L_DENSE ? 1 : b->H * b->W);
+  DEMON_CHECK_CUDA(cudaMemcpy2DAsync(to, width, src, pitch, width, rows, cudaMemcpyDeviceToDevice, stream));
+  return DEMON_OK;
+}
+
+// `dst`: see build_problems.  With a trace set (demon_debug_trace_layers), the layer's input slice is copied out before it
+// runs and its output slice after.
+int run_layer_profiled(demon_net* n, int idx, cudaStream_t stream, float* dst = nullptr) {
+  if (!n->tracing) return run_layer_timed(n, idx, stream, dst);
+  const Layer& l = *n->layers[idx];
+  int rc = n->trace_in[idx] ? trace_copy(n, l, true, dst, n->trace_in[idx], stream) : DEMON_OK;
+  if (rc == DEMON_OK) rc = run_layer_timed(n, idx, stream, dst);
+  if (rc == DEMON_OK && n->trace_out[idx]) rc = trace_copy(n, l, false, dst, n->trace_out[idx], stream);
   return rc;
 }
 
@@ -1121,7 +1147,14 @@ static int pipeline_body(demon_net* n, const PipelineCall& c, cudaStream_t s) {
   return DEMON_OK;
 }
 
+// The fused pipeline is not traced: a graph captured with the trace's copies inside would replay them after it is cleared
+static int refuse_while_tracing(const demon_net* n) {
+  if (n->tracing) return fail(DEMON_E_STATE, "pipeline: a layer trace is set (demon_debug_trace_layers); only the stage-wise entries are traced");
+  return DEMON_OK;
+}
+
 static int pipeline_forward_impl(demon_net* n, const PipelineCall& c, void* stream) {
+  if (int rc = refuse_while_tracing(n)) return rc;
   DEMON_REQUIRE(c.iterations >= 0 && c.iterations <= 7, "pipeline: iterations %d", (int)c.iterations);
   int* launch_record = c.snapshots != NO_SNAPSHOTS ? n->snapshot_launches : n->pipeline_launches;
   DEMON_REQUIRE(n->RH == 192 && n->RW == 256, "pipeline: net was created with a %dx%d refinement block", n->RH, n->RW);
@@ -1240,6 +1273,7 @@ int demon_pipeline_forward_views_u8(demon_net* n, const uint8_t* images, int64_t
 static int pipeline_host(demon_net* n, const void* images_host, const void* image2_2_host, bool u8, int iterations, float* depth0_host,
                          float* rotation_host, float* translation_host, void* stream, bool sync) {
   REQUIRE_READY(n);
+  if (int rc = refuse_while_tracing(n)) return rc;
   DEMON_REQUIRE(images_host && depth0_host, "pipeline_host: null pointer");
   cudaStream_t s = (cudaStream_t)stream;
   const size_t px = (size_t)n->B * 192 * 256;
@@ -1307,6 +1341,18 @@ int demon_debug_describe_layers(const demon_net* n, char* buf, int buflen) {
     off += snprintf(buf + off, buflen - off, "\n");
   }
   return off;
+}
+
+// debug: per-layer input / output copies of the stage-wise entries (run_layer_profiled)
+int demon_debug_trace_layers(demon_net* n, float* const* in, float* const* out) {
+  DEMON_REQUIRE(n, "trace: null net");
+  const size_t L = n->layers.size();
+  n->trace_in.assign(L, nullptr);
+  n->trace_out.assign(L, nullptr);
+  if (in) std::copy(in, in + L, n->trace_in.begin());
+  if (out) std::copy(out, out + L, n->trace_out.begin());
+  n->tracing = in || out;
+  return DEMON_OK;
 }
 
 // debug, no device needed: the plan of one convolution shape ([B,H,W,Cin] NHWC, channel pitches given)

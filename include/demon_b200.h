@@ -380,6 +380,16 @@ int demon_debug_tc_timing(int enable, int64_t* host_out, int nblocks);
  * see tools/describe_plan.py for the offline variant). Returns bytes written. */
 int demon_debug_describe_layers(const demon_net* net, char* buf, int buflen);
 
+/* debug, a test entry like demon_conv_slice_nhwc: while set, the stage-wise entries (demon_bootstrap_forward,
+ * demon_iterative_forward, demon_refine_forward) copy every layer's input slice (cin_buf channels, just before the layer
+ * runs) to in[i] and its output slice (cout channels, just after) to out[i], as dense float32 [B,H,W,C] (dense layers:
+ * [B,cin_buf] in the buffer's NHWC order and [B,cout]), on the launching stream; a null pointer skips that copy.  The last
+ * refinement layer's output is read from the caller's depth0.  `in` and `out` are arrays of demon_net_num_layers(net)
+ * device pointers in layer order (demon_net_layer_name); in == out == NULL clears the trace.  While a trace is set, every
+ * demon_pipeline_forward* entry returns DEMON_E_STATE, so that no CUDA graph is captured with the copies inside it.
+ * Without a trace the forward passes are unchanged. */
+int demon_debug_trace_layers(demon_net* net, float* const* in, float* const* out);
+
 /* debug, no device needed: the kernel family and tiling plan one convolution shape would get */
 int demon_debug_describe_conv(int B, int H, int W, int Cin, int in_pitch, int Cout, int out_pitch, int kh, int kw, int sy, int sx,
                               int deconv, int precision, char* buf, int buflen);

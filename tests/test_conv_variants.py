@@ -116,6 +116,26 @@ def describe(row, precision):
                 tiles=int(tiles), ksplit=int(ksplit), wres=int(wres), tb=int(tb), th=int(th), tw=int(tw), widths=widths, text=text)
 
 
+def tc_error_bound(precision, Cin, kh, kw, deconv, ksplit):
+    """The coefficient of the tensor-core convolution's per-element error bound |err| <= bound * S, S = sum |x||w| + |b| over
+    the terms of an output element; Cin is the channel count the kernel reads (a layer's cin_buf), ksplit the plan's.  With
+    n8 = the number of K = 8 wgmma slices summed into an output element:
+
+    * 3xTF32: A_hi = trunc(A) and A_lo = A - A_hi (exact), |A_lo| < 2^-10 |A|, and the tensor cores truncate A_lo to TF32:
+      2^-20 |A|.  W_hi = rne(W), |W_lo| <= 2^-11 |W|, truncated to TF32: 2^-21 |W|.  The dropped A_lo W_lo: 2^-21 |A W|.  The
+      split costs at most 2^-19 S.  Every one of the 3 n8 wgmma rounds twice (its internal sum and the accumulator add), at
+      most one float32 ulp of a partial sum <= S each, 2^-23 S; split-K adds ksplit sums, the epilogue the bias add and the
+      leaky ReLU's product: 2 more.  |err| <= (2^-19 + (2 * 3 n8 + ksplit + 2) 2^-23) S.
+    * TF32: both operands truncated to TF32, 2^-10 relative each: 2^-9 S, and n8 wgmma: |err| <= (2^-9 + (2 n8 + ksplit + 2) 2^-23) S.
+
+    The split terms follow from the operand formats alone.  The accumulation terms do not: NVIDIA does not document how a
+    wgmma rounds its internal sum, and "at most one float32 ulp of S per wgmma" is an assumption about Hopper's tensor
+    cores that rests on measurement (tests/test_gpu_conv_variants.py: test_variant_realistic)."""
+    n8 = (4 * Cin // 8) if deconv else ((-(-kh * kw // 4)) * 4 if Cin == 8 else kh * kw * Cin // 8)
+    split, mult = (2.0 ** -19, 3) if precision == X3TF32 else (2.0 ** -9, 1)
+    return split + (2 * mult * n8 + ksplit + 2) * 2.0 ** -23
+
+
 SMS = 132    # the launch grid is min(work items, SMs): an H100 SXM's 132 (a GPU with fewer SMs gives each CTA more work)
 W_RING = 4   # weight ring slots of the kernel (kRing)
 

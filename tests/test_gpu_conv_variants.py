@@ -17,7 +17,8 @@ import torch
 import torch.nn.functional as F
 
 from demon_b200 import _lib
-from test_conv_variants import DATASETS, FP32, TF32, TC_PRECISIONS, VARIANTS, X3TF32, describe, exact_data, geometry, pitches
+from test_conv_variants import (DATASETS, FP32, TF32, TC_PRECISIONS, VARIANTS, X3TF32, describe, exact_data, geometry, pitches,
+                                tc_error_bound)
 
 pytestmark = pytest.mark.gpu
 
@@ -139,19 +140,12 @@ def log_uniform(shape, rng):
 @pytest.mark.parametrize("precision", TC_PRECISIONS, ids=["3xtf32", "tf32"])
 @pytest.mark.parametrize("row", VARIANTS, ids=[row_id(r) for r in VARIANTS])
 def test_variant_realistic(row, precision):
-    """Random signs, magnitudes log-uniform in 2^-8 .. 2^8 (x, w and bias).  With S = sum |x||w| + |b| over the terms of an
-    output element and n8 = the number of K = 8 wgmma slices summed into it:
+    """Random signs, magnitudes log-uniform in 2^-8 .. 2^8 (x, w and bias), under the per-element bound |err| <= bound * S of
+    tests/test_conv_variants.py: tc_error_bound (S = sum |x||w| + |b| over the terms of an output element).
 
-    * 3xTF32: A_hi = trunc(A) and A_lo = A - A_hi (exact), |A_lo| < 2^-10 |A|, and the tensor cores truncate A_lo to TF32:
-      2^-20 |A|.  W_hi = rne(W), |W_lo| <= 2^-11 |W|, truncated to TF32: 2^-21 |W|.  The dropped A_lo W_lo: 2^-21 |A W|.  The
-      split costs at most 2^-19 S.  Every one of the 3 n8 wgmma rounds twice (its internal sum and the accumulator add), at
-      most one float32 ulp of a partial sum <= S each, 2^-23 S; split-K adds ksplit sums, the epilogue the bias add and the
-      leaky ReLU's product: 2 more.  |err| <= (2^-19 + (2 * 3 n8 + ksplit + 2) 2^-23) S.
-    * TF32: both operands truncated to TF32, 2^-10 relative each: 2^-9 S, and n8 wgmma: |err| <= (2^-9 + (2 n8 + ksplit + 2) 2^-23) S.
-
-    The split terms follow from the operand formats alone.  The accumulation terms do not: NVIDIA does not document how a
-    wgmma rounds its internal sum, and "at most one float32 ulp of S per wgmma" is an assumption about Hopper's tensor
-    cores that rests on measurement, not on a derivation.  On an H100 (seeds as below) the largest |err| / S was 4.7e-6
+    The split terms of that bound follow from the operand formats alone.  The accumulation terms do not: NVIDIA does not
+    document how a wgmma rounds its internal sum, and "at most one float32 ulp of S per wgmma" is an assumption about Hopper's
+    tensor cores that rests on measurement, not on a derivation.  On an H100 (seeds as below) the largest |err| / S was 4.7e-6
     for 3xTF32, under a tenth of its bound, where the accumulation terms dominate; and 1.8e-3 for TF32, 0.91 of its bound, where
     the operand truncation (a hard bound: a product of two truncated operands is never off by 2^-9 of itself) dominates.
     """
@@ -170,9 +164,7 @@ def test_variant_realistic(row, precision):
         y = torch.maximum(float(np.float32(0.1)) * y, y)
     got = run_slice(xd, in_off, in_pitch, k, b, Cout, out_off, out_pitch, geom, deconv, leaky, precision).double()
     d = describe(row, precision)
-    n8 = (4 * Cin // 8) if deconv else ((-(-kh * kw // 4)) * 4 if Cin == 8 else kh * kw * Cin // 8)
-    split, mult = (2.0 ** -19, 3) if precision == X3TF32 else (2.0 ** -9, 1)
-    bound = split + (2 * mult * n8 + d["ksplit"] + 2) * 2.0 ** -23
+    bound = tc_error_bound(precision, Cin, kh, kw, deconv, d["ksplit"])
     ratio = ((got - y).abs() / S).max().item()
     if ratio > WORST.get(precision, (-1,))[0]:
         WORST[precision] = (ratio, ratio / bound, row)
@@ -197,11 +189,17 @@ def net_layers(batch, refine_hw, precision):
     ptr = ctypes.c_void_p()
     _lib.check(lib.demon_net_create(ctypes.byref(ptr), batch, refine_hw[0], refine_hw[1], precision))
     try:
-        n = lib.demon_net_num_layers(ptr)
-        buf = ctypes.create_string_buffer(1 << 20)
-        lib.demon_debug_describe_layers(ptr, buf, 1 << 20)
+        return describe_layers(ptr)
     finally:
         lib.demon_net_destroy(ptr)
+
+
+def describe_layers(ptr):
+    """net_layers of the net `ptr` (a demon_net*)."""
+    lib = _lib.load()
+    n = lib.demon_net_num_layers(ptr)
+    buf = ctypes.create_string_buffer(1 << 20)
+    lib.demon_debug_describe_layers(ptr, buf, 1 << 20)
     lines = buf.value.decode().splitlines()
     assert len(lines) == n
     out = []

@@ -1,7 +1,9 @@
 """CPU: pins the torch calls of oracle/network.py against naive numpy loops written from TensorFlow's
 documented definitions of the layers the reference graph uses, checks the variable table against the
-numbers in SURVEY.md / BASELINE.md, and replays the committed golden outputs (BASELINE.json configs[0])."""
+numbers in SURVEY.md / BASELINE.md, replays the committed golden outputs (BASELINE.json configs[0]), and checks that
+forcing the oracle's layer outputs (the hook tests/test_gpu_layer_trace.py uses) changes nothing else."""
 import os
+import re
 
 import numpy as np
 import pytest
@@ -125,3 +127,58 @@ def test_golden_pipeline_fp32_vs_fp64(golden_dir):
     assert np.abs(d32 - d64).sum() / np.abs(d64).sum() < 1e-6
     f32, f64 = g["predict_flow2_f32"], g["predict_flow2_f64"]
     assert np.sqrt(((f32 - f64) ** 2).sum(1)).mean() < 1e-6
+
+
+# stride of the strided layers (helpers.py:105-153 / blocks_original.py:459-465): conv1..conv5 of the trunks split into a y
+# and an x conv, netRefine's conv1 and conv2; every other layer has stride 1
+_STRIDED = re.compile(r"net\w+/conv[1-5]([yx]?)")
+_LINEAR = ("predict_flow5/conv2", "predict_flow2/conv2", "predict_depthnormal2/conv2", "predict_depth0/conv2",
+           "upsample_flow5to4/upconv", "motion_fc3")   # the layers without a leaky ReLU
+
+
+def own_layer_outputs(W_, record):
+    """A `force` for the oracle that computes every layer itself, with the oracle's own arithmetic, and records its name.
+    The scaled depth channel of predict_depthnormal2/conv2 is scale * conv, with the scale of the same block's motion_fc3."""
+    scales = {}
+
+    def force(name, x):
+        assert name not in record, "layer %s forced twice" % name
+        record.append(name)
+        act = not name.endswith(_LINEAR)
+        if name.endswith("upconv"):
+            y = onet._upconv(W_, name, x)
+            return onet.my_leaky_relu(y) if act else y
+        if name.split("/")[-1].startswith("motion_fc"):
+            y = onet.dense(W_, name, x, act)
+            if name.endswith("motion_fc3"):
+                scales[name.split("/")[0]] = y[:, 6:7]
+            return y
+        m = _STRIDED.fullmatch(name)
+        stride = 1 if not m else {"y": (2, 1), "x": (1, 2), "": 2}[m.group(1)]
+        y = onet.conv2d_caffe_padding(W_, name, x, stride, activation=act)
+        if name.endswith("predict_depthnormal2/conv2"):
+            y = torch.cat((scales[name.split("/")[0]].reshape(-1, 1, 1, 1) * y[:, 0:1], y[:, 1:4]), dim=1)
+        return y
+    return force
+
+
+def test_forced_oracle_with_its_own_layer_outputs_is_the_oracle(sculpture, synthetic_weights):
+    """The oracle's `force` hook changes nothing but where each layer's output comes from: forced with its own fp32 layer
+    outputs, all three stages reproduce the unforced oracle bit for bit, and every one of the 121 layers is forced once."""
+    nets = onet.OracleNets(synthetic_weights)
+    ip, i22 = sculpture["image_pair"], sculpture["image2_2"]
+    record = []
+    force = own_layer_outputs(nets.W, record)
+    stages = []
+    r0 = nets.bootstrap(ip, i22, full=True)
+    stages.append((r0, nets.bootstrap(ip, i22, full=True, force=force)))
+    args = tuple(r0[k].numpy() for k in ("predict_depth2", "predict_normal2", "predict_rotation", "predict_translation"))
+    stages.append((nets.iterative(ip, i22, *args, full=True), nets.iterative(ip, i22, *args, full=True, force=force)))
+    image1 = np.ascontiguousarray(ip[:, 0:3])
+    stages.append((nets.refine(image1, r0["predict_depth2"]), nets.refine(image1, r0["predict_depth2"], force=force)))
+    for want, got in stages:
+        assert set(want) == set(got)
+        for k in want:
+            assert torch.equal(want[k], got[k]), k
+    layers = sorted({n.rsplit("/", 1)[0] for n in W.variable_specs()})
+    assert sorted(record) == layers
