@@ -70,6 +70,10 @@ PROTOTYPES = {
     "demon_pipeline_forward_images_u8": [_P, _P, c_int64, c_int64, c_int64] + [c_int] * 5 + [_P] * 6 + [_P],
     "demon_adjust_intrinsics_u8": [_P, c_int64, c_int64, c_int, c_int, c_int, _P] + [c_double] * 4 + [_P, c_int, c_int, _P, _P],
     "demon_pipeline_forward_views_u8": [_P, _P, c_int64, c_int64, c_int64, c_int, c_int, _P, _P] + [c_int] * 3 + [_P] * 6 + [_P],
+    "demon_sharpness_u8": [_P, c_int64, c_int64, c_int, c_int, c_int, _P, _P],
+    "demon_sun3d_depth_u16": [_P, c_int, c_int, c_int, _P, _P, _P],
+    "demon_depth_ratios_f32": [_P] * 5 + [c_int] * 3 + [_P, c_int, _P, _P],
+    "demon_depth_consistency_counts_f32": [_P] * 5 + [c_int] * 3 + [_P, c_int, c_float, c_float, _P, _P],
     "demon_net_batch": [_P],
     "demon_net_workspace_bytes": [_P],
     "demon_net_pipeline_launches": [_P, c_int],

@@ -1,9 +1,11 @@
 // Ground-truth preparation of the DeMoN evaluation (python/depthmotionnet/evaluation/evaluate_to_xarray.py:93-124) on the
 // device: the mask of the pixels of view 1 that are visible in view 2, compute_visible_points_mask
 // (dataset_tools/view_tools_cython.pyx:9-58).  The .pyx computes in float32 C arithmetic in a fixed order; the kernel does
-// the same operations in the same order with round-to-nearest intrinsics (no contraction into FMAs), so the mask equals
-// the compiled Cython bit for bit.  One thread per pixel, K1, R1^T and t1 of the sample in shared memory.
+// the same operations in the same order with round-to-nearest intrinsics (no contraction into FMAs; the projection is
+// view_projection.cuh's, shared with the depth ratios), so the mask equals the compiled Cython bit for bit.  One thread
+// per pixel, K1, R1^T and t1 of the sample in shared memory.
 #include "common.cuh"
+#include "view_projection.cuh"
 #include <cstdint>
 
 namespace demon {
@@ -35,26 +37,9 @@ __global__ void __launch_bounds__(256) visible_points_mask_kernel(const float* _
   float d = __ldg(depth + n * hw + i);
   if (kInverse) d = fdiv(1.0f, d);   // abs_depth = 1/depth (evaluate_to_xarray.py:110)
   uint8_t m = 0;
-  if (isfinite(d) && d > 0.0f) {
-    const float px = fadd((float)x, 0.5f), py = fadd((float)y, 0.5f);
-    float p0 = fdiv(fmul(d, fsub(px, K[2])), K[0]);
-    float p1 = fdiv(fmul(d, fsub(py, K[5])), K[4]);
-    float p2 = d;
-    p0 = fsub(p0, t[0]);
-    p1 = fsub(p1, t[1]);
-    p2 = fsub(p2, t[2]);
-    float q[3];
-#pragma unroll
-    for (int r = 0; r < 3; ++r) q[r] = fadd(fadd(fmul(RT[3 * r], p0), fmul(RT[3 * r + 1], p1)), fmul(RT[3 * r + 2], p2));
-    float pr[3];
-#pragma unroll
-    for (int r = 0; r < 3; ++r)
-      pr[r] = fadd(fadd(fadd(fmul(__ldg(P + 4 * r), q[0]), fmul(__ldg(P + 4 * r + 1), q[1])), fmul(__ldg(P + 4 * r + 2), q[2])),
-                   fmul(__ldg(P + 4 * r + 3), 1.0f));
-    if (pr[2] > 0.0f) {
-      const float u = fdiv(pr[0], pr[2]), v = fdiv(pr[1], pr[2]);
-      if (u > (float)borderx && v > (float)bordery && u < (float)(width2 - borderx) && v < (float)(height2 - bordery)) m = 1;
-    }
+  float u, v, z;
+  if (isfinite(d) && d > 0.0f && project_into_view2(d, x, y, K, RT, t, P, u, v, z)) {
+    if (u > (float)borderx && v > (float)bordery && u < (float)(width2 - borderx) && v < (float)(height2 - bordery)) m = 1;
   }
   mask[n * hw + i] = m;
 }

@@ -223,6 +223,29 @@ int demon_adjust_intrinsics_u8(const uint8_t* src, int64_t src_sn, int64_t src_s
                                void* stream);
 
 /* ------------------------------------------------------------------------
+ * Dataset tools (python/depthmotionnet/dataset_tools): selecting multi-view samples from RGB-D sequences.
+ * ---------------------------------------------------------------------- */
+/* measure_sharpness (helpers.py:23-31) of n RGB uint8 frames, bit for bit: out[i] = np.var(laplace(grey)) as float32, with
+ * grey Pillow's convert('L'), laplace scipy's (mode 'reflect') and the variance numpy's pairwise float32 sums.  images
+ * [n,h,w,3] with `stride_n` bytes between frames and `stride_y` between rows (pixel stride 3, channel stride 1).
+ * h*w < 2^24 (n must be exact in float32), n >= 0. */
+int demon_sharpness_u8(const uint8_t* images, int64_t stride_n, int64_t stride_y, int n, int h, int w, float* out, void* stream);
+/* sun3d_utils.read_depth (sun3d_utils.py:60-72) on n decoded depth PNGs, bit for bit: raw [n,h,w] uint16 ->
+ * depth [n,h,w] float32 = float32(double((d >> 3) | (d << 13) in uint16) / 1000), and valid_counts [n] int64 = the number of
+ * finite depths > 0 of each frame.  n up to 65535. */
+int demon_sun3d_depth_u16(const uint16_t* raw, int n, int h, int w, float* depth, int64_t* valid_counts, void* stream);
+/* compute_depth_ratios (view_tools_cython.pyx:107-191) of n_pairs ordered view pairs, bit for bit: depth [n_views,h,w]
+ * camera z; per view K [3,3], R [3,3], t [3] and P = K [R|t] [3,4] (float32, built as the .pyx wrapper builds them);
+ * pairs [n_pairs,2] int32 (i, j) -> ratios [n_pairs,h,w] = the ratio map of view i against view j.  Where the .pyx would
+ * read past depth j (a lookup at flat index y2*w + x2 >= h*w) the ratio is NaN.  h*w < 2^24. */
+int demon_depth_ratios_f32(const float* depth, const float* K, const float* R, const float* t, const float* P, int n_views, int h, int w,
+                           const int* pairs, int n_pairs, float* ratios, void* stream);
+/* the same without the maps: counts [n_pairs,2] int64 = (finite ratios, finite ratios r with lo < r < hi) of each pair,
+ * what check_depth_consistency (view_tools.py:62-94) needs from a map.  Exact integer counts, independent of scheduling. */
+int demon_depth_consistency_counts_f32(const float* depth, const float* K, const float* R, const float* t, const float* P, int n_views,
+                                       int h, int w, const int* pairs, int n_pairs, float lo, float hi, int64_t* counts, void* stream);
+
+/* ------------------------------------------------------------------------
  * Network graphs (python/depthmotionnet/networks_original.py).
  * One handle = the five blocks netFlow1, netDM1, netFlow2, netDM2, netRefine for a
  * fixed batch size at 256x192 (networks_original.py:38-42), plus a refinement block that
