@@ -59,6 +59,13 @@ PROTOTYPES = {
     "demon_bootstrap_forward": [_P] + [_P] * 8 + [c_int, _P],
     "demon_iterative_forward": [_P] + [_P] * 12 + [c_int, _P],
     "demon_refine_forward": [_P, _P, _P, _P, c_int, _P],
+    "demon_net_create_v2": [ctypes.POINTER(c_void_p), c_int, c_int, c_int, c_int],
+    "demon_net_variant": [_P],
+    "demon_bootstrap_forward_v2": [_P] + [_P] * 8 + [c_int, _P],
+    "demon_iterative_forward_v2": [_P] + [_P] * 12 + [c_int, _P],
+    "demon_refine_forward_v2": [_P] * 6 + [c_int, _P],
+    "demon_pipeline_forward_v2": [_P, _P, _P, c_int] + [_P] * 7 + [_P],
+    "demon_debug_describe_plan": [c_int] * 5 + [_P, c_int],
     "demon_pipeline_forward": [_P, _P, _P, c_int] + [_P] * 6 + [_P],
     "demon_pipeline_forward_snapshots": [_P, _P, _P, c_int] + [_P] * 6 + [_P],
     "demon_pipeline_forward_host": [_P, _P, _P, c_int, _P, _P, _P, _P],
@@ -92,6 +99,7 @@ PROTOTYPES = {
     "demon_debug_last_conv_ms": [],
     "demon_debug_tc_timing": [c_int, _P, c_int],
     "demon_conv_slice_nhwc": [_P, c_int, _P] + [c_int] * 11 + [_P, _P, c_int, c_int, _P],
+    "demon_conv_slice_nhwc_same": [_P, c_int, _P] + [c_int] * 10 + [_P, _P, c_int, c_int, _P],
     "demon_conv2d_nhwc": [_P, _P] + [c_int] * 9 + [_P, _P, c_int, c_int, _P],
     "demon_deconv4x4s2_nhwc": [_P, _P] + [c_int] * 5 + [_P, _P, c_int, c_int, _P],
     "demon_last_error": [],

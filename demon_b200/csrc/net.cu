@@ -53,6 +53,15 @@ struct Layer {
   int scale_stride = 0;
   bool dense_nchw_flatten = false;  // motion_fc1: TF flattens NCHW (blocks_original.py:388-392)
   int dense_c = 0, dense_hw = 0;
+  // v2 only.  tf_same: the taps of a conv sit where tf.layers.conv2d(padding='same') puts them (pad_before below) instead
+  // of k/2 (caffe padding).  dense_nchw_unflatten: the output columns are reshaped to NCHW [dense_c, H, W] by TF
+  // (v2/blocks.py:215), so they are permuted like the input rows.  nhwc: the dense layer reads channels [0, dense_c) of
+  // every pixel of this buffer (gathered into `in` before it runs) and its output is scattered back into channels
+  // [nhwc_out_coff, nhwc_out_coff + dense_c) of it (conv5_1_dense5, v2/blocks.py:198-215).
+  bool tf_same = false;
+  bool dense_nchw_unflatten = false;
+  Buf* nhwc = nullptr;
+  int nhwc_out_coff = 0;
   // expected TF variable shapes
   std::vector<int64_t> kshape;
   // device parameters
@@ -71,8 +80,8 @@ struct Layer {
 // The refinement block has no head (head_end == begin).
 struct Block { int begin = 0, head_end = 0, end = 0; };
 
-// The outputs of a fused-pipeline call, in the C ABI's order; any pointer may be null
-struct PipelineOutputs { float *depth0, *rotation, *translation, *flow2, *depth2, *normal2; };
+// The outputs of a fused-pipeline call, in the C ABI's order; any pointer may be null (normal0: v2 nets only)
+struct PipelineOutputs { float *depth0, *rotation, *translation, *flow2, *depth2, *normal2, *normal0; };
 
 enum PipelineInput : int64_t { IN_FP32, IN_U8, IN_RESIZE, IN_VIEWS };
 // NO_SNAPSHOTS: the last iteration's predictions and the refinement block; otherwise snapshot k (0 = bootstrap, k = after
@@ -105,6 +114,7 @@ using namespace demon;
 struct demon_net {
   int B = 0, RH = 0, RW = 0;
   int precision = DEMON_PREC_FP32_SIMT;
+  int variant = 1;           // 1: networks_original (demon_net_create), 2: v2.networks (demon_net_create_v2); fixed at creation
   int device = 0;            // the CUDA device the handle was created on; every entry point checks it is current
   bool finalized = false;
   float* ws = nullptr;
@@ -138,6 +148,8 @@ struct demon_net {
   Buf *img8, *i22, *i22_half, *c1y, *c1, *c2y, *cat2, *extra_in, *exy, *c21y, *concat2, *c3y, *c3, *c31y, *concat3, *c4y, *c4,
       *c41y, *concat4, *c5y, *c5, *c51y, *c51, *pf5a, *pf5, *p2a, *flowconf2, *dn2, *mc1, *fc1, *fc2, *motion;
   Buf *rin, *concat0, *rc1, *concat1, *rc2, *rc21, *pd0a, *rdepth0, *splitk;
+  // v2 only (build_plan_v2): dense5's gathered input and its output row, the motion branch (its concat is mc1)
+  Buf *d5in = nullptr, *d5out = nullptr, *mc3y = nullptr, *mc3 = nullptr, *mc4y = nullptr, *mc4 = nullptr, *mc5y = nullptr;
   // staging roles of the buffers above (see build_plan)
   Buf *pair_bytes, *i22_bytes, *planes2, *host_depth0, *host_motion;
   // the five blocks' layer ranges
@@ -172,6 +184,24 @@ struct demon_net {
     Layer* y = add_layer(name + "y", L_CONV, in, in_coff, cin, mid, 0, cmid, k, 1, stride, 1, true);
     add_layer(name + "x", L_CONV, mid, 0, cmid, out, out_coff, cout, 1, k, 1, stride, true);
     return y;
+  }
+  // v2 convrelu2 (v2/helpers.py:46-91): the same pair with 'same' padding; the x conv reads its input in whole chunks of 32
+  // channels, so a 24 / 48-channel y half sits in a 32 / 64-channel pixel whose other channels are never written (zero)
+  // and carry zero weights, which keeps the x conv on the tensor cores
+  Layer* add_sep_v2(const std::string& name, int k, int stride, Buf* in, int in_coff, int cin, Buf* mid, int cmid, Buf* out,
+                    int out_coff, int cout) {
+    Layer* y = add_sep(name, k, stride, in, in_coff, cin, mid, cmid, out, out_coff, cout);
+    Layer* x = layers.back().get();
+    y->tf_same = x->tf_same = true;
+    x->cin_buf = (cmid + 31) / 32 * 32;
+    return y;
+  }
+  // a v2 single conv (v2/helpers.py:24-43)
+  Layer* add_conv_v2(const std::string& name, Buf* in, int in_coff, int cin, Buf* out, int out_coff, int cout, int k, int stride,
+                     bool leaky) {
+    Layer* l = add_layer(name, L_CONV, in, in_coff, cin, out, out_coff, cout, k, k, stride, stride, leaky);
+    l->tf_same = true;
+    return l;
   }
 };
 
@@ -327,6 +357,158 @@ void build_plan(demon_net* n) {
   n->refine = build_refine_block(n, "netRefine");
 }
 
+// ---- v2 (python/depthmotionnet/v2/blocks.py): the same kernels over a second plan ----------------------------------------
+// returns the index of the first layer after conv2 (as build_trunk)
+int build_trunk_v2(demon_net* n, const std::string& s, bool flow, bool iterative) {
+  const bool wide2 = flow && !iterative;   // the bootstrap flow block's conv2 is (48, 64) and has no extra inputs
+  Buf* cat2 = iterative ? (flow ? n->cat2_f2 : n->cat2_d2) : n->cat2;
+  n->add_sep_v2(s + "conv1", 9, 2, n->img8, 0, 6, n->c1y, 24, n->c1, 0, 32);
+  n->add_sep_v2(s + "conv2", 7, 2, n->c1, 0, 32, n->c2y, wide2 ? 48 : 32, cat2, 0, wide2 ? 64 : 32);
+  const int head_end = (int)n->layers.size();
+  if (!wide2) {
+    const int extra = flow ? 9 : (iterative ? 8 : 7);
+    Layer* ey = n->add_sep_v2(s + "conv2_extra_inputs", 3, 1, n->extra_in, 0, extra, n->exy, 32, cat2, 32, 32);
+    ey->cin_buf = 32;   // as in build_trunk
+  }
+  n->add_sep_v2(s + "conv2_1", 3, 1, cat2, 0, 64, n->c21y, 64, n->concat2, 64, 64);
+  n->add_sep_v2(s + "conv3", 5, 2, n->concat2, 64, 64, n->c3y, 96, n->c3, 0, 128);
+  n->add_sep_v2(s + "conv3_1", 3, 1, n->c3, 0, 128, n->c31y, 128, n->concat3, 128, 128);
+  n->add_sep_v2(s + "conv4", 5, 2, n->concat3, 128, 128, n->c4y, 192, n->c4, 0, 256);
+  n->add_sep_v2(s + "conv4_1", 3, 1, n->c4, 0, 256, n->c41y, 256, n->concat4, 256, 256);
+  n->add_sep_v2(s + "conv5", flow ? 5 : 3, 2, n->concat4, 256, 256, n->c5y, 384, n->c5, 0, 384);
+  n->add_sep_v2(s + "conv5_1", 3, 1, n->c5, 0, 384, n->c51y, 384, n->c51, 0, 384);
+  // dense5 over conv5_1[:, 0:96] flattened NCHW, reshaped [96,6,8] and concatenated after conv5_1: channels 384..479 of
+  // c51 (conv5_1_dense5)
+  Layer* d5 = n->add_layer(s + "dense5", L_DENSE, n->d5in, 0, 4608, n->d5out, 0, 4608, 1, 1, 1, 1, true);
+  d5->dense_nchw_flatten = d5->dense_nchw_unflatten = true; d5->dense_c = 96; d5->dense_hw = 48;
+  d5->nhwc = n->c51; d5->nhwc_out_coff = 384;
+  // 72 column tiles x 16 K slices of 288 rows: at batch 1 the layer is a read of its 85 MB weight, and 1152 CTAs keep enough
+  // loads in flight for it (4 slices, 288 CTAs, reached a fifth of HBM bandwidth); build_plan_v2 sizes the split-K buffer
+  d5->ksplit = 16;
+  return head_end;
+}
+
+Block build_flow_block_v2(demon_net* n, const std::string& scope, bool iterative) {
+  const std::string s = scope + "/";
+  const int begin = (int)n->layers.size();
+  const int head_end = build_trunk_v2(n, s, true, iterative);
+  n->add_conv_v2(s + "predict_flow5/conv1", n->c51, 0, 480, n->pf5a, 0, 24, 3, 1, true);
+  n->add_conv_v2(s + "predict_flow5/conv2", n->pf5a, 0, 24, n->pf5, 0, 4, 3, 1, false);
+  n->add_layer(s + "upsample_flow5to4/upconv", L_DECONV, n->pf5, 0, 4, n->concat4, 512, 2, 4, 4, 2, 2, false);
+  n->add_layer(s + "refine4/upconv", L_DECONV, n->c51, 0, 480, n->concat4, 0, 256, 4, 4, 2, 2, true);
+  Layer* r3 = n->add_layer(s + "refine3/upconv", L_DECONV, n->concat4, 0, 514, n->concat3, 0, 128, 4, 4, 2, 2, true);
+  r3->cin_buf = 576;   // as in build_flow_block
+  n->add_layer(s + "refine2/upconv", L_DECONV, n->concat3, 0, 256, n->concat2, 0, 64, 4, 4, 2, 2, true);
+  n->add_conv_v2(s + "predict_flow2/conv1", n->concat2, 0, 128, n->p2a, 0, 24, 3, 1, true);
+  n->add_conv_v2(s + "predict_flow2/conv2", n->p2a, 0, 24, n->flowconf2, 0, 4, 3, 1, false);
+  return {begin, head_end, (int)n->layers.size()};
+}
+
+Block build_dm_block_v2(demon_net* n, const std::string& scope, bool iterative) {
+  const std::string s = scope + "/";
+  const int begin = (int)n->layers.size();
+  const int head_end = build_trunk_v2(n, s, false, iterative);
+  // motion branch (v2/blocks.py:417-429): three separable stride-2 pairs on conv2_1 and a 3x3 conv on conv5_1_dense5, each
+  // into one half of the 128-channel concat that motion_fc1 flattens NCHW
+  n->add_sep_v2(s + "motion_conv3", 5, 2, n->concat2, 64, 64, n->mc3y, 64, n->mc3, 0, 64);
+  n->add_sep_v2(s + "motion_conv4", 5, 2, n->mc3, 0, 64, n->mc4y, 64, n->mc4, 0, 64);
+  n->add_sep_v2(s + "motion_conv5a", 3, 2, n->mc4, 0, 64, n->mc5y, 64, n->mc1, 0, 64);
+  n->add_conv_v2(s + "motion_conv5b", n->c51, 0, 480, n->mc1, 64, 64, 3, 1, true);
+  Layer* f1 = n->add_layer(s + "motion_fc1", L_DENSE, n->mc1, 0, 6144, n->fc1, 0, 1024, 1, 1, 1, 1, true);
+  f1->dense_nchw_flatten = true; f1->dense_c = 128; f1->dense_hw = 48;
+  f1->ksplit = 24;
+  Layer* f2 = n->add_layer(s + "motion_fc2", L_DENSE, n->fc1, 0, 1024, n->fc2, 0, 128, 1, 1, 1, 1, true);
+  f2->ksplit = 16;
+  n->add_layer(s + "motion_fc3", L_DENSE, n->fc2, 0, 128, n->motion, 0, 7, 1, 1, 1, 1, false);
+  n->add_layer(s + "refine4/upconv", L_DECONV, n->c51, 0, 384, n->concat4, 0, 256, 4, 4, 2, 2, true);   // conv5_1 alone
+  n->add_layer(s + "refine3/upconv", L_DECONV, n->concat4, 0, 512, n->concat3, 0, 128, 4, 4, 2, 2, true);
+  n->add_layer(s + "refine2/upconv", L_DECONV, n->concat3, 0, 256, n->concat2, 0, 64, 4, 4, 2, 2, true);
+  n->add_conv_v2(s + "predict_depthnormal2/conv1", n->concat2, 0, 128, n->p2a, 0, 24, 3, 1, true);
+  Layer* dn = n->add_conv_v2(s + "predict_depthnormal2/conv2", n->p2a, 0, 24, n->dn2, 0, 4, 3, 1, false);
+  dn->scale = n->motion; dn->scale_coff = 6; dn->scale_stride = 8;
+  return {begin, head_end, (int)n->layers.size()};
+}
+
+// v2/blocks.py:499-560: as build_refine_block, with 'same' padding and depth0 + normal0 out of predict_depth0/conv2
+Block build_refine_block_v2(demon_net* n, const std::string& scope) {
+  const std::string s = scope + "/";
+  const int begin = (int)n->layers.size();
+  Layer* c0 = n->add_conv_v2(s + "conv0", n->rin, 0, 4, n->concat0, 32, 32, 3, 1, true);
+  c0->cin_buf = 8;
+  n->add_conv_v2(s + "conv1", n->concat0, 32, 32, n->rc1, 0, 64, 3, 2, true);
+  n->add_conv_v2(s + "conv1_1", n->rc1, 0, 64, n->concat1, 64, 64, 3, 1, true);
+  n->add_conv_v2(s + "conv2", n->concat1, 64, 64, n->rc2, 0, 128, 3, 2, true);
+  n->add_conv_v2(s + "conv2_1", n->rc2, 0, 128, n->rc21, 0, 128, 3, 1, true);
+  n->add_layer(s + "refine1/upconv", L_DECONV, n->rc21, 0, 128, n->concat1, 0, 64, 4, 4, 2, 2, true);
+  n->add_layer(s + "refine0/upconv", L_DECONV, n->concat1, 0, 128, n->concat0, 0, 32, 4, 4, 2, 2, true);
+  n->add_conv_v2(s + "predict_depth0/conv1", n->concat0, 0, 64, n->pd0a, 0, 16, 3, 1, true);
+  n->add_conv_v2(s + "predict_depth0/conv2", n->pd0a, 0, 16, n->rdepth0, 0, 4, 3, 1, false);
+  return {begin, begin, (int)n->layers.size()};
+}
+
+void build_plan_v2(demon_net* n) {
+  const int H = 192, W = 256;
+  n->img8 = n->add_buf(H, W, 8);
+  n->i22_half = n->add_buf(3, 96, 128);
+  n->i22 = n->add_buf(3, 48, 64);
+  n->c1y = n->add_buf(96, 256, 32);      // 24 channels written
+  n->c1 = n->add_buf(96, 128, 32);
+  n->c2y = n->add_buf(48, 128, 64);      // 48 (bootstrap flow block) or 32 channels written
+  n->cat2 = n->add_buf(48, 64, 64);
+  n->cat2_f2 = n->add_buf(48, 64, 64);
+  n->cat2_d2 = n->add_buf(48, 64, 64);
+  n->extra_in = n->add_buf(48, 64, 32);
+  n->exy = n->add_buf(48, 64, 32);
+  n->c21y = n->add_buf(48, 64, 64);
+  n->concat2 = n->add_buf(48, 64, 128);
+  n->c3y = n->add_buf(24, 64, 96);
+  n->c3 = n->add_buf(24, 32, 128);
+  n->c31y = n->add_buf(24, 32, 128);
+  n->concat3 = n->add_buf(24, 32, 256);
+  n->c4y = n->add_buf(12, 32, 192);
+  n->c4 = n->add_buf(12, 16, 256);
+  n->c41y = n->add_buf(12, 16, 256);
+  n->concat4 = n->add_buf(12, 16, 576);
+  n->c5y = n->add_buf(6, 16, 384);
+  n->c5 = n->add_buf(6, 8, 384);
+  n->c51y = n->add_buf(6, 8, 384);
+  n->c51 = n->add_buf(6, 8, 480);        // conv5_1_dense5: conv5_1 (384) ++ dense5 reshaped (96)
+  n->d5in = n->add_buf(1, 1, 4608);
+  n->d5out = n->add_buf(1, 1, 4608);
+  n->pf5a = n->add_buf(6, 8, 24);
+  n->pf5 = n->add_buf(6, 8, 4);
+  n->p2a = n->add_buf(48, 64, 24);
+  n->flowconf2 = n->add_buf(48, 64, 4);
+  n->dn2 = n->add_buf(48, 64, 4);
+  n->mc3y = n->add_buf(24, 64, 64);
+  n->mc3 = n->add_buf(24, 32, 64);
+  n->mc4y = n->add_buf(12, 32, 64);
+  n->mc4 = n->add_buf(12, 16, 64);
+  n->mc5y = n->add_buf(6, 16, 64);
+  n->mc1 = n->add_buf(6, 8, 128);        // motion_conv5a ++ motion_conv5b
+  n->fc1 = n->add_buf(1, 1, 1024);
+  n->fc2 = n->add_buf(1, 1, 128);
+  n->motion = n->add_buf(1, 1, 8);
+  n->splitk = n->add_buf(1, 16, 4608);   // split-K partial sums: dense5 [16][B][4608], motion_fc1 [24][B][1024]
+  const int RH = n->RH, RW = n->RW;
+  n->rin = n->add_buf(RH, RW, 8);
+  n->concat0 = n->add_buf(RH, RW, 64);
+  n->rc1 = n->add_buf(RH / 2, RW / 2, 64);
+  n->concat1 = n->add_buf(RH / 2, RW / 2, 128);
+  n->rc2 = n->add_buf(RH / 4, RW / 4, 128);
+  n->rc21 = n->add_buf(RH / 4, RW / 4, 128);
+  n->pd0a = n->add_buf(RH, RW, 16);
+  n->rdepth0 = n->add_buf(RH, RW, 4);    // depth0 ++ normal0
+  // v2 has only float32 device entries: no staging roles
+  n->pair_bytes = n->i22_bytes = n->planes2 = n->host_depth0 = n->host_motion = nullptr;
+
+  n->flow1 = build_flow_block_v2(n, "netFlow1", false);
+  n->dm1 = build_dm_block_v2(n, "netDM1", false);
+  n->flow2 = build_flow_block_v2(n, "netFlow2", true);
+  n->dm2 = build_dm_block_v2(n, "netDM2", true);
+  n->refine = build_refine_block_v2(n, "netRefine");
+}
+
 // ---------------------------------------------------------------------------------------------
 // weight packing: TF layout -> [tap][cin_buf][cout_pad]
 // ---------------------------------------------------------------------------------------------
@@ -357,6 +539,9 @@ void pack_deconv_class(const Layer& l, const float* k, int py, int px, std::vect
     }
 }
 
+// dense5 (v2): buffer column j = hw*C + c holds TF column c*HW + hw (TF reshapes the output to NCHW [C, H, W])
+int dense_unflatten_src(const Layer& l, int j) { return (j % l.dense_c) * l.dense_hw + j / l.dense_c; }
+
 void pack_dense(const Layer& l, const float* k, std::vector<float>& out) {
   out.assign((size_t)l.cin_buf * l.cout_pad, 0.f);
   for (int i = 0; i < l.cin; ++i) {
@@ -365,7 +550,11 @@ void pack_dense(const Layer& l, const float* k, std::vector<float>& out) {
       const int hw = i / l.dense_c, c = i % l.dense_c;
       src = c * l.dense_hw + hw;
     }
-    for (int co = 0; co < l.cout; ++co) out[(size_t)i * l.cout_pad + co] = k[(size_t)src * l.cout + co];
+    if (!l.dense_nchw_unflatten) {
+      for (int co = 0; co < l.cout; ++co) out[(size_t)i * l.cout_pad + co] = k[(size_t)src * l.cout + co];
+      continue;
+    }
+    for (int co = 0; co < l.cout; ++co) out[(size_t)i * l.cout_pad + co] = k[(size_t)src * l.cout + dense_unflatten_src(l, co)];
   }
 }
 
@@ -381,6 +570,14 @@ int upload(std::vector<void*>& allocs, const std::vector<float>& host, float** d
 // ---------------------------------------------------------------------------------------------
 // layer execution
 // ---------------------------------------------------------------------------------------------
+// tf.nn.conv2d(padding='SAME') along one axis: out = ceil(in / s), pad_total = max((out - 1) * s + k - in, 0), and the
+// smaller half goes before.  Equal to k / 2 (caffe padding) for s = 1 and odd k, and for s = 2 on an odd input; one less
+// for s = 2 on an even input.
+int tf_same_pad_before(int in, int k, int s) {
+  const int out = ceil_div(in, s);
+  return std::max((out - 1) * s + k - in, 0) / 2;
+}
+
 // The convolution problem(s) of a layer: 1 for conv / dense, 4 sub-pixel classes for a transposed conv.
 // `dst`, if given, replaces the base of the layer's output buffer (same shape and channel pitch).
 int build_problems(const Layer& l, int B, ConvProblem* out, float* dst = nullptr) {
@@ -414,8 +611,10 @@ int build_problems(const Layer& l, int B, ConvProblem* out, float* dst = nullptr
     p.Ho = ceil_div(p.Hi, l.sy); p.Wo = ceil_div(p.Wi, l.sx);
     p.Hfull = p.Ho; p.Wfull = p.Wo;
     p.ntaps = l.kh * l.kw;
+    const int py = l.tf_same ? tf_same_pad_before(p.Hi, l.kh, l.sy) : l.kh / 2;
+    const int px = l.tf_same ? tf_same_pad_before(p.Wi, l.kw, l.sx) : l.kw / 2;
     for (int ky = 0; ky < l.kh; ++ky)
-      for (int kx = 0; kx < l.kw; ++kx) { p.dy[ky * l.kw + kx] = ky - l.kh / 2; p.dx[ky * l.kw + kx] = kx - l.kw / 2; }
+      for (int kx = 0; kx < l.kw; ++kx) { p.dy[ky * l.kw + kx] = ky - py; p.dx[ky * l.kw + kx] = kx - px; }
     p.w = l.w_dev[0];
     out[0] = p;
     return 1;
@@ -458,6 +657,8 @@ int run_layer(const Layer& l, int B, cudaStream_t stream, float* splitk_ws, floa
 int upload_layer(Layer& l, const float* k, const float* bias_host, int B, int precision, std::vector<void*>& allocs) {
   std::vector<float> bias(l.cout_pad, 0.f);
   std::copy(bias_host, bias_host + l.cout, bias.begin());
+  if (l.dense_nchw_unflatten)
+    for (int j = 0; j < l.cout; ++j) bias[j] = bias_host[dense_unflatten_src(l, j)];
   int rc;
   if ((rc = upload(allocs, bias, &l.bias_dev))) return rc;
   std::vector<float> w[4];
@@ -543,14 +744,26 @@ int trace_copy(const demon_net* n, const Layer& l, bool input, float* dst, float
   return DEMON_OK;
 }
 
+int dense_nhwc_copy(const demon_net* n, const Layer& l, bool gather, cudaStream_t s);
+
 // `dst`: see build_problems.  With a trace set (demon_debug_trace_layers), the layer's input slice is copied out before it
 // runs and its output slice after.
-int run_layer_profiled(demon_net* n, int idx, cudaStream_t stream, float* dst = nullptr) {
+int run_layer_traced(demon_net* n, int idx, cudaStream_t stream, float* dst) {
   if (!n->tracing) return run_layer_timed(n, idx, stream, dst);
   const Layer& l = *n->layers[idx];
   int rc = n->trace_in[idx] ? trace_copy(n, l, true, dst, n->trace_in[idx], stream) : DEMON_OK;
   if (rc == DEMON_OK) rc = run_layer_timed(n, idx, stream, dst);
   if (rc == DEMON_OK && n->trace_out[idx]) rc = trace_copy(n, l, false, dst, n->trace_out[idx], stream);
+  return rc;
+}
+
+// A dense layer over pixels (v2's dense5) gathers its input row before it runs and scatters its output after
+int run_layer_profiled(demon_net* n, int idx, cudaStream_t stream, float* dst = nullptr) {
+  const Layer& l = *n->layers[idx];
+  if (!l.nhwc) return run_layer_traced(n, idx, stream, dst);
+  int rc = dense_nhwc_copy(n, l, true, stream);
+  if (rc == DEMON_OK) rc = run_layer_traced(n, idx, stream, dst);
+  if (rc == DEMON_OK) rc = dense_nhwc_copy(n, l, false, stream);
   return rc;
 }
 
@@ -600,6 +813,16 @@ int strided_copy(const float* src, float* dst, int N, int P, int C, Strides s, S
   (void)launch_pdl(strided_copy_kernel, dim3((int)blocks), dim3(256), 0, stream, src, dst, N, P, C, s.n, s.p, s.c, d.n, d.p, d.c);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
+}
+
+// dense5's two copies (Layer::nhwc): gather channels [0, dense_c) of every pixel into the row [B, HW*C] the dense kernel
+// reads, or scatter its output row into channels [nhwc_out_coff, +dense_c).  Two small copies of B x 18 KB rather than a
+// pixel pitch inside the dense kernel and its split-K reduction, which v1's layers share.
+int dense_nhwc_copy(const demon_net* n, const Layer& l, bool gather, cudaStream_t s) {
+  const Buf* b = l.nhwc;
+  const Strides row{(long)l.dense_hw * l.dense_c, l.dense_c, 1};
+  if (gather) return strided_copy(b->p, l.in->p, n->B, l.dense_hw, l.dense_c, buf_strides(b), row, s);
+  return strided_copy(l.out->p, b->p + l.nhwc_out_coff, n->B, l.dense_hw, l.dense_c, row, buf_strides(b), s);
 }
 
 // median3x3_downsample over planes with a batch stride (image_pair[:,3:6] -> image2_2,
@@ -664,7 +887,16 @@ __global__ void __launch_bounds__(256) flow_extra_kernel(const float* __restrict
   o[2] = make_float4(d.w, 0.f, 0.f, 0.f);
 }
 
-// DM extra inputs (blocks_original.py:336-364): warp2d(image2_2, flow2) ++ flowconf2 (++ flow_to_depth) -> NHWC8
+// tf.clip_by_value(x, 0, 50) of TF 1.4 (v2/blocks.py:379): minimum(x, 50) then maximum(., 0) with the compare order of
+// std::min / std::max, so +inf -> 50, -inf -> 0 and NaN stays NaN (neither less than 0 nor greater than 50)
+__device__ __forceinline__ float clip_0_50(float x) {
+  const float t = (50.f < x) ? 50.f : x;
+  return (t < 0.f) ? 0.f : t;
+}
+
+// DM extra inputs (blocks_original.py:336-364): warp2d(image2_2, flow2) ++ flowconf2 (++ flow_to_depth) -> NHWC8.
+// kClip (v2): the depth from flow is clipped to [0, 50] (v2/blocks.py:379)
+template <bool kClip>
 __global__ void __launch_bounds__(128) dm_extra_kernel(const float* __restrict__ flowconf2, const float* __restrict__ motion_prev,
                                                       const float* __restrict__ image2_2, float* __restrict__ extra, int H, int W,
                                                       int extra_pitch, bool with_depth) {
@@ -694,7 +926,8 @@ __global__ void __launch_bounds__(128) dm_extra_kernel(const float* __restrict__
     }
     wv[c] = r;
   }
-  const float dff = with_depth ? f2d_pixel(fc.x, fc.y, x, y, cam, true, true) : 0.f;
+  float dff = with_depth ? f2d_pixel(fc.x, fc.y, x, y, cam, true, true) : 0.f;
+  if (kClip) dff = clip_0_50(dff);
   float* o = extra + ((size_t)n * hw + i) * extra_pitch;
   *reinterpret_cast<float4*>(o) = make_float4(wv[0], wv[1], wv[2], fc.x);
   *reinterpret_cast<float4*>(o + 4) = make_float4(fc.y, fc.z, fc.w, dff);
@@ -831,8 +1064,8 @@ int run_dm_block(demon_net* n, const Block& b, bool iterative, cudaStream_t s, b
   int rc;
   if (head && (rc = run_layers(n, b.begin, b.head_end, s))) return rc;
   // the previous motion is still in n->motion here: this block's motion_fc3 overwrites it later
-  (void)launch_pdl(dm_extra_kernel, dim3(dim3(ceil_div(48 * 64, 128), n->B)), dim3(128), 0, s, n->flowconf2->p, n->motion->p, n->i22->p, n->extra_in->p, 48, 64,
-                                                                   n->extra_in->C, iterative);
+  (void)launch_pdl(n->variant == 2 ? dm_extra_kernel<true> : dm_extra_kernel<false>, dim3(dim3(ceil_div(48 * 64, 128), n->B)), dim3(128), 0, s,
+                   n->flowconf2->p, n->motion->p, n->i22->p, n->extra_in->p, 48, 64, n->extra_in->C, iterative);
   DEMON_LAUNCH_CHECK();
   return run_layers(n, b.head_end, b.end, s);
 }
@@ -852,6 +1085,14 @@ int run_refine_block(demon_net* n, const float* image1, Strides img, const float
   return run_layer_profiled(n, b.end - 1, s, depth0);
 }
 
+// v2: predict_depth0/conv2 writes depth0 ++ normal0 into rdepth0, from where the two are exported in `data_format`
+int run_refine_block_v2(demon_net* n, const float* image1, Strides img, const float* depth, Strides dep, int dh, int dw, float* depth0,
+                        float* normal0, int data_format, cudaStream_t s) {
+  int rc = run_refine_block(n, image1, img, depth, dep, dh, dw, nullptr, s);
+  if (rc || (rc = export_slice(n, n->rdepth0, 0, 1, depth0, data_format, s))) return rc;
+  return export_slice(n, n->rdepth0, 1, 3, normal0, data_format, s);
+}
+
 }  // namespace
 }  // namespace demon
 
@@ -860,15 +1101,16 @@ int run_refine_block(demon_net* n, const float* image1, Strides img, const float
 // ---------------------------------------------------------------------------------------------
 extern "C" {
 
-int demon_net_create(demon_net** out, int batch, int refine_h, int refine_w, int precision) {
+static int net_create(demon_net** out, int batch, int refine_h, int refine_w, int precision, int variant) {
   DEMON_REQUIRE(out, "demon_net_create: null out");
   DEMON_REQUIRE(batch >= 1 && batch <= 4096, "demon_net_create: batch %d", batch);
   DEMON_REQUIRE(refine_h >= 4 && refine_w >= 4 && refine_h % 4 == 0 && refine_w % 4 == 0, "demon_net_create: refine size %dx%d must be a multiple of 4", refine_h, refine_w);
   DEMON_REQUIRE(precision >= 0 && precision <= 2, "demon_net_create: precision %d", precision);
   std::unique_ptr<demon_net> n(new demon_net());
-  n->B = batch; n->RH = refine_h; n->RW = refine_w; n->precision = precision;
+  n->B = batch; n->RH = refine_h; n->RW = refine_w; n->precision = precision; n->variant = variant;
   DEMON_CHECK_CUDA(cudaGetDevice(&n->device));
-  build_plan(n.get());
+  if (variant == 2) build_plan_v2(n.get());
+  else build_plan(n.get());
   void* p = nullptr;
   DEMON_CHECK_CUDA(cudaMalloc(&p, n->ws_floats * sizeof(float)));
   n->ws = (float*)p;
@@ -877,6 +1119,16 @@ int demon_net_create(demon_net** out, int batch, int refine_h, int refine_w, int
   *out = n.release();
   return DEMON_OK;
 }
+
+int demon_net_create(demon_net** out, int batch, int refine_h, int refine_w, int precision) {
+  return net_create(out, batch, refine_h, refine_w, precision, 1);
+}
+
+int demon_net_create_v2(demon_net** out, int batch, int refine_h, int refine_w, int precision) {
+  return net_create(out, batch, refine_h, refine_w, precision, 2);
+}
+
+int demon_net_variant(const demon_net* n) { return n ? n->variant : 0; }
 
 void demon_net_destroy(demon_net* n) {
   if (!n) return;
@@ -1012,25 +1264,27 @@ int demon_net_layer_profile(const demon_net* n, int i, double* ms, int64_t* call
   if (ms) *ms = i < (int)n->prof_ms.size() ? n->prof_ms[i] : 0.0;
   if (calls) *calls = i < (int)n->prof_calls.size() ? n->prof_calls[i] : 0;
   const Layer& l = *n->layers[i];
-  if (launches_per_call) *launches_per_call = l.use_tc() ? 1 : (l.kind == L_DECONV ? 4 : (l.ksplit > 1 ? 2 : 1));
+  if (launches_per_call) *launches_per_call = (l.use_tc() ? 1 : (l.kind == L_DECONV ? 4 : (l.ksplit > 1 ? 2 : 1))) + (l.nhwc ? 2 : 0);
   // kernel family: 0 conv_simt_kernel, 2 conv_tc_halo_kernel (halo), 3 conv_tc_halo_kernel (per tap)
   if (uses_tc) *uses_tc = !l.use_tc() ? 0 : (l.tc.per_tap ? 3 : 2);
   return DEMON_OK;
 }
 
-#define REQUIRE_READY(n)                                                         \
+// A forward entry of network variant v (1: the demon_* entries, 2: the demon_*_v2 entries) takes only a net of that variant
+#define REQUIRE_READY_AS(n, v)                                                   \
   do {                                                                           \
     DEMON_REQUIRE(n, "null net");                                                \
+    DEMON_REQUIRE((n)->variant == (v), "a v%d net handle was passed to a v%d entry", (n)->variant, (v)); \
     if (!(n)->finalized) return fail(DEMON_E_STATE, "forward before demon_net_finalize"); \
     int _dev = -1;                                                               \
     cudaGetDevice(&_dev);                                                        \
     if (_dev != (n)->device)                                                     \
       return fail(DEMON_E_STATE, "net handle belongs to CUDA device %d but device %d is current", (n)->device, _dev); \
   } while (0)
+#define REQUIRE_READY(n) REQUIRE_READY_AS(n, 1)
 
-int demon_bootstrap_forward(demon_net* n, const float* image_pair, const float* image2_2, float* flow5, float* flow2, float* depth2,
-                            float* normal2, float* rotation, float* translation, int data_format, void* stream) {
-  REQUIRE_READY(n);
+static int bootstrap_impl(demon_net* n, const float* image_pair, const float* image2_2, float* flow5, float* flow2, float* depth2,
+                          float* normal2, float* rotation, float* translation, int data_format, void* stream) {
   DEMON_REQUIRE(image_pair && image2_2, "bootstrap: null input");
   DEMON_REQUIRE(data_format == 0 || data_format == 1, "bootstrap: data_format %d", data_format);
   cudaStream_t s = (cudaStream_t)stream;
@@ -1042,10 +1296,21 @@ int demon_bootstrap_forward(demon_net* n, const float* image_pair, const float* 
   return export_predictions(n, flow5, flow2, depth2, normal2, rotation, translation, data_format, s);
 }
 
-int demon_iterative_forward(demon_net* n, const float* image_pair, const float* image2_2, const float* depth2_in, const float* normal2_in,
-                            const float* rotation_in, const float* translation_in, float* flow5, float* flow2, float* depth2,
+int demon_bootstrap_forward(demon_net* n, const float* image_pair, const float* image2_2, float* flow5, float* flow2, float* depth2,
                             float* normal2, float* rotation, float* translation, int data_format, void* stream) {
   REQUIRE_READY(n);
+  return bootstrap_impl(n, image_pair, image2_2, flow5, flow2, depth2, normal2, rotation, translation, data_format, stream);
+}
+
+int demon_bootstrap_forward_v2(demon_net* n, const float* image_pair, const float* image2_2, float* flow5, float* flow2, float* depth2,
+                               float* normal2, float* rotation, float* translation, int data_format, void* stream) {
+  REQUIRE_READY_AS(n, 2);
+  return bootstrap_impl(n, image_pair, image2_2, flow5, flow2, depth2, normal2, rotation, translation, data_format, stream);
+}
+
+static int iterative_impl(demon_net* n, const float* image_pair, const float* image2_2, const float* depth2_in, const float* normal2_in,
+                          const float* rotation_in, const float* translation_in, float* flow5, float* flow2, float* depth2,
+                          float* normal2, float* rotation, float* translation, int data_format, void* stream) {
   DEMON_REQUIRE(image_pair && image2_2 && depth2_in && normal2_in && rotation_in && translation_in, "iterative: null input");
   DEMON_REQUIRE(data_format == 0 || data_format == 1, "iterative: data_format %d", data_format);
   cudaStream_t s = (cudaStream_t)stream;
@@ -1063,6 +1328,22 @@ int demon_iterative_forward(demon_net* n, const float* image_pair, const float* 
   return export_predictions(n, flow5, flow2, depth2, normal2, rotation, translation, data_format, s);
 }
 
+int demon_iterative_forward(demon_net* n, const float* image_pair, const float* image2_2, const float* depth2_in, const float* normal2_in,
+                            const float* rotation_in, const float* translation_in, float* flow5, float* flow2, float* depth2,
+                            float* normal2, float* rotation, float* translation, int data_format, void* stream) {
+  REQUIRE_READY(n);
+  return iterative_impl(n, image_pair, image2_2, depth2_in, normal2_in, rotation_in, translation_in, flow5, flow2, depth2, normal2,
+                        rotation, translation, data_format, stream);
+}
+
+int demon_iterative_forward_v2(demon_net* n, const float* image_pair, const float* image2_2, const float* depth2_in, const float* normal2_in,
+                               const float* rotation_in, const float* translation_in, float* flow5, float* flow2, float* depth2,
+                               float* normal2, float* rotation, float* translation, int data_format, void* stream) {
+  REQUIRE_READY_AS(n, 2);
+  return iterative_impl(n, image_pair, image2_2, depth2_in, normal2_in, rotation_in, translation_in, flow5, flow2, depth2, normal2,
+                        rotation, translation, data_format, stream);
+}
+
 int demon_refine_forward(demon_net* n, const float* image1, const float* depth2, float* depth0, int data_format, void* stream) {
   REQUIRE_READY(n);
   DEMON_REQUIRE(image1 && depth2 && depth0, "refine: null pointer");
@@ -1071,6 +1352,19 @@ int demon_refine_forward(demon_net* n, const float* image1, const float* depth2,
   const int dh = n->RH / 4, dw = n->RW / 4;
   return run_refine_block(n, image1, api_strides(data_format, P, 3), depth2, api_strides(data_format, (long)dh * dw, 1), dh, dw, depth0,
                           (cudaStream_t)stream);
+}
+
+// normal2 is accepted and not read, as by the reference's RefinementNet.eval (v2/networks.py:204-228)
+int demon_refine_forward_v2(demon_net* n, const float* image1, const float* depth2, const float* normal2, float* depth0, float* normal0,
+                            int data_format, void* stream) {
+  REQUIRE_READY_AS(n, 2);
+  (void)normal2;
+  DEMON_REQUIRE(image1 && depth2 && depth0, "refine_v2: null pointer");
+  DEMON_REQUIRE(data_format == 0 || data_format == 1, "refine_v2: data_format %d", data_format);
+  const long P = (long)n->RH * n->RW;
+  const int dh = n->RH / 4, dw = n->RW / 4;
+  return run_refine_block_v2(n, image1, api_strides(data_format, P, 3), depth2, api_strides(data_format, (long)dh * dw, 1), dh, dw, depth0,
+                             normal0, data_format, (cudaStream_t)stream);
 }
 
 // The intrinsics DeMoN was trained for (examples/example.py:51-61), in pixels of the 256x192 input
@@ -1086,6 +1380,9 @@ static int export_outputs(demon_net* n, const PipelineCall& c, int k, cudaStream
   int rc = export_predictions(n, nullptr, at(o.flow2, B * 2 * P2), at(o.depth2, B * P2), at(o.normal2, B * 3 * P2), at(o.rotation, B * 3),
                               at(o.translation, B * 3), 0, s);
   if (rc || c.snapshots == SNAPSHOTS) return rc;
+  if (n->variant == 2)
+    return run_refine_block_v2(n, n->img8->p, buf_strides(n->img8), n->dn2->p, buf_strides(n->dn2), 48, 64, at(o.depth0, B * P0),
+                               at(o.normal0, B * 3 * P0), 0, s);
   // image1 is read back from img8 (NHWC8: the first three channels), whatever the input kind; no depth0: into rdepth0
   return run_refine_block(n, n->img8->p, buf_strides(n->img8), n->dn2->p, buf_strides(n->dn2), 48, 64, at(o.depth0, B * P0), s);
 }
@@ -1211,6 +1508,16 @@ int demon_pipeline_forward(demon_net* n, const float* image_pair, const float* i
   return pipeline_forward_impl(n, c, stream);
 }
 
+int demon_pipeline_forward_v2(demon_net* n, const float* image_pair, const float* image2_2, int iterations, float* depth0, float* normal0,
+                              float* rotation, float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
+  REQUIRE_READY_AS(n, 2);
+  DEMON_REQUIRE(image_pair, "pipeline_v2: null image_pair");
+  PipelineCall c{};
+  c.input = IN_FP32; c.image_pair = image_pair; c.image2_2 = image2_2; c.iterations = iterations;
+  c.out = {depth0, rotation, translation, flow2, depth2, normal2, normal0};
+  return pipeline_forward_impl(n, c, stream);
+}
+
 int demon_pipeline_forward_snapshots(demon_net* n, const float* image_pair, const float* image2_2, int iterations, float* flow2,
                                      float* depth2, float* normal2, float* rotation, float* translation, float* depth0, void* stream) {
   REQUIRE_READY(n);
@@ -1325,7 +1632,8 @@ int demon_pipeline_forward_host_u8_async(demon_net* n, const uint8_t* images_hos
   return pipeline_host(n, images_host, image2_2_host, true, iterations, depth0_host, rotation_host, translation_host, stream, false);
 }
 
-// debug: the geometry of every layer of the net and which kernel family / plan it got (one line per layer)
+// debug: the geometry of every layer of the net and which kernel family / plan it got (one line per layer).  A v2 conv's
+// line also gives its first tap (dy, dx): minus the 'same' padding before the first row / column.
 int demon_debug_describe_layers(const demon_net* n, char* buf, int buflen) {
   DEMON_REQUIRE(n && buf && buflen > 0, "describe: null");
   static const char* const kKind[] = {"conv", "deconv", "dense"};
@@ -1337,10 +1645,32 @@ int demon_debug_describe_layers(const demon_net* n, char* buf, int buflen) {
                     "%-40s %s H %d W %d cin %d cin_buf %d in_pitch %d in_off %d cout %d out_pitch %d out_off %d kh %d kw %d sy %d sx %d leaky %d scale %d : ",
                     l.name.c_str(), kKind[l.kind], l.in->H, l.in->W, l.cin, l.cin_buf, l.in->C, l.in_coff, l.cout, l.out->C, l.out_coff,
                     l.kh, l.kw, l.sy, l.sx, l.leaky ? 1 : 0, l.scale ? 1 : 0);
+    if (l.tf_same) {
+      ConvProblem p;
+      build_problems(l, n->B, &p);
+      off += snprintf(buf + off, buflen - off, "tap0 %d %d : ", p.dy[0], p.dx[0]);
+    }
     off += describe_layer(l, n->B, n->precision, buf + off, buflen - off);
     off += snprintf(buf + off, buflen - off, "\n");
   }
   return off;
+}
+
+// debug, no device needed: demon_debug_describe_layers of the plan a net of this variant (1 or 2), batch, refinement size
+// and precision gets, without creating it
+int demon_debug_describe_plan(int variant, int batch, int refine_h, int refine_w, int precision, char* buf, int buflen) {
+  DEMON_REQUIRE(variant == 1 || variant == 2, "describe_plan: variant %d", variant);
+  DEMON_REQUIRE(batch >= 1 && refine_h >= 4 && refine_w >= 4 && refine_h % 4 == 0 && refine_w % 4 == 0, "describe_plan: shape");
+  DEMON_REQUIRE(precision >= 0 && precision <= 2, "describe_plan: precision %d", precision);
+  std::unique_ptr<demon_net> n(new demon_net());
+  n->B = batch; n->RH = refine_h; n->RW = refine_w; n->precision = precision; n->variant = variant;
+  if (variant == 2) build_plan_v2(n.get());
+  else build_plan(n.get());
+  // the buffers at their workspace offsets from a 256-byte aligned base that is never dereferenced (the planner looks at
+  // alignment only)
+  float* base = reinterpret_cast<float*>(uintptr_t(1) << 32);
+  for (auto& b : n->bufs) b->p = base + b->offset;
+  return demon_debug_describe_layers(n.get(), buf, buflen);
 }
 
 // debug: per-layer input / output copies of the stage-wise entries (run_layer_profiled)
@@ -1368,7 +1698,8 @@ static double g_last_conv_ms = -1.0;
 double demon_debug_last_conv_ms(void) { return g_last_conv_ms; }
 
 static int standalone_conv(const float* in, int in_pitch, float* out, int out_pitch, int B, int H, int W, int Cin, int Cout, int kh, int kw,
-                           int sy, int sx, const float* kernel_host, const float* bias_host, int leaky, int precision, bool deconv, void* stream) {
+                           int sy, int sx, const float* kernel_host, const float* bias_host, int leaky, int precision, bool deconv, void* stream,
+                           bool tf_same = false) {
   DEMON_REQUIRE(in && out && kernel_host && bias_host, "conv: null pointer");
   DEMON_REQUIRE(Cin % 4 == 0, "conv test entry: Cin must be a multiple of 4");
   DEMON_REQUIRE(B >= 1 && H >= 1 && W >= 1 && Cout >= 1 && in_pitch >= Cin && out_pitch >= Cout, "conv test entry: shape or pitch");
@@ -1378,6 +1709,7 @@ static int standalone_conv(const float* in, int in_pitch, float* out, int out_pi
   std::vector<void*> allocs;
   StandaloneLayer s(in, out, H, W, Cin, in_pitch, Cout, out_pitch, kh, kw, sy, sx, deconv, leaky != 0);
   Layer& l = s.layer;
+  l.tf_same = tf_same;
   int rc = upload_layer(l, kernel_host, bias_host, B, precision, allocs);
   if (rc == DEMON_OK && precision != DEMON_PREC_FP32_SIMT && !l.use_tc())
     rc = fail(DEMON_E_INVALID, "conv test entry: shape not supported by the tensor-core path");
@@ -1414,6 +1746,14 @@ int demon_conv_slice_nhwc(const float* in, int in_pitch, float* out, int out_pit
                           int sy, int sx, int deconv, const float* kernel_host, const float* bias_host, int leaky, int precision, void* stream) {
   return standalone_conv(in, in_pitch, out, out_pitch, B, H, W, Cin, Cout, kh, kw, sy, sx, kernel_host, bias_host, leaky, precision,
                          deconv != 0, stream);
+}
+
+// demon_conv_slice_nhwc of a convolution with the taps of tf.layers.conv2d(padding='same') (the v2 network's layers):
+// along each axis the first tap reads pad_before = max((ceil(n/s) - 1) s + k - n, 0) / 2 before the output's first pixel
+int demon_conv_slice_nhwc_same(const float* in, int in_pitch, float* out, int out_pitch, int B, int H, int W, int Cin, int Cout, int kh,
+                               int kw, int sy, int sx, const float* kernel_host, const float* bias_host, int leaky, int precision, void* stream) {
+  return standalone_conv(in, in_pitch, out, out_pitch, B, H, W, Cin, Cout, kh, kw, sy, sx, kernel_host, bias_host, leaky, precision, false,
+                         stream, true);
 }
 
 int demon_conv2d_nhwc(const float* in, float* out, int B, int H, int W, int Cin, int Cout, int kh, int kw, int sy, int sx,

@@ -33,6 +33,8 @@ def _stream():
 class _NetHandle:
     """RAII wrapper of a finalized `demon_net*`."""
 
+    _create = "demon_net_create"   # the C entry that lays out the plan (demon_b200.v2.networks: demon_net_create_v2)
+
     def __init__(self, weights, batch, refine_hw, precision):
         if not torch.cuda.is_available():
             raise RuntimeError("demon_b200 networks need a CUDA device (there is no CPU fallback)")
@@ -40,7 +42,7 @@ class _NetHandle:
         self._lib = lib
         self.ptr = ctypes.c_void_p()
         self.batch, self.refine_hw, self.precision = batch, refine_hw, precision
-        _lib.check(lib.demon_net_create(ctypes.byref(self.ptr), batch, refine_hw[0], refine_hw[1], PRECISIONS[precision]))
+        _lib.check(getattr(lib, self._create)(ctypes.byref(self.ptr), batch, refine_hw[0], refine_hw[1], PRECISIONS[precision]))
         for i in range(lib.demon_net_num_variables(self.ptr)):
             name = lib.demon_net_variable_name(self.ptr, i).decode()
             if name not in weights:
@@ -70,6 +72,8 @@ class _NetHandle:
 class Session:
     """Owner of the variables, in place of the tf.Session of the reference (examples/example.py:70-83)."""
 
+    _handle = _NetHandle   # the network the session's handles run (demon_b200.v2.networks: v2)
+
     def __init__(self, precision=DEFAULT_PRECISION):
         if precision not in PRECISIONS:
             raise ValueError("precision must be one of %s" % sorted(PRECISIONS))
@@ -78,7 +82,7 @@ class Session:
         self._nets = {}
 
     def load_weights(self, weights):
-        """weights: dict TF variable name -> numpy array in TF layout (see demon_b200.weights)."""
+        """weights: dict TF variable name -> numpy array in TF layout (see demon_b200.weights, demon_b200.v2.weights)."""
         self.weights = weights
         self._nets = {}
 
@@ -96,7 +100,7 @@ class Session:
             raise RuntimeError("Session.load_weights() has not been called")
         key = (int(batch), tuple(refine_hw))
         if key not in self._nets:
-            self._nets[key] = _NetHandle(self.weights, key[0], key[1], self.precision)
+            self._nets[key] = self._handle(self.weights, key[0], key[1], self.precision)
         return self._nets[key]
 
 

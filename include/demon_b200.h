@@ -304,6 +304,35 @@ int demon_pipeline_forward(demon_net* net, const float* image_pair, const float*
                            float* depth0, float* rotation, float* translation,
                            float* flow2, float* depth2, float* normal2, void* stream);
 
+/* ------------------------------------------------------------------------
+ * The v2 network (python/depthmotionnet/v2/networks.py, the one training/v2/training.py trains): a second plan over the
+ * same kernels, with TF 'same' padding, the dense5 layer of every trunk, the motion branch of v2 and a refinement block
+ * that also predicts normal0.  demon_net_set_weight / _num_variables / _variable_name / _finalize / _destroy, the profile
+ * and the debug entries take either kind of handle; every forward entry takes one kind only and returns DEMON_E_INVALID
+ * for the other (the entries above are v1's, the *_v2 entries below v2's).  float32 device entries only.
+ * ---------------------------------------------------------------------- */
+int demon_net_create_v2(demon_net** net, int batch, int refine_h, int refine_w, int precision);
+/* 1 for a handle of demon_net_create, 2 for one of demon_net_create_v2, 0 for NULL */
+int demon_net_variant(const demon_net* net);
+/* BootstrapNet.eval / IterativeNet.eval of v2 (v2/networks.py:48-75,127-172): arguments and outputs as the v1 entries */
+int demon_bootstrap_forward_v2(demon_net* net, const float* image_pair, const float* image2_2,
+                               float* flow5, float* flow2, float* depth2, float* normal2,
+                               float* rotation, float* translation, int data_format, void* stream);
+int demon_iterative_forward_v2(demon_net* net, const float* image_pair, const float* image2_2,
+                               const float* depth2_in, const float* normal2_in,
+                               const float* rotation_in, const float* translation_in,
+                               float* flow5, float* flow2, float* depth2, float* normal2,
+                               float* rotation, float* translation, int data_format, void* stream);
+/* RefinementNet.eval of v2 (v2/networks.py:204-228): image1 [B,3,H,W], depth2 [B,1,H/4,W/4] -> depth0 [B,1,H,W] and
+ * normal0 [B,3,H,W] (may be NULL).  normal2 is taken like the reference takes it and not read (may be NULL). */
+int demon_refine_forward_v2(demon_net* net, const float* image1, const float* depth2, const float* normal2,
+                            float* depth0, float* normal0, int data_format, void* stream);
+/* bootstrap, `iterations` x iterative and refinement of v2 in one call, as demon_pipeline_forward (one CUDA graph per
+ * distinct call, image2_2 may be NULL, any output may be NULL); normal0 [B,3,192,256].  channels_first only. */
+int demon_pipeline_forward_v2(demon_net* net, const float* image_pair, const float* image2_2, int iterations,
+                              float* depth0, float* normal0, float* rotation, float* translation,
+                              float* flow2, float* depth2, float* normal2, void* stream);
+
 /* The pipeline as examples/evaluation.py:225-255 runs it for an accuracy table: every intermediate prediction is kept.
  * Snapshot k = 0 is the bootstrap block's output, snapshot k = 1..iterations the output after iteration k; the arrays hold
  * S = iterations + 1 snapshots of the batch: flow2 [S,B,2,48,64], depth2 [S,B,1,48,64], normal2 [S,B,3,48,64],
@@ -402,6 +431,10 @@ int demon_debug_tc_timing(int enable, int64_t* host_out, int nblocks);
  * kernel family and tiling plan it gets (works without a device as long as the net was created -- creation needs one;
  * see tools/describe_plan.py for the offline variant). Returns bytes written. */
 int demon_debug_describe_layers(const demon_net* net, char* buf, int buflen);
+/* debug, no device needed: demon_debug_describe_layers of the plan that demon_net_create (variant 1) or
+ * demon_net_create_v2 (variant 2) would lay out for this batch, refinement size and precision.  A v2 conv's line carries
+ * "tap0 <dy> <dx> :" after the geometry: the input offset of its first tap, minus TF's 'same' padding before. */
+int demon_debug_describe_plan(int variant, int batch, int refine_h, int refine_w, int precision, char* buf, int buflen);
 
 /* debug, a test entry like demon_conv_slice_nhwc: while set, the stage-wise entries (demon_bootstrap_forward,
  * demon_iterative_forward, demon_refine_forward) copy every layer's input slice (cin_buf channels, just before the layer
@@ -430,6 +463,13 @@ double demon_debug_last_conv_ms(void);
 int demon_conv_slice_nhwc(const float* in, int in_pitch, float* out, int out_pitch, int B, int H, int W, int Cin, int Cout,
                           int kh, int kw, int sy, int sx, int deconv, const float* kernel_host, const float* bias_host,
                           int leaky, int precision, void* stream);
+
+/* demon_conv_slice_nhwc (no transposed conv) with TF's 'same' padding, the padding of the v2 network's convolutions: along
+ * each axis of size n with kernel k and stride s the first tap reads max((ceil(n/s) - 1) s + k - n, 0) / 2 pixels before the
+ * output's first one (demon_conv_slice_nhwc uses k / 2, caffe padding). */
+int demon_conv_slice_nhwc_same(const float* in, int in_pitch, float* out, int out_pitch, int B, int H, int W, int Cin, int Cout,
+                               int kh, int kw, int sy, int sx, const float* kernel_host, const float* bias_host,
+                               int leaky, int precision, void* stream);
 
 /* Standalone convolution entry used by tests to compare the tensor-core path with the fp32 SIMT path on
  * the same NHWC tensors.  in [B,H,W,Cin], kernel TF layout [kh,kw,cin,cout] (host), bias [cout] (host)
