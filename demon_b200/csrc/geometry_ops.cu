@@ -172,7 +172,8 @@ static int warp2d_launch(const T* in, const T* disp, T* out, int n, int c, int h
   DEMON_REQUIRE(border_mode == DEMON_BORDER_CLAMP || border_mode == DEMON_BORDER_VALUE, "warp2d: border_mode %d", border_mode);
   if ((int64_t)n * c * h * w == 0) return DEMON_OK;
   DEMON_REQUIRE(in && disp && out, "warp2d: null pointer");
-  DEMON_REQUIRE(h <= 65535 && n <= 65535, "warp2d: h and n must be <= 65535");
+  DEMON_REQUIRE(n <= 65535, "warp2d: n must be <= 65535 (got %d)", n);
+  DEMON_REQUIRE(h <= 65535, "warp2d: h must be <= 65535 (got %d)", h);
   dim3 grid(ceil_div(w, 128), h, n), block(128);
   cudaStream_t s = (cudaStream_t)stream;
   if (warp2d_fast<T>(in, disp, out, n, c, h, w, normalized, border_mode, border_value, s)) {
@@ -274,7 +275,8 @@ template <class T>
 static int depth_to_flow_launch(const T* depth, const T* intrinsics, const T* rotation, const T* translation, T* flow,
                                 int n, int h, int w, int rotation_format, int inverse_depth, int normalize_flow, void* stream) {
   DEMON_REQUIRE(rotation_format >= 0 && rotation_format <= 2, "depth_to_flow: rotation_format %d", rotation_format);
-  DEMON_REQUIRE(n >= 0 && h >= 0 && w >= 0 && n <= 65535, "depth_to_flow: bad size");
+  DEMON_REQUIRE(n >= 0 && h >= 0 && w >= 0, "depth_to_flow: negative size");
+  DEMON_REQUIRE(n <= 65535, "depth_to_flow: n must be <= 65535 (got %d)", n);
   if ((int64_t)n * h * w == 0) return DEMON_OK;
   DEMON_REQUIRE(depth && intrinsics && rotation && translation && flow, "depth_to_flow: null pointer");
   if (d2f_fast<T>(depth, intrinsics, rotation, translation, flow, n, h, w, rotation_format, inverse_depth, normalize_flow, (cudaStream_t)stream)) {
@@ -326,7 +328,8 @@ template <class T>
 static int flow_to_depth_launch(const T* flow, const T* intrinsics, const T* rotation, const T* translation, T* depth,
                                 int n, int h, int w, int rotation_format, int inverse_depth, int normalized_flow, void* stream) {
   DEMON_REQUIRE(rotation_format >= 0 && rotation_format <= 2, "flow_to_depth: rotation_format %d", rotation_format);
-  DEMON_REQUIRE(n >= 0 && h >= 0 && w >= 0 && n <= 65535, "flow_to_depth: bad size");
+  DEMON_REQUIRE(n >= 0 && h >= 0 && w >= 0, "flow_to_depth: negative size");
+  DEMON_REQUIRE(n <= 65535, "flow_to_depth: n must be <= 65535 (got %d)", n);
   if ((int64_t)n * h * w == 0) return DEMON_OK;
   DEMON_REQUIRE(flow && intrinsics && rotation && translation && depth, "flow_to_depth: null pointer");
   flow_to_depth_kernel<T><<<dim3(ceil_div(h * w, 128 * kF2DPixPerThread), n), 128, 0, (cudaStream_t)stream>>>(
@@ -479,7 +482,7 @@ static int median3x3_launch(const T* in, T* out, int64_t z, int h, int w, void* 
   if (z * h * w == 0) return DEMON_OK;
   DEMON_REQUIRE(in && out, "median3x3_downsample: null pointer");
   const int ho = (h + 1) / 2, wo = (w + 1) / 2;
-  DEMON_REQUIRE(ho <= 65535, "median3x3_downsample: height too large");
+  DEMON_REQUIRE(ho <= 65535, "median3x3_downsample: (h + 1) / 2 must be <= 65535 (got h = %d)", h);
   // (the last column 2*xo+7 <= W-1 needs no clamp when W is a multiple of 8)
   const bool fast = sizeof(T) == 4 && (w & 7) == 0 && w >= 256 && z * h * w < (1ll << 31) &&
                     ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
@@ -597,7 +600,7 @@ static int sig_launch(const T* in, T* out, int64_t z, int h, int w, const int* d
   DEMON_REQUIRE(num == 0 || (deltas && weights), "scale_invariant_gradient: null deltas/weights");
   if (z * h * w == 0) return DEMON_OK;
   DEMON_REQUIRE(in && out, "scale_invariant_gradient: null pointer");
-  DEMON_REQUIRE(h <= 65535, "scale_invariant_gradient: height too large");
+  DEMON_REQUIRE(h <= 65535, "scale_invariant_gradient: h must be <= 65535 (got %d)", h);
   SigParams<T> prm;
   prm.num = num;
   prm.eps = eps;

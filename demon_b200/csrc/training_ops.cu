@@ -81,7 +81,7 @@ int sig_grad_launch(const T* grad, const T* in, T* out, int64_t z, int h, int w,
   DEMON_REQUIRE(num == 0 || (deltas && weights), "scale_invariant_gradient_grad: null deltas/weights");
   if (z * h * w == 0) return DEMON_OK;
   DEMON_REQUIRE(in && grad && out, "scale_invariant_gradient_grad: null pointer");
-  DEMON_REQUIRE(h <= 65535, "scale_invariant_gradient_grad: height too large");
+  DEMON_REQUIRE(h <= 65535, "scale_invariant_gradient_grad: h must be <= 65535 (got %d)", h);
   SigGradParams<T> prm;
   prm.num = num;
   prm.eps = eps;
@@ -220,7 +220,7 @@ static int depth_to_normals_launch(const T* depth, const T* intrinsics, T* out, 
   DEMON_REQUIRE(z >= 0 && h >= 0 && w >= 0, "depth_to_normals: negative size");
   if (z * h * w == 0) return DEMON_OK;
   DEMON_REQUIRE(depth && intrinsics && out, "depth_to_normals: null pointer");
-  DEMON_REQUIRE(h <= 65535, "depth_to_normals: height too large");
+  DEMON_REQUIRE(h <= 65535, "depth_to_normals: h must be <= 65535 (got %d)", h);
   for (int64_t z0 = 0; z0 < z; z0 += 32768) {
     const int zn = (int)((z - z0 < 32768) ? (z - z0) : 32768);
     depth_to_normals_kernel<T><<<dim3(ceil_div(w, 128), h, zn), 128, 0, (cudaStream_t)stream>>>(depth, intrinsics, out, h, w, (int)z0, inverse_depth != 0);
