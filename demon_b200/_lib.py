@@ -38,6 +38,10 @@ PROTOTYPES = {
     "demon_replace_nonfinite_grad_f64": [_P, _P, _P, c_int64, _P],
     "demon_depth_to_normals_f32": [_P, _P, _P, c_int64, c_int, c_int, c_int, _P],
     "demon_depth_to_normals_f64": [_P, _P, _P, c_int64, c_int, c_int, c_int, _P],
+    "demon_correlation_f32": [_P, _P, _P] + [c_int] * 11 + [_P],
+    "demon_correlation_grad_f32": [_P] * 5 + [c_int] * 11 + [_P],
+    "demon_correlation_1d_f32": [_P, _P, _P] + [c_int] * 12 + [_P],
+    "demon_correlation_1d_grad_f32": [_P] * 5 + [c_int] * 12 + [_P],
     "demon_metric_workspace_bytes": [c_int, c_int64],
     "demon_depth_error_sums_f32": [_P, _P, c_int, c_int64, c_int, c_int, _P, _P, _P, _P, _P],
     "demon_depth_scale_factor": [_P, c_int, c_int, _P, _P],

@@ -11,7 +11,7 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB_DIR = os.path.join(_HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libdemon_b200.so")
 SOURCES = ["geometry_ops.cu", "metrics.cu", "evaluation.cu", "training_ops.cu", "conv_simt.cu", "conv_tc_halo.cu", "images.cu", "vis.cu", "dataset_tools.cu",
-           "net.cu"]
+           "correlation.cu", "net.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]

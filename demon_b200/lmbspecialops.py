@@ -338,3 +338,148 @@ class _SIGFunction(torch.autograd.Function):
 def scale_invariant_gradient_autograd(input, deltas=(1,), weights=(1.0,), epsilon=0.001):
     """scale_invariant_gradient on a torch CUDA tensor with the reference's analytic gradient attached."""
     return _SIGFunction.apply(input, tuple(deltas), tuple(weights), float(epsilon))
+
+
+# ---- FlowNet cost volumes (correlation.cc, correlation_1d.cc, correlation_cuda.cu, correlation_1d_cuda.cu) ----------------
+_CORR_TYPES = {"mult": 1, "subt": 2}   # DEMON_CORR_MULT, DEMON_CORR_SUBT
+
+
+def correlation_top_shape(shape, max_displacement, kernel_size, stride1=1, stride2=1, pad_size=0, one_d=False, single_dir=0):
+    """[N, top_channels, top_h, top_w] of correlation (one_d False, correlation.cc:62-77) or correlation_1d
+    (correlation_1d.cc:47-67): the top size is a ceil taken in float32, as the reference takes it."""
+    n, _, h, w = (int(s) for s in shape)
+    kr = (int(kernel_size) - 1) // 2
+    f = np.float32
+    tw = int(np.ceil(f(w + 2 * pad_size - 2 * (max_displacement + kr)) / f(stride1)))
+    th = int(np.ceil(f(h - 2 * kr) / f(stride1))) if one_d else int(np.ceil(f(h + 2 * pad_size - 2 * (max_displacement + kr)) / f(stride1)))
+    r = int(max_displacement) // int(stride2)
+    if one_d:
+        tc = r + 1 if single_dir != 0 else 2 * r + 1
+    else:
+        tc = (2 * r + 1) ** 2
+    return (n, tc, th, tw)
+
+
+def _corr_inputs(input1, input2):
+    s1, s2 = _shp(input1), _shp(input2)
+    if len(s1) != 4:
+        raise ValueError("Shape must be rank 4 but is rank %d" % len(s1))
+    if len(s2) != 4:
+        raise ValueError("Shape must be rank 4 but is rank %d" % len(s2))
+    if tuple(s1) != tuple(s2):
+        raise ValueError("Dimensions must be equal, but are %s and %s" % (tuple(s1), tuple(s2)))
+    _no_float64(input1)
+    _no_float64(input2)
+    a, was_np = _as_cuda(input1)
+    b, _ = _as_cuda(input2, torch.float32)
+    return a, b, was_np
+
+
+def _no_float64(x):
+    dt = x.dtype if isinstance(x, torch.Tensor) else np.asarray(x).dtype
+    if dt in (torch.float64, np.float64):
+        raise TypeError("correlation is registered for float32 only (T: {float}), got %s" % dt)
+
+
+def _corr_type(corr_type):
+    if corr_type not in _CORR_TYPES:
+        raise ValueError("corr_type must be 'mult' or 'subt', got %r" % (corr_type,))
+    return _CORR_TYPES[corr_type]
+
+
+def _corr_forward(one_d, input1, input2, kernel_size, max_displacement, stride1, stride2, pad_size, do_abs, corr_type, single_dir):
+    ct = _corr_type(corr_type)
+    a, b, was_np = _corr_inputs(input1, input2)
+    shape = correlation_top_shape(a.shape, max_displacement, kernel_size, stride1, stride2, pad_size, one_d, single_dir)
+    out = torch.empty(tuple(max(0, s) for s in shape), dtype=torch.float32, device=a.device)
+    n, c, h, w = a.shape
+    args = [a.data_ptr(), b.data_ptr(), out.data_ptr(), n, c, h, w, ct, int(kernel_size), int(max_displacement), int(stride1),
+            int(stride2), int(pad_size), int(bool(do_abs))]
+    if one_d:
+        _call("demon_correlation_1d_f32", *args, int(single_dir), _stream())
+    else:
+        _call("demon_correlation_f32", *args, _stream())
+    return _ret(out, was_np)
+
+
+def _corr_grad(one_d, gradient, input1, input2, kernel_size, max_displacement, stride1, stride2, pad_size, do_abs, corr_type,
+               single_dir):
+    ct = _corr_type(corr_type)
+    _no_float64(gradient)
+    a, b, was_np = _corr_inputs(input1, input2)
+    g, _ = _as_cuda(gradient, torch.float32)
+    shape = correlation_top_shape(a.shape, max_displacement, kernel_size, stride1, stride2, pad_size, one_d, single_dir)
+    if tuple(g.shape) != tuple(shape):
+        raise ValueError("Dimensions must be equal: gradient %s, output of the forward op %s" % (tuple(g.shape), tuple(shape)))
+    g1, g2 = torch.empty_like(a), torch.empty_like(b)
+    n, c, h, w = a.shape
+    args = [a.data_ptr(), b.data_ptr(), g.data_ptr(), g1.data_ptr(), g2.data_ptr(), n, c, h, w, ct, int(kernel_size),
+            int(max_displacement), int(stride1), int(stride2), int(pad_size), int(bool(do_abs))]
+    if one_d:
+        _call("demon_correlation_1d_grad_f32", *args, int(single_dir), _stream())
+    else:
+        _call("demon_correlation_grad_f32", *args, _stream())
+    return _ret(g1, was_np), _ret(g2, was_np)
+
+
+def correlation(input1, input2, max_displacement, kernel_size, stride1=1, stride2=1, pad_size=0, do_abs=False, corr_type="mult"):
+    """Correlation (correlation.cc:25-104): for every K x K patch of input1 (NCHW, float32) its correlation with the patches
+    of input2 displaced by (2R+1)^2 offsets, R = max_displacement // stride2 -> [N, (2R+1)^2, top_h, top_w].  'mult': mean
+    of the products, 'subt': mean of the absolute differences.  do_abs has no effect, as in the reference."""
+    return _corr_forward(False, input1, input2, kernel_size, max_displacement, stride1, stride2, pad_size, do_abs, corr_type, 0)
+
+
+def correlation_1d(input1, input2, max_displacement, kernel_size, stride1=1, stride2=1, pad_size=0, do_abs=False,
+                   corr_type="mult", single_dir=0):
+    """Correlation1D (correlation_1d.cc): correlation along x only, pad_size columns each side and no vertical padding.
+    single_dir 0: displacements -R..R times stride2; 1: 0..R; -1: the reference's -(R+1)..-1 (not -R..0), kept for
+    drop-in compatibility.  The reference reads before the start of a padded row there; those reads are 0 here."""
+    return _corr_forward(True, input1, input2, kernel_size, max_displacement, stride1, stride2, pad_size, do_abs, corr_type,
+                         single_dir)
+
+
+def correlation_grad(gradient, input1, input2, max_displacement, kernel_size, stride1=1, stride2=1, pad_size=0, do_abs=False,
+                     corr_type="mult"):
+    """CorrelationGrad (correlation.cc:106-128): (input1_grad, input2_grad) of `gradient` [N, top_c, top_h, top_w].  For
+    'subt' this is the reference's gradient, which takes the sign of input1 - input2 at the displaced position for both
+    inputs, not the derivative of the forward op."""
+    return _corr_grad(False, gradient, input1, input2, kernel_size, max_displacement, stride1, stride2, pad_size, do_abs,
+                      corr_type, 0)
+
+
+def correlation_1d_grad(gradient, input1, input2, max_displacement, kernel_size, stride1=1, stride2=1, pad_size=0, do_abs=False,
+                        corr_type="mult", single_dir=0):
+    """Correlation1DGrad (correlation_1d.cc:95-118): (input1_grad, input2_grad); see correlation_1d and correlation_grad."""
+    return _corr_grad(True, gradient, input1, input2, kernel_size, max_displacement, stride1, stride2, pad_size, do_abs,
+                      corr_type, single_dir)
+
+
+class _CorrelationFunction(torch.autograd.Function):
+    """torch.autograd counterpart of the reference binding's registered Correlation / Correlation1D gradients."""
+
+    @staticmethod
+    def forward(ctx, input1, input2, one_d, attrs):
+        ctx.save_for_backward(input1, input2)
+        ctx.one_d, ctx.attrs = one_d, attrs
+        return _corr_forward(one_d, input1, input2, *attrs)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        input1, input2 = ctx.saved_tensors
+        g1, g2 = _corr_grad(ctx.one_d, grad_out.contiguous(), input1, input2, *ctx.attrs)
+        return g1, g2, None, None
+
+
+def correlation_autograd(input1, input2, max_displacement, kernel_size, stride1=1, stride2=1, pad_size=0, do_abs=False,
+                         corr_type="mult"):
+    """correlation on torch CUDA tensors with the reference's gradient attached."""
+    attrs = (int(kernel_size), int(max_displacement), int(stride1), int(stride2), int(pad_size), bool(do_abs), corr_type, 0)
+    return _CorrelationFunction.apply(input1, input2, False, attrs)
+
+
+def correlation_1d_autograd(input1, input2, max_displacement, kernel_size, stride1=1, stride2=1, pad_size=0, do_abs=False,
+                            corr_type="mult", single_dir=0):
+    """correlation_1d on torch CUDA tensors with the reference's gradient attached."""
+    attrs = (int(kernel_size), int(max_displacement), int(stride1), int(stride2), int(pad_size), bool(do_abs), corr_type,
+             int(single_dir))
+    return _CorrelationFunction.apply(input1, input2, True, attrs)

@@ -118,6 +118,33 @@ int demon_depth_to_normals_f32(const float* depth, const float* intrinsics, floa
 int demon_depth_to_normals_f64(const double* depth, const double* intrinsics, double* output, int64_t z, int h, int w, int inverse_depth, void* stream);
 
 /* ------------------------------------------------------------------------
+ * FlowNet cost volumes: Correlation / Correlation1D and their gradients (correlation.cc, correlation_1d.cc,
+ * correlation_cuda.cu, correlation_1d_cuda.cu), float32 NCHW, bit for bit the reference's CUDA kernels (NaNs included).
+ * input1, input2 [n,c,h,w] -> output [n,top_c,top_h,top_w] with
+ *   top_w = ceil((float)(w + 2 pad_size - 2 (max_displacement + k)) / stride1), k = (kernel_size - 1) / 2,
+ *   top_h = the same over h for the 2D op, ceil((float)(h - 2 k) / stride1) for the 1D op (no vertical padding),
+ *   top_c = (2 R + 1)^2 (2D), 2 R + 1 (1D, single_dir 0) or R + 1 (1D, single_dir +-1), R = max_displacement / stride2.
+ * The 1D op's single_dir -1 uses the reference's displacements -(R+1) stride2 .. -stride2; a read outside the padded input
+ * is 0.  do_abs is accepted and has no effect, as in the reference.  Gradients: gradient [n,top_c,top_h,top_w] ->
+ * input1_grad, input2_grad [n,c,h,w], deterministic (no atomics).  DEMON_E_INVALID before any launch for an even or
+ * non-positive kernel_size, stride1 or stride2 < 1, a negative max_displacement or pad_size, single_dir not in {-1,0,1}
+ * or a top size < 1.  No workspace, no allocation; everything runs on `stream`.
+ * ---------------------------------------------------------------------- */
+#define DEMON_CORR_MULT 1   /* correlation_cuda.cu: enum CorrType {MULT = 1, SUBT = 2} */
+#define DEMON_CORR_SUBT 2
+int demon_correlation_f32(const float* input1, const float* input2, float* output, int n, int c, int h, int w, int corr_type,
+                          int kernel_size, int max_displacement, int stride1, int stride2, int pad_size, int do_abs, void* stream);
+int demon_correlation_grad_f32(const float* input1, const float* input2, const float* gradient, float* input1_grad, float* input2_grad,
+                               int n, int c, int h, int w, int corr_type, int kernel_size, int max_displacement, int stride1,
+                               int stride2, int pad_size, int do_abs, void* stream);
+int demon_correlation_1d_f32(const float* input1, const float* input2, float* output, int n, int c, int h, int w, int corr_type,
+                             int kernel_size, int max_displacement, int stride1, int stride2, int pad_size, int do_abs, int single_dir,
+                             void* stream);
+int demon_correlation_1d_grad_f32(const float* input1, const float* input2, const float* gradient, float* input1_grad,
+                                  float* input2_grad, int n, int c, int h, int w, int corr_type, int kernel_size, int max_displacement,
+                                  int stride1, int stride2, int pad_size, int do_abs, int single_dir, void* stream);
+
+/* ------------------------------------------------------------------------
  * Evaluation metrics on the device (python/depthmotionnet/evaluation/metrics.py; SURVEY.md section 8 f3).
  * One streaming pass per call; all pointers are device pointers, nothing synchronises.
  * ---------------------------------------------------------------------- */
