@@ -42,6 +42,12 @@ PROTOTYPES = {
     "demon_correlation_grad_f32": [_P] * 5 + [c_int] * 11 + [_P],
     "demon_correlation_1d_f32": [_P, _P, _P] + [c_int] * 12 + [_P],
     "demon_correlation_1d_grad_f32": [_P] * 5 + [c_int] * 12 + [_P],
+    "demon_flow_warp_f32": [_P, _P, _P] + [c_int] * 5 + [_P],
+    "demon_flow_warp_grad_workspace_bytes": [c_int, c_int, c_int],
+    "demon_flow_warp_grad_f32": [_P] * 5 + [c_int] * 4 + [_P, c_int64, _P],
+    "demon_flow_out_of_frame_f32": [_P, _P, _P, c_int, c_int, c_int, _P],
+    "demon_resample_f32": [_P, _P] + [c_int] * 8 + [_P],
+    "demon_resample_f64": [_P, _P] + [c_int] * 8 + [_P],
     "demon_metric_workspace_bytes": [c_int, c_int64],
     "demon_depth_error_sums_f32": [_P, _P, c_int, c_int64, c_int, c_int, _P, _P, _P, _P, _P],
     "demon_depth_scale_factor": [_P, c_int, c_int, _P, _P],
@@ -116,6 +122,7 @@ _RESTYPES = {
     "demon_net_layer_name": c_char_p,
     "demon_net_workspace_bytes": c_int64,
     "demon_metric_workspace_bytes": c_int64,
+    "demon_flow_warp_grad_workspace_bytes": c_int64,
     "demon_point_cloud_scratch_bytes": c_int64,
     "demon_last_error": c_char_p,
     "demon_version": c_char_p,

@@ -483,3 +483,130 @@ def correlation_1d_autograd(input1, input2, max_displacement, kernel_size, strid
     attrs = (int(kernel_size), int(max_displacement), int(stride1), int(stride2), int(pad_size), bool(do_abs), corr_type,
              int(single_dir))
     return _CorrelationFunction.apply(input1, input2, True, attrs)
+
+
+# ---- FlowNet warping and resampling (flowwarp.cc, flowwarp_cuda.cu, flow_out_of_frame.cc, resample.cc, resample_cuda.cu) ----
+_FLOW_WARP_FILL = {"zero": 1, "not_a_number": 2}              # DEMON_FLOW_WARP_ZERO, DEMON_FLOW_WARP_NAN
+_RESAMPLE_TYPES = {"NEAREST": 1, "CUBIC": 2, "LINEAR": 3}     # DEMON_LMB_RESAMPLE_*
+
+
+def _float32_only(op, *xs):
+    for x in xs:
+        dt = x.dtype if isinstance(x, torch.Tensor) else np.asarray(x).dtype
+        if dt in (torch.float64, np.float64):
+            raise TypeError("%s is registered for float32 only (T: {float}), got %s" % (op, dt))
+
+
+def _rank4(*shapes):
+    for s in shapes:
+        if len(s) != 4:
+            raise ValueError("Shape must be rank 4 but is rank %d" % len(s))
+
+
+def _warp_inputs(image, flow):
+    ishape, fshape = _shp(image), _shp(flow)
+    _rank4(ishape, fshape)
+    if tuple(ishape[2:]) != tuple(fshape[2:]):
+        raise ValueError("Dimensions must be equal, but are %s and %s" % (tuple(ishape[2:]), tuple(fshape[2:])))
+    if ishape[0] != fshape[0]:
+        raise ValueError("Dimensions must be equal, but are %d and %d" % (ishape[0], fshape[0]))
+    if fshape[1] != 2:
+        raise ValueError("Dimension must be 2 but is %d" % fshape[1])
+    return ishape
+
+
+def flow_warp(image, flow, fill_parameter="zero"):
+    """FlowWarp (flowwarp.cc:29-78): image [N,C,H,W] sampled bilinearly at (x + flow_x, y + flow_y), float32 NCHW.
+    Positions out of the image (a NaN flow included) get the fill: 0 for 'zero', and for 'not_a_number' the NaN with bits
+    0xFFE00000 that the reference's GPU kernel writes."""
+    if fill_parameter not in _FLOW_WARP_FILL:
+        raise ValueError("fill_parameter must be 'zero' or 'not_a_number', got %r" % (fill_parameter,))
+    n, c, h, w = _warp_inputs(image, flow)
+    _float32_only("flow_warp", image, flow)
+    img, was_np = _as_cuda(image, torch.float32)
+    fl, _ = _as_cuda(flow, torch.float32)
+    out = torch.empty_like(img)
+    _call("demon_flow_warp_f32", img.data_ptr(), fl.data_ptr(), out.data_ptr(), n, c, h, w, _FLOW_WARP_FILL[fill_parameter],
+          _stream())
+    return _ret(out, was_np)
+
+
+def flow_warp_grad(image, flow, gradient):
+    """FlowWarpGrad (flowwarp.cc:193-208): (image_grad [N,C,H,W], flow_grad [N,2,H,W]) of `gradient` [N,C,H,W].
+    image_grad is deterministic: the reference CPU kernel's sum, in its order.  flow_grad is the reference's formula, which
+    at the clamped last row and column is not the derivative of flow_warp."""
+    n, c, h, w = _warp_inputs(image, flow)
+    gshape = _shp(gradient)
+    _rank4(gshape)
+    if tuple(gshape) != (n, c, h, w):
+        raise ValueError("Dimensions must be equal: gradient %s, image %s" % (tuple(gshape), (n, c, h, w)))
+    _float32_only("flow_warp_grad", image, flow, gradient)
+    img, was_np = _as_cuda(image, torch.float32)
+    fl, _ = _as_cuda(flow, torch.float32)
+    g, _ = _as_cuda(gradient, torch.float32)
+    lib = _lib.load()
+    nbytes = lib.demon_flow_warp_grad_workspace_bytes(n, h, w)
+    if nbytes < 0:
+        _lib.check(-1)
+    ws = torch.empty(max(1, nbytes), dtype=torch.uint8, device=img.device)   # the caching allocator aligns to 512 bytes
+    image_grad = torch.empty_like(img)
+    flow_grad = torch.empty_like(fl)
+    _call("demon_flow_warp_grad_f32", img.data_ptr(), fl.data_ptr(), g.data_ptr(), image_grad.data_ptr(), flow_grad.data_ptr(),
+          n, c, h, w, ws.data_ptr(), nbytes, _stream())
+    return _ret(image_grad, was_np), _ret(flow_grad, was_np)
+
+
+def flow_out_of_frame(flow, occ):
+    """FlowOutOfFrame (flow_out_of_frame.cc): [N,1,H,W], `occ` (N*H*W elements) where x + flow rounded half away from zero
+    lies in the image, 1 elsewhere; a NaN occ stays.  flow must be [N,2,H,W] (the reference does not check C)."""
+    fshape = _shp(flow)
+    _rank4(fshape)
+    if fshape[1] != 2:
+        raise ValueError("Dimension must be 2 but is %d" % fshape[1])
+    n, _, h, w = fshape
+    if _prod(_shp(occ)) != n * h * w:
+        raise ValueError("occ must have N*H*W = %d elements, has %d" % (n * h * w, _prod(_shp(occ))))
+    _float32_only("flow_out_of_frame", flow, occ)
+    fl, was_np = _as_cuda(flow, torch.float32)
+    oc, _ = _as_cuda(occ, torch.float32)
+    out = torch.empty((n, 1, h, w), dtype=torch.float32, device=fl.device)
+    _call("demon_flow_out_of_frame_f32", fl.data_ptr(), oc.data_ptr(), out.data_ptr(), n, h, w, _stream())
+    return _ret(out, was_np)
+
+
+def resample(input, width, height, antialias=True, type="LINEAR"):
+    """Resample (resample.cc, resample_cuda.cu): input [N,C,H,W] (float32 or float64) -> [N,C,height,width], 'NEAREST',
+    'LINEAR' or 'CUBIC', antialiased when `antialias` and either axis downsamples.  Bit for bit the reference's kernels,
+    except that NEAREST clamps its source pixel to the image where the reference reads outside it."""
+    if type not in _RESAMPLE_TYPES:
+        raise ValueError("type must be one of 'NEAREST', 'CUBIC', 'LINEAR', got %r" % (type,))
+    if int(width) < 1 or int(height) < 1:
+        raise ValueError("width and height must be >= 1, got %d and %d" % (int(width), int(height)))
+    s = _shp(input)
+    _rank4(s)
+    x, was_np = _as_cuda(input)
+    n, c, ih, iw = x.shape
+    out = torch.empty((n, c, int(height), int(width)), dtype=x.dtype, device=x.device)
+    _call("demon_resample" + _sfx(x), x.data_ptr(), out.data_ptr(), n, c, ih, iw, int(height), int(width), int(bool(antialias)),
+          _RESAMPLE_TYPES[type], _stream())
+    return _ret(out, was_np)
+
+
+class _FlowWarpFunction(torch.autograd.Function):
+    """torch.autograd counterpart of the reference binding's registered FlowWarp gradient (__init__.py:336-341)."""
+
+    @staticmethod
+    def forward(ctx, image, flow, fill_parameter):
+        ctx.save_for_backward(image, flow)
+        return flow_warp(image, flow, fill_parameter)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        image, flow = ctx.saved_tensors
+        image_grad, flow_grad = flow_warp_grad(image, flow, grad_out.contiguous())
+        return image_grad, flow_grad, None
+
+
+def flow_warp_autograd(image, flow, fill_parameter="zero"):
+    """flow_warp on torch CUDA tensors with the reference's gradient attached."""
+    return _FlowWarpFunction.apply(image, flow, fill_parameter)

@@ -145,6 +145,49 @@ int demon_correlation_1d_grad_f32(const float* input1, const float* input2, cons
                                   int stride1, int stride2, int pad_size, int do_abs, int single_dir, void* stream);
 
 /* ------------------------------------------------------------------------
+ * FlowNet warping: FlowWarp / FlowWarpGrad (flowwarp.cc, flowwarp_cuda.cu) and FlowOutOfFrame (flow_out_of_frame.cc),
+ * float32 NCHW.  image [n,c,h,w], flow [n,2,h,w] (x then y displacement in pixels).
+ *   flow_warp       warped [n,c,h,w]: bilinear at (x + fx, y + fy), bit for bit the reference's GPU kernel; out of frame
+ *                   (a NaN flow included) the fill: 0 (DEMON_FLOW_WARP_ZERO) or the NaN with bits 0xFFE00000
+ *                   (DEMON_FLOW_WARP_NAN).
+ *   flow_warp_grad  gradient [n,c,h,w] -> image_grad [n,c,h,w], flow_grad [n,2,h,w].  flow_grad is bit for bit the
+ *                   reference's GPU kernel (its formula, which at the clamped last row and column is not the derivative
+ *                   of the forward op).  image_grad is bit for bit the reference's CPU kernel, whose GPU kernel adds
+ *                   the same products with atomics in scheduling order.  workspace: device memory of at least
+ *                   demon_flow_warp_grad_workspace_bytes(n, h, w) bytes, 256-byte aligned; that query returns -1 (and
+ *                   sets the error) for n*h*w >= 2^31 - 1 or when the device cannot be queried.
+ *   flow_out_of_frame  occ [n*h*w] -> output [n,1,h,w], bit for bit the reference's CPU kernel: occ where the rounded
+ *                   target (x + fx, y + fy) lies in the image, else 1; a NaN occ passes through; a NaN, infinite or
+ *                   out-of-int-range target is out of frame.
+ * Deterministic: no float atomics, the same bits on every call.  DEMON_E_INVALID before any launch for a negative size,
+ * an unknown fill or too small a workspace.  No allocation; everything runs on `stream`.
+ * ---------------------------------------------------------------------- */
+#define DEMON_FLOW_WARP_ZERO 1   /* flowwarp_cuda.cu: #define ZERO 1, NOT_A_NUMBER 2 */
+#define DEMON_FLOW_WARP_NAN 2
+int demon_flow_warp_f32(const float* image, const float* flow, float* warped, int n, int c, int h, int w, int fill, void* stream);
+int64_t demon_flow_warp_grad_workspace_bytes(int n, int h, int w);
+int demon_flow_warp_grad_f32(const float* image, const float* flow, const float* gradient, float* image_grad, float* flow_grad, int n, int c,
+                             int h, int w, void* workspace, int64_t workspace_bytes, void* stream);
+int demon_flow_out_of_frame_f32(const float* flow, const float* occ, float* output, int n, int h, int w, void* stream);
+
+/* ------------------------------------------------------------------------
+ * Resample (resample.cc, resample_cuda.cu): input [n,c,in_h,in_w] -> output [n,c,out_h,out_w], float32 and float64, bit
+ * for bit the reference's NearestNeighborKernel / InterpolationKernel: scale fx = in_w / out_w, fy = in_h / out_h in
+ * float, source position (x fx + fy/2 - 0.5, y fy + fx/2 - 0.5) (the reference's swapped half offsets), LINEAR (triangle)
+ * or CUBIC (Keys, a = -0.5) weights, antialiased on both axes when `antialias` and either axis downsamples.  One
+ * deviation: NEAREST clamps its source pixel to the image, where the reference reads outside it (fy / 2 >~ fx).
+ * DEMON_E_INVALID for an unknown type or an output side < 1.  Deterministic, no allocation, runs on `stream`.
+ * ---------------------------------------------------------------------- */
+/* resample_cuda.cu: enum InterpolationType {NEAREST = 1, CUBIC = 2, LINEAR = 3}; DEMON_RESAMPLE_* are the image resize's */
+#define DEMON_LMB_RESAMPLE_NEAREST 1
+#define DEMON_LMB_RESAMPLE_CUBIC 2
+#define DEMON_LMB_RESAMPLE_LINEAR 3
+int demon_resample_f32(const float* input, float* output, int n, int c, int in_h, int in_w, int out_h, int out_w, int antialias, int type,
+                       void* stream);
+int demon_resample_f64(const double* input, double* output, int n, int c, int in_h, int in_w, int out_h, int out_w, int antialias, int type,
+                       void* stream);
+
+/* ------------------------------------------------------------------------
  * Evaluation metrics on the device (python/depthmotionnet/evaluation/metrics.py; SURVEY.md section 8 f3).
  * One streaming pass per call; all pointers are device pointers, nothing synchronises.
  * ---------------------------------------------------------------------- */
