@@ -48,6 +48,16 @@ PROTOTYPES = {
     "demon_flow_out_of_frame_f32": [_P, _P, _P, c_int, c_int, c_int, _P],
     "demon_resample_f32": [_P, _P] + [c_int] * 8 + [_P],
     "demon_resample_f64": [_P, _P] + [c_int] * 8 + [_P],
+    "demon_loss_workspace_bytes": [_P, c_int, c_int, c_int],
+    "demon_loss_forward_f32": [_P, c_int, _P, c_int64, _P],
+    "demon_loss_forward_f64": [_P, c_int, _P, c_int64, _P],
+    "demon_loss_backward_f32": [_P, c_int, _P, c_int64, _P],
+    "demon_loss_backward_f64": [_P, c_int, _P, c_int64, _P],
+    "demon_confidence_map_f32": [_P, _P, _P, c_int64, c_double, _P],
+    "demon_confidence_map_f64": [_P, _P, _P, c_int64, c_double, _P],
+    "demon_loss_ground_truth_workspace_bytes": [c_int, c_int, c_int, c_int],
+    "demon_loss_ground_truth_f32": [_P] * 4 + [c_int] * 3 + [_P] * 9 + [_P, c_int64, _P],
+    "demon_loss_ground_truth_f64": [_P] * 4 + [c_int] * 3 + [_P] * 9 + [_P, c_int64, _P],
     "demon_metric_workspace_bytes": [c_int, c_int64],
     "demon_depth_error_sums_f32": [_P, _P, c_int, c_int64, c_int, c_int, _P, _P, _P, _P, _P],
     "demon_depth_scale_factor": [_P, c_int, c_int, _P, _P],
@@ -122,6 +132,8 @@ _RESTYPES = {
     "demon_net_layer_name": c_char_p,
     "demon_net_workspace_bytes": c_int64,
     "demon_metric_workspace_bytes": c_int64,
+    "demon_loss_workspace_bytes": c_int64,
+    "demon_loss_ground_truth_workspace_bytes": c_int64,
     "demon_flow_warp_grad_workspace_bytes": c_int64,
     "demon_point_cloud_scratch_bytes": c_int64,
     "demon_last_error": c_char_p,

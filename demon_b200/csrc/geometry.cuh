@@ -264,4 +264,98 @@ __device__ __forceinline__ T median9_reference_order(T v[9]) {
   return v[4];
 }
 
+// ---- scale_invariant_gradient: one delta's term of one axis, scaleinvariantgradient.cc:174-189 --------------------
+// wgt * (vn - v0) / (|v0| + |vn| + eps); vn is the neighbour at +delta, or v0 itself where that lies outside the image.
+template <class T>
+__device__ __forceinline__ T sig_term(T v0, T vn, T wgt, T eps) {
+  return fdiv(fmul(wgt, fsub(vn, v0)), fadd(fadd(tabs(v0), tabs(vn)), eps));
+}
+
+// its partial derivatives by the centre and by the neighbour, scaleinvariantgradient.cc:247-268
+template <class T>
+__device__ __forceinline__ T sig_dcenter(T c, T n, T eps) {
+  const T sum_abs = fadd(fadd(tabs(c), tabs(n)), eps);
+  const T sign = (c < 0) ? (T)1 : (T)-1;
+  return fadd(fdiv((T)-1, sum_abs), fdiv(fmul(sign, fsub(n, c)), fmul(sum_abs, sum_abs)));
+}
+template <class T>
+__device__ __forceinline__ T sig_dneighbour(T c, T n, T eps) {
+  const T sum_abs = fadd(fadd(tabs(c), tabs(n)), eps);
+  const T sign = (n < 0) ? (T)1 : (T)-1;
+  return fadd(fdiv((T)1, sum_abs), fdiv(fmul(sign, fsub(n, c)), fmul(sum_abs, sum_abs)));
+}
+
+// ---- depth_to_normals (depthtonormals.cc:147-238) --------------------------------------------------------------------------
+// inv_K of K = [[fx*W, 0, cx*W], [0, fy*H, cy*H], [0, 0, 1]] the way Eigen 3.3 inverts a fixed 3x3 matrix
+// (Eigen/src/LU/InverseImpl.h, compute_inverse<.,.,3>: cofactors times 1/det), restricted to the four entries the op reads.
+template <class T>
+struct D2NCamera { T i00, i02, i11, i12; };
+
+template <class T>
+__device__ __forceinline__ void d2n_point(T p[3], int x, int y, T depth, const D2NCamera<T>& c) {   // compute3dPoint, depthtonormals.cc:95-101
+  p[0] = fmul(fadd(fmul(fadd((T)x, (T)0.5), c.i00), c.i02), depth);
+  p[1] = fmul(fadd(fmul(fadd((T)y, (T)0.5), c.i11), c.i12), depth);
+  p[2] = depth;
+}
+template <class T>
+__device__ __forceinline__ void d2n_cross(T r[3], const T a[3], const T b[3]) {
+  r[0] = fsub(fmul(a[1], b[2]), fmul(a[2], b[1]));
+  r[1] = fsub(fmul(a[2], b[0]), fmul(a[0], b[2]));
+  r[2] = fsub(fmul(a[0], b[1]), fmul(a[1], b[0]));
+}
+template <class T>
+__device__ __forceinline__ void d2n_normalize(T v[3]) {   // MatrixBase::normalize(): z = squaredNorm(); if (z > 0) v /= sqrt(z)
+  const T z = fadd(fadd(fmul(v[0], v[0]), fmul(v[1], v[1])), fmul(v[2], v[2]));
+  if (z > (T)0) {
+    const T n = sqrt(z);   // IEEE sqrt (sqrt.rn for float: no -use_fast_math in this build)
+    v[0] = fdiv(v[0], n); v[1] = fdiv(v[1], n); v[2] = fdiv(v[2], n);
+  }
+}
+
+// The normal of pixel (x, y) of the depth plane dm [H][W] with the sample's normalised intrinsics k[4]; NaN on the border
+// and next to a non-positive / non-finite depth.
+template <class T>
+__device__ __forceinline__ void d2n_pixel(T nrm[3], const T* __restrict__ dm, const T* __restrict__ k, int x, int y, int H, int W,
+                                          bool inverse_depth) {
+  const T nan = (T)NAN;
+  nrm[0] = nan; nrm[1] = nan; nrm[2] = nan;
+  if (x == 0 || y == 0 || x == W - 1 || y == H - 1) return;
+  const size_t i = (size_t)y * W + x;
+  T d = __ldg(dm + i), d_y0 = __ldg(dm + i - W), d_x0 = __ldg(dm + i - 1), d_y1 = __ldg(dm + i + W), d_x1 = __ldg(dm + i + 1);
+  if (inverse_depth) { d = fdiv((T)1, d); d_y0 = fdiv((T)1, d_y0); d_x0 = fdiv((T)1, d_x0); d_y1 = fdiv((T)1, d_y1); d_x1 = fdiv((T)1, d_x1); }
+  const bool bad = d <= 0 || !isfinite(d) || d_y0 <= 0 || !isfinite(d_y0) || d_x0 <= 0 || !isfinite(d_x0) || d_y1 <= 0 || !isfinite(d_y1) ||
+                   d_x1 <= 0 || !isfinite(d_x1);
+  if (bad) return;
+  D2NCamera<T> c;
+  {
+    const T a = fmul(__ldg(k + 0), (T)W), b = fmul(__ldg(k + 1), (T)H), cx = fmul(__ldg(k + 2), (T)W), cy = fmul(__ldg(k + 3), (T)H);
+    // cofactors of column 0: (b*1 - cy*0, 0*cx - 1*0, 0*cy - cx*b); det = (c0*a + c1*0) + c2*0; invdet = 1 / det
+    const T c0 = fsub(fmul(b, (T)1), fmul(cy, (T)0));
+    const T c1 = fsub(fmul((T)0, cx), fmul((T)1, (T)0));
+    const T c2 = fsub(fmul((T)0, cy), fmul(cx, b));
+    const T det = fadd(fadd(fmul(c0, a), fmul(c1, (T)0)), fmul(c2, (T)0));
+    const T invdet = fdiv((T)1, det);
+    c.i00 = fmul(c0, invdet);                                                     // result.row(0) = cofactors_col0 * invdet
+    c.i02 = fmul(c2, invdet);
+    c.i11 = fmul(fsub(fmul((T)1, a), fmul((T)0, cx)), invdet);                    // cofactor<1,1> = m22*m00 - m20*m02
+    c.i12 = fmul(fsub(fmul(cx, (T)0), fmul(a, cy)), invdet);                      // cofactor<2,1> = m02*m10 - m00*m12
+  }
+  T p[3], p_y0[3], p_x0[3], p_y1[3], p_x1[3];
+  d2n_point(p, x, y, d, c);
+  d2n_point(p_y0, x, y - 1, d_y0, c);
+  d2n_point(p_x0, x - 1, y, d_x0, c);
+  d2n_point(p_y1, x, y + 1, d_y1, c);
+  d2n_point(p_x1, x + 1, y, d_x1, c);
+  T a1[3], b1[3], a0[3], b0[3], v1[3], v0[3];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) { a1[j] = fsub(p[j], p_x1[j]); b1[j] = fsub(p_y1[j], p[j]); a0[j] = fsub(p[j], p_x0[j]); b0[j] = fsub(p_y0[j], p[j]); }
+  d2n_cross(v1, a1, b1);
+  d2n_cross(v0, a0, b0);
+  d2n_normalize(v1);
+  d2n_normalize(v0);
+  T v[3] = {fadd(v1[0], v0[0]), fadd(v1[1], v0[1]), fadd(v1[2], v0[2])};
+  d2n_normalize(v);
+  nrm[0] = v[0]; nrm[1] = v[1]; nrm[2] = v[2];
+}
+
 }  // namespace demon

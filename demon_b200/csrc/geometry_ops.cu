@@ -527,8 +527,8 @@ __global__ void __launch_bounds__(128) sig_kernel(const T* __restrict__ in, T* _
     const T wgt = prm.weights[c];
     const T vx = (x + d >= 0 && x + d < W) ? __ldg(p + (size_t)y * W + x + d) : v0;
     const T vy = (y + d >= 0 && y + d < H) ? __ldg(p + (size_t)(y + d) * W + x) : v0;
-    gx = fadd(gx, fdiv(fmul(wgt, fsub(vx, v0)), fadd(fadd(tabs(v0), tabs(vx)), prm.eps)));
-    gy = fadd(gy, fdiv(fmul(wgt, fsub(vy, v0)), fadd(fadd(tabs(v0), tabs(vy)), prm.eps)));
+    gx = fadd(gx, sig_term(v0, vx, wgt, prm.eps));
+    gy = fadd(gy, sig_term(v0, vy, wgt, prm.eps));
   }
   T* o = out + z * 2 * hw + (size_t)y * W + x;
   o[0] = gx;
@@ -575,8 +575,8 @@ __global__ void __launch_bounds__(128) sig_v4_kernel(const float* __restrict__ i
     }
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      gx[k] = fadd(gx[k], fdiv(fmul(wgt, fsub(vx[k], v0[k])), fadd(fadd(tabs(v0[k]), tabs(vx[k])), prm.eps)));
-      gy[k] = fadd(gy[k], fdiv(fmul(wgt, fsub(vy[k], v0[k])), fadd(fadd(tabs(v0[k]), tabs(vy[k])), prm.eps)));
+      gx[k] = fadd(gx[k], sig_term(v0[k], vx[k], wgt, prm.eps));
+      gy[k] = fadd(gy[k], sig_term(v0[k], vy[k], wgt, prm.eps));
     }
   }
   float* o = out + z * 2 * hw + y * W + x;

@@ -188,6 +188,62 @@ int demon_resample_f64(const double* input, double* output, int n, int c, int in
                        void* stream);
 
 /* ------------------------------------------------------------------------
+ * DeMoN v2's training losses (python/depthmotionnet/v2/losses.py) and their gradients (csrc/losses.cu).
+ * All tensor pointers are device pointers of the entry's T (float for _f32, double for _f64), NCHW and contiguous.
+ * Nothing allocates or synchronises; scratch comes from the caller.
+ * ---------------------------------------------------------------------- */
+#define DEMON_LOSS_L2   0   /* pointwise_l2_loss: mean of sqrt(sum_c d_c^2 + eps), d = replace_nonfinite(pr - gt)       */
+#define DEMON_LOSS_SIG  1   /* pointwise_l2_loss of the prediction's 5-delta SIG stack (never stored) against gt's     */
+#define DEMON_LOSS_L1   2   /* l1_loss: sum of sqrt(x^2 + eps), x = pr - gt (pr alone when gt is NULL)                */
+#define DEMON_LOSS_MAX_TERMS 8
+typedef struct demon_loss_term {
+  int kind;                 /* DEMON_LOSS_*                                                                            */
+  int c;                    /* L2: channels summed per pixel; L1: elements per row; SIG: 1                             */
+  int h, w;                 /* L2, SIG: plane size                                                                     */
+  int gt_plane;             /* SIG: gt is a plane [n,h,w] whose SIG stack is taken on the fly (eps gt_sig_eps);
+                               otherwise gt is the stack [n,10,h,w], channels (2i, 2i+1) = (x, y) of delta 2^i          */
+  int accumulate;           /* backward: 0 writes grad, 1 adds to it                                                   */
+  int64_t n;                /* L2: samples [n,c,h,w]; SIG: planes [n,h,w] (a flow [N,2,h,w] is 2N planes); L1: rows   */
+  const void* pr;
+  const void* gt;
+  double eps;               /* the loss epsilon, converted to T                                                        */
+  double sig_eps;           /* SIG: epsilon of the prediction's SIG (converted to T)                                   */
+  double gt_sig_eps;        /* SIG with gt_plane: epsilon of the ground truth's SIG                                    */
+  double weight;            /* the weight, converted to T, unless weight_dev                                           */
+  const void* weight_dev;   /* device T scalar or NULL                                                                  */
+  void* out;                /* device T scalar: T(mean) * weight (L1: T(sum) * weight), or NULL                         */
+  void* out0;               /* device T scalar: the mean (sum) with eps 0, not weighted, or NULL                        */
+  void* terms;              /* L2: the per-pixel terms [n,h,w] (eps), or NULL                                          */
+  const void* grad_out;     /* backward: device T scalar, the upstream gradient of `out` (NULL: 0)                     */
+  void* grad;               /* backward: d(out)/d(pr), pr's shape; NULL: no gradient for this term                    */
+} demon_loss_term;
+/* Scratch bytes of the forward entries (backward = 0) or the backward entries (backward = 1) for this table; -1 if invalid. */
+int64_t demon_loss_workspace_bytes(const demon_loss_term* terms, int num, int elem_size, int backward);
+/* Every term's `out` and `out0` in two launches.  Sums are double in an order fixed by the shapes: same bits every call. */
+int demon_loss_forward_f32(const demon_loss_term* terms, int num, void* workspace, int64_t workspace_bytes, void* stream);
+int demon_loss_forward_f64(const demon_loss_term* terms, int num, void* workspace, int64_t workspace_bytes, void* stream);
+/* Each term's gradient into its `grad`, terms in table order (one launch per L2 / L1 term, two per SIG term).  L2:
+ * g*w*d_c/(M*t), 0 where d_c is not finite; L1: g*w*x/sqrt(x^2+eps); SIG: the same per SIG channel, through each delta's
+ * SIG derivative (ScaleInvariantGradientGrad's, summed over the deltas). */
+int demon_loss_backward_f32(const demon_loss_term* terms, int num, void* workspace, int64_t workspace_bytes, void* stream);
+int demon_loss_backward_f64(const demon_loss_term* terms, int num, void* workspace, int64_t workspace_bytes, void* stream);
+/* compute_confidence_map: out = T(exp((double)(T(-scale) * |pr - gt|))), exp in double and rounded once */
+int demon_confidence_map_f32(const float* pr, const float* gt, float* out, int64_t size, double scale, void* stream);
+int demon_confidence_map_f64(const double* pr, const double* gt, double* out, int64_t size, double scale, void* stream);
+/* prepare_ground_truth_tensors for depth [n,h,w] (inverse depth), intrinsics [n,4], rotation [n,3] (angle axis),
+ * translation [n,3]: depth2 [n,h2,w2], flow0/2/5 [n,2,.,.], normal0/2 [n,3,.,.], depth0_sig / depth2_sig [n,10,.,.],
+ * flow2_sig [2n,10,h2,w2] (level k has the size (s+1)/2 applied k times).  Six launches (five medians, one for the rest);
+ * each output bit for bit the composition of the standalone ops.  Scratch: demon_loss_ground_truth_workspace_bytes. */
+int64_t demon_loss_ground_truth_workspace_bytes(int n, int h, int w, int elem_size);
+int demon_loss_ground_truth_f32(const float* depth, const float* intrinsics, const float* rotation, const float* translation, int n, int h, int w,
+                                float* depth2, float* flow0, float* flow2, float* flow5, float* normal0, float* normal2, float* depth0_sig,
+                                float* depth2_sig, float* flow2_sig, void* workspace, int64_t workspace_bytes, void* stream);
+int demon_loss_ground_truth_f64(const double* depth, const double* intrinsics, const double* rotation, const double* translation, int n, int h,
+                                int w, double* depth2, double* flow0, double* flow2, double* flow5, double* normal0, double* normal2,
+                                double* depth0_sig, double* depth2_sig, double* flow2_sig, void* workspace, int64_t workspace_bytes,
+                                void* stream);
+
+/* ------------------------------------------------------------------------
  * Evaluation metrics on the device (python/depthmotionnet/evaluation/metrics.py; SURVEY.md section 8 f3).
  * One streaming pass per call; all pointers are device pointers, nothing synchronises.
  * ---------------------------------------------------------------------- */
