@@ -9,6 +9,8 @@
 // CUDA's logf / log10f, within 1-2 ulp of numpy's), accumulation is double in a FIXED order (per-thread strided partial
 // sums -> warp shuffle tree -> per-CTA slots -> one warp folds the slots in index order), so results are deterministic
 // run to run; the reference accumulates pairwise in float32, which is where the documented 1e-5 tolerance comes from.
+// Promotion is NumPy 1.x's: the gt divide and the prediction's scale are float32, and the ratio thresholds compare the
+// float32 |ld| with float32(log t), which is what logf(t) gives here (DESIGN.md §3.4, tests/test_gpu_metrics_oracle.py).
 #include "common.cuh"
 #include <cmath>
 
@@ -253,7 +255,8 @@ using namespace demon;
 extern "C" {
 
 int64_t demon_metric_workspace_bytes(int n, int64_t hw) {
-  if (n <= 0 || hw <= 0) return 0;
+  // hw == 0 still launches one slot per sample, which writes its (zero) partial sums
+  if (n <= 0 || hw < 0) return 0;
   return (int64_t)n * slots_for(hw) * kSums * (int64_t)sizeof(double);
 }
 

@@ -10,8 +10,9 @@ arrays in, Python floats out -- plus batched forms that keep everything on the G
 One streaming pass over prediction and ground truth yields all sums the eleven distances and the least-squares scale
 factor need; the scale factor itself is computed on the device, so `evaluate_depth` is two kernel passes and one
 [n,16]-double copy.  Tolerance against the numpy reference: 1e-5 relative (float32 pairwise summation there, double
-accumulation here; `logf` vs numpy's log); counts (`num_valid`, the ratio thresholds) can differ by pixels whose
-log-ratio sits within an ulp of the threshold.  There is no CPU fallback.
+accumulation here; `logf` vs numpy's log).  Mixed scalar / array arithmetic follows NumPy 1.x promotion: the
+ground truth's divide and the scaled prediction are float32, and the ratio thresholds compare the float32 |log ratio|
+with float32(log t) (DESIGN.md §3.4).  There is no CPU fallback.
 """
 import ctypes
 import math

@@ -8,6 +8,8 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import metrics as om
+
 pytestmark = pytest.mark.gpu
 
 NAMES = ['l1', 'l1_inverse', 'scale_invariant', 'abs_relative', 'sq_relative', 'avg_log10', 'rmse_log', 'rmse',
@@ -20,14 +22,22 @@ def golden(golden_dir):
     return np.load(os.path.join(golden_dir, "metrics_golden.npz"))
 
 
-def check(errs, want, npix):
+def gt_div_of(t):
+    norm = np.sqrt(t.dot(t))
+    return None if np.isclose(1.0, norm) else np.array([norm])
+
+
+def check(errs, want, account):
+    """account: oracle/metrics.py's threshold_account of the same compute_errors call."""
     assert abs(errs['num_valid'] - want[0]) <= 0, (errs['num_valid'], want[0])
     for k, w in zip(NAMES, want[1:]):
         g = errs[k]
         if np.isnan(w):
             assert np.isnan(g), k
         elif k.startswith('ratio_threshold'):
-            assert abs(g - w) <= 3.0 / max(1, want[0]), (k, g, w)          # at most 3 borderline pixels
+            a = account[om.THRESHOLDS.index(float(k.split('_')[-1]))]
+            borderline = len(set(a['ambiguous']) | set(a['disagree']))
+            assert abs(round(g * want[0]) - round(w * want[0])) <= borderline, (k, g * want[0], w * want[0], a)
         else:
             assert abs(g - w) <= RTOL * abs(w) + 1e-9, (k, g, w)
 
@@ -38,14 +48,15 @@ def test_evaluate_depth_matches_reference(golden, ci, scaling):
     from demon_b200 import evaluation as ev
     gt, pred, t = golden["gt_%d" % ci], golden["pred_%d" % ci], golden["t_%d" % ci]
     errs, errs_scaled = ev.evaluate_depth(t, gt, pred, depth_scaling=scaling)
-    check(errs, golden["errs_%d_%s" % (ci, scaling)], gt.size)
-    check(errs_scaled, golden["errs_scaled_%d_%s" % (ci, scaling)], gt.size)
+    check(errs, golden["errs_%d_%s" % (ci, scaling)], om.threshold_account(pred[None], gt[None], True, gt_div_of(t)))
+    check(errs_scaled, golden["errs_scaled_%d_%s" % (ci, scaling)], om.threshold_account(pred[None], gt[None], True, gt_div_of(t), scaling))
 
 
 @pytest.mark.parametrize("ci", (0, 1, 2))
 def test_compute_errors_and_flow_epe_match_reference(golden, ci):
     from demon_b200 import evaluation as ev
-    check(ev.compute_errors(golden["dpred_%d" % ci], golden["dgt_%d" % ci]), golden["errs_plain_%d" % ci], golden["dgt_%d" % ci].size)
+    dpred, dgt = golden["dpred_%d" % ci], golden["dgt_%d" % ci]
+    check(ev.compute_errors(dpred, dgt), golden["errs_plain_%d" % ci], om.threshold_account(dpred[None], dgt[None]))
     epe = ev.compute_flow_epe(golden["f1_%d" % ci], golden["f2_%d" % ci])
     assert abs(epe - float(golden["epe_%d" % ci])) <= RTOL * float(golden["epe_%d" % ci])
 
