@@ -473,13 +473,18 @@ int loss_backward(const demon_loss_term* terms, int num, void* ws, int64_t ws_by
   int slots = 0;
   const int rc = make_terms(tt, terms, num, &slots);
   if (rc != DEMON_OK) return rc;
+  // every SIG term's scratch is checked before the first launch, so a refused call writes no gradient
+  for (int i = 0; i < num; ++i) {
+    const Term<T>& t = tt.t[i];
+    if (!t.grad || t.kind != DEMON_LOSS_SIG) continue;
+    const int64_t need = t.n * kSigChannels * t.h * t.w * (int64_t)sizeof(T);
+    DEMON_REQUIRE(ws && ws_bytes >= need, "loss_backward: workspace of %lld bytes, %lld needed", (long long)ws_bytes, (long long)need);
+  }
   cudaStream_t s = (cudaStream_t)stream;
   for (int i = 0; i < num; ++i) {
     const Term<T>& t = tt.t[i];
     if (!t.grad) continue;
     if (t.kind == DEMON_LOSS_SIG) {
-      const int64_t need = t.n * kSigChannels * t.h * t.w * (int64_t)sizeof(T);
-      DEMON_REQUIRE(ws && ws_bytes >= need, "loss_backward: workspace of %lld bytes, %lld needed", (long long)ws_bytes, (long long)need);
       T* U = static_cast<T*>(ws);
       const int64_t tiles = sig_tiles(t.n, t.h, t.w);
       sig_u_kernel<T><<<(int)(tiles < 132 * 8 ? tiles : 132 * 8), kLossThreads, 0, s>>>(t, U);
