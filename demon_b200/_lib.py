@@ -97,6 +97,15 @@ PROTOTYPES = {
     "demon_pipeline_forward_images_u8": [_P, _P, c_int64, c_int64, c_int64] + [c_int] * 5 + [_P] * 6 + [_P],
     "demon_adjust_intrinsics_u8": [_P, c_int64, c_int64, c_int, c_int, c_int, _P] + [c_double] * 4 + [_P, c_int, c_int, _P, _P],
     "demon_pipeline_forward_views_u8": [_P, _P, c_int64, c_int64, c_int64, c_int, c_int, _P, _P] + [c_int] * 3 + [_P] * 6 + [_P],
+    "demon_pipeline_forward_snapshots_v2": [_P, _P, _P, c_int, c_int] + [_P] * 7 + [_P],
+    "demon_pipeline_forward_u8_v2": [_P, _P, _P, c_int, c_int] + [_P] * 7 + [_P],
+    "demon_pipeline_forward_images_u8_v2": [_P, _P, c_int64, c_int64, c_int64] + [c_int] * 5 + [_P] * 7 + [_P],
+    "demon_pipeline_forward_views_u8_v2": [_P, _P, c_int64, c_int64, c_int64, c_int, c_int, _P, _P] + [c_int] * 3 + [_P] * 7 + [_P],
+    "demon_pipeline_forward_host_v2": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P],
+    "demon_pipeline_forward_host_async_v2": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P],
+    "demon_pipeline_forward_host_u8_v2": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P],
+    "demon_pipeline_forward_host_u8_async_v2": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P],
+    "demon_resize_area_f32": [_P, c_int64, _P] + [c_int] * 6 + [_P],
     "demon_sharpness_u8": [_P, c_int64, c_int64, c_int, c_int, c_int, _P, _P],
     "demon_sun3d_depth_u16": [_P, c_int, c_int, c_int, _P, _P, _P],
     "demon_depth_ratios_f32": [_P] * 5 + [c_int] * 3 + [_P, c_int, _P, _P],

@@ -150,8 +150,8 @@ struct demon_net {
   Buf *rin, *concat0, *rc1, *concat1, *rc2, *rc21, *pd0a, *rdepth0, *splitk;
   // v2 only (build_plan_v2): dense5's gathered input and its output row, the motion branch (its concat is mc1)
   Buf *d5in = nullptr, *d5out = nullptr, *mc3y = nullptr, *mc3 = nullptr, *mc4y = nullptr, *mc4 = nullptr, *mc5y = nullptr;
-  // staging roles of the buffers above (see build_plan)
-  Buf *pair_bytes, *i22_bytes, *planes2, *host_depth0, *host_motion;
+  // staging roles of the buffers above (see build_plan, build_plan_v2); host_normal0: v2 only
+  Buf *pair_bytes, *i22_bytes, *planes2, *host_depth0, *host_motion, *host_normal0 = nullptr;
   // the five blocks' layer ranges
   Block flow1, dm1, flow2, dm2, refine;
 
@@ -499,8 +499,19 @@ void build_plan_v2(demon_net* n) {
   n->rc21 = n->add_buf(RH / 4, RW / 4, 128);
   n->pd0a = n->add_buf(RH, RW, 16);
   n->rdepth0 = n->add_buf(RH, RW, 4);    // depth0 ++ normal0
-  // v2 has only float32 device entries: no staging roles
-  n->pair_bytes = n->i22_bytes = n->planes2 = n->host_depth0 = n->host_motion = nullptr;
+  // Staging roles as in build_plan, for the same reasons: pair_bytes, i22_bytes and planes2 are consumed into img8 / i22
+  // before the first block, c1y is next written by conv1y, concat0 and pd0a only by the refinement block, which reads img8
+  // and dn2 alone; fc1 is free after the last DM block.  Unlike v1's, rdepth0 is not free for a host entry's depth0: it
+  // holds depth0 ++ normal0 (predict_depth0/conv2), which export_outputs reads.  The host outputs are exported after the
+  // refinement block's last layer instead, into buffers whose last reader that block has already run: pd0a (read by
+  // predict_depth0/conv2) takes depth0 and concat0 (read by predict_depth0/conv1) takes normal0.  A host entry takes no
+  // snapshots, so the block runs once, and nothing runs after the export but the copies to the host.
+  n->pair_bytes = n->concat0;    // the image pair as uint8 [B,2,192,256,3] (resized / adapted), or a host entry's image pair
+  n->i22_bytes = n->pd0a;        // image2_2 as uint8 [B,48,64,3] (resized), or a host entry's image2_2
+  n->planes2 = n->c1y;           // image 2 as NCHW fp32 planes, input of the median or area downsampling of a uint8 call
+  n->host_depth0 = n->pd0a;      // a host entry's depth0 [B,1,192,256] before its copy to the host
+  n->host_normal0 = n->concat0;  // a host entry's normal0 [B,3,192,256] before its copy to the host
+  n->host_motion = n->fc1;       // a host entry's rotation and translation ([B,3] each) before their copy to the host
 
   n->flow1 = build_flow_block_v2(n, "netFlow1", false);
   n->dm1 = build_dm_block_v2(n, "netDM1", false);
@@ -845,6 +856,55 @@ __global__ void __launch_bounds__(128) median_planes_kernel(const float* __restr
   out[n * out_sn + (long)c * Ho * Wo + (size_t)yo * Wo + xo] = median9_reference_order(v);
 }
 
+// tf.image.resize_area (align_corners=False) by integer factors fy = H / Ho, fx = W / Wo, over NCHW planes with a batch stride
+// (training/v2/training.py:179 makes image2_2 with it).  Every weight of TF's area kernel is 1 for an integer factor, and
+// this project defines the result, in float32, as: each source row's fx pixels summed left to right from +0, the fy row sums
+// summed top to bottom from +0, times `scale` = float32(1 / (fy fx)) (DESIGN.md §3.6).  Rounded adds and one rounded
+// multiply, so no contraction can change the bits.  One output per thread; grid-stride over N*C*Ho*Wo.
+__global__ void __launch_bounds__(256) area_planes_kernel(const float* __restrict__ in, float* __restrict__ out, int N, int C, int H, int W,
+                                                         int Ho, int Wo, long in_sn, float scale) {
+  pdl_launch_dependents();   // common.cuh: programmatic dependent launch
+  pdl_wait();
+  const int fy = H / Ho, fx = W / Wo;
+  const long total = (long)N * C * Ho * Wo;
+  for (long i = (long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long)gridDim.x * 256) {
+    const int xo = (int)(i % Wo);
+    long r = i / Wo;
+    const int yo = (int)(r % Ho);
+    r /= Ho;
+    const int c = (int)(r % C);
+    const long n = r / C;
+    const float* p = in + n * in_sn + ((long)c * H + (long)yo * fy) * W + (long)xo * fx;
+    float sum = 0.f;
+    for (int y = 0; y < fy; ++y) {
+      float row = 0.f;
+      for (int x = 0; x < fx; ++x) row = fadd(row, __ldg(p + (long)y * W + x));
+      sum = fadd(sum, row);
+    }
+    out[i] = fmul(sum, scale);
+  }
+}
+
+// Argument checks of area_launch
+int area_check(int N, int C, int H, int W, int Ho, int Wo, long in_sn, const char* who) {
+  DEMON_REQUIRE(N >= 0 && C >= 0 && H >= 1 && W >= 1 && Ho >= 1 && Wo >= 1, "%s: size %dx%dx%dx%d -> %dx%d", who, N, C, H, W, Ho, Wo);
+  DEMON_REQUIRE(H % Ho == 0 && W % Wo == 0, "%s: %dx%d -> %dx%d is not a downsampling by integer factors", who, H, W, Ho, Wo);
+  DEMON_REQUIRE(in_sn >= (long)C * H * W, "%s: batch stride %ld below one sample's %ld floats", who, in_sn, (long)C * H * W);
+  return DEMON_OK;
+}
+
+// [N,C,H,W] planes `in_sn` floats apart -> packed [N,C,Ho,Wo]; the factors must be integers (area_check)
+int area_launch(const float* in, float* out, int N, int C, int H, int W, int Ho, int Wo, long in_sn, cudaStream_t s) {
+  const long total = (long)N * C * Ho * Wo;
+  if (total == 0) return DEMON_OK;
+  long blocks = (total + 255) / 256;
+  if (blocks > 132 * 32) blocks = 132 * 32;
+  const float scale = 1.0f / (float)((H / Ho) * (W / Wo));   // float32(1 / (fy fx)): one correctly rounded division
+  (void)launch_pdl(area_planes_kernel, dim3((int)blocks), dim3(256), 0, s, in, out, N, C, H, W, Ho, Wo, in_sn, scale);
+  DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
+}
+
 // Flow2 extra inputs (blocks_original.py:155-183): depth_to_flow(inverse_depth, normalize_flow) ->
 // zero where |flow| >= 1 or NaN -> warp2d(image2_2, normalized, 'value') -> NHWC12
 // [warped(3), flow(2), depth(1), normal(3), 0, 0, 0].  dn2 = [depth, normal] NHWC4, motion [B,8] = rot|trans|scale.
@@ -1027,6 +1087,13 @@ int median_image2_2(demon_net* n, const float* planes, long sn, cudaStream_t s) 
   (void)launch_pdl(median_planes_kernel, dim3(dim3(1, 48, B * 3)), dim3(128), 0, s, n->i22_half->p, n->i22->p, 3, 96, 128, 48, 64, 3L * 96 * 128, 3L * 48 * 64);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
+}
+
+// image2_2 made from image 2's planes when the call brings none: image2_2_mode 2 is resize_area to 48x64
+// (training/v2/training.py:179), any other the median pair
+int downsample_image2_2(demon_net* n, const float* planes, long sn, int64_t image2_2_mode, cudaStream_t s) {
+  if (image2_2_mode == 2) return area_launch(planes, n->i22->p, n->B, 3, 192, 256, 48, 64, sn, s);
+  return median_image2_2(n, planes, sn, s);
 }
 
 // export one NHWC channel slice to the API layout
@@ -1418,7 +1485,7 @@ static int pipeline_body(demon_net* n, const PipelineCall& c, cudaStream_t s) {
       long b2 = ((long)n->B * 48 * 64 + 255) / 256;
       (void)launch_pdl(u8_planes_kernel, dim3((int)b2), dim3(256), 0, s, image2_2_u8, n->i22->p, n->B, 48 * 64);
       DEMON_LAUNCH_CHECK();
-    } else if ((rc = median_image2_2(n, planes2, 3 * P, s))) {
+    } else if ((rc = downsample_image2_2(n, planes2, 3 * P, c.image2_2_mode, s))) {
       return rc;
     }
   } else {
@@ -1426,7 +1493,7 @@ static int pipeline_body(demon_net* n, const PipelineCall& c, cudaStream_t s) {
     if (c.image2_2) {
       if ((rc = import_image2_2(n, c.image2_2, 0, s))) return rc;
     } else {
-      if ((rc = median_image2_2(n, c.image_pair + 3 * P, 6 * P, s))) return rc;
+      if ((rc = downsample_image2_2(n, c.image_pair + 3 * P, 6 * P, c.image2_2_mode, s))) return rc;
     }
   }
   // k = 0: the bootstrap blocks; k > 0: iteration k
@@ -1518,47 +1585,115 @@ int demon_pipeline_forward_v2(demon_net* n, const float* image_pair, const float
   return pipeline_forward_impl(n, c, stream);
 }
 
+// The image2_2 source of a v2 entry that takes pairs at the network's size (uint8 or float32): 0 (the given image2_2, or
+// the median pair without one) or 2 (resize_area of image 2; then there is no given image2_2)
+static int check_pair_mode(int image2_2_mode, const void* image2_2, const char* who) {
+  DEMON_REQUIRE(image2_2_mode == 0 || image2_2_mode == 2, "%s: image2_2_mode %d is not 0 (median) or 2 (area)", who, image2_2_mode);
+  DEMON_REQUIRE(image2_2_mode == 0 || !image2_2, "%s: image2_2_mode 2 (area) computes image2_2, which must then be NULL", who);
+  return DEMON_OK;
+}
+
+// snapshot k of every output at slice k; the refinement block runs on every snapshot iff depth0 is given
+static int snapshots_impl(demon_net* n, const float* image_pair, const float* image2_2, int image2_2_mode, int iterations,
+                          const PipelineOutputs& o, void* stream) {
+  DEMON_REQUIRE(image_pair, "pipeline_snapshots: null image_pair");
+  DEMON_REQUIRE(o.depth0 || !o.normal0, "pipeline_snapshots: normal0 without depth0 (normal0 comes out of the refinement block)");
+  PipelineCall c{};
+  c.input = IN_FP32; c.image_pair = image_pair; c.image2_2 = image2_2; c.image2_2_mode = image2_2_mode; c.iterations = iterations;
+  c.out = o;
+  c.snapshots = o.depth0 ? SNAPSHOTS_REFINED : SNAPSHOTS;
+  return pipeline_forward_impl(n, c, stream);
+}
+
 int demon_pipeline_forward_snapshots(demon_net* n, const float* image_pair, const float* image2_2, int iterations, float* flow2,
                                      float* depth2, float* normal2, float* rotation, float* translation, float* depth0, void* stream) {
   REQUIRE_READY(n);
-  DEMON_REQUIRE(image_pair, "pipeline_snapshots: null image_pair");
+  return snapshots_impl(n, image_pair, image2_2, 0, iterations, {depth0, rotation, translation, flow2, depth2, normal2}, stream);
+}
+
+int demon_pipeline_forward_snapshots_v2(demon_net* n, const float* image_pair, const float* image2_2, int image2_2_mode, int iterations,
+                                        float* depth0, float* normal0, float* rotation, float* translation, float* flow2, float* depth2,
+                                        float* normal2, void* stream) {
+  REQUIRE_READY_AS(n, 2);
+  if (int rc = check_pair_mode(image2_2_mode, image2_2, "pipeline_snapshots_v2")) return rc;
+  return snapshots_impl(n, image_pair, image2_2, image2_2_mode, iterations, {depth0, rotation, translation, flow2, depth2, normal2, normal0},
+                        stream);
+}
+
+static int u8_impl(demon_net* n, const uint8_t* images, const uint8_t* image2_2, int image2_2_mode, int iterations, const PipelineOutputs& o,
+                   void* stream) {
+  DEMON_REQUIRE(images, "pipeline_u8: null images");
   PipelineCall c{};
-  c.input = IN_FP32; c.image_pair = image_pair; c.image2_2 = image2_2; c.iterations = iterations;
-  c.out = {depth0, rotation, translation, flow2, depth2, normal2};
-  c.snapshots = depth0 ? SNAPSHOTS_REFINED : SNAPSHOTS;
+  c.input = IN_U8; c.images = images; c.image2_2_u8 = image2_2; c.image2_2_mode = image2_2_mode; c.iterations = iterations;
+  c.out = o;
   return pipeline_forward_impl(n, c, stream);
 }
 
 int demon_pipeline_forward_u8(demon_net* n, const uint8_t* images, const uint8_t* image2_2, int iterations, float* depth0, float* rotation,
                               float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
   REQUIRE_READY(n);
-  DEMON_REQUIRE(images, "pipeline_u8: null images");
-  PipelineCall c{};
-  c.input = IN_U8; c.images = images; c.image2_2_u8 = image2_2; c.iterations = iterations;
-  c.out = {depth0, rotation, translation, flow2, depth2, normal2};
-  return pipeline_forward_impl(n, c, stream);
+  return u8_impl(n, images, image2_2, 0, iterations, {depth0, rotation, translation, flow2, depth2, normal2}, stream);
 }
 
-// The argument checks shared by the entries that take uint8 pairs of any size, which then fill the source fields of `c`
-static int set_source(PipelineCall& c, PipelineInput input, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w,
-                      int resample, int image2_2_mode, const char* who) {
+int demon_pipeline_forward_u8_v2(demon_net* n, const uint8_t* images, const uint8_t* image2_2, int image2_2_mode, int iterations,
+                                 float* depth0, float* normal0, float* rotation, float* translation, float* flow2, float* depth2,
+                                 float* normal2, void* stream) {
+  REQUIRE_READY_AS(n, 2);
+  if (int rc = check_pair_mode(image2_2_mode, image2_2, "pipeline_u8_v2")) return rc;
+  return u8_impl(n, images, image2_2, image2_2_mode, iterations, {depth0, rotation, translation, flow2, depth2, normal2, normal0}, stream);
+}
+
+// The argument checks shared by the entries that take uint8 pairs of any size, which then fill the source fields of `c`.
+// image2_2_mode 2 (area) is v2's only: it is the input training/v2/training.py feeds v2, and v1 never saw it
+static int set_source(const demon_net* n, PipelineCall& c, PipelineInput input, const uint8_t* images, int64_t sn, int64_t si, int64_t sy,
+                      int h, int w, int resample, int image2_2_mode, const char* who) {
   DEMON_REQUIRE(sn >= 0 && si >= 0 && sy >= 0, "%s: negative stride", who);
-  DEMON_REQUIRE(image2_2_mode == 0 || image2_2_mode == 1, "%s: image2_2_mode %d is not 0 (median) or 1 (resize)", who, image2_2_mode);
+  if (n->variant == 2)
+    DEMON_REQUIRE(image2_2_mode >= 0 && image2_2_mode <= 2, "%s: image2_2_mode %d is not 0 (median), 1 (resize) or 2 (area)", who,
+                  image2_2_mode);
+  else
+    DEMON_REQUIRE(image2_2_mode == 0 || image2_2_mode == 1, "%s: image2_2_mode %d is not 0 (median) or 1 (resize)", who, image2_2_mode);
   c.input = input; c.images = images; c.sn = sn; c.si = si; c.sy = sy; c.h = h; c.w = w; c.resample = resample;
   c.image2_2_mode = image2_2_mode;
   return DEMON_OK;
+}
+
+static int images_impl(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, int resample,
+                       int image2_2_mode, int iterations, const PipelineOutputs& o, void* stream) {
+  DEMON_REQUIRE(images, "pipeline_images_u8: null images");
+  PipelineCall c{};
+  int rc = set_source(n, c, IN_RESIZE, images, sn, si, sy, h, w, resample, image2_2_mode, "pipeline_images_u8");
+  if (rc || (rc = resize_u8_check(h, w, 192, 256, resample, "pipeline_images_u8"))) return rc;
+  c.iterations = iterations;
+  c.out = o;
+  return pipeline_forward_impl(n, c, stream);
 }
 
 int demon_pipeline_forward_images_u8(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, int resample,
                                      int image2_2_mode, int iterations, float* depth0, float* rotation, float* translation, float* flow2,
                                      float* depth2, float* normal2, void* stream) {
   REQUIRE_READY(n);
-  DEMON_REQUIRE(images, "pipeline_images_u8: null images");
+  return images_impl(n, images, sn, si, sy, h, w, resample, image2_2_mode, iterations, {depth0, rotation, translation, flow2, depth2, normal2},
+                     stream);
+}
+
+int demon_pipeline_forward_images_u8_v2(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, int resample,
+                                        int image2_2_mode, int iterations, float* depth0, float* normal0, float* rotation, float* translation,
+                                        float* flow2, float* depth2, float* normal2, void* stream) {
+  REQUIRE_READY_AS(n, 2);
+  return images_impl(n, images, sn, si, sy, h, w, resample, image2_2_mode, iterations,
+                     {depth0, rotation, translation, flow2, depth2, normal2, normal0}, stream);
+}
+
+static int views_impl(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, const double* K, uint8_t* status,
+                      int resample, int image2_2_mode, int iterations, const PipelineOutputs& o, void* stream) {
+  DEMON_REQUIRE(images && K && status, "pipeline_views_u8: null images, K or status");
   PipelineCall c{};
-  int rc = set_source(c, IN_RESIZE, images, sn, si, sy, h, w, resample, image2_2_mode, "pipeline_images_u8");
-  if (rc || (rc = resize_u8_check(h, w, 192, 256, resample, "pipeline_images_u8"))) return rc;
-  c.iterations = iterations;
-  c.out = {depth0, rotation, translation, flow2, depth2, normal2};
+  int rc = set_source(n, c, IN_VIEWS, images, sn, si, sy, h, w, resample, image2_2_mode, "pipeline_views_u8");
+  if (rc || (rc = adjust_intrinsics_check(h, w, kNetIntrinsics, 192, 256, "pipeline_views_u8"))) return rc;
+  if ((rc = resize_u8_check(192, 256, 48, 64, resample, "pipeline_views_u8"))) return rc;
+  c.K = K; c.status = status; c.iterations = iterations;
+  c.out = o;
   return pipeline_forward_impl(n, c, stream);
 }
 
@@ -1566,22 +1701,28 @@ int demon_pipeline_forward_views_u8(demon_net* n, const uint8_t* images, int64_t
                                     uint8_t* status, int resample, int image2_2_mode, int iterations, float* depth0, float* rotation,
                                     float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
   REQUIRE_READY(n);
-  DEMON_REQUIRE(images && K && status, "pipeline_views_u8: null images, K or status");
-  PipelineCall c{};
-  int rc = set_source(c, IN_VIEWS, images, sn, si, sy, h, w, resample, image2_2_mode, "pipeline_views_u8");
-  if (rc || (rc = adjust_intrinsics_check(h, w, kNetIntrinsics, 192, 256, "pipeline_views_u8"))) return rc;
-  if ((rc = resize_u8_check(192, 256, 48, 64, resample, "pipeline_views_u8"))) return rc;
-  c.K = K; c.status = status; c.iterations = iterations;
-  c.out = {depth0, rotation, translation, flow2, depth2, normal2};
-  return pipeline_forward_impl(n, c, stream);
+  return views_impl(n, images, sn, si, sy, h, w, K, status, resample, image2_2_mode, iterations,
+                    {depth0, rotation, translation, flow2, depth2, normal2}, stream);
 }
 
-// H2D of the inputs into the staging buffers (build_plan), the pipeline, D2H of depth0 / rotation / translation
-static int pipeline_host(demon_net* n, const void* images_host, const void* image2_2_host, bool u8, int iterations, float* depth0_host,
-                         float* rotation_host, float* translation_host, void* stream, bool sync) {
-  REQUIRE_READY(n);
+int demon_pipeline_forward_views_u8_v2(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, const double* K,
+                                       uint8_t* status, int resample, int image2_2_mode, int iterations, float* depth0, float* normal0,
+                                       float* rotation, float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
+  REQUIRE_READY_AS(n, 2);
+  return views_impl(n, images, sn, si, sy, h, w, K, status, resample, image2_2_mode, iterations,
+                    {depth0, rotation, translation, flow2, depth2, normal2, normal0}, stream);
+}
+
+// H2D of the inputs into the staging buffers (build_plan, build_plan_v2), the pipeline of network `variant`, D2H of depth0 /
+// normal0 (v2) / rotation / translation
+static int pipeline_host(demon_net* n, int variant, const void* images_host, const void* image2_2_host, bool u8, int image2_2_mode,
+                         int iterations, float* depth0_host, float* normal0_host, float* rotation_host, float* translation_host, void* stream,
+                         bool sync) {
+  REQUIRE_READY_AS(n, variant);
   if (int rc = refuse_while_tracing(n)) return rc;
   DEMON_REQUIRE(images_host && depth0_host, "pipeline_host: null pointer");
+  if (variant == 2)
+    if (int rc = check_pair_mode(image2_2_mode, image2_2_host, "pipeline_host_v2")) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   const size_t px = (size_t)n->B * 192 * 256;
   const size_t ip_bytes = u8 ? px * 6 : px * 6 * sizeof(float);
@@ -1594,13 +1735,16 @@ static int pipeline_host(demon_net* n, const void* images_host, const void* imag
   PipelineCall c{};
   if (u8) { c.input = IN_U8; c.images = static_cast<const uint8_t*>(ip_dev); c.image2_2_u8 = static_cast<const uint8_t*>(i22_dev); }
   else { c.input = IN_FP32; c.image_pair = static_cast<const float*>(ip_dev); c.image2_2 = static_cast<const float*>(i22_dev); }
+  c.image2_2_mode = image2_2_mode;
   c.iterations = iterations;
   c.out.depth0 = n->host_depth0->p;
+  c.out.normal0 = normal0_host ? n->host_normal0->p : nullptr;
   c.out.rotation = rotation_host ? rt_dev : nullptr;
   c.out.translation = translation_host ? rt_dev + 3 * n->B : nullptr;
   int rc = pipeline_forward_impl(n, c, stream);
   if (rc) return rc;
   DEMON_CHECK_CUDA(cudaMemcpyAsync(depth0_host, c.out.depth0, px * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if (normal0_host) DEMON_CHECK_CUDA(cudaMemcpyAsync(normal0_host, c.out.normal0, px * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
   if (rotation_host) DEMON_CHECK_CUDA(cudaMemcpyAsync(rotation_host, rt_dev, (size_t)n->B * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
   if (translation_host)
     DEMON_CHECK_CUDA(cudaMemcpyAsync(translation_host, rt_dev + 3 * n->B, (size_t)n->B * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
@@ -1614,22 +1758,61 @@ static int pipeline_host(demon_net* n, const void* images_host, const void* imag
 
 int demon_pipeline_forward_host(demon_net* n, const float* image_pair_host, const float* image2_2_host, int iterations, float* depth0_host,
                                 float* rotation_host, float* translation_host, void* stream) {
-  return pipeline_host(n, image_pair_host, image2_2_host, false, iterations, depth0_host, rotation_host, translation_host, stream, true);
+  return pipeline_host(n, 1, image_pair_host, image2_2_host, false, 0, iterations, depth0_host, nullptr, rotation_host, translation_host,
+                       stream, true);
 }
 
 int demon_pipeline_forward_host_async(demon_net* n, const float* image_pair_host, const float* image2_2_host, int iterations,
                                       float* depth0_host, float* rotation_host, float* translation_host, void* stream) {
-  return pipeline_host(n, image_pair_host, image2_2_host, false, iterations, depth0_host, rotation_host, translation_host, stream, false);
+  return pipeline_host(n, 1, image_pair_host, image2_2_host, false, 0, iterations, depth0_host, nullptr, rotation_host, translation_host,
+                       stream, false);
 }
 
 int demon_pipeline_forward_host_u8(demon_net* n, const uint8_t* images_host, const uint8_t* image2_2_host, int iterations, float* depth0_host,
                                    float* rotation_host, float* translation_host, void* stream) {
-  return pipeline_host(n, images_host, image2_2_host, true, iterations, depth0_host, rotation_host, translation_host, stream, true);
+  return pipeline_host(n, 1, images_host, image2_2_host, true, 0, iterations, depth0_host, nullptr, rotation_host, translation_host, stream,
+                       true);
 }
 
 int demon_pipeline_forward_host_u8_async(demon_net* n, const uint8_t* images_host, const uint8_t* image2_2_host, int iterations,
                                          float* depth0_host, float* rotation_host, float* translation_host, void* stream) {
-  return pipeline_host(n, images_host, image2_2_host, true, iterations, depth0_host, rotation_host, translation_host, stream, false);
+  return pipeline_host(n, 1, images_host, image2_2_host, true, 0, iterations, depth0_host, nullptr, rotation_host, translation_host, stream,
+                       false);
+}
+
+int demon_pipeline_forward_host_v2(demon_net* n, const float* image_pair_host, const float* image2_2_host, int image2_2_mode, int iterations,
+                                   float* depth0_host, float* normal0_host, float* rotation_host, float* translation_host, void* stream) {
+  return pipeline_host(n, 2, image_pair_host, image2_2_host, false, image2_2_mode, iterations, depth0_host, normal0_host, rotation_host,
+                       translation_host, stream, true);
+}
+
+int demon_pipeline_forward_host_async_v2(demon_net* n, const float* image_pair_host, const float* image2_2_host, int image2_2_mode,
+                                         int iterations, float* depth0_host, float* normal0_host, float* rotation_host,
+                                         float* translation_host, void* stream) {
+  return pipeline_host(n, 2, image_pair_host, image2_2_host, false, image2_2_mode, iterations, depth0_host, normal0_host, rotation_host,
+                       translation_host, stream, false);
+}
+
+int demon_pipeline_forward_host_u8_v2(demon_net* n, const uint8_t* images_host, const uint8_t* image2_2_host, int image2_2_mode, int iterations,
+                                      float* depth0_host, float* normal0_host, float* rotation_host, float* translation_host, void* stream) {
+  return pipeline_host(n, 2, images_host, image2_2_host, true, image2_2_mode, iterations, depth0_host, normal0_host, rotation_host,
+                       translation_host, stream, true);
+}
+
+int demon_pipeline_forward_host_u8_async_v2(demon_net* n, const uint8_t* images_host, const uint8_t* image2_2_host, int image2_2_mode,
+                                            int iterations, float* depth0_host, float* normal0_host, float* rotation_host,
+                                            float* translation_host, void* stream) {
+  return pipeline_host(n, 2, images_host, image2_2_host, true, image2_2_mode, iterations, depth0_host, normal0_host, rotation_host,
+                       translation_host, stream, false);
+}
+
+// resize_area over NCHW planes (area_planes_kernel): input [N,C,h,w] with `in_sn` floats between samples -> packed
+// [N,C,oh,ow]; h / oh and w / ow must be integers
+int demon_resize_area_f32(const float* input, int64_t in_sn, float* output, int n, int c, int h, int w, int oh, int ow, void* stream) {
+  if (int rc = area_check(n, c, h, w, oh, ow, (long)in_sn, "resize_area")) return rc;
+  if ((int64_t)n * c == 0) return DEMON_OK;
+  DEMON_REQUIRE(input && output, "resize_area: null pointer");
+  return area_launch(input, output, n, c, h, w, oh, ow, (long)in_sn, (cudaStream_t)stream);
 }
 
 // debug: the geometry of every layer of the net and which kernel family / plan it got (one line per layer).  A v2 conv's

@@ -380,7 +380,7 @@ def evaluate_batch(predictions, depth_gt, motion_gt, intrinsics=None, flow_gt=No
                    depth_scaling='abs', snapshot='snapshot_1', first_sample=0):
     """evaluate_to_xarray.evaluate (lines 216-316) for one batch of predictions that never left the device.
 
-    predictions: DemonPipeline.forward_snapshots' dict (predict_flow2 [S,B,2,h,w], predict_depth2 [S,B,1,h,w],
+    predictions: DemonPipeline.forward_snapshots' dict (or DemonPipelineV2's; keys it does not use are ignored) (predict_flow2 [S,B,2,h,w], predict_depth2 [S,B,1,h,w],
         predict_rotation / predict_translation [S,B,3], optional predict_depth0 [S,B,1,H,W]); the first n samples are used
     depth_gt: [n,gh,gw] INVERSE depth (the ground-truth file's 'depth'), motion_gt [n,6] ('motion', angle axis |
         translation), intrinsics [n,4] normalised ('intrinsics') or None for the sun3d default, flow_gt [n,2,gh,gw]
@@ -481,12 +481,15 @@ class Evaluator:
 
     Every batch is one forward_snapshots call (bootstrap, `iterations` iterations, the refinement net on every snapshot)
     and one evaluate_batch; only the table's numbers leave the GPU.  A last, smaller batch is padded to the batch size
-    and only its real samples are evaluated."""
+    and only its real samples are evaluated.  A v2 Session (demon_b200.v2.networks, e.g. restored from a checkpoint of
+    training/v2/training.py) is evaluated with DemonPipelineV2; its predict_normal0 is not part of the table."""
 
     def __init__(self, session, batch_size, iterations=3, depthmask=False, eigen_crop_gt_and_pred=False, depth_scaling='abs',
                  refine=True):
         from .networks_original import DemonPipeline
-        self.pipeline = DemonPipeline(session, batch_size, iterations)
+        from .v2.networks import DemonPipelineV2, Session as SessionV2
+        self.v2 = isinstance(session, SessionV2)
+        self.pipeline = (DemonPipelineV2 if self.v2 else DemonPipeline)(session, batch_size, iterations)
         self.batch_size = int(batch_size)
         self.options = dict(depthmask=depthmask, eigen_crop_gt_and_pred=eigen_crop_gt_and_pred, depth_scaling=depth_scaling)
         self.refine = refine
@@ -494,17 +497,21 @@ class Evaluator:
         self._count = 0
 
     def add(self, image_pair, depth_gt, motion_gt, intrinsics=None, flow_gt=None, image2_2=None):
-        """image_pair [m,6,192,256] (m <= batch size), image2_2 [m,3,48,64] or None (median3x3 twice); ground truth as
+        """image_pair [m,6,192,256] (m <= batch size), image2_2 [m,3,48,64], None (median3x3 twice) or, for a v2 session,
+        'area' (tf.image.resize_area of the second image, the input training/v2/training.py trains v2 on); ground truth as
         evaluate_batch takes it.  Returns this batch's EvaluationResult."""
+        if isinstance(image2_2, str) and not (self.v2 and image2_2 == 'area'):
+            raise ValueError("image2_2 must be a tensor, None%s, got %r (v1 was never trained on resize_area's image2_2)"
+                             % (" or 'area'" if self.v2 else "", image2_2))
         ip = _dev(image_pair)
         m = ip.shape[0]
         if m > self.batch_size:
             raise ValueError("%d pairs in a batch of %d" % (m, self.batch_size))
-        i2 = None if image2_2 is None else _dev(image2_2)
+        i2 = image2_2 if image2_2 is None or isinstance(image2_2, str) else _dev(image2_2)
         if m < self.batch_size:
             pad = self.batch_size - m
             ip = torch.cat([ip, ip[-1:].expand(pad, -1, -1, -1)])
-            i2 = None if i2 is None else torch.cat([i2, i2[-1:].expand(pad, -1, -1, -1)])
+            i2 = i2 if i2 is None or isinstance(i2, str) else torch.cat([i2, i2[-1:].expand(pad, -1, -1, -1)])
         preds = self.pipeline.forward_snapshots(ip, i2, refine=self.refine)
         r = evaluate_batch(preds, depth_gt, motion_gt, intrinsics, flow_gt, first_sample=self._count, **self.options)
         self._parts.append(r)

@@ -122,6 +122,64 @@ def prepare_input_data(img1, img2, data_format="channels_first", resample="bicub
     return {"image_pair": pair.contiguous(), "image1": i1.contiguous(), "image2_2": i22.contiguous()}
 
 
+def _check_area(x, size):
+    """The checks of resize_area that need no device: x torch or numpy float32 [N,C,h,w] or [C,h,w], size (oh, ow) dividing
+    (h, w).  Returns (oh, ow)."""
+    if not isinstance(x, (torch.Tensor, np.ndarray)):
+        raise ValueError("images: expected a torch CUDA tensor or a numpy array, got %s" % type(x).__name__)
+    if x.dtype != (torch.float32 if isinstance(x, torch.Tensor) else np.float32):
+        raise ValueError("images: expected float32, got %s" % x.dtype)
+    if x.ndim not in (3, 4):
+        raise ValueError("images: expected [N,C,h,w] or [C,h,w], got shape %s" % (tuple(x.shape),))
+    if isinstance(x, torch.Tensor) and not x.is_cuda:
+        raise ValueError("images: a torch tensor must be on a CUDA device (or pass a numpy array)")
+    try:
+        oh, ow = (int(v) for v in size)
+    except (TypeError, ValueError):
+        raise ValueError("size must be (height, width), got %r" % (size,))
+    h, w = x.shape[-2:]
+    if not (1 <= oh <= h and 1 <= ow <= w and h % oh == 0 and w % ow == 0):
+        raise ValueError("resize_area: %dx%d -> %dx%d (height x width) is not a downsampling by integer factors" % (h, w, oh, ow))
+    if x.shape[-3] * h * w >= 2 ** 31 or (x.ndim == 4 and x.shape[0] >= 2 ** 31):
+        raise ValueError("images: shape %s too large" % (tuple(x.shape),))
+    return oh, ow
+
+
+def _resize_area_into(x, out):
+    """resize_area of CUDA float32 [N,C,h,w] (rows and planes packed, any sample stride) into `out` [N,C,oh,ow] contiguous,
+    on the current stream."""
+    n, c, h, w = x.shape
+    if x.stride()[1:] != (h * w, w, 1) or (n > 1 and x.stride(0) < c * h * w):
+        x = x.contiguous()
+    with torch.cuda.device(x.device):
+        _lib.check(_lib.load().demon_resize_area_f32(x.data_ptr(), x.stride(0) if n > 1 else c * h * w, out.data_ptr(), n, c, h, w,
+                                                     out.shape[2], out.shape[3], ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
+    return out
+
+
+def resize_area(images, size):
+    """`tf.image.resize_area(images, size)` (align_corners=False) for integer factors, the image2_2 of
+    training/v2/training.py:179 (`resize_area(image2, (48, 64))`): images float32 [N,C,h,w] or [C,h,w] (NCHW, unlike TF's
+    NHWC), size (height, width) as TF takes it, h and w multiples of them; other sizes raise ValueError.  A torch CUDA tensor
+    gives a new torch CUDA tensor (asynchronous, current stream; a channel slice such as image_pair[:, 3:6] is read in place),
+    a numpy array a numpy array.  Every output is the fy x fx block's rows summed left to right, the row sums top to bottom,
+    times float32(1 / (fy fx)), in float32 (this project's definition; DESIGN.md §3.6)."""
+    oh, ow = _check_area(images, size)
+    was_np = isinstance(images, np.ndarray)
+    if was_np:
+        if not torch.cuda.is_available():
+            raise RuntimeError("resize_area needs a CUDA device (there is no CPU fallback)")
+        x = torch.from_numpy(np.ascontiguousarray(images)).cuda()
+    else:
+        x = images
+    single = x.dim() == 3
+    x4 = x.unsqueeze(0) if single else x
+    out = torch.empty((x4.shape[0], x4.shape[1], oh, ow), dtype=torch.float32, device=x4.device)
+    _resize_area_into(x4, out)
+    out = out[0] if single else out
+    return out.cpu().numpy() if was_np else out
+
+
 def demon_intrinsics(width=256, height=192):
     """The intrinsics DeMoN was trained for in pixels of a width x height image: numpy float64 K [3,3]."""
     fx, fy, cx, cy = NETWORK_INTRINSICS

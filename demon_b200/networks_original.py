@@ -243,15 +243,25 @@ class RefinementNet(_NetBase):
         return self._finish(out, t1 and t2)
 
 
-class DemonPipeline:
-    """examples/example.py:87-99 as one device-resident call (channels_first only)."""
+class _Pipeline:
+    """The fused pipeline's methods, written once for DemonPipeline (networks_original) and DemonPipelineV2 (v2.networks).
+    A subclass names its network handle, the suffix of its C entries, its output keys in C ABI order and the image2_2 modes
+    it takes; v2's entries also take an image2_2_mode and return normal0."""
 
-    def __init__(self, session=None, batch_size=1, iterations=3, private_net=False):
-        self.session = session if session is not None else default_session()
+    _handle = _NetHandle
+    _suffix = ""                                 # C entry names: demon_pipeline_forward<kind><suffix>
+    _keys = _OUTPUTS                             # outputs of the device entries, in C ABI order
+    _snapshot_keys = _SNAPSHOT_OUTPUTS
+    _host_keys = ("predict_depth0", "predict_rotation", "predict_translation")
+    _modes = {"resize": 1, "median": 0}          # image2_2 of forward_images / forward_views -> image2_2_mode
+    _area = False                                # image2_2='area' (tf.image.resize_area of image 2, v2 only)
+
+    def __init__(self, session, batch_size, iterations, private_net):
+        self.session = session
         self.batch_size = int(batch_size)
         self.iterations = int(iterations)
         # private_net: an own network handle (own workspace), so that two pipelines can be in flight on two streams
-        self.net = (_NetHandle(self.session.weights, self.batch_size, (192, 256), self.session.precision) if private_net
+        self.net = (self._handle(self.session.weights, self.batch_size, (192, 256), self.session.precision) if private_net
                     else self.session.net(self.batch_size))
         # The C call replays ONE CUDA graph per set of pointer arguments, so the pipeline owns persistent input staging
         # and output buffers: the graph key is then the same for every call, whatever tensors the caller passes.
@@ -259,42 +269,71 @@ class DemonPipeline:
         self._snap = self._snap_refined = None
         self._K = self._status = None   # forward_views: intrinsics staging [B,2,4] float64 and status [B,2] uint8
 
+    def _mode_args(self, mode):
+        """The image2_2_mode argument of the entries at the network's input size: v1's take none (mode 0 only)."""
+        return ()
+
+    def _image2_2_source(self, image2_2):
+        """image2_2 of the uint8 and host entries -> (the tensor or None, image2_2_mode)."""
+        if isinstance(image2_2, str):
+            if not (self._area and image2_2 == "area"):
+                raise ValueError("image2_2 must be %sNone or a tensor, got %r" % ("'area', " if self._area else "", image2_2))
+            return None, 2
+        return image2_2, 0
+
+    def _staging(self, device):
+        if self._ip is None:
+            b = self.batch_size
+            self._ip = torch.empty((b, 6, 192, 256), dtype=torch.float32, device=device)
+            self._i22 = torch.empty((b, 3, 48, 64), dtype=torch.float32, device=device)
+
+    def _stage_image2_2(self, ip, image2_2):
+        """image2_2 in the pipeline's own buffer: a copy of the given one, or resize_area of ip's second image."""
+        i2, mode = self._image2_2_source(image2_2)
+        self._staging(ip.device)
+        if mode == 2:
+            from .images import _resize_area_into
+            return _resize_area_into(ip[:, 3:6], self._i22)
+        if i2 is None:
+            return None
+        i2, _ = _to_dev(i2, (self.batch_size, 3, 48, 64), "image2_2")
+        if i2.data_ptr() != self._i22.data_ptr():
+            self._i22.copy_(i2, non_blocking=True)
+        return self._i22
+
     def stage(self, image_pair, image2_2=None):
         """Copies the inputs into the pipeline's own device buffers (asynchronous, current stream) and returns them."""
-        b = self.batch_size
-        ip, _ = _to_dev(image_pair, (b, 6, 192, 256), "image_pair")
-        if self._ip is None:
-            self._ip = torch.empty((b, 6, 192, 256), dtype=torch.float32, device=ip.device)
-            self._i22 = torch.empty((b, 3, 48, 64), dtype=torch.float32, device=ip.device)
+        ip, _ = _to_dev(image_pair, (self.batch_size, 6, 192, 256), "image_pair")
+        self._staging(ip.device)
         if ip.data_ptr() != self._ip.data_ptr():
             self._ip.copy_(ip, non_blocking=True)
-        i2 = None
-        if image2_2 is not None:
-            i2, _ = _to_dev(image2_2, (b, 3, 48, 64), "image2_2")
-            if i2.data_ptr() != self._i22.data_ptr():
-                self._i22.copy_(i2, non_blocking=True)
-            i2 = self._i22
-        return self._ip, i2
+        return self._ip, self._stage_image2_2(self._ip, image2_2)
 
-    def _own(self, attr, shapes):
+    def _own(self, attr, shapes, device=None):
         """The persistent float32 buffers `attr` of the pipeline (name -> shape), made on the first call."""
         if getattr(self, attr) is None:
-            dev = self._ip.device if self._ip is not None else torch.device("cuda", torch.cuda.current_device())
-            setattr(self, attr, {k: torch.empty(s, dtype=torch.float32, device=dev) for k, s in shapes.items()})
+            if device is None:
+                device = self._ip.device if self._ip is not None else torch.device("cuda", torch.cuda.current_device())
+            setattr(self, attr, {k: torch.empty(s, dtype=torch.float32, device=device) for k, s in shapes.items()})
         return getattr(self, attr)
 
-    def own_outputs(self):
+    def _output_shapes(self):
         b = self.batch_size
-        return self._own("_out", {"predict_depth0": (b, 1, 192, 256), "predict_rotation": (b, 3), "predict_translation": (b, 3),
-                                  "predict_flow2": (b, 2, 48, 64), "predict_depth2": (b, 1, 48, 64), "predict_normal2": (b, 3, 48, 64)})
+        return {"predict_depth0": (b, 1, 192, 256), "predict_rotation": (b, 3), "predict_translation": (b, 3),
+                "predict_flow2": (b, 2, 48, 64), "predict_depth2": (b, 1, 48, 64), "predict_normal2": (b, 3, 48, 64)}
 
-    def _run(self, entry, args, outputs=None, keys=_OUTPUTS):
-        """Calls the C entry `entry` on the net with `args`, the iteration count, the pointers of `outputs` (default: the
-        pipeline's own) in the order of `keys` (null for a missing one) and the current stream; raises on an error code."""
+    def own_outputs(self):
+        return self._own("_out", self._output_shapes())
+
+    def _run(self, entry, args, outputs=None, keys=None, iterations=None):
+        """Calls the C entry `entry` (+ the class's suffix) on the net with `args`, the iteration count, the pointers of
+        `outputs` (default: the pipeline's own) in the order of `keys` (default: the class's; null for a missing one) and the
+        current stream; raises on an error code."""
         if outputs is None:
             outputs = self.own_outputs()
-        fn = getattr(_lib.load(), entry)
-        _lib.check(fn(self.net.ptr, *args, self.iterations, *(_ptr(outputs.get(k)) for k in keys), _stream()))
+        fn = getattr(_lib.load(), entry + self._suffix)
+        it = self.iterations if iterations is None else int(iterations)
+        _lib.check(fn(self.net.ptr, *args, it, *(_ptr(outputs.get(k)) for k in (keys or self._keys)), _stream()))
         return outputs
 
     def forward(self, image_pair, image2_2=None, outputs=None, stage_inputs=True):
@@ -304,15 +343,17 @@ class DemonPipeline:
         the pipeline and are overwritten by the next call (clone them to keep them).  `stage_inputs=False` skips the
         device-to-device copy into the pipeline's own input buffers; pass the same tensors every call then, or every
         new pointer set costs an eager ~270-launch pass plus a graph capture."""
-        b = self.batch_size
+        return self._forward(image_pair, image2_2, outputs, stage_inputs, None)
+
+    def _forward(self, image_pair, image2_2, outputs, stage_inputs, iterations):
         if stage_inputs:
             ip, i2 = self.stage(image_pair, image2_2)
         else:
-            ip, _ = _to_dev(image_pair, (b, 6, 192, 256), "image_pair")
-            i2 = None
-            if image2_2 is not None:
-                i2, _ = _to_dev(image2_2, (b, 3, 48, 64), "image2_2")
-        return self.forward_staged(outputs, ip, i2)
+            ip, _ = _to_dev(image_pair, (self.batch_size, 6, 192, 256), "image_pair")
+            i2 = self._stage_image2_2(ip, image2_2) if isinstance(image2_2, str) else image2_2
+            if i2 is not None and i2 is not self._i22:
+                i2, _ = _to_dev(i2, (self.batch_size, 3, 48, 64), "image2_2")
+        return self._run("demon_pipeline_forward", (ip.data_ptr(), _ptr(i2)), outputs, iterations=iterations)
 
     def forward_staged(self, outputs=None, ip=None, i2=None, use_image2_2=False):
         """The pipeline on inputs that are already in place: by default the pipeline's own staging buffers (filled by
@@ -326,11 +367,10 @@ class DemonPipeline:
 
     def own_snapshot_outputs(self, refine=True):
         """The persistent output buffers of forward_snapshots (S = iterations + 1 snapshots); one set per `refine`."""
-        b, s = self.batch_size, self.iterations + 1
-        shapes = {"predict_flow2": (s, b, 2, 48, 64), "predict_depth2": (s, b, 1, 48, 64), "predict_normal2": (s, b, 3, 48, 64),
-                  "predict_rotation": (s, b, 3), "predict_translation": (s, b, 3)}
-        if refine:
-            shapes["predict_depth0"] = (s, b, 1, 192, 256)
+        s = self.iterations + 1
+        shapes = {k: (s,) + v for k, v in self._output_shapes().items()}
+        if not refine:
+            shapes = {k: v for k, v in shapes.items() if k not in ("predict_depth0", "predict_normal0")}
         return self._own("_snap_refined" if refine else "_snap", shapes)
 
     def forward_snapshots(self, image_pair, image2_2=None, refine=True, outputs=None):
@@ -344,8 +384,8 @@ class DemonPipeline:
         if outputs is None:
             outputs = self.own_snapshot_outputs(refine)
         # without `refine` no depth0 pointer, which is what skips the refinement
-        self._run("demon_pipeline_forward_snapshots", (ip.data_ptr(), _ptr(i2)),
-                  outputs if refine else dict(outputs, predict_depth0=None), _SNAPSHOT_OUTPUTS)
+        self._run("demon_pipeline_forward_snapshots", (ip.data_ptr(), _ptr(i2)) + self._mode_args(0),
+                  outputs if refine else dict(outputs, predict_depth0=None, predict_normal0=None), self._snapshot_keys)
         return outputs
 
     def snapshot_launches(self):
@@ -356,6 +396,7 @@ class DemonPipeline:
         PIL gives them (HWC RGB), image2_2 [B,48,64,3] or None (median3x3_downsample twice).  /255 - 0.5 and the pair
         concat run on the device (examples/example.py:15-42); same outputs as forward(), bit for bit."""
         b = self.batch_size
+        image2_2, mode = self._image2_2_source(image2_2)
         if not (isinstance(images, torch.Tensor) and images.is_cuda and images.dtype == torch.uint8 and tuple(images.shape) == (b, 2, 192, 256, 3)):
             raise ValueError("images: expected a CUDA uint8 tensor of shape %s" % ((b, 2, 192, 256, 3),))
         if image2_2 is not None and not (isinstance(image2_2, torch.Tensor) and image2_2.is_cuda and image2_2.dtype == torch.uint8
@@ -364,18 +405,18 @@ class DemonPipeline:
         images = images.contiguous()
         if image2_2 is not None:
             image2_2 = image2_2.contiguous()
-        return self._run("demon_pipeline_forward_u8", (images.data_ptr(), _ptr(image2_2)), outputs)
+        return self._run("demon_pipeline_forward_u8", (images.data_ptr(), _ptr(image2_2)) + self._mode_args(mode), outputs)
 
     def _check_pairs(self, images, resample, image2_2):
         """The checks of forward_images / forward_views; returns h, w, the resample code and the image2_2 mode."""
         from .images import check_images, resample_code
         code = resample_code(resample)
-        if image2_2 not in ("resize", "median"):
-            raise ValueError("image2_2 must be 'resize' or 'median', got %r" % (image2_2,))
+        if image2_2 not in self._modes:
+            raise ValueError("image2_2 must be %s, got %r" % (" or ".join(", ".join(repr(m) for m in self._modes).rsplit(", ", 1)), image2_2))
         check_images(images, "images", 5)
         if tuple(images.shape[:2]) != (self.batch_size, 2):
             raise ValueError("images: expected shape (%d, 2, h, w, 3), got %s" % (self.batch_size, tuple(images.shape)))
-        return images.shape[2], images.shape[3], code, 1 if image2_2 == "resize" else 0
+        return images.shape[2], images.shape[3], code, self._modes[image2_2]
 
     def forward_images(self, images, resample="bicubic", image2_2="resize", outputs=None):
         """The pipeline on image pairs of any size (examples/example.py:15-42 and :87-99 in one call): images CUDA uint8
@@ -409,27 +450,41 @@ class DemonPipeline:
                         (images.data_ptr(), *images.stride()[:3], h, w, self._K.data_ptr(), self._status.data_ptr(), code, mode), outputs)
         return dict(out, status=self._status)
 
+    def _host(self, entry, inputs, image2_2, outputs, stream):
+        """A host entry: `inputs` and `image2_2` host buffers (image2_2 may also be None or a mode name), `outputs` the host
+        buffers by key (the class's _host_keys; depth0 is required)."""
+        image2_2, mode = self._image2_2_source(image2_2)
+        s = ctypes.c_void_p((stream or torch.cuda.current_stream()).cuda_stream)
+        fn = getattr(_lib.load(), entry + self._suffix)
+        _lib.check(fn(self.net.ptr, _ptr(inputs), _ptr(image2_2), *self._mode_args(mode), self.iterations,
+                      *(_ptr(outputs.get(k)) for k in self._host_keys), s))
+
     def forward_host_u8(self, images, image2_2, depth0, rotation, translation, stream=None, sync=True):
         """End to end from HOST uint8 images [B,2,192,256,3] (numpy or pinned torch CPU uint8): H2D of the bytes, the
         pipeline, D2H of depth0 / rotation / translation.  sync=False: asynchronous on `stream` like forward_host_async."""
-        s = ctypes.c_void_p((stream or torch.cuda.current_stream()).cuda_stream)
-        fn = _lib.load().demon_pipeline_forward_host_u8 if sync else _lib.load().demon_pipeline_forward_host_u8_async
-        _lib.check(fn(self.net.ptr, _ptr(images), _ptr(image2_2), self.iterations, _ptr(depth0), _ptr(rotation), _ptr(translation), s))
+        self._host("demon_pipeline_forward_host_u8" if sync else "demon_pipeline_forward_host_u8_async", images, image2_2,
+                   {"predict_depth0": depth0, "predict_rotation": rotation, "predict_translation": translation}, stream)
 
     def forward_host(self, image_pair, image2_2, depth0, rotation, translation):
         """End-to-end call on HOST buffers (pinned torch CPU tensors or numpy arrays): H2D, pipeline, D2H and a
         stream synchronise inside the C call."""
-        _lib.check(_lib.load().demon_pipeline_forward_host(
-            self.net.ptr, _ptr(image_pair), _ptr(image2_2), self.iterations, _ptr(depth0), _ptr(rotation), _ptr(translation), _stream()))
+        self._host("demon_pipeline_forward_host", image_pair, image2_2,
+                   {"predict_depth0": depth0, "predict_rotation": rotation, "predict_translation": translation}, None)
         # (the C call synchronises and returns DEMON_E_STATE itself if a tensor-core pipeline wait timed out)
 
     def forward_host_async(self, image_pair, image2_2, depth0, rotation, translation, stream=None):
         """forward_host without the final synchronisation, on `stream` (a torch.cuda.Stream; default: current).  The host
         buffers must be pinned and are valid after `stream.synchronize()`.  Two DemonPipeline objects on two Sessions'
         nets and two streams overlap one batch's copies with the other's compute."""
-        s = ctypes.c_void_p((stream or torch.cuda.current_stream()).cuda_stream)
-        _lib.check(_lib.load().demon_pipeline_forward_host_async(
-            self.net.ptr, _ptr(image_pair), _ptr(image2_2), self.iterations, _ptr(depth0), _ptr(rotation), _ptr(translation), s))
+        self._host("demon_pipeline_forward_host_async", image_pair, image2_2,
+                   {"predict_depth0": depth0, "predict_rotation": rotation, "predict_translation": translation}, stream)
 
     def launches(self):
         return _lib.load().demon_net_pipeline_launches(self.net.ptr, self.iterations)
+
+
+class DemonPipeline(_Pipeline):
+    """examples/example.py:87-99 as one device-resident call (channels_first only)."""
+
+    def __init__(self, session=None, batch_size=1, iterations=3, private_net=False):
+        super().__init__(session if session is not None else default_session(), batch_size, iterations, private_net)

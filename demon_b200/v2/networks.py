@@ -126,48 +126,61 @@ _OUTPUTS = ("predict_depth0", "predict_normal0", "predict_rotation", "predict_tr
             "predict_normal2")
 
 
-class DemonPipelineV2:
-    """examples/example_v2.py's bootstrap -> iterations -> refinement as one device-resident call (channels_first).  Like
-    networks_original.DemonPipeline it owns its input staging and output buffers, so every call replays one CUDA graph."""
+class DemonPipelineV2(_v1._Pipeline):
+    """examples/example_v2.py's bootstrap -> iterations -> refinement as one device-resident call (channels_first), with
+    every method of networks_original.DemonPipeline (stage, forward_staged, forward_snapshots, forward_u8, forward_images,
+    forward_views, the host entries) and v2's outputs: predict_normal0 [B,3,192,256] comes with predict_depth0 wherever the
+    refinement block runs.  Like DemonPipeline it owns its input staging and output buffers, so every call replays one CUDA
+    graph.
 
-    def __init__(self, session=None, batch_size=1, iterations=3):
-        self.session = session if session is not None else default_session()
-        self.batch_size = int(batch_size)
-        self.iterations = int(iterations)
-        self.net = self.session.net(self.batch_size)
-        self._ip = self._i22 = self._out = None
+    image2_2 may also be 'area': tf.image.resize_area of the second image to 48x64 (images.resize_area), the input
+    training/v2/training.py:179 trains v2 on.  forward / forward_snapshots stage it with images.resize_area, the uint8,
+    images, views and host entries compute it inside the pipeline from image 2's float planes (x/255 - 0.5 for uint8)."""
 
-    def own_outputs(self, device):
-        if self._out is None:
-            b = self.batch_size
-            shapes = {"predict_depth0": (b, 1, 192, 256), "predict_normal0": (b, 3, 192, 256), "predict_rotation": (b, 3),
-                      "predict_translation": (b, 3), "predict_flow2": (b, 2, 48, 64), "predict_depth2": (b, 1, 48, 64),
-                      "predict_normal2": (b, 3, 48, 64)}
-            self._out = {k: torch.empty(s, dtype=torch.float32, device=device) for k, s in shapes.items()}
-        return self._out
+    _handle = _NetHandleV2
+    _suffix = "_v2"
+    _keys = _snapshot_keys = _OUTPUTS
+    _host_keys = ("predict_depth0", "predict_normal0", "predict_rotation", "predict_translation")
+    _modes = {"resize": 1, "median": 0, "area": 2}
+    _area = True
 
-    def forward(self, image_pair, image2_2=None, iterations=None, outputs=None):
-        """image_pair [B,6,192,256], image2_2 [B,3,48,64] or None (median3x3_downsample twice of the second image);
+    def __init__(self, session=None, batch_size=1, iterations=3, private_net=False):
+        super().__init__(session if session is not None else default_session(), batch_size, iterations, private_net)
+
+    def _mode_args(self, mode):
+        return (mode,)
+
+    def _output_shapes(self):
+        return dict(super()._output_shapes(), predict_normal0=(self.batch_size, 3, 192, 256))
+
+    def own_outputs(self, device=None):
+        return self._own("_out", self._output_shapes(), device)
+
+    def forward(self, image_pair, image2_2=None, iterations=None, outputs=None, stage_inputs=True):
+        """image_pair [B,6,192,256], image2_2 [B,3,48,64], None (median3x3_downsample twice of the second image) or 'area';
         torch CUDA tensors or host arrays.  Returns a dict of torch CUDA tensors: predict_depth0, predict_normal0,
         predict_flow2, predict_depth2, predict_normal2, predict_rotation, predict_translation; no host synchronisation.
-        With `outputs=None` they belong to the pipeline and are overwritten by the next call."""
-        b = self.batch_size
-        ip, _ = _to_dev(image_pair, (b, 6, 192, 256), "image_pair")
-        if self._ip is None:
-            self._ip = torch.empty((b, 6, 192, 256), dtype=torch.float32, device=ip.device)
-            self._i22 = torch.empty((b, 3, 48, 64), dtype=torch.float32, device=ip.device)
-        self._ip.copy_(ip, non_blocking=True)
-        i2 = None
-        if image2_2 is not None:
-            t, _ = _to_dev(image2_2, (b, 3, 48, 64), "image2_2")
-            self._i22.copy_(t, non_blocking=True)
-            i2 = self._i22
-        if outputs is None:
-            outputs = self.own_outputs(ip.device)
-        it = self.iterations if iterations is None else int(iterations)
-        _lib.check(_lib.load().demon_pipeline_forward_v2(self.net.ptr, self._ip.data_ptr(), _ptr(i2), it,
-                                                         *(_ptr(outputs.get(k)) for k in _OUTPUTS), _stream()))
-        return outputs
+        With `outputs=None` they belong to the pipeline and are overwritten by the next call.  `stage_inputs` as in
+        DemonPipeline.forward."""
+        return self._forward(image_pair, image2_2, outputs, stage_inputs, iterations)
+
+    def forward_host_u8(self, images, image2_2, depth0, rotation, translation, stream=None, sync=True, normal0=None):
+        """DemonPipeline.forward_host_u8 with v2's optional normal0 [B,3,192,256] host buffer; image2_2 may be 'area'."""
+        self._host("demon_pipeline_forward_host_u8" if sync else "demon_pipeline_forward_host_u8_async", images, image2_2,
+                   {"predict_depth0": depth0, "predict_normal0": normal0, "predict_rotation": rotation, "predict_translation": translation},
+                   stream)
+
+    def forward_host(self, image_pair, image2_2, depth0, rotation, translation, normal0=None):
+        """DemonPipeline.forward_host with v2's optional normal0 [B,3,192,256] host buffer; image2_2 may be 'area'."""
+        self._host("demon_pipeline_forward_host", image_pair, image2_2,
+                   {"predict_depth0": depth0, "predict_normal0": normal0, "predict_rotation": rotation, "predict_translation": translation},
+                   None)
+
+    def forward_host_async(self, image_pair, image2_2, depth0, rotation, translation, stream=None, normal0=None):
+        """DemonPipeline.forward_host_async with v2's optional normal0 [B,3,192,256] host buffer; image2_2 may be 'area'."""
+        self._host("demon_pipeline_forward_host_async", image_pair, image2_2,
+                   {"predict_depth0": depth0, "predict_normal0": normal0, "predict_rotation": rotation, "predict_translation": translation},
+                   stream)
 
     def launches(self, iterations=None):
         return _lib.load().demon_net_pipeline_launches(self.net.ptr, self.iterations if iterations is None else int(iterations))

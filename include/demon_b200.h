@@ -85,6 +85,13 @@ int demon_leaky_relu_f64(const double* input, double* output, int64_t size, doub
 int demon_median3x3_downsample_f32(const float* input, float* output, int64_t z, int h, int w, void* stream);
 int demon_median3x3_downsample_f64(const double* input, double* output, int64_t z, int h, int w, void* stream);
 
+/* tf.image.resize_area(align_corners=False) by integer factors, the image2_2 of training/v2/training.py:179 (192x256 ->
+ * 48x64).  input [n,c,h,w] float32 with `in_sn` floats between samples (>= c*h*w; a channel slice of a wider batch is read
+ * in place) -> output [n,c,oh,ow] packed.  h % oh and w % ow must be 0 (DEMON_E_INVALID otherwise).  Every output is, in
+ * float32: each of the fy = h/oh source rows' fx = w/ow pixels summed left to right from +0, the fy row sums summed top to
+ * bottom from +0, times float32(1/(fy*fx)) -- this project's definition (DESIGN.md section 3.6). */
+int demon_resize_area_f32(const float* input, int64_t in_sn, float* output, int n, int c, int h, int w, int oh, int ow, void* stream);
+
 /* Replaces ScaleInvariantGradientOp forward (scaleinvariantgradient.cc:98-207,
  * scaleinvariantgradient_cuda.cu:56-102,205-320).  input [z,h,w] -> output [z,2,h,w].
  * deltas / weights are HOST arrays of length num (<= 16); they are op attributes in the reference. */
@@ -512,6 +519,42 @@ int demon_pipeline_forward_images_u8(demon_net* net, const uint8_t* images, int6
 int demon_pipeline_forward_views_u8(demon_net* net, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w,
                                     const double* K, uint8_t* status, int resample, int image2_2_mode, int iterations, float* depth0,
                                     float* rotation, float* translation, float* flow2, float* depth2, float* normal2, void* stream);
+
+/* The entries above for a v2 handle (demon_net_create_v2).  Arguments as their v1 twins, with two differences: the outputs
+ * come in demon_pipeline_forward_v2's order with normal0 [B,3,192,256] (snapshots: [S,B,3,192,256]) after depth0, and every
+ * entry takes an image2_2_mode:
+ *   0: the given image2_2, or without one median3x3_downsample twice of image 2 (examples/evaluation.py:170-173);
+ *   1: image 2 resized to 64x48 with the call's filter (examples/example_v2.py) -- images_u8 / views_u8 only;
+ *   2: tf.image.resize_area of image 2's float planes to 48x64, the input training/v2/training.py:179 trains v2 on
+ *      (demon_resize_area_f32 on x/255 - 0.5 for uint8 input); image2_2 must then be NULL.
+ * The v1 entries refuse mode 2.  Any device output may be NULL.  demon_pipeline_forward_snapshots_v2 runs the refinement block
+ * on every snapshot iff depth0 is given, and refuses normal0 without depth0.  The host entries need depth0_host; normal0_host,
+ * rotation_host and translation_host may be NULL. */
+int demon_pipeline_forward_snapshots_v2(demon_net* net, const float* image_pair, const float* image2_2, int image2_2_mode, int iterations,
+                                        float* depth0, float* normal0, float* rotation, float* translation, float* flow2, float* depth2,
+                                        float* normal2, void* stream);
+int demon_pipeline_forward_u8_v2(demon_net* net, const uint8_t* images, const uint8_t* image2_2, int image2_2_mode, int iterations,
+                                 float* depth0, float* normal0, float* rotation, float* translation, float* flow2, float* depth2,
+                                 float* normal2, void* stream);
+int demon_pipeline_forward_images_u8_v2(demon_net* net, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w,
+                                        int resample, int image2_2_mode, int iterations, float* depth0, float* normal0, float* rotation,
+                                        float* translation, float* flow2, float* depth2, float* normal2, void* stream);
+int demon_pipeline_forward_views_u8_v2(demon_net* net, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w,
+                                       const double* K, uint8_t* status, int resample, int image2_2_mode, int iterations, float* depth0,
+                                       float* normal0, float* rotation, float* translation, float* flow2, float* depth2, float* normal2,
+                                       void* stream);
+int demon_pipeline_forward_host_v2(demon_net* net, const float* image_pair_host, const float* image2_2_host, int image2_2_mode,
+                                   int iterations, float* depth0_host, float* normal0_host, float* rotation_host, float* translation_host,
+                                   void* stream);
+int demon_pipeline_forward_host_async_v2(demon_net* net, const float* image_pair_host, const float* image2_2_host, int image2_2_mode,
+                                         int iterations, float* depth0_host, float* normal0_host, float* rotation_host,
+                                         float* translation_host, void* stream);
+int demon_pipeline_forward_host_u8_v2(demon_net* net, const uint8_t* images_host, const uint8_t* image2_2_host, int image2_2_mode,
+                                      int iterations, float* depth0_host, float* normal0_host, float* rotation_host, float* translation_host,
+                                      void* stream);
+int demon_pipeline_forward_host_u8_async_v2(demon_net* net, const uint8_t* images_host, const uint8_t* image2_2_host, int image2_2_mode,
+                                            int iterations, float* depth0_host, float* normal0_host, float* rotation_host,
+                                            float* translation_host, void* stream);
 
 /* introspection for tests and bench */
 int demon_net_batch(const demon_net* net);
