@@ -110,6 +110,8 @@ PROTOTYPES = {
     "demon_sun3d_depth_u16": [_P, c_int, c_int, c_int, _P, _P, _P],
     "demon_depth_ratios_f32": [_P] * 5 + [c_int] * 3 + [_P, c_int, _P, _P],
     "demon_depth_consistency_counts_f32": [_P] * 5 + [c_int] * 3 + [_P, c_int, c_float, c_float, _P, _P],
+    "demon_datareader_prepare": [_P, _P, c_int, c_int, c_int, _P, _P, _P],
+    "demon_datareader_batch": [_P, _P, c_int, c_int, _P, c_int, c_int] + [c_float] * 4 + [c_int] * 4 + [_P] * 5,
     "demon_net_batch": [_P],
     "demon_net_workspace_bytes": [_P],
     "demon_net_pipeline_launches": [_P, c_int],

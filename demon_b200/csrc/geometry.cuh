@@ -286,10 +286,27 @@ __device__ __forceinline__ T sig_dneighbour(T c, T n, T eps) {
 }
 
 // ---- depth_to_normals (depthtonormals.cc:147-238) --------------------------------------------------------------------------
-// inv_K of K = [[fx*W, 0, cx*W], [0, fy*H, cy*H], [0, 0, 1]] the way Eigen 3.3 inverts a fixed 3x3 matrix
-// (Eigen/src/LU/InverseImpl.h, compute_inverse<.,.,3>: cofactors times 1/det), restricted to the four entries the op reads.
+// inv_K of K = [[a, s, cx], [0, b, cy], [0, 0, 1]] the way Eigen 3.3 inverts a fixed 3x3 matrix
+// (Eigen/src/LU/InverseImpl.h, compute_inverse<.,.,3>: cofactors times 1/det), restricted to the four entries the callers
+// read.  depth_to_normals passes s = 0; the multi-view reader's cameras (multivih5datareader.cpp:385,446,1497) keep a skew.
 template <class T>
 struct D2NCamera { T i00, i02, i11, i12; };
+
+template <class T>
+__device__ __forceinline__ D2NCamera<T> eigen_inverse_k(T a, T s, T b, T cx, T cy) {
+  // cofactors of column 0: (b*1 - cy*0, 0*cx - 1*s, s*cy - cx*b); det = (c0*a + c1*0) + c2*0; invdet = 1 / det
+  const T c0 = fsub(fmul(b, (T)1), fmul(cy, (T)0));
+  const T c1 = fsub(fmul((T)0, cx), fmul((T)1, s));
+  const T c2 = fsub(fmul(s, cy), fmul(cx, b));
+  const T det = fadd(fadd(fmul(c0, a), fmul(c1, (T)0)), fmul(c2, (T)0));
+  const T invdet = fdiv((T)1, det);
+  D2NCamera<T> c;
+  c.i00 = fmul(c0, invdet);                                                     // result.row(0) = cofactors_col0 * invdet
+  c.i02 = fmul(c2, invdet);
+  c.i11 = fmul(fsub(fmul((T)1, a), fmul((T)0, cx)), invdet);                    // cofactor<1,1> = m22*m00 - m20*m02
+  c.i12 = fmul(fsub(fmul(cx, (T)0), fmul(a, cy)), invdet);                      // cofactor<2,1> = m02*m10 - m00*m12
+  return c;
+}
 
 template <class T>
 __device__ __forceinline__ void d2n_point(T p[3], int x, int y, T depth, const D2NCamera<T>& c) {   // compute3dPoint, depthtonormals.cc:95-101
@@ -326,20 +343,8 @@ __device__ __forceinline__ void d2n_pixel(T nrm[3], const T* __restrict__ dm, co
   const bool bad = d <= 0 || !isfinite(d) || d_y0 <= 0 || !isfinite(d_y0) || d_x0 <= 0 || !isfinite(d_x0) || d_y1 <= 0 || !isfinite(d_y1) ||
                    d_x1 <= 0 || !isfinite(d_x1);
   if (bad) return;
-  D2NCamera<T> c;
-  {
-    const T a = fmul(__ldg(k + 0), (T)W), b = fmul(__ldg(k + 1), (T)H), cx = fmul(__ldg(k + 2), (T)W), cy = fmul(__ldg(k + 3), (T)H);
-    // cofactors of column 0: (b*1 - cy*0, 0*cx - 1*0, 0*cy - cx*b); det = (c0*a + c1*0) + c2*0; invdet = 1 / det
-    const T c0 = fsub(fmul(b, (T)1), fmul(cy, (T)0));
-    const T c1 = fsub(fmul((T)0, cx), fmul((T)1, (T)0));
-    const T c2 = fsub(fmul((T)0, cy), fmul(cx, b));
-    const T det = fadd(fadd(fmul(c0, a), fmul(c1, (T)0)), fmul(c2, (T)0));
-    const T invdet = fdiv((T)1, det);
-    c.i00 = fmul(c0, invdet);                                                     // result.row(0) = cofactors_col0 * invdet
-    c.i02 = fmul(c2, invdet);
-    c.i11 = fmul(fsub(fmul((T)1, a), fmul((T)0, cx)), invdet);                    // cofactor<1,1> = m22*m00 - m20*m02
-    c.i12 = fmul(fsub(fmul(cx, (T)0), fmul(a, cy)), invdet);                      // cofactor<2,1> = m02*m10 - m00*m12
-  }
+  const D2NCamera<T> c = eigen_inverse_k(fmul(__ldg(k + 0), (T)W), (T)0, fmul(__ldg(k + 1), (T)H), fmul(__ldg(k + 2), (T)W),
+                                         fmul(__ldg(k + 3), (T)H));
   T p[3], p_y0[3], p_x0[3], p_y1[3], p_x1[3];
   d2n_point(p, x, y, d, c);
   d2n_point(p_y0, x, y - 1, d_y0, c);

@@ -379,6 +379,44 @@ int demon_depth_consistency_counts_f32(const float* depth, const float* K, const
                                        int h, int w, const int* pairs, int n_pairs, float lo, float hi, int64_t* counts, void* stream);
 
 /* ------------------------------------------------------------------------
+ * Multi-view training reader (multivih5datareaderop/multivih5datareader.cpp): its per-pixel compute.
+ * ---------------------------------------------------------------------- */
+/* One view of a demon_datareader_prepare call.  image_offset / depth_offset are byte offsets into `staging`: the source
+ * image uint8 [height,width,3] RGB and its depth [height,width], float32 or (depth_f16) IEEE half.  k = the intrinsics
+ * normalised like prepareScene (:1393-1396) and cast to float: fx/W, skew (in pixels, not normalised), cx/W, fy/H, cy/H.
+ * ray_length: the depth is the distance along the ray and is converted to camera z. */
+typedef struct {
+  int64_t image_offset, depth_offset, pool_index;
+  int32_t width, height, depth_f16, ray_length;
+  float k[5];
+  int32_t pad;
+} demon_datareader_view;
+
+/* One batch item of demon_datareader_batch.  flags bit 0 = rot180, bit 1 = mirror_x.  aug = the colour draws hue, sat,
+ * val, contrast, brightness, gamma.  cam[i] = view i's [fx, skew, cx, fy, cy] as in demon_datareader_view, then R
+ * row-major [9] and t [3], cast to float from the unrotated double pose. */
+typedef struct {
+  int32_t view1, view2, flags, pad;
+  double depth_scale_factor;
+  float aug[6];
+  float cam[2][17];
+} demon_datareader_item;
+
+/* prepareScene (:1384-1520) of n_views views into the pool at their pool_index: pool_image [*,h,w,3] uint8 and pool_depth
+ * [*,h,w] float32 camera z.  The image is downscaled as cv::resize(INTER_AREA) defines it for width >= w and height >= h
+ * (the exact area-weighted mean rounded half to even, DESIGN.md section 3.8), the depth by cv::resize(INTER_NEAREST).
+ * One launch.  The caller guarantees width >= w, height >= h, both <= 8192, and offsets inside staging. */
+int demon_datareader_prepare(const uint8_t* staging, const demon_datareader_view* views, int n_views, int h, int w, uint8_t* pool_image,
+                             float* pool_depth, void* stream);
+/* The batch loop's outputs (:1585-1950) of `batch` items (a device table) from the prepared pool, in one launch:
+ * image_pair [batch,6,h,w], flow [batch,2,h,w], depth and depthmasks [batch,1 or 2 (depth_pair),h,w]; a NULL output is
+ * skipped.  colour applies augmentImage (:641-714) with each item's draws.  The caller guarantees view indices inside the
+ * pool. */
+int demon_datareader_batch(const uint8_t* pool_image, const float* pool_depth, int h, int w, const demon_datareader_item* items, int batch,
+                           int colour, float range_min, float range_max, float min_depth, float max_depth, int inverse_depth, int depth_pair,
+                           int border1, int border2, float* image_pair, float* flow, float* depth, float* depthmasks, void* stream);
+
+/* ------------------------------------------------------------------------
  * Network graphs (python/depthmotionnet/networks_original.py).
  * One handle = the five blocks netFlow1, netDM1, netFlow2, netDM2, netRefine for a
  * fixed batch size at 256x192 (networks_original.py:38-42), plus a refinement block that
