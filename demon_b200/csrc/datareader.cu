@@ -2,8 +2,10 @@
 // the device; demon_b200/datareader.py drives it and does the per-item pose math on the host.
 //
 // * prepare_kernel: prepareScene (:1384-1520) for a table of views of any source size: INTER_AREA downscaling of the uint8
-//   image (the exact area-weighted mean, rounded half to even), half -> float depth, INTER_NEAREST scaling of the depth and
-//   ray length -> camera z with the scaled float K.  One thread per output pixel, blockIdx.y = view.
+//   image by the path OpenCV's cv::resize takes for the view (the 2x2 vector path, the other integer factors, or the
+//   general float-weighted path), half -> float depth, INTER_NEAREST scaling of the depth and ray length -> camera z with
+//   the scaled float K.  One thread per output pixel, blockIdx.y = view.  Both resizes are bit for bit OpenCV 4.13.0's
+//   (tests/golden/datareader_resize_digests.json).
 // * batch_kernel: the batch loop (:1585-1950) for every item of a batch in one launch.  Each output pixel is remapped
 //   through the item's rot180 / mirror_x to the pixel of the prepared pool it comes from; IMAGE_PAIR (:344-363 and
 //   augmentImage :641-714), DEPTH (:1857-1908), FLOW (computeFlow :370-424 on the unrotated cameras, then negated) and
@@ -13,6 +15,7 @@
 // places where x86 and CUDA differ on NaN or on out-of-range conversions are restated explicitly (DESIGN.md section 3.8).
 #include "common.cuh"
 #include "geometry.cuh"
+#include <cfloat>
 #include <cstdint>
 
 namespace demon {
@@ -41,10 +44,78 @@ __device__ __forceinline__ float half_bits_to_float(uint16_t h) {
   return __uint_as_float(sign | ((e + 112u) << 23) | (m << 13));
 }
 
-// the source cells [i0, i1] that output cell `o` of an n -> m downscale covers, and the overlap of cell i with it, in units
-// of 1/m source cells: output cell o is [o*n, (o+1)*n), source cell i is [i*m, (i+1)*m)
-__device__ __forceinline__ int area_overlap(int i, int o, int n, int m) {
-  return min((i + 1) * m, (o + 1) * n) - max(i * m, o * n);
+// cv::resize(INTER_AREA) of uint8 images, downscaling only (imgproc/src/resize.cpp).  An axis of n -> m cells has the scale
+// 1 / (m / (double)n); it is integral when |scale - cvRound(scale)| < DBL_EPSILON, and for sides up to 8192 that implies
+// n = scale * m (the converse fails: 98 -> 2 has the scale 49.00000000000001).  Returns the integer factor, or 0.
+__device__ __forceinline__ int area_factor(double scale) {
+  const int k = __double2int_rn(scale);
+  return fabs(fsub(scale, (double)k)) < DBL_EPSILON ? k : 0;
+}
+
+// computeResizeAreaTab's entries of output index d: source cells lo..hi, consecutive, with the weight `lead` on cell lo if
+// `has_lead` (the leading partial cell), `trail` on cell hi if `has_trail` (the trailing one) and `full` on the others.
+// Each weight is computed in double and cast to float, as the table stores it.
+struct AreaCells {
+  int lo, hi;
+  bool has_lead, has_trail;
+  float lead, full, trail;
+  __device__ __forceinline__ float weight(int i) const { return (has_lead && i == lo) ? lead : (has_trail && i == hi) ? trail : full; }
+};
+
+__device__ __forceinline__ AreaCells area_cells(int d, int n, double scale) {
+  const double fs1 = fmul((double)d, scale), fs2 = fadd(fs1, scale);
+  const double cell = fmin(scale, fsub((double)n, fs1));
+  const int s2 = min((int)floor(fs2), n - 1);
+  const int s1 = min((int)ceil(fs1), s2);
+  AreaCells c;
+  c.has_lead = fsub((double)s1, fs1) > 1e-3;   // a sliver of at most 1e-3 of a cell gets no entry
+  c.has_trail = fsub(fs2, (double)s2) > 1e-3;
+  c.lo = c.has_lead ? s1 - 1 : s1;
+  c.hi = c.has_trail ? s2 : s2 - 1;
+  c.lead = __double2float_rn(fdiv(fsub((double)s1, fs1), cell));
+  c.full = __double2float_rn(fdiv(1.0, cell));
+  c.trail = __double2float_rn(fdiv(fmin(fmin(fsub(fs2, (double)s2), 1.0), cell), cell));
+  return c;
+}
+
+// Output pixel (x, y) of INTER_AREA, per channel, by the path OpenCV takes for the view (both axes integral or not):
+//   2x2          (a + b + c + d + 2) >> 2, ties up (ResizeAreaFastVec);
+//   other k x l  float(int block sum) * (1.f / (k * l)), cvRound: ties to even (resizeAreaFast_);
+//   otherwise    ResizeArea_Invoker: per source row, buf = buf + S * alpha over the x cells in order, in float; then
+//                sum = beta * buf for the first row, sum = sum + beta * buf for the rest; cvRound.
+__device__ __forceinline__ void area_pixel(const uint8_t* __restrict__ img, int sh, int sw, int x, int y, double scale_x,
+                                           double scale_y, uint8_t out[3]) {
+  const int kx = area_factor(scale_x), ky = area_factor(scale_y);
+  if (kx && ky) {
+    unsigned acc[3] = {0, 0, 0};   // OpenCV's block sum is an int, which wraps (two's complement) above 2^31 - 1
+    for (int sy = y * ky; sy < (y + 1) * ky; ++sy) {
+      const uint8_t* q = img + ((long)sy * sw + (long)x * kx) * 3;
+      for (int i = 0; i < kx * 3; i += 3)
+#pragma unroll
+        for (int c = 0; c < 3; ++c) acc[c] += __ldg(q + i + c);
+    }
+    const float inv_area = fdiv(1.0f, (float)(kx * ky));   // 1.f / area: an area above 2^24 is rounded to float first
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      out[c] = (kx == 2 && ky == 2) ? (uint8_t)((acc[c] + 2) >> 2) : (uint8_t)min(max(__float2int_rn(fmul((float)(int)acc[c], inv_area)), 0), 255);
+    return;
+  }
+  const AreaCells cx = area_cells(x, sw, scale_x), cy = area_cells(y, sh, scale_y);
+  float sum[3] = {0.0f, 0.0f, 0.0f};
+  for (int sy = cy.lo; sy <= cy.hi; ++sy) {
+    const uint8_t* row = img + (long)sy * sw * 3;
+    float buf[3] = {0.0f, 0.0f, 0.0f};
+    for (int sx = cx.lo; sx <= cx.hi; ++sx) {
+      const float alpha = cx.weight(sx);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) buf[c] = fadd(buf[c], fmul((float)__ldg(row + sx * 3 + c), alpha));
+    }
+    const float beta = cy.weight(sy);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) sum[c] = sy == cy.lo ? fmul(beta, buf[c]) : fadd(sum[c], fmul(beta, buf[c]));
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) out[c] = (uint8_t)min(max(__float2int_rn(sum[c]), 0), 255);
 }
 
 __global__ void __launch_bounds__(kThreads) prepare_kernel(const uint8_t* __restrict__ staging, const demon_datareader_view* __restrict__ views,
@@ -54,33 +125,16 @@ __global__ void __launch_bounds__(kThreads) prepare_kernel(const uint8_t* __rest
   const demon_datareader_view v = views[blockIdx.y];
   const int x = p % w, y = p / w;
   const int sw = v.width, sh = v.height;
+  // cv::resize's scale of each axis, 1 / inv_scale with inv_scale = dsize / (double)ssize: both calls use it
+  const double ifx = fdiv(1.0, fdiv((double)w, (double)sw)), ify = fdiv(1.0, fdiv((double)h, (double)sh));
 
-  // cv::resize(INTER_AREA) for sw >= w, sh >= h: sum(v * ox * oy) / (sw * sh), exact in 64-bit integers
-  const int x0 = (int)(((long)x * sw) / w), x1 = (int)(((long)(x + 1) * sw - 1) / w);
-  const int y0 = (int)(((long)y * sh) / h), y1 = (int)(((long)(y + 1) * sh - 1) / h);
-  const uint8_t* img = staging + v.image_offset;
-  unsigned long long acc[3] = {0, 0, 0};
-  for (int sy = y0; sy <= y1; ++sy) {
-    const unsigned long long oy = (unsigned long long)area_overlap(sy, y, sh, h);
-    for (int sx = x0; sx <= x1; ++sx) {
-      const unsigned long long o = oy * (unsigned long long)area_overlap(sx, x, sw, w);
-      const uint8_t* q = img + ((long)sy * sw + sx) * 3;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) acc[c] += o * __ldg(q + c);
-    }
-  }
-  const unsigned long long den = (unsigned long long)sw * (unsigned long long)sh;
+  uint8_t rgb[3];
+  area_pixel(staging + v.image_offset, sh, sw, x, y, ifx, ify, rgb);
   uint8_t* out = pool_image + ((long)v.pool_index * h * w + p) * 3;
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    unsigned long long q = acc[c] / den;
-    const unsigned long long r2 = 2 * (acc[c] - q * den);
-    if (r2 > den || (r2 == den && (q & 1))) ++q;   // round half to even
-    out[c] = (uint8_t)q;
-  }
+  for (int c = 0; c < 3; ++c) out[c] = rgb[c];
 
-  // cv::resize(INTER_NEAREST): sx = cvFloor(x * (1 / (w / (double)sw))), clamped
-  const double ifx = fdiv(1.0, fdiv((double)w, (double)sw)), ify = fdiv(1.0, fdiv((double)h, (double)sh));
+  // cv::resize(INTER_NEAREST): sx = cvFloor(x * ifx), clamped
   const int sx = min((int)floor(fmul((double)x, ifx)), sw - 1), sy = min((int)floor(fmul((double)y, ify)), sh - 1);
   const long si = (long)sy * sw + sx;
   float d = v.depth_f16 ? half_bits_to_float(__ldg(reinterpret_cast<const uint16_t*>(staging + v.depth_offset) + si))

@@ -403,8 +403,9 @@ typedef struct {
 } demon_datareader_item;
 
 /* prepareScene (:1384-1520) of n_views views into the pool at their pool_index: pool_image [*,h,w,3] uint8 and pool_depth
- * [*,h,w] float32 camera z.  The image is downscaled as cv::resize(INTER_AREA) defines it for width >= w and height >= h
- * (the exact area-weighted mean rounded half to even, DESIGN.md section 3.8), the depth by cv::resize(INTER_NEAREST).
+ * [*,h,w] float32 camera z.  The image is downscaled as cv::resize(INTER_AREA) does for width >= w and height >= h, in
+ * OpenCV's three paths (2x2, other integer factors, general; DESIGN.md section 3.8), the depth by cv::resize(INTER_NEAREST);
+ * both bit for bit OpenCV 4.13.0.
  * One launch.  The caller guarantees width >= w, height >= h, both <= 8192, and offsets inside staging. */
 int demon_datareader_prepare(const uint8_t* staging, const demon_datareader_view* views, int n_views, int h, int w, uint8_t* pool_image,
                              float* pool_depth, void* stream);

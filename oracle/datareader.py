@@ -7,8 +7,10 @@ numpy's IEEE float32 element-wise ops, which are not contracted into FMAs, as th
 the reader calls into Eigen or OpenCV, the published algorithm is restated and says so:
   - Matrix products sum left to right, the 3x3 inverse is cofactors times 1/det (as oracle/ref_stub/eigen_stub.h);
   - the 4x4 determinant, Quaternion(Matrix3d) and AngleAxis(Quaternion) are Eigen 3.3's formulas;
-  - cv::resize INTER_AREA for downscaling is the exact area-weighted mean rounded half to even (the project's definition,
-    DESIGN.md section 3.8; unverified against OpenCV), INTER_NEAREST is sx = floor(x * (1 / (dw / sw))).
+  - cv::resize INTER_AREA for downscaling is OpenCV's three paths (below; DESIGN.md section 3.8) and INTER_NEAREST is
+    sx = floor(x * (1 / (dw / sw))), clamped.  Both are held bit for bit to OpenCV 4.13.0's results
+    (tests/test_datareader_opencv.py and tests/golden/datareader_resize_digests.json); the reference's build used
+    OpenCV 2.4.9, whose resize code is believed to be the same but has not been run against this.
 The pose math is float64.  The flips are applied as the reader applies them: the whole plane reversed, rows reversed.
 """
 import math
@@ -20,25 +22,90 @@ _NAN = np.array([0x7fc00000], np.uint32).view(np.float32)[0]   # the C macro NAN
 
 
 # ---- prepareScene (:1384-1520) -----------------------------------------------------------------------------------------
-def _area_weights(n, m):
-    """[m, n] integer overlap of output cell o = [o*n, (o+1)*n) with source cell i = [i*m, (i+1)*m)."""
-    o = np.arange(m)[:, None]
-    i = np.arange(n)[None, :]
-    return np.maximum(0, np.minimum((i + 1) * m, (o + 1) * n) - np.maximum(i * m, o * n)).astype(np.int64)
+# cv::resize(INTER_AREA) of uint8 images, downscaling only (imgproc/src/resize.cpp), in one of three paths per view:
+#   '2x2'      both axes at the integer factor 2: (a + b + c + d + 2) >> 2, half up (ResizeAreaFastVec);
+#   'fast'     both axes at an integer factor, any other pair: float(int block sum) * (1.f / area), cvRound (resizeAreaFast_);
+#   'general'  otherwise: computeResizeAreaTab's float weights, float accumulation (ResizeArea_Invoker).
+# An axis takes an integer factor when |scale - cvRound(scale)| < DBL_EPSILON for scale = 1 / (dsize / (double)ssize):
+# not the same as "ssize divisible by dsize" (98 -> 2 is divisible, and its scale 49.00000000000001 is not integral).
+DBL_EPSILON = float(np.finfo(np.float64).eps)
+
+
+def area_scale(n, m):
+    """cv::resize's scale along an axis of n source cells -> m output cells: 1 / inv_scale, inv_scale = m / (double)n."""
+    return 1.0 / (m / float(n))
+
+
+def area_factor(n, m):
+    """The integer factor of n -> m when INTER_AREA's integer test passes along that axis, else None."""
+    s = area_scale(n, m)
+    k = round(s)   # saturate_cast<int>(double) is cvRound: half to even, as Python's round
+    return k if abs(s - k) < DBL_EPSILON else None
+
+
+def area_path(sh, sw, h, w):
+    """'2x2', 'fast' or 'general': which of INTER_AREA's paths an sh x sw -> h x w downscale takes."""
+    ky, kx = area_factor(sh, h), area_factor(sw, w)
+    if ky is None or kx is None:
+        return 'general'
+    return '2x2' if (ky, kx) == (2, 2) else 'fast'
+
+
+def area_table(n, m):
+    """computeResizeAreaTab for n -> m as [m, K] source indices and float32 weights: row d holds output d's entries in the
+    table's order (the leading partial cell, the full cells, the trailing partial cell; consecutive source cells), padded
+    with (0, +0).  Every step is the double arithmetic of the table, element-wise."""
+    scale = area_scale(n, m)
+    fs1 = np.arange(m) * scale
+    fs2 = fs1 + scale
+    cell = np.minimum(scale, n - fs1)
+    s2 = np.minimum(np.floor(fs2), n - 1)
+    s1 = np.minimum(np.ceil(fs1), s2)
+    lead, trail = s1 - fs1 > 1e-3, fs2 - s2 > 1e-3
+    lo = np.where(lead, s1 - 1, s1).astype(np.int64)
+    hi = np.where(trail, s2, s2 - 1).astype(np.int64)
+    k = int((hi - lo).max()) + 1
+    idx = lo[:, None] + np.arange(k)[None, :]
+    wt = np.broadcast_to((1.0 / cell).astype(np.float32)[:, None], (m, k)).copy()
+    wt[lead, 0] = ((s1 - fs1) / cell).astype(np.float32)[lead]
+    rows = np.nonzero(trail)[0]
+    wt[rows, (hi - lo)[rows]] = (np.minimum(np.minimum(fs2 - s2, 1.0), cell) / cell).astype(np.float32)[rows]
+    pad = idx > hi[:, None]
+    idx[pad], wt[pad] = 0, 0
+    return idx, wt
+
+
+def _area_general(img, h, w):
+    sh, sw = img.shape[:2]
+    xi, xa = area_table(sw, w)
+    yi, ya = area_table(sh, h)
+    src = img.astype(np.float32)
+    # horizontal: buf[dx] = buf[dx] + S[sx] * alpha per source row, in the x table's order (a padded +0 term adds nothing)
+    buf = np.zeros((sh, w, img.shape[2]), np.float32)
+    for k in range(xi.shape[1]):
+        buf = buf + src[:, xi[:, k]] * xa[None, :, k, None]
+    # vertical: sum = beta * buf for an output row's first source row, then sum = sum + beta * buf
+    acc = ya[:, 0, None, None] * buf[yi[:, 0]]
+    for k in range(1, yi.shape[1]):
+        acc = acc + ya[:, k, None, None] * buf[yi[:, k]]
+    return np.clip(np.rint(acc), 0, 255).astype(np.uint8)   # saturate_cast<uchar>: cvRound, half to even
 
 
 def area_downscale(img, h, w):
+    """cv::resize(img, (w, h), INTER_AREA) of a uint8 [sh, sw, c] image with h <= sh and w <= sw."""
+    img = np.asarray(img, np.uint8)
     sh, sw = img.shape[:2]
-    wy, wx = _area_weights(sh, h), _area_weights(sw, w)
-    den = sh * sw
-    out = np.empty((h, w, img.shape[2]), np.uint8)
-    for c in range(img.shape[2]):
-        # integer sums below 2^53: exact in float64, whatever order the matrix product sums in
-        acc = np.rint(wy.astype(np.float64) @ img[:, :, c].astype(np.float64) @ wx.T.astype(np.float64)).astype(np.int64)
-        q, r = acc // den, acc % den
-        q = q + ((2 * r > den) | ((2 * r == den) & (q % 2 == 1)))   # round half to even
-        out[:, :, c] = q
-    return out
+    assert h <= sh and w <= sw, "INTER_AREA's upscaling is not restated"
+    path = area_path(sh, sw, h, w)
+    if path == 'general':
+        return _area_general(img, h, w)
+    ky, kx = sh // h, sw // w
+    blocks = img.reshape(h, ky, w, kx, img.shape[2]).astype(np.int64).sum((1, 3))
+    if path == '2x2':
+        return ((blocks + 2) >> 2).astype(np.uint8)
+    blocks = ((blocks + 2 ** 31) % 2 ** 32 - 2 ** 31).astype(np.int32)   # the sum is an int: it wraps above 2^31 - 1
+    scale = f32(1) / f32(kx * ky)   # 1.f / area: above 2^24 the area itself is rounded to float first
+    return np.clip(np.rint(blocks.astype(np.float32) * scale), 0, 255).astype(np.uint8)
 
 
 def nearest_indices(n, m):   # cv::resize INTER_NEAREST: cvFloor(x * ifx), ifx = 1 / (m / (double)n), clamped

@@ -126,14 +126,18 @@ def test_refusals_before_the_device():
         dr.build_batch(pool, [(0, 1)], {'batch_size': 1, 'scaled_width': 640}, aug)
 
 
-def test_oracle_area_scaling_definition():
-    """The area mean at factor 2.5 is k/25 (no ties) and equals the float64 box mean rounded; at factor 2 a constructed
-    tie rounds to even."""
+def test_oracle_area_scaling_is_opencvs():
+    """cv::resize(INTER_AREA) as the oracle restates it: at 640x480 -> 256x192 (factor 2.5) every value is the exact
+    area mean k/25 rounded (the 2x-upsampled image's 5x5 block sums over 25); at factor 2 a tie rounds up; at factor 3
+    the value is float(sum) * (1.f / 9), rounded half to even."""
     rng = np.random.default_rng(5)
     img = rng.integers(0, 256, (480, 640, 3), dtype=np.uint8)
     out = od.area_downscale(img, 192, 256)
-    wy, wx = od._area_weights(480, 192) / 480.0, od._area_weights(640, 256) / 640.0
-    exact = np.stack([wy @ img[:, :, c].astype(np.float64) @ wx.T for c in range(3)], -1)
-    assert np.array_equal(out, np.rint(exact).astype(np.uint8))
-    tie = np.array([[[1, 2, 0], [2, 3, 0]], [[1, 2, 0], [2, 3, 0]]], np.uint8)   # means 1.5, 2.5 -> 2, 2
-    assert list(od.area_downscale(tie, 1, 1)[0, 0]) == [2, 2, 0]
+    up = img.repeat(2, 0).repeat(2, 1).astype(np.int64)
+    sums = up.reshape(192, 5, 256, 5, 3).sum((1, 3))
+    assert np.array_equal(out, np.rint(sums / 25).astype(np.uint8))
+    tie = np.array([[[1, 2, 0], [2, 3, 0]], [[1, 2, 0], [2, 3, 0]]], np.uint8)   # means 1.5, 2.5, 0
+    assert list(od.area_downscale(tie, 1, 1)[0, 0]) == [2, 3, 0]
+    block = rng.integers(0, 256, (3, 3, 3), dtype=np.uint8)
+    s = block.astype(np.int64).sum((0, 1))
+    assert np.array_equal(od.area_downscale(block, 1, 1)[0, 0], np.rint(s.astype(np.float32) * (np.float32(1) / np.float32(9))))

@@ -115,18 +115,19 @@ def test_odd_sizes_ray_length_half_depth_pair(fmt, colour):
 
 
 @pytest.mark.parametrize("colour", [False, True])
-def test_integer_factor_with_ties_and_equal_size(colour):
-    """128x96 -> 64x48 (factor 2) with constructed ties, and 64x48 -> 64x48, in one pool with a 131x97 source."""
+def test_integer_factor_ties_round_up_and_equal_size(colour):
+    """128x96 -> 64x48 (factor 2, OpenCV's 2x2 path: ties round up) with constructed ties, and 64x48 -> 64x48, in one
+    pool with a 131x97 source."""
     raw = od.synthetic_views(3, 96, 128, 31)
     img = raw[0][3]
-    img[0:2, 0:2] = [[[1, 2, 3], [2, 3, 3]], [[1, 2, 4], [2, 3, 4]]]   # means 1.5, 2.5, 3.5 -> 2, 2, 4
+    img[0:2, 0:2] = [[[1, 2, 3], [2, 3, 3]], [[1, 2, 4], [2, 3, 4]]]   # means 1.5, 2.5, 3.5 -> 2, 3, 4 (ties up)
     img[2:4, 0:2] = 0
-    img[2, 0] = [2, 2, 2]                                               # mean 0.5 -> 0
+    img[2, 0] = [2, 2, 2]                                               # mean 0.5 -> 1
     raw += od.synthetic_views(2, 48, 64, 32) + od.synthetic_views(1, 97, 131, 33)
     pool = dr.ViewPool(64, 48)
     idx = pool.add([View(*v) for v in raw])
     prepared = _check_pool(pool, idx, raw, 48, 64)
-    assert list(pool.images[0, 0, 0].cpu().numpy()) == [2, 2, 4] and list(pool.images[0, 1, 0].cpu().numpy()) == [0, 0, 0]
+    assert list(pool.images[0, 0, 0].cpu().numpy()) == [2, 3, 4] and list(pool.images[0, 1, 0].cpu().numpy()) == [1, 1, 1]
     assert np.array_equal(pool.images[3].cpu().numpy(), raw[3][3])   # equal size: a copy
     params = {'batch_size': 8, 'motion_format': 'ANGLEAXIS7', 'inverse_depth': True}
     _compare(pool, prepared, [(0, 1), (1, 2), (3, 4), (4, 3), (0, 5), (5, 1), (2, 0), (3, 5)], params, _aug(8, colour, 5))
