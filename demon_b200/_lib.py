@@ -84,6 +84,8 @@ PROTOTYPES = {
     "demon_bootstrap_forward_v2": [_P] + [_P] * 8 + [c_int, _P],
     "demon_iterative_forward_v2": [_P] + [_P] * 12 + [c_int, _P],
     "demon_refine_forward_v2": [_P] * 6 + [c_int, _P],
+    "demon_flow_block_forward_v2": [_P, c_char_p] + [_P] * 9 + [c_int, _P],
+    "demon_depthmotion_block_forward_v2": [_P, c_char_p] + [_P] * 12 + [c_int, _P],
     "demon_pipeline_forward_v2": [_P, _P, _P, c_int] + [_P] * 7 + [_P],
     "demon_debug_describe_plan": [c_int] * 5 + [_P, c_int],
     "demon_pipeline_forward": [_P, _P, _P, c_int] + [_P] * 6 + [_P],

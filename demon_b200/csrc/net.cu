@@ -908,16 +908,18 @@ int area_launch(const float* in, float* out, int N, int C, int H, int W, int Ho,
 // Flow2 extra inputs (blocks_original.py:155-183): depth_to_flow(inverse_depth, normalize_flow) ->
 // zero where |flow| >= 1 or NaN -> warp2d(image2_2, normalized, 'value') -> NHWC12
 // [warped(3), flow(2), depth(1), normal(3), 0, 0, 0].  dn2 = [depth, normal] NHWC4, motion [B,8] = rot|trans|scale.
+// intrinsics: [B,4] normalised (fx, fy, cx, cy) of each sample (v2/blocks.py:154-161), or null for the constant the
+// networks use (networks_original.py:108, v2/networks.py:90)
 __global__ void __launch_bounds__(256) flow_extra_kernel(const float* __restrict__ dn2, const float* __restrict__ motion,
                                                         const float* __restrict__ image2_2, float* __restrict__ extra, int H, int W,
-                                                        int extra_pitch) {
+                                                        int extra_pitch, const float* __restrict__ intrinsics) {
   pdl_launch_dependents();   // common.cuh: programmatic dependent launch
   pdl_wait();
   __shared__ D2FCamera<float> cam;
   const int n = blockIdx.y;
   if (threadIdx.x == 0) {
     const float K[4] = {0.89115971f, 1.18821287f, 0.5f, 0.5f};  // networks_original.py:108
-    d2f_camera(cam, K, motion + 8 * n, motion + 8 * n + 3, DEMON_ROT_ANGLEAXIS3, W, H);
+    d2f_camera(cam, intrinsics ? intrinsics + 4 * n : K, motion + 8 * n, motion + 8 * n + 3, DEMON_ROT_ANGLEAXIS3, W, H);
   }
   __syncthreads();
   const int hw = H * W;
@@ -955,18 +957,21 @@ __device__ __forceinline__ float clip_0_50(float x) {
 }
 
 // DM extra inputs (blocks_original.py:336-364): warp2d(image2_2, flow2) ++ flowconf2 (++ flow_to_depth) -> NHWC8.
-// kClip (v2): the depth from flow is clipped to [0, 50] (v2/blocks.py:379)
+// kClip (v2): the depth from flow is clipped to [0, 50] (v2/blocks.py:379).  intrinsics as in flow_extra_kernel.
+// flow2: the flow that is warped with and turned into depth, NHWC with `flow2_pitch` floats per pixel, or null for the
+// first two channels of flowconf2 (the networks' case: prev_flow2 is a slice of prev_flowconf2)
 template <bool kClip>
 __global__ void __launch_bounds__(128) dm_extra_kernel(const float* __restrict__ flowconf2, const float* __restrict__ motion_prev,
                                                       const float* __restrict__ image2_2, float* __restrict__ extra, int H, int W,
-                                                      int extra_pitch, bool with_depth) {
+                                                      int extra_pitch, bool with_depth, const float* __restrict__ intrinsics,
+                                                      const float* __restrict__ flow2, int flow2_pitch) {
   pdl_launch_dependents();   // common.cuh: programmatic dependent launch
   pdl_wait();
   __shared__ F2DCamera cam;
   const int n = blockIdx.y;
   if (with_depth && threadIdx.x == 0) {
     const float K[4] = {0.89115971f, 1.18821287f, 0.5f, 0.5f};
-    f2d_camera(cam, K, motion_prev + 8 * n, motion_prev + 8 * n + 3, DEMON_ROT_ANGLEAXIS3, W, H);
+    f2d_camera(cam, intrinsics ? intrinsics + 4 * n : K, motion_prev + 8 * n, motion_prev + 8 * n + 3, DEMON_ROT_ANGLEAXIS3, W, H);
   }
   __syncthreads();
   const int hw = H * W;
@@ -974,7 +979,12 @@ __global__ void __launch_bounds__(128) dm_extra_kernel(const float* __restrict__
   if (i >= hw) return;
   const int y = i / W, x = i - y * W;
   const float4 fc = __ldg(reinterpret_cast<const float4*>(flowconf2) + (size_t)n * hw + i);
-  const WarpTap<float> t = warp2d_tap<float>(x, y, fc.x, fc.y, W, H, true);
+  float fx = fc.x, fy = fc.y;
+  if (flow2) {
+    const float* f = flow2 + ((size_t)n * hw + i) * flow2_pitch;
+    fx = __ldg(f); fy = __ldg(f + 1);
+  }
+  const WarpTap<float> t = warp2d_tap<float>(x, y, fx, fy, W, H, true);
   const bool valid = warp2d_valid(t.x0, t.y0, W, H);
   float wv[3];
 #pragma unroll
@@ -986,7 +996,7 @@ __global__ void __launch_bounds__(128) dm_extra_kernel(const float* __restrict__
     }
     wv[c] = r;
   }
-  float dff = with_depth ? f2d_pixel(fc.x, fc.y, x, y, cam, true, true) : 0.f;
+  float dff = with_depth ? f2d_pixel(fx, fy, x, y, cam, true, true) : 0.f;
   if (kClip) dff = clip_0_50(dff);
   float* o = extra + ((size_t)n * hw + i) * extra_pitch;
   *reinterpret_cast<float4*>(o) = make_float4(wv[0], wv[1], wv[2], fc.x);
@@ -1116,23 +1126,27 @@ int export_predictions(demon_net* n, float* flow5, float* flow2, float* depth2, 
 }
 
 // flow block (blocks_original.py:190-235); `head`: run conv1 / conv2 (false when the pipeline has hoisted them out of the
-// iteration loop)
-int run_flow_block(demon_net* n, const Block& b, bool iterative, cudaStream_t s, bool head = true) {
+// iteration loop); `intrinsics`: the cameras of the samples [B,4] on the device, or null for the networks' constant
+int run_flow_block(demon_net* n, const Block& b, bool iterative, cudaStream_t s, bool head = true, const float* intrinsics = nullptr) {
   int rc;
   if (head && (rc = run_layers(n, b.begin, b.head_end, s))) return rc;
   if (iterative) {
-    (void)launch_pdl(flow_extra_kernel, dim3(dim3(ceil_div(48 * 64, 256), n->B)), dim3(256), 0, s, n->dn2->p, n->motion->p, n->i22->p, n->extra_in->p, 48, 64, n->extra_in->C);
+    (void)launch_pdl(flow_extra_kernel, dim3(dim3(ceil_div(48 * 64, 256), n->B)), dim3(256), 0, s, n->dn2->p, n->motion->p, n->i22->p, n->extra_in->p, 48, 64, n->extra_in->C,
+                     intrinsics);
     DEMON_LAUNCH_CHECK();
   }
   return run_layers(n, b.head_end, b.end, s);
 }
 
-int run_dm_block(demon_net* n, const Block& b, bool iterative, cudaStream_t s, bool head = true) {
+// `flow2`: the flow the extra inputs warp with (NHWC, `flow2_pitch` floats per pixel), or null for flowconf2's first two
+// channels; `intrinsics` as in run_flow_block
+int run_dm_block(demon_net* n, const Block& b, bool iterative, cudaStream_t s, bool head = true, const float* intrinsics = nullptr,
+                 const float* flow2 = nullptr, int flow2_pitch = 0) {
   int rc;
   if (head && (rc = run_layers(n, b.begin, b.head_end, s))) return rc;
   // the previous motion is still in n->motion here: this block's motion_fc3 overwrites it later
   (void)launch_pdl(n->variant == 2 ? dm_extra_kernel<true> : dm_extra_kernel<false>, dim3(dim3(ceil_div(48 * 64, 128), n->B)), dim3(128), 0, s,
-                   n->flowconf2->p, n->motion->p, n->i22->p, n->extra_in->p, 48, 64, n->extra_in->C, iterative);
+                   n->flowconf2->p, n->motion->p, n->i22->p, n->extra_in->p, 48, 64, n->extra_in->C, iterative, intrinsics, flow2, flow2_pitch);
   DEMON_LAUNCH_CHECK();
   return run_layers(n, b.head_end, b.end, s);
 }
@@ -1375,21 +1389,31 @@ int demon_bootstrap_forward_v2(demon_net* n, const float* image_pair, const floa
   return bootstrap_impl(n, image_pair, image2_2, flow5, flow2, depth2, normal2, rotation, translation, data_format, stream);
 }
 
+// previous predictions -> dn2 (NHWC4) and motion [B,8], where the flow and DM blocks' extra inputs read them
+static int import_prev_depth_normal(demon_net* n, const float* depth2, const float* normal2, int data_format, cudaStream_t s) {
+  const int P = 48 * 64;
+  int rc;
+  if ((rc = strided_copy(depth2, n->dn2->p, n->B, P, 1, api_strides(data_format, P, 1), buf_strides(n->dn2), s))) return rc;
+  return strided_copy(normal2, n->dn2->p + 1, n->B, P, 3, api_strides(data_format, P, 3), buf_strides(n->dn2), s);
+}
+
+static int import_prev_motion(demon_net* n, const float* rotation, const float* translation, cudaStream_t s) {
+  int rc;
+  if ((rc = strided_copy(rotation, n->motion->p, n->B, 1, 3, {3, 0, 1}, {8, 0, 1}, s))) return rc;
+  return strided_copy(translation, n->motion->p + 3, n->B, 1, 3, {3, 0, 1}, {8, 0, 1}, s);
+}
+
 static int iterative_impl(demon_net* n, const float* image_pair, const float* image2_2, const float* depth2_in, const float* normal2_in,
                           const float* rotation_in, const float* translation_in, float* flow5, float* flow2, float* depth2,
                           float* normal2, float* rotation, float* translation, int data_format, void* stream) {
   DEMON_REQUIRE(image_pair && image2_2 && depth2_in && normal2_in && rotation_in && translation_in, "iterative: null input");
   DEMON_REQUIRE(data_format == 0 || data_format == 1, "iterative: data_format %d", data_format);
   cudaStream_t s = (cudaStream_t)stream;
-  const int P = 48 * 64;
   int rc;
   if ((rc = import_image_pair(n, image_pair, data_format, s))) return rc;
   if ((rc = import_image2_2(n, image2_2, data_format, s))) return rc;
-  // previous predictions -> dn2 (NHWC4) and motion
-  if ((rc = strided_copy(depth2_in, n->dn2->p, n->B, P, 1, api_strides(data_format, P, 1), buf_strides(n->dn2), s))) return rc;
-  if ((rc = strided_copy(normal2_in, n->dn2->p + 1, n->B, P, 3, api_strides(data_format, P, 3), buf_strides(n->dn2), s))) return rc;
-  if ((rc = strided_copy(rotation_in, n->motion->p, n->B, 1, 3, {3, 0, 1}, {8, 0, 1}, s))) return rc;
-  if ((rc = strided_copy(translation_in, n->motion->p + 3, n->B, 1, 3, {3, 0, 1}, {8, 0, 1}, s))) return rc;
+  if ((rc = import_prev_depth_normal(n, depth2_in, normal2_in, data_format, s))) return rc;
+  if ((rc = import_prev_motion(n, rotation_in, translation_in, s))) return rc;
   if ((rc = run_flow_block(n, n->flow2, true, s))) return rc;
   if ((rc = run_dm_block(n, n->dm2, true, s))) return rc;
   return export_predictions(n, flow5, flow2, depth2, normal2, rotation, translation, data_format, s);
@@ -1432,6 +1456,78 @@ int demon_refine_forward_v2(demon_net* n, const float* image1, const float* dept
   const int dh = n->RH / 4, dw = n->RW / 4;
   return run_refine_block_v2(n, image1, api_strides(data_format, P, 3), depth2, api_strides(data_format, (long)dh * dw, 1), dh, dw, depth0,
                              normal0, data_format, (cudaStream_t)stream);
+}
+
+// The scope of a block entry: `second` is set for the iterative block's scope (netFlow2 / netDM2), whose weights include
+// conv2_extra_inputs over the previous predictions.  Each argument in `args` must be given for that scope and absent for
+// the bootstrap one (netFlow1 / netDM1).
+struct BlockArg { const char* name; const void* p; };
+static int check_block_args(const char* entry, const char* scope, const char* first, const char* second_name, bool* second,
+                            const BlockArg* args, int nargs) {
+  DEMON_REQUIRE(scope, "%s: null scope", entry);
+  *second = strcmp(scope, second_name) == 0;
+  DEMON_REQUIRE(*second || strcmp(scope, first) == 0, "%s: scope must be %s or %s, got '%s'", entry, first, second_name, scope);
+  for (int k = 0; k < nargs; ++k) {
+    if (*second) DEMON_REQUIRE(args[k].p, "%s: scope %s needs %s", entry, scope, args[k].name);
+    else DEMON_REQUIRE(!args[k].p, "%s: scope %s takes no %s (its weights have no input for it)", entry, scope, args[k].name);
+  }
+  return DEMON_OK;
+}
+
+int demon_flow_block_forward_v2(demon_net* n, const char* scope, const float* image_pair, const float* image2_2, const float* intrinsics,
+                                const float* prev_depth2, const float* prev_normal2, const float* prev_rotation,
+                                const float* prev_translation, float* flowconf5, float* flowconf2, int data_format, void* stream) {
+  REQUIRE_READY_AS(n, 2);
+  bool iterative = false;
+  const BlockArg args[] = {{"intrinsics", intrinsics}, {"prev_predictions['predict_depth2']", prev_depth2},
+                           {"prev_predictions['predict_normal2']", prev_normal2},
+                           {"prev_predictions['predict_rotation']", prev_rotation},
+                           {"prev_predictions['predict_translation']", prev_translation}};
+  int rc;
+  if ((rc = check_block_args("flow_block", scope, "netFlow1", "netFlow2", &iterative, args, 5))) return rc;
+  // netFlow1 does not read image2_2 (v2/blocks.py:142-144), so there it may come or not
+  if (iterative) DEMON_REQUIRE(image2_2, "flow_block: scope %s needs image2_2", scope);
+  DEMON_REQUIRE(image_pair, "flow_block: null image_pair");
+  DEMON_REQUIRE(data_format == 0 || data_format == 1, "flow_block: data_format %d", data_format);
+  cudaStream_t s = (cudaStream_t)stream;
+  if ((rc = import_image_pair(n, image_pair, data_format, s))) return rc;
+  if (iterative) {
+    if ((rc = import_image2_2(n, image2_2, data_format, s))) return rc;
+    if ((rc = import_prev_depth_normal(n, prev_depth2, prev_normal2, data_format, s))) return rc;
+    if ((rc = import_prev_motion(n, prev_rotation, prev_translation, s))) return rc;
+  }
+  if ((rc = run_flow_block(n, iterative ? n->flow2 : n->flow1, iterative, s, true, intrinsics))) return rc;
+  if ((rc = export_slice(n, n->pf5, 0, 4, flowconf5, data_format, s))) return rc;
+  return export_slice(n, n->flowconf2, 0, 4, flowconf2, data_format, s);
+}
+
+int demon_depthmotion_block_forward_v2(demon_net* n, const char* scope, const float* image_pair, const float* image2_2,
+                                       const float* prev_flow2, const float* prev_flowconf2, const float* prev_rotation,
+                                       const float* prev_translation, const float* intrinsics, float* depth2, float* normal2,
+                                       float* rotation, float* translation, float* scale, int data_format, void* stream) {
+  REQUIRE_READY_AS(n, 2);
+  bool iterative = false;
+  const BlockArg args[] = {{"prev_rotation", prev_rotation}, {"prev_translation", prev_translation}, {"intrinsics", intrinsics}};
+  int rc;
+  if ((rc = check_block_args("depthmotion_block", scope, "netDM1", "netDM2", &iterative, args, 3))) return rc;
+  DEMON_REQUIRE(image_pair, "depthmotion_block: null image_pair");
+  DEMON_REQUIRE(image2_2, "depthmotion_block: null image2_2");
+  DEMON_REQUIRE(prev_flow2, "depthmotion_block: null prev_flow2");
+  DEMON_REQUIRE(prev_flowconf2, "depthmotion_block: null prev_flowconf2");
+  DEMON_REQUIRE(data_format == 0 || data_format == 1, "depthmotion_block: data_format %d", data_format);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int P = 48 * 64;
+  if ((rc = import_image_pair(n, image_pair, data_format, s))) return rc;
+  if ((rc = import_image2_2(n, image2_2, data_format, s))) return rc;
+  // prev_flowconf2 -> flowconf2 (NHWC4), prev_flow2 -> p2a's first two channels: p2a is next written by
+  // predict_depthnormal2/conv1, after the extra inputs have read it
+  if ((rc = strided_copy(prev_flowconf2, n->flowconf2->p, n->B, P, 4, api_strides(data_format, P, 4), buf_strides(n->flowconf2), s)))
+    return rc;
+  if ((rc = strided_copy(prev_flow2, n->p2a->p, n->B, P, 2, api_strides(data_format, P, 2), buf_strides(n->p2a), s))) return rc;
+  if (iterative && (rc = import_prev_motion(n, prev_rotation, prev_translation, s))) return rc;
+  if ((rc = run_dm_block(n, iterative ? n->dm2 : n->dm1, iterative, s, true, intrinsics, n->p2a->p, n->p2a->C))) return rc;
+  if ((rc = export_predictions(n, nullptr, nullptr, depth2, normal2, rotation, translation, data_format, s))) return rc;
+  return scale ? strided_copy(n->motion->p + 6, scale, n->B, 1, 1, {8, 0, 1}, {1, 0, 1}, s) : DEMON_OK;
 }
 
 // The intrinsics DeMoN was trained for (examples/example.py:51-61), in pixels of the 256x192 input

@@ -36,6 +36,18 @@ class Session(_v1.Session):
 
     _handle = _NetHandleV2
 
+    def load_weights(self, weights):
+        super().load_weights(weights)
+        self._kernel_l2 = None
+
+    def kernel_l2(self):
+        """v2.weights.kernel_l2 of the loaded weights, computed once per load_weights (v2.objective's regularisation)."""
+        if self.weights is None:
+            raise RuntimeError("Session.load_weights() has not been called")
+        if getattr(self, "_kernel_l2", None) is None:
+            self._kernel_l2 = W.kernel_l2(self.weights)
+        return self._kernel_l2
+
     def restore(self, save_path):
         if isinstance(save_path, dict):
             return self.load_weights(save_path)

@@ -91,6 +91,18 @@ def variable_specs():
     return out
 
 
+def kernel_l2(weights):
+    """OrderedDict: scope -> the sum over the scope's kernels (every conv, transposed conv and dense layer) of
+    tf.nn.l2_loss(kernel) = sum(kernel^2) / 2, in float64 over the float32 values, in the order of variable_specs.  Biases
+    carry no regulariser in v2/blocks.py."""
+    out = OrderedDict((scope, 0.0) for scope in SCOPES)
+    for name, (kind, _) in variable_specs().items():
+        if kind != "bias":
+            a = np.asarray(weights[name], dtype=np.float32).astype(np.float64).ravel()
+            out[name.split("/", 1)[0]] += 0.5 * float(np.dot(a, a))
+    return out
+
+
 # output resolution of every conv, input resolution of every transposed conv (as demon_b200.weights._TRUNK_RES)
 _TRUNK_RES = dict(_v1._TRUNK_RES, **{
     "motion_conv3y": (24, 64), "motion_conv3x": (24, 32), "motion_conv4y": (12, 32), "motion_conv4x": (12, 16),

@@ -499,6 +499,25 @@ int demon_iterative_forward_v2(demon_net* net, const float* image_pair, const fl
  * normal0 [B,3,H,W] (may be NULL).  normal2 is taken like the reference takes it and not read (may be NULL). */
 int demon_refine_forward_v2(demon_net* net, const float* image1, const float* depth2, const float* normal2,
                             float* depth0, float* normal0, int data_format, void* stream);
+/* One block of v2/blocks.py under a variable scope of training/v2/training.py, on each sample's own camera.
+ * demon_flow_block_forward_v2: flow_block, scope "netFlow1" or "netFlow2" -> flowconf5 [B,4,6,8] and flowconf2 [B,4,48,64]
+ * (flow x, y, confidence x, y).  netFlow2 needs image2_2 [B,3,48,64], intrinsics and the previous prediction's depth2
+ * [B,1,48,64], normal2 [B,3,48,64], rotation [B,3] and translation [B,3]; netFlow1 takes none of them (image2_2 is
+ * accepted and not read).
+ * demon_depthmotion_block_forward_v2: depthmotion_block, scope "netDM1" or "netDM2": image_pair, image2_2, prev_flow2
+ * [B,2,48,64] and prev_flowconf2 [B,4,48,64] always; netDM2 also needs prev_rotation, prev_translation and intrinsics, which
+ * netDM1 refuses -> depth2, normal2, rotation, translation and scale [B,1]; any output may be NULL.
+ * intrinsics: device float32 [B,4], normalised fx, fy, cx, cy of each sample (datareader INTRINSICS).  A mismatch between
+ * the scope and the arguments returns DEMON_E_INVALID with the argument's name.  The blocks run on the net's buffers
+ * like the stage entries above: calls on one handle must not overlap. */
+int demon_flow_block_forward_v2(demon_net* net, const char* scope, const float* image_pair, const float* image2_2,
+                                const float* intrinsics, const float* prev_depth2, const float* prev_normal2,
+                                const float* prev_rotation, const float* prev_translation, float* flowconf5, float* flowconf2,
+                                int data_format, void* stream);
+int demon_depthmotion_block_forward_v2(demon_net* net, const char* scope, const float* image_pair, const float* image2_2,
+                                       const float* prev_flow2, const float* prev_flowconf2, const float* prev_rotation,
+                                       const float* prev_translation, const float* intrinsics, float* depth2, float* normal2,
+                                       float* rotation, float* translation, float* scale, int data_format, void* stream);
 /* bootstrap, `iterations` x iterative and refinement of v2 in one call, as demon_pipeline_forward (one CUDA graph per
  * distinct call, image2_2 may be NULL, any output may be NULL); normal0 [B,3,192,256].  channels_first only. */
 int demon_pipeline_forward_v2(demon_net* net, const float* image_pair, const float* image2_2, int iterations,
