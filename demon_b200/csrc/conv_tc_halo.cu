@@ -31,7 +31,20 @@
 // Narrow single-n-tile layers keep their whole packed weight set (<= 96 KB) RESIDENT in shared memory, loaded once per CTA
 // instead of one small bulk copy per step.  Layers with few tiles split their K loop over several work items (split-K,
 // halo_splitk_reduce_kernel).  Variants: PER_TAP (images that are not made of whole 16 x 8 tiles: one 128-pixel TMA box per
-// step instead of a halo) and CIN8 (8-channel inputs: four taps x 8 channels per K = 32 step).
+// step instead of a halo), CIN8 (8-channel inputs: four taps x 8 channels per K = 32 step) and FOLD (below).
+//
+// Fold mode (FOLD = 9 or 3: narrow 3x3 stride-1 layers, Cout 16 or 20 / 24, on images of whole 12 x 16 tiles).  At N = 16 or
+// 32 a step's dozen tiny wgmma cost less than loading and splitting its A fragment, so these layers run INPUT-stationary
+// with the taps in N: the GEMM rows are the pixels of the tile's 14 x 18 halo box (padded to 256 rows), the columns are
+// (tap, output channel), and one K step multiplies a pixel with the weights of every folded tap:
+//
+//     acc[pixel][t][co] = sum_ci in[pixel][ci] * W[t][ci][co],     out[y][x][co] = sum_t acc[(y + dy_t, x + dx_t)][t][co]
+//
+// FOLD 9 (Cout 16): all nine taps, N = 144, one step per chunk.  FOLD 3 (Cout 24; N = 216 would not fit the registers):
+// the three dx taps of a row, N = 72, and dy as three steps per chunk that shift the A rows by whole halo rows (GEMM row
+// = pixel (r, c) of the 12 x 18 rows r + dy of the box).  Every pixel is loaded and split once per step instead of once
+// per tap.  The epilogue (col2im) stages a third of the accumulator columns at a time in shared memory and sums the taps
+// of each output in ascending tap order (deterministic), then adds the bias.
 //
 // Host side: tc_plan is the only place that decides whether a layer runs on this kernel and in which mode; tc_prepare
 // plans and packs a layer, conv_tc_launch launches it, and the per-device launch state and timeout flag live here too.
@@ -56,6 +69,7 @@ constexpr int kThreads = 384;            // producer warpgroup + two consumer wa
 constexpr int kConsumerWarps = 8;
 constexpr int kMaxAStages = 4;
 constexpr int kTileH = 16, kTileW = 8;
+constexpr int kFoldH = 12, kFoldW = 16;  // fold mode output tile: a 14 x 18 = 252-pixel halo box in 256 GEMM rows
 constexpr int kMaxPlanes = 4;
 constexpr int kPlanSms = 132;            // SM count the tiling model plans for (H100 SXM); the launch uses the device's count
 constexpr int kSmemBudget = 224 * 1024;  // dynamic shared memory of the plan's operand stages (+ 1 KB for alignment)
@@ -93,6 +107,9 @@ struct HaloParams {
   // describe the real taps, -1 = missing tap -> zero columns)
   int cin8, ntaps_real;
   int g_plane[kMaxTaps], g_aoff[kMaxTaps];
+  // fold mode: taps folded into N (9, 3; 0 in the other modes) and the GEMM's N = fold x (Cout rounded up to 8); the
+  // epilogue's staging buffer follows the weights
+  int fold, fold_n;
   HaloPlane planes[kMaxPlanes];
   int a_region_bytes;   // one halo stage (all planes)
   int sa;               // A (halo, shared memory) stages
@@ -136,7 +153,7 @@ __device__ __forceinline__ void wait_t(uint32_t bar, uint32_t parity, int* err, 
 // x / d for small d by one multiply (mul = 2^32 / d + 1, exact while x * d < 2^32; d == 1 -> mul = 0)
 __device__ __forceinline__ int fast_div(int x, int d, uint32_t mul) { return mul ? (int)__umulhi((uint32_t)x, mul) : x; }
 
-template <bool PER_TAP>
+template <bool PER_TAP, int FOLD>
 __device__ __forceinline__ void halo_decode_tile(const HaloParams& p, int tile, int& nt, int& n, int& y0, int& x0) {
   int m = fast_div(tile, p.n_tiles, p.mul_n_tiles);
   nt = tile - m * p.n_tiles;
@@ -145,6 +162,7 @@ __device__ __forceinline__ void halo_decode_tile(const HaloParams& p, int tile, 
   n = fast_div(m1, p.tiles_y, p.mul_tiles_y);
   const int yb = m1 - n * p.tiles_y;
   if (PER_TAP) { n *= p.tb; y0 = yb * p.th; x0 = xb * p.tw; }
+  else if (FOLD) { y0 = yb * kFoldH; x0 = xb * kFoldW; }
   else { y0 = yb * kTileH; x0 = xb * kTileW; }
 }
 
@@ -163,7 +181,161 @@ __device__ __forceinline__ void issue_block(float* acc, const uint32_t* hi, cons
   }
 }
 
-template <bool PER_TAP, bool CIN8, int MODE, int N, int NCLS>
+// Fold mode epilogue staging: a third of the N columns of all 256 GEMM rows per round, rows padded so that a warp's float2
+// stores (8 rows x 4 column pairs) hit distinct banks
+__host__ __device__ constexpr int fold_stage_pitch(int n) { return (n / 3) % 16 == 0 ? n / 3 + 8 : n / 3; }
+__host__ __device__ constexpr int fold_stage_bytes(int n) { return 256 * fold_stage_pitch(n) * 4; }
+
+// The fold-mode consumers (warpgroups 1, 2: GEMM rows 128 wg .. 128 wg + 127 as two m64 blocks).  One step (one dy of
+// a chunk for FOLD 3, the whole chunk for FOLD 9) loads and splits each block's A fragment once and issues its 12
+// wgmma of N = 72 / 144; the next block's pixels are read from shared memory while they run.
+template <int MODE, int N, int FOLD>
+__device__ __forceinline__ void fold_consumers(const HaloParams& p, unsigned char* smem, uint32_t afull0, uint32_t aempty0,
+                                               uint32_t wfull0, uint32_t wempty0, uint32_t wres_bar) {
+  constexpr int CO = N / FOLD;                        // columns of one tap: Cout rounded up to 8
+  constexpr int BW = kFoldW + 2;                      // halo box width
+  constexpr int MROWS = (FOLD == 9 ? kFoldH + 2 : kFoldH) * BW;   // GEMM rows that are pixels; rows MROWS .. 255 pad
+  constexpr int TG = FOLD / 3;                        // taps per epilogue round (one dy row of taps, or one tap)
+  constexpr int GC = N / 3;                           // accumulator columns per round
+  constexpr int SP = fold_stage_pitch(N);
+  constexpr int NQ = kFoldH * kFoldW * CO / 4;        // float4 outputs of a tile
+  constexpr int OQ = (NQ + 255) / 256;                // ... per consumer thread
+  static_assert(N % FOLD == 0 && CO % 8 == 0 && GC % 8 == 0, "fold geometry");
+  const int ct = threadIdx.x - 128;                   // consumer thread 0 .. 255
+  const int wg = ct >> 7, warp = ct >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, tq = lane & 3;
+  const int m0 = 128 * wg + 16 * (warp & 3) + g;      // this thread's GEMM rows: m0 + 64 b + 8 h
+  const uint32_t smem_u = smem_u32(smem);
+  const uint32_t w_ring_u = smem_u + (uint32_t)(p.sa * p.a_region_bytes);
+  float* stage = reinterpret_cast<float*>(smem + (size_t)p.sa * p.a_region_bytes + p.w_region_bytes);
+  const float slope = p.leaky ? 0.1f : 1.0f;
+  long long w_afull = 0, w_wfull = 0;
+  const long long t_begin = clock64();
+  int sa = 0, slot = 0;
+  uint32_t pa = 0, use = 0;
+  if (p.w_resident) wait_t(wres_bar, 0u, p.err, w_wfull);
+  pdl_wait();   // the output buffer may still be read (or written) by the previous kernel
+  float acc[2][N / 2];
+  for (int item = blockIdx.x; item < p.total_items; item += gridDim.x) {
+    int nt, n, y0, x0;
+    halo_decode_tile<false, FOLD>(p, item, nt, n, y0, x0);
+#pragma unroll
+    for (int b = 0; b < 2; ++b)
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) acc[b][i] = 0.f;
+    int l_res = 0;
+    for (int kc = 0; kc < p.k_chunks; ++kc) {
+      wait_t(afull0 + 8 * sa, pa, p.err, w_afull);
+      const uint32_t abase = smem_u + (uint32_t)(sa * p.a_region_bytes);
+      for (int s = 0; s < p.nsteps; ++s) {
+        // channels 8 tq .. 8 tq + 7 of the pixels of rows m0 + 64 b and m0 + 64 b + 8 (padding rows read pixel 0)
+        float v[2][8];
+        auto load = [&](int b) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int m = m0 + 64 * b + 8 * h;
+            const uint32_t row = abase + (uint32_t)((m < MROWS ? m + BW * s : 0) * 128);
+            const uint32_t phase = (row >> 7) & 7u;
+            const float4 a = lds128(row + (((uint32_t)(2 * tq) ^ phase) << 4));
+            const float4 c = lds128(row + (((uint32_t)(2 * tq + 1) ^ phase) << 4));
+            v[h][0] = a.x; v[h][1] = a.y; v[h][2] = a.z; v[h][3] = a.w; v[h][4] = c.x; v[h][5] = c.y; v[h][6] = c.z; v[h][7] = c.w;
+          }
+        };
+        load(0);
+        uint32_t wb;
+        if (p.w_resident) {
+          wb = w_ring_u + (uint32_t)(l_res++) * (uint32_t)p.w_stage_bytes;
+        } else {
+          wait_t(wfull0 + 8 * slot, use, p.err, w_wfull);
+          wb = w_ring_u + (uint32_t)slot * (uint32_t)p.w_stage_bytes;
+        }
+#pragma unroll
+        for (int b = 0; b < 2; ++b) {
+          uint32_t hi[16], lo[16];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float f[4] = {v[0][2 * j], v[1][2 * j], v[0][2 * j + 1], v[1][2 * j + 1]};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const uint32_t u = __float_as_uint(f[e]);
+              hi[4 * j + e] = (MODE == 2) ? (u & 0xFFFFE000u) : u;
+              lo[4 * j + e] = __float_as_uint(f[e] - __uint_as_float(u & 0xFFFFE000u));
+            }
+          }
+#pragma unroll
+          for (int i = 0; i < N / 2; ++i) reg_fence(acc[b][i]);
+          wgmma_fence();
+          issue_block<N, MODE>(acc[b], hi, lo, wb);
+          wgmma_commit();
+          if (b == 0) load(1);
+          wgmma_wait0();
+#pragma unroll
+          for (int i = 0; i < N / 2; ++i) reg_fence(acc[b][i]);
+        }
+        if (!p.w_resident) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(wempty0 + 8 * slot);
+          if (++slot == kRing) { slot = 0; use ^= 1; }
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(aempty0 + 8 * sa);   // this warp is done reading the halo stage
+      if (++sa == p.sa) { sa = 0; pa ^= 1; }
+    }
+    // ---- epilogue (col2im): round r stages the columns of taps r TG .. r TG + TG - 1 of every row, then each thread adds
+    // them into its float4 outputs (output pixel q / (CO / 4), channels 4 (q % (CO / 4)) ..), taps in ascending order
+    float4 o[OQ];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      asm volatile("bar.sync 1, 256;" ::: "memory");   // the staging buffer's previous round (or tile) has been read
+#pragma unroll
+      for (int b = 0; b < 2; ++b)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float* srow = stage + (size_t)(m0 + 64 * b + 8 * h) * SP + 2 * tq;
+#pragma unroll
+          for (int i = 0; i < GC / 8; ++i)
+            *reinterpret_cast<float2*>(srow + 8 * i) =
+                make_float2(acc[b][4 * (r * GC / 8 + i) + 2 * h], acc[b][4 * (r * GC / 8 + i) + 2 * h + 1]);
+        }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+#pragma unroll
+      for (int j = 0; j < OQ; ++j) {
+        const int q = ct + 256 * j;
+        if (NQ % 256 != 0 && q >= NQ) break;
+        const int pix = q / (CO / 4), c = 4 * (q % (CO / 4));
+        const int y = pix / kFoldW, x = pix % kFoldW;
+#pragma unroll
+        for (int tl = 0; tl < TG; ++tl) {
+          const int t = r * TG + tl;
+          const int row = (FOLD == 9) ? (y + t / 3) * BW + x + t % 3 : y * BW + x + t;
+          const float4 a = *reinterpret_cast<const float4*>(stage + (size_t)row * SP + tl * CO + c);
+          if (t == 0) o[j] = a;
+          else { o[j].x += a.x; o[j].y += a.y; o[j].z += a.z; o[j].w += a.w; }
+        }
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < OQ; ++j) {
+      const int q = ct + 256 * j;
+      if (NQ % 256 != 0 && q >= NQ) break;
+      const int pix = q / (CO / 4), c = 4 * (q % (CO / 4));
+      if (c >= p.Cout) continue;
+      const int y = pix / kFoldW, x = pix % kFoldW;
+      float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (p.bias) {
+        const float2 b0 = __ldg(reinterpret_cast<const float2*>(p.bias + c)), b1 = __ldg(reinterpret_cast<const float2*>(p.bias + c + 2));
+        b = make_float4(b0.x, b0.y, b1.x, b1.y);
+      }
+      float4 r = make_float4(o[j].x + b.x, o[j].y + b.y, o[j].z + b.z, o[j].w + b.w);
+      r.x = fmaxf(slope * r.x, r.x); r.y = fmaxf(slope * r.y, r.y); r.z = fmaxf(slope * r.z, r.z); r.w = fmaxf(slope * r.w, r.w);
+      *reinterpret_cast<float4*>(p.out + ((size_t)(n * p.Hfull + y0 + y) * p.Wfull + x0 + x) * p.out_pitch + c) = r;
+    }
+  }
+  if (p.timing && threadIdx.x == 128) { p.timing[blockIdx.x * 16 + 6] = w_afull; p.timing[blockIdx.x * 16 + 3] = w_wfull; p.timing[blockIdx.x * 16 + 9] = clock64() - t_begin; }
+}
+
+template <bool PER_TAP, bool CIN8, int MODE, int N, int NCLS, int FOLD>
 __global__ void __launch_bounds__(kThreads, 1) conv_tc_halo_kernel(const __grid_constant__ HaloMaps maps, const HaloParams p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -218,7 +390,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_halo_kernel(const __grid_
       const int tile = fast_div(item, p.ksplit, p.mul_ksplit);
       const int kc0 = (item - tile * p.ksplit) * p.kc_split;
       int nt, n, y0, x0;
-      halo_decode_tile<PER_TAP>(p, tile, nt, n, y0, x0);
+      halo_decode_tile<PER_TAP, FOLD>(p, tile, nt, n, y0, x0);
       const unsigned char* wsrc = p.w + ((size_t)nt * p.k_chunks + kc0) * p.w_chunk_bytes;
       for (int kc = kc0; kc < kc0 + p.kc_split; ++kc, wsrc += p.w_chunk_bytes) {
         if (!PER_TAP) {
@@ -255,6 +427,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_halo_kernel(const __grid_
 
   // ===== consumers ======================================================================================================
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  if constexpr (FOLD != 0) {
+    fold_consumers<MODE, N, FOLD>(p, smem, afull0, aempty0, wfull0, wempty0, wres_bar);
+    return;
+  }
   const int wg = (warp >> 2) - 1;            // 0, 1: GEMM rows 64 wg .. 64 wg + 63
   const int wq = warp & 3;                   // warp inside the warpgroup: rows + 16 wq
   const int g = lane >> 2, tq = lane & 3;
@@ -281,7 +457,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_halo_kernel(const __grid_
     const int tile = fast_div(item, p.ksplit, p.mul_ksplit);
     const int z = item - tile * p.ksplit;
     int nt, n, y0, x0;
-    halo_decode_tile<PER_TAP>(p, tile, nt, n, y0, x0);
+    halo_decode_tile<PER_TAP, 0>(p, tile, nt, n, y0, x0);
 #pragma unroll
     for (int k = 0; k < NCLS; ++k)
 #pragma unroll
@@ -455,6 +631,8 @@ static int popcount4(int m) { return (m & 1) + ((m >> 1) & 1) + ((m >> 2) & 1) +
 // max_cls: at most this many classes per step (a wide step needs a wide weight slot; a shift is repeated if necessary).
 struct ShiftStep { int ry, rx, qy, qx, cmask, tap[4]; };
 
+static bool plan_tail(const ConvProblem* probs, int nclass, HaloPlan& plan);
+
 // The tiling of one layer (no tensor maps, no weights).  force_per_tap: per-tap mode even for images made of whole
 // 16 x 8 tiles (the fallback for shapes the halo mode refuses).
 static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPlan& plan, bool force_per_tap) {
@@ -606,6 +784,13 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
     break;
   }
   if (!found || prm.sa < 2) return false;
+  return plan_tail(probs, nclass, plan);
+}
+
+// What every mode's plan derives from its tiling: work items, split-K, the fast_div multipliers, the output.
+static bool plan_tail(const ConvProblem* probs, int nclass, HaloPlan& plan) {
+  const ConvProblem& p = probs[0];
+  HaloParams& prm = plan.prm;
   prm.B = p.B;
   const int m_tiles = prm.tiles_x * prm.tiles_y * prm.tiles_b;
   prm.total_tiles = m_tiles * prm.n_tiles;
@@ -613,7 +798,7 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
   // idle and run their K loop serially.  Cost model in cycles: rounds of kPlanSms items x (steps of an item x ~600 + ~3000
   // of prologue / epilogue), + ~12000 for the second pass + the partial sums' trip through L2; a split has to win 10 %.
   prm.ksplit = 1;
-  if (!prm.cin8 && !prm.w_resident && prm.k_chunks >= 4) {
+  if (!prm.cin8 && !prm.fold && !prm.w_resident && prm.k_chunks >= 4) {
     // the partial sums travel to the second pass through L2 (~4000 B per cycle for write + read back)
     const long out_bytes = (long)p.B * p.Hfull * p.Wfull * ((p.Cout + 3) / 4 * 4) * 4;
     auto cost = [&](int ks) {
@@ -641,6 +826,56 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
   return true;
 }
 
+// The fold mode's plan (see the top of this file), or false for a layer it does not take: one class of a plain 3x3
+// stride-1 convolution (taps in row-major order), Cin >= 64, Cout 16 (FOLD 9, N 144) or 20 / 24 (FOLD 3, N 72: the
+// kernel's two fold instantiations), an output of whole 12 x 16 tiles.  Weights resident when they fit, else the ring.
+static bool fold_build(const ConvProblem* probs, int nclass, int nsplit, HaloPlan& plan) {
+  const ConvProblem& p = probs[0];
+  if (nclass != 1 || p.ntaps != 9 || p.sy != 1 || p.sx != 1 || p.Cin < 64 || (p.Ho % kFoldH) != 0 || (p.Wo % kFoldW) != 0) return false;
+  if (p.osy != 1 || p.osx != 1 || p.ooy != 0 || p.oox != 0) return false;
+  for (int t = 0; t < 9; ++t)
+    if (p.dy[t] != t / 3 - 1 || p.dx[t] != t % 3 - 1) return false;
+  const int co8 = (p.Cout + 7) / 8 * 8;
+  const int fold = (co8 == 16) ? 9 : (co8 == 24 ? 3 : 0);
+  if (!fold) return false;
+  HaloParams& prm = plan.prm;
+  memset(&prm, 0, sizeof(prm));
+  memset(plan.st_tap, -1, sizeof(plan.st_tap));
+  prm.fold = fold;
+  prm.fold_n = fold * co8;
+  prm.nclass = 1;
+  prm.nsplit = nsplit;
+  prm.mode = (nsplit == 1) ? 0 : 2;
+  prm.n_tile = pow2_ceil_h((p.Cout + 15) / 16 * 16);   // the output channels of a tile, as in the halo mode
+  prm.n_tiles = 1;
+  prm.k_chunks = p.Cin / 32;
+  prm.nsteps = 9 / fold;
+  prm.nplanes = 1;
+  HaloPlane& pl = prm.planes[0];
+  pl.qx_min = -1; pl.qy_min = -1;
+  pl.cols = kFoldW + 2; pl.rows = kFoldH + 2;
+  pl.bytes = pl.rows * pl.cols * 128;
+  prm.a_region_bytes = (pl.bytes + 1023) / 1024 * 1024;
+  prm.cls_bytes = (nsplit == 3) ? prm.fold_n * 256 : prm.fold_n * 128;   // [W_hi ; W_lo] or W, multiples of 1024
+  for (int t = 0; t < prm.nsteps; ++t) {
+    prm.st_cmask[t] = 1;
+    prm.st_woff[t] = t * prm.cls_bytes;
+    prm.st_wbytes[t] = prm.cls_bytes;
+  }
+  prm.w_chunk_bytes = prm.nsteps * prm.cls_bytes;
+  prm.w_stage_bytes = prm.cls_bytes;
+  const int w_total = prm.k_chunks * prm.w_chunk_bytes;
+  const int stage = fold_stage_bytes(prm.fold_n);
+  prm.w_resident = (w_total <= 96 * 1024 && kSmemBudget - w_total - stage >= 2 * prm.a_region_bytes) ? 1 : 0;
+  prm.w_region_bytes = prm.w_resident ? w_total : kRing * prm.cls_bytes;
+  const int rest = kSmemBudget - prm.w_region_bytes - stage;
+  if (rest < 2 * prm.a_region_bytes) return false;
+  prm.sa = std::min(kMaxAStages, rest / prm.a_region_bytes);
+  plan.smem_bytes = prm.sa * prm.a_region_bytes + prm.w_region_bytes + stage + 1024;
+  prm.tiles_x = p.Wo / kFoldW; prm.tiles_y = p.Ho / kFoldH; prm.tiles_b = p.B;
+  return plan_tail(probs, nclass, plan);
+}
+
 // The shape rules of the kernel, for one problem
 static bool tc_shape_supported(const ConvProblem& p) {
   const bool cin8 = p.Cin == 8 && p.in_pitch == 8;   // 8-channel mode: four taps x 8 channels per K = 32 step
@@ -655,7 +890,8 @@ static bool tc_shape_supported(const ConvProblem& p) {
   return true;
 }
 
-// The one decision of the tensor-core path: whether a layer gets a plan, and in which mode.  The halo plan picks the
+// The one decision of the tensor-core path: whether a layer gets a plan, and in which mode.  The fold mode takes the
+// narrow 3x3 layers it was made for (fold_build); the halo plan picks the
 // per-tap mode itself for images not made of whole 16 x 8 tiles; shapes it refuses (e.g. more than kMaxPlanes stride-parity
 // planes) get the per-tap mode forced, which takes every 32-channel multiple but no 8-channel input.
 static bool tc_plan(const ConvProblem* probs, int nclass, int nsplit, HaloPlan& plan) {
@@ -664,7 +900,8 @@ static bool tc_plan(const ConvProblem* probs, int nclass, int nsplit, HaloPlan& 
     if (!tc_shape_supported(probs[c])) return false;
     if (probs[c].in != probs[0].in || probs[c].Cout != probs[0].Cout || probs[c].sy != probs[0].sy || probs[c].sx != probs[0].sx) return false;
   }
-  return halo_build(probs, nclass, nsplit, plan, false) || halo_build(probs, nclass, nsplit, plan, true);
+  return fold_build(probs, nclass, nsplit, plan) || halo_build(probs, nclass, nsplit, plan, false) ||
+         halo_build(probs, nclass, nsplit, plan, true);
 }
 
 static int nsplit_of(int precision) { return (precision == DEMON_PREC_TF32) ? 1 : 3; }
@@ -702,12 +939,13 @@ int tc_describe(const ConvProblem* probs, int nclass, int precision, char* buf, 
   HaloPlan plan;
   if (!tc_plan(probs, nclass, nsplit_of(precision), plan)) return 0;
   const HaloParams& q = plan.prm;
-  // per-tap mode: a pixel tile is tb images x th rows x tw columns (halo mode: 1 x 16 x 8)
+  // per-tap mode: a pixel tile is tb images x th rows x tw columns (halo mode: 1 x 16 x 8, fold mode 1 x 12 x 16; the fold
+  // mode's kind is "halo", its halo box, and `fold` the taps it puts into N)
   int n = snprintf(buf, buflen,
-                   "halo %s mode %d n_tile %d x%d steps %d x %d chunks sa %d a_stage %d w_slot %d smem %d tiles %d ksplit %d wres %d tb %d th %d tw %d |",
-                   q.per_tap ? "per-tap" : (q.cin8 ? "cin8" : "halo"), q.mode, q.n_tile, q.n_tiles, q.nsteps, q.k_chunks, q.sa,
+                   "halo %s mode %d n_tile %d x%d steps %d x %d chunks sa %d fold %d a_stage %d w_slot %d smem %d tiles %d ksplit %d wres %d tb %d th %d tw %d |",
+                   q.per_tap ? "per-tap" : (q.cin8 ? "cin8" : "halo"), q.mode, q.n_tile, q.n_tiles, q.nsteps, q.k_chunks, q.sa, q.fold,
                    q.a_region_bytes, q.w_stage_bytes, plan.smem_bytes, q.total_tiles, q.ksplit, q.w_resident, q.per_tap ? q.tb : 1,
-                   q.per_tap ? q.th : kTileH, q.per_tap ? q.tw : kTileW);
+                   q.per_tap ? q.th : (q.fold ? kFoldH : kTileH), q.per_tap ? q.tw : (q.fold ? kFoldW : kTileW));
   for (int t = 0; t < q.nsteps && n < buflen - 32; ++t)
     n += snprintf(buf + n, buflen - n, " [c%x w%d+%d]", q.st_cmask[t], q.st_woff[t], q.st_wbytes[t]);
   return n;
@@ -732,7 +970,9 @@ int tc_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts
   if (!encode_maps(p, *plan)) return fail(DEMON_E_CUDA, "tc_prepare: tensor map encode failed");
   const HaloParams& prm = plan->prm;
   // weights: [n tile][chunk][step][class of the step] blocks of [W_hi | W_lo], n_tile rows x 32 fp32, K-major, pre-swizzled;
-  // K position k of a row holds input channel kphys (the K order of the kernel's A fragment, see the top of this file)
+  // K position k of a row holds input channel kphys (the K order of the kernel's A fragment, see the top of this file).
+  // Fold mode: fold_n rows per block, row (tap of the step, co) with the tap's columns co8 = fold_n / fold apart.
+  const int rows = prm.fold ? prm.fold_n : prm.n_tile;
   const size_t total = (size_t)prm.n_tiles * prm.k_chunks * prm.w_chunk_bytes;
   std::vector<unsigned char> packed(total, 0);
   for (int nt = 0; nt < prm.n_tiles; ++nt)
@@ -743,9 +983,13 @@ int tc_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts
           if (!((prm.st_cmask[tt] >> cls) & 1)) continue;
           unsigned char* blk = packed.data() + ((size_t)nt * prm.k_chunks + kc) * prm.w_chunk_bytes + prm.st_woff[tt] + (size_t)idx * prm.cls_bytes;
           ++idx;
-          const int tap = prm.cin8 ? 0 : plan->st_tap[tt][cls];
-          for (int r = 0; r < prm.n_tile; ++r) {
-            const int co = nt * prm.n_tile + r;
+          for (int r = 0; r < rows; ++r) {
+            int tap = prm.cin8 ? 0 : plan->st_tap[tt][cls], co = nt * prm.n_tile + r;
+            if (prm.fold) {
+              const int co8 = prm.fold_n / prm.fold;
+              tap = (prm.fold == 3 ? 3 * tt : 0) + r / co8;   // taps in row-major order: 3 dy + dx
+              co = r % co8;
+            }
             for (int k = 0; k < 32; ++k) {
               const int kk = k & 7, kphys = 8 * (kk & 3) + 2 * (k >> 3) + (kk >> 2);
               float w = 0.f;
@@ -759,7 +1003,7 @@ int tc_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts
               const float lo = w - hi;
               const size_t off = (size_t)r * 128 + (size_t)(((k >> 2) ^ (r & 7)) << 4) + (size_t)(k & 3) * 4;
               memcpy(blk + off, &hi, 4);
-              if (nsplit == 3) memcpy(blk + (size_t)prm.n_tile * 128 + off, &lo, 4);
+              if (nsplit == 3) memcpy(blk + (size_t)rows * 128 + off, &lo, 4);
             }
           }
         }
@@ -837,15 +1081,15 @@ int tc_halo_read_timing(long long* host, int nblocks) {
   return 0;
 }
 
-template <bool PER_TAP, bool CIN8, int MODE, int N, int NCLS>
+template <bool PER_TAP, bool CIN8, int MODE, int N, int NCLS, int FOLD = 0>
 static int launch_variant(const HaloPlan* plan, const HaloParams& prm, int grid, cudaStream_t stream) {
   TcDeviceState& ds = tc_device_state();
   static int attr_device = -1;   // per instantiation: the device whose shared-memory limit was raised last
   if (attr_device != ds.device) {
-    DEMON_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_halo_kernel<PER_TAP, CIN8, MODE, N, NCLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
+    DEMON_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_halo_kernel<PER_TAP, CIN8, MODE, N, NCLS, FOLD>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxDynSmem));
     attr_device = ds.device;
   }
-  cudaError_t le = launch_pdl(conv_tc_halo_kernel<PER_TAP, CIN8, MODE, N, NCLS>, dim3(grid), dim3(kThreads), (size_t)plan->smem_bytes, stream, plan->maps, prm);
+  cudaError_t le = launch_pdl(conv_tc_halo_kernel<PER_TAP, CIN8, MODE, N, NCLS, FOLD>, dim3(grid), dim3(kThreads), (size_t)plan->smem_bytes, stream, plan->maps, prm);
   if (le != cudaSuccess) return fail(DEMON_E_CUDA, "conv_tc_halo launch: %s", cudaGetErrorString(le));
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
@@ -866,6 +1110,13 @@ static int launch_n(const HaloPlan* plan, const HaloParams& prm, int grid, cudaS
 template <bool PER_TAP, bool CIN8, int NCLS>
 static int launch_mode(const HaloPlan* plan, const HaloParams& prm, int grid, cudaStream_t stream) {
   return prm.mode == 0 ? launch_n<PER_TAP, CIN8, 0, NCLS>(plan, prm, grid, stream) : launch_n<PER_TAP, CIN8, 2, NCLS>(plan, prm, grid, stream);
+}
+
+template <int FOLD, int N>
+static int launch_fold(const HaloPlan* plan, const HaloParams& prm, int grid, cudaStream_t stream) {
+  if (prm.fold_n != N) return fail(DEMON_E_STATE, "conv_tc_halo: no fold kernel for %d taps at N %d", prm.fold, prm.fold_n);
+  return prm.mode == 0 ? launch_variant<false, false, 0, N, 1, FOLD>(plan, prm, grid, stream)
+                       : launch_variant<false, false, 2, N, 1, FOLD>(plan, prm, grid, stream);
 }
 
 int conv_tc_launch(const TcLayer& t, const ConvProblem* probs, cudaStream_t stream) {
@@ -891,7 +1142,8 @@ int conv_tc_launch(const TcLayer& t, const ConvProblem* probs, cudaStream_t stre
   }
   const int grid = std::min(prm.total_items, ds.sms);
   int rc;
-  if (prm.cin8) rc = launch_mode<false, true, 1>(plan, prm, grid, stream);
+  if (prm.fold) rc = prm.fold == 9 ? launch_fold<9, 144>(plan, prm, grid, stream) : launch_fold<3, 72>(plan, prm, grid, stream);
+  else if (prm.cin8) rc = launch_mode<false, true, 1>(plan, prm, grid, stream);
   else if (prm.per_tap) rc = prm.nclass == 1 ? launch_mode<true, false, 1>(plan, prm, grid, stream) : launch_mode<true, false, 4>(plan, prm, grid, stream);
   else rc = prm.nclass == 1 ? launch_mode<false, false, 1>(plan, prm, grid, stream) : launch_mode<false, false, 4>(plan, prm, grid, stream);
   if (rc != DEMON_OK || prm.ksplit == 1) return rc;
