@@ -15,11 +15,14 @@ struct TcLayer {
 
 // tc_prepare's result for a layer the tensor-core path does not take (not an error: the layer stays on the SIMT path)
 constexpr int kTcNoPlan = 1;
+// tc_prepare's result at DEMON_PREC_FP16 for a layer that has a plan but a weight FP16 cannot hold (|w| > 65504 or not
+// finite); nothing is allocated, the caller names the variable
+constexpr int kTcWeightRange = 2;
 
 // Decides whether a layer runs on the tensor cores and in which mode, and if so uploads its weights packed for the
 // kernel.  `nclass` problems that share input, tiling and Cout (1 for a convolution, 4 for the sub-pixel classes of a
 // transposed convolution) run in ONE launch.  w_hosts[c]: [ntaps][Cin][Cout_pad] fp32, the same packing the SIMT path
-// uses.  Returns DEMON_OK, kTcNoPlan or an error code.
+// uses.  Returns DEMON_OK, kTcNoPlan, kTcWeightRange or an error code.
 int tc_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts, int nclass, int precision);
 int conv_tc_launch(const TcLayer& t, const ConvProblem* probs, cudaStream_t stream);
 // The plan tc_prepare would choose, as text (no device needed); 0 if the layer has no plan.

@@ -25,8 +25,13 @@
 // so that a thread's four slices are the 8 CONSECUTIVE channels 8t .. 8t + 7 of its two pixels (two 16-byte loads per
 // pixel); the host packs the weights in the same order.
 //
-// Precision: 3xTF32 = A_hi * W_lo + A_lo * W_hi + A_hi * W_hi (W split on the host), three wgmma per K = 8 slice and
-// class; the dropped term A_lo * W_lo is ~2^-21 relative.  nsplit = 1 is plain single-pass TF32.
+// Precision (MODE): 2 = 3xTF32 = A_hi * W_lo + A_lo * W_hi + A_hi * W_hi (W split on the host), three wgmma per K = 8
+// slice and class; the dropped term A_lo * W_lo is ~2^-21 relative.  0 = plain single-pass TF32.  1 = FP16: the same 8
+// channels of a thread's two pixels are converted (cvt.rn.f16x2.f32, round to nearest even) into two K = 16 slices of
+// m64nNk16 kind f16, slice j column kk = input channel 8 ((kk % 8) >> 1) + 4 j + 2 (kk >> 3) + (kk & 1), so that register
+// R0 = (row g, channels 4j, 4j + 1), R1 = (row g + 8, same), R2 = (row g, 4j + 2, 4j + 3), R3 = (row g + 8, same) of the
+// thread's eight (PTX ISA, wgmma .f16 A fragment).  The weights are packed as FP16 (round to nearest even) with 64-byte
+// rows and 64-byte swizzle (TcFormat below); accumulators, epilogue and the fp32 halo staging are those of the TF32 modes.
 //
 // Narrow single-n-tile layers keep their whole packed weight set (<= 96 KB) RESIDENT in shared memory, loaded once per CTA
 // instead of one small bulk copy per step.  Layers with few tiles split their K loop over several work items (split-K,
@@ -49,8 +54,10 @@
 // Host side: tc_plan is the only place that decides whether a layer runs on this kernel and in which mode; tc_prepare
 // plans and packs a layer, conv_tc_launch launches it, and the per-device launch state and timeout flag live here too.
 #include <cuda.h>
+#include <cuda_fp16.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <memory>
 #include <mutex>
@@ -58,6 +65,7 @@
 
 #include "conv_tc.cuh"
 #include "conv_tc_ptx.cuh"
+#include "wgmma_f16.cuh"
 #include "wgmma_tf32.cuh"
 
 namespace demon {
@@ -117,9 +125,9 @@ struct HaloParams {
   int w_stage_bytes;    // weight ring slot = the largest step
   int w_region_bytes;   // shared memory of the weights: kRing slots, or the whole layer when resident
   int w_resident;       // 1: ALL weight blocks of the (single) n tile live in shared memory for the whole kernel, loaded once
-  int cls_bytes;        // one class block: [W_hi ; W_lo] (3xTF32) or W alone
-  int n_tile, nsplit;
-  int mode;             // 0 single pass TF32, 2 three-instruction 3xTF32
+  int cls_bytes;        // one class block: [W_hi ; W_lo] (3xTF32) or W alone (TF32, FP16)
+  int n_tile;
+  int mode;             // 0 single pass TF32, 1 FP16, 2 three-instruction 3xTF32
   const unsigned char* w;
   float* out;
   int out_pitch, Ho, Wo, Hfull, Wfull, osy, osx, Cout;
@@ -166,18 +174,53 @@ __device__ __forceinline__ void halo_decode_tile(const HaloParams& p, int tile, 
   else { y0 = yb * kTileH; x0 = xb * kTileW; }
 }
 
-// All wgmma of ONE class block of a step: K = 32 as four K = 8 slices.  hi/lo[8 j + 0..3] = the A fragment of slice j.
+// The A fragment of one step from a thread's 8 channels of its rows g (v[0]) and g + 8 (v[1]).  TF32 modes: slice j
+// (K = 8) is hi/lo[4 j + 0..3], a0 = (row g, col tq) = v[0][2j], a1 = (row g + 8, col tq), a2 = (row g, col tq + 4) =
+// v[0][2j + 1], a3; A_hi = trunc_tf32(A) for 3xTF32.  FP16: slice j (K = 16) is hi[4 j + 0..3] (see the top of this file),
+// lo is unused.
+template <int MODE>
+__device__ __forceinline__ void a_fragment(const float (&v)[2][8], uint32_t* hi, uint32_t* lo) {
+  if constexpr (MODE == 1) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {   // e = 2 q + h: row g + 8 h, channels 4 j + 2 q, 4 j + 2 q + 1 (the lower one in the low half)
+        const int h = e & 1, c = 4 * j + 2 * (e >> 1);
+        asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(hi[4 * j + e]) : "f"(v[h][c + 1]), "f"(v[h][c]));
+      }
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float f[4] = {v[0][2 * j], v[1][2 * j], v[0][2 * j + 1], v[1][2 * j + 1]};
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const uint32_t u = __float_as_uint(f[e]);
+        hi[4 * j + e] = (MODE == 2) ? (u & 0xFFFFE000u) : u;
+        lo[4 * j + e] = __float_as_uint(f[e] - __uint_as_float(u & 0xFFFFE000u));
+      }
+    }
+  }
+}
+
+// All wgmma of ONE class block of a step: K = 32 as four K = 8 slices (TF32 modes) or two K = 16 slices (FP16).
 template <int N, int MODE>
 __device__ __forceinline__ void issue_block(float* acc, const uint32_t* hi, const uint32_t* lo, uint32_t wb) {
-  const uint64_t w_hi = wgmma_desc_sw128(wb);
-  const uint64_t w_lo = wgmma_desc_sw128(wb + N * 128u);
+  if constexpr (MODE == 1) {
+    const uint64_t w = wgmma_desc_sw64(wb);
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {   // + 32 bytes inside the swizzled weight row per K = 8 slice
-    if (MODE == 2) {
-      Wgmma<N>::mma(acc, hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3], w_lo + (uint64_t)(2 * j));
-      Wgmma<N>::mma(acc, lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3], w_hi + (uint64_t)(2 * j));
+    for (int j = 0; j < 2; ++j)   // + 32 bytes inside the swizzled 64-byte weight row per K = 16 slice
+      WgmmaF16<N>::mma(acc, hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3], w + (uint64_t)(2 * j));
+  } else {
+    const uint64_t w_hi = wgmma_desc_sw128(wb);
+    const uint64_t w_lo = wgmma_desc_sw128(wb + N * 128u);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {   // + 32 bytes inside the swizzled weight row per K = 8 slice
+      if (MODE == 2) {
+        Wgmma<N>::mma(acc, hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3], w_lo + (uint64_t)(2 * j));
+        Wgmma<N>::mma(acc, lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3], w_hi + (uint64_t)(2 * j));
+      }
+      Wgmma<N>::mma(acc, hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3], w_hi + (uint64_t)(2 * j));
     }
-    Wgmma<N>::mma(acc, hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3], w_hi + (uint64_t)(2 * j));
   }
 }
 
@@ -252,16 +295,7 @@ __device__ __forceinline__ void fold_consumers(const HaloParams& p, unsigned cha
 #pragma unroll
         for (int b = 0; b < 2; ++b) {
           uint32_t hi[16], lo[16];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float f[4] = {v[0][2 * j], v[1][2 * j], v[0][2 * j + 1], v[1][2 * j + 1]};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const uint32_t u = __float_as_uint(f[e]);
-              hi[4 * j + e] = (MODE == 2) ? (u & 0xFFFFE000u) : u;
-              lo[4 * j + e] = __float_as_uint(f[e] - __uint_as_float(u & 0xFFFFE000u));
-            }
-          }
+          a_fragment<MODE>(v, hi, lo);
 #pragma unroll
           for (int i = 0; i < N / 2; ++i) reg_fence(acc[b][i]);
           wgmma_fence();
@@ -502,18 +536,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_halo_kernel(const __grid_
             v[h][0] = a.x; v[h][1] = a.y; v[h][2] = a.z; v[h][3] = a.w; v[h][4] = b.x; v[h][5] = b.y; v[h][6] = b.z; v[h][7] = b.w;
           }
         }
-        // slice j: a0 = (row g, col tq) = v[0][2j], a1 = (row g + 8, col tq), a2 = (row g, col tq + 4) = v[0][2j + 1], a3
         uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float f[4] = {v[0][2 * j], v[1][2 * j], v[0][2 * j + 1], v[1][2 * j + 1]};
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const uint32_t u = __float_as_uint(f[e]);
-            hi[4 * j + e] = (MODE == 2) ? (u & 0xFFFFE000u) : u;
-            lo[4 * j + e] = __float_as_uint(f[e] - __uint_as_float(u & 0xFFFFE000u));
-          }
-        }
+        a_fragment<MODE>(v, hi, lo);
         uint32_t wb;
         if (p.w_resident) {
           wb = w_ring_u + (uint32_t)(l_res++) * (uint32_t)p.w_stage_bytes;
@@ -625,6 +649,36 @@ struct HaloPlan {
 };
 
 static int pow2_ceil_h(int v) { int r = 1; while (r < v) r <<= 1; return r; }
+
+// The operand format of a tensor-core precision: the kernel's MODE and the packed weight blocks it reads.  A block is
+// `rows` rows (output channels) of one 32-channel chunk, K-major: 128 bytes per fp32 row (TF32 modes, 128-byte swizzle,
+// wgmma_desc_sw128) or 64 bytes per FP16 row (64-byte swizzle, wgmma_desc_sw64); 3xTF32 stores [W_hi ; W_lo].  A block is
+// aligned to its swizzle atom of 8 rows.
+struct TcFormat {
+  int mode;        // the kernel's MODE: 0 TF32, 1 FP16, 2 3xTF32
+  int row_bytes;   // one packed row of a chunk
+  int parts;       // weight images per block: 2 for [W_hi ; W_lo], else 1
+  int block_bytes(int rows) const {
+    const int atom = 8 * row_bytes;
+    return (rows * row_bytes * parts + atom - 1) / atom * atom;
+  }
+  // byte offset of K position k (0 .. 31) of row r inside one weight image of a block, and the input channel of the chunk
+  // that K position holds (the K order of the kernel's A fragment, see the top of this file)
+  int offset(int r, int k) const {
+    return mode == 1 ? r * 64 + (((k >> 3) ^ ((r >> 1) & 3)) << 4) + (k & 7) * 2 : r * 128 + (((k >> 2) ^ (r & 7)) << 4) + (k & 3) * 4;
+  }
+  int channel(int k) const {
+    if (mode == 1) { const int j = k >> 4, kk = k & 15; return 8 * ((kk & 7) >> 1) + 4 * j + 2 * (kk >> 3) + (kk & 1); }
+    const int kk = k & 7;
+    return 8 * (kk & 3) + 2 * (k >> 3) + (kk >> 2);
+  }
+};
+
+static TcFormat tc_format(int precision) {
+  if (precision == DEMON_PREC_TF32) return {0, 128, 1};
+  if (precision == DEMON_PREC_FP16) return {1, 64, 1};
+  return {2, 128, 2};
+}
 static int popcount4(int m) { return (m & 1) + ((m >> 1) & 1) + ((m >> 2) & 1) + ((m >> 3) & 1); }
 
 // Steps of one chunk: the distinct input shifts of all classes, each with the mask of the classes that use it.
@@ -635,7 +689,7 @@ static bool plan_tail(const ConvProblem* probs, int nclass, HaloPlan& plan);
 
 // The tiling of one layer (no tensor maps, no weights).  force_per_tap: per-tap mode even for images made of whole
 // 16 x 8 tiles (the fallback for shapes the halo mode refuses).
-static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPlan& plan, bool force_per_tap) {
+static bool halo_build(const ConvProblem* probs, int nclass, const TcFormat& fmt, HaloPlan& plan, bool force_per_tap) {
   const ConvProblem& p = probs[0];
   HaloParams& prm = plan.prm;
   const int budget = kSmemBudget;
@@ -651,7 +705,6 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
     memset(&prm, 0, sizeof(prm));
     memset(plan.st_tap, -1, sizeof(plan.st_tap));
     prm.nclass = nclass;
-    prm.nsplit = nsplit;
     prm.cin8 = (p.Cin == 8) ? 1 : 0;
     const int px_bytes = prm.cin8 ? 32 : 128;   // bytes of one pixel of a halo plane in shared memory
     prm.per_tap = (force_per_tap || (p.Ho % kTileH) != 0 || (p.Wo % kTileW) != 0) ? 1 : 0;
@@ -750,13 +803,13 @@ static bool halo_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
     int n_tile = std::min(pow2_ceil_h(std::max(cout16, 16)), std::min(nclass > 1 ? 64 : 128, cand.n_cap));
     // narrow the N tile (down to 64) while the layer would leave SMs idle
     while (n_tile >= 128 && (long)m_tiles * ceil_div(p.Cout, n_tile) < kPlanSms) n_tile /= 2;
-    prm.mode = (nsplit == 1) ? 0 : 2;
+    prm.mode = fmt.mode;
     prm.n_tile = n_tile;
     prm.n_tiles = ceil_div(p.Cout, n_tile);
     prm.k_chunks = prm.cin8 ? 1 : p.Cin / 32;
-    // ---- weights: one class block = [W_hi ; W_lo] (3xTF32) or W alone, 1024-byte aligned; a step holds the blocks of its
-    // classes in ascending class order; the ring slot is as large as the widest step
-    prm.cls_bytes = (nsplit == 3) ? n_tile * 256 : (n_tile * 128 + 1023) / 1024 * 1024;
+    // ---- weights: one class block of the precision's format (TcFormat); a step holds the blocks of its classes in
+    // ascending class order; the ring slot is as large as the widest step
+    prm.cls_bytes = fmt.block_bytes(n_tile);
     int woff = 0, wmax = 0;
     for (int t = 0; t < prm.nsteps; ++t) {
       prm.st_woff[t] = woff;
@@ -829,7 +882,7 @@ static bool plan_tail(const ConvProblem* probs, int nclass, HaloPlan& plan) {
 // The fold mode's plan (see the top of this file), or false for a layer it does not take: one class of a plain 3x3
 // stride-1 convolution (taps in row-major order), Cin >= 64, Cout 16 (FOLD 9, N 144) or 20 / 24 (FOLD 3, N 72: the
 // kernel's two fold instantiations), an output of whole 12 x 16 tiles.  Weights resident when they fit, else the ring.
-static bool fold_build(const ConvProblem* probs, int nclass, int nsplit, HaloPlan& plan) {
+static bool fold_build(const ConvProblem* probs, int nclass, const TcFormat& fmt, HaloPlan& plan) {
   const ConvProblem& p = probs[0];
   if (nclass != 1 || p.ntaps != 9 || p.sy != 1 || p.sx != 1 || p.Cin < 64 || (p.Ho % kFoldH) != 0 || (p.Wo % kFoldW) != 0) return false;
   if (p.osy != 1 || p.osx != 1 || p.ooy != 0 || p.oox != 0) return false;
@@ -844,8 +897,7 @@ static bool fold_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
   prm.fold = fold;
   prm.fold_n = fold * co8;
   prm.nclass = 1;
-  prm.nsplit = nsplit;
-  prm.mode = (nsplit == 1) ? 0 : 2;
+  prm.mode = fmt.mode;
   prm.n_tile = pow2_ceil_h((p.Cout + 15) / 16 * 16);   // the output channels of a tile, as in the halo mode
   prm.n_tiles = 1;
   prm.k_chunks = p.Cin / 32;
@@ -856,7 +908,7 @@ static bool fold_build(const ConvProblem* probs, int nclass, int nsplit, HaloPla
   pl.cols = kFoldW + 2; pl.rows = kFoldH + 2;
   pl.bytes = pl.rows * pl.cols * 128;
   prm.a_region_bytes = (pl.bytes + 1023) / 1024 * 1024;
-  prm.cls_bytes = (nsplit == 3) ? prm.fold_n * 256 : prm.fold_n * 128;   // [W_hi ; W_lo] or W, multiples of 1024
+  prm.cls_bytes = fmt.block_bytes(prm.fold_n);
   for (int t = 0; t < prm.nsteps; ++t) {
     prm.st_cmask[t] = 1;
     prm.st_woff[t] = t * prm.cls_bytes;
@@ -894,17 +946,15 @@ static bool tc_shape_supported(const ConvProblem& p) {
 // narrow 3x3 layers it was made for (fold_build); the halo plan picks the
 // per-tap mode itself for images not made of whole 16 x 8 tiles; shapes it refuses (e.g. more than kMaxPlanes stride-parity
 // planes) get the per-tap mode forced, which takes every 32-channel multiple but no 8-channel input.
-static bool tc_plan(const ConvProblem* probs, int nclass, int nsplit, HaloPlan& plan) {
+static bool tc_plan(const ConvProblem* probs, int nclass, const TcFormat& fmt, HaloPlan& plan) {
   if (nclass < 1 || nclass > 4) return false;
   for (int c = 0; c < nclass; ++c) {
     if (!tc_shape_supported(probs[c])) return false;
     if (probs[c].in != probs[0].in || probs[c].Cout != probs[0].Cout || probs[c].sy != probs[0].sy || probs[c].sx != probs[0].sx) return false;
   }
-  return fold_build(probs, nclass, nsplit, plan) || halo_build(probs, nclass, nsplit, plan, false) ||
-         halo_build(probs, nclass, nsplit, plan, true);
+  return fold_build(probs, nclass, fmt, plan) || halo_build(probs, nclass, fmt, plan, false) ||
+         halo_build(probs, nclass, fmt, plan, true);
 }
-
-static int nsplit_of(int precision) { return (precision == DEMON_PREC_TF32) ? 1 : 3; }
 
 // TMA descriptors: 5-D view {sx*C, W/sx, sy, H/sy, B} of the input slice, one box shape per plane
 static bool encode_maps(const ConvProblem& p, HaloPlan& plan) {
@@ -937,7 +987,7 @@ static bool encode_maps(const ConvProblem& p, HaloPlan& plan) {
 
 int tc_describe(const ConvProblem* probs, int nclass, int precision, char* buf, int buflen) {
   HaloPlan plan;
-  if (!tc_plan(probs, nclass, nsplit_of(precision), plan)) return 0;
+  if (!tc_plan(probs, nclass, tc_format(precision), plan)) return 0;
   const HaloParams& q = plan.prm;
   // per-tap mode: a pixel tile is tb images x th rows x tw columns (halo mode: 1 x 16 x 8, fold mode 1 x 12 x 16; the fold
   // mode's kind is "halo", its halo box, and `fold` the taps it puts into N)
@@ -964,13 +1014,13 @@ static float tf32_round_h(float x) {
 
 int tc_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts, int nclass, int precision) {
   const ConvProblem& p = probs[0];
-  const int nsplit = nsplit_of(precision);
+  const TcFormat fmt = tc_format(precision);
   std::unique_ptr<HaloPlan> plan(new HaloPlan());
-  if (!tc_plan(probs, nclass, nsplit, *plan)) return kTcNoPlan;
+  if (!tc_plan(probs, nclass, fmt, *plan)) return kTcNoPlan;
   if (!encode_maps(p, *plan)) return fail(DEMON_E_CUDA, "tc_prepare: tensor map encode failed");
   const HaloParams& prm = plan->prm;
-  // weights: [n tile][chunk][step][class of the step] blocks of [W_hi | W_lo], n_tile rows x 32 fp32, K-major, pre-swizzled;
-  // K position k of a row holds input channel kphys (the K order of the kernel's A fragment, see the top of this file).
+  // weights: [n tile][chunk][step][class of the step] blocks of the precision's format (TcFormat: [W_hi | W_lo], W or FP16
+  // W), n_tile rows x 32 K positions, K-major, pre-swizzled; K position k of a row holds input channel fmt.channel(k).
   // Fold mode: fold_n rows per block, row (tap of the step, co) with the tap's columns co8 = fold_n / fold apart.
   const int rows = prm.fold ? prm.fold_n : prm.n_tile;
   const size_t total = (size_t)prm.n_tiles * prm.k_chunks * prm.w_chunk_bytes;
@@ -991,7 +1041,7 @@ int tc_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts
               co = r % co8;
             }
             for (int k = 0; k < 32; ++k) {
-              const int kk = k & 7, kphys = 8 * (kk & 3) + 2 * (k >> 3) + (kk >> 2);
+              const int kphys = fmt.channel(k);
               float w = 0.f;
               if (prm.cin8) {   // channel index = (tap within the group of four, channel)
                 const int rt = 4 * tt + kphys / 8;
@@ -999,11 +1049,17 @@ int tc_prepare(TcLayer& t, const ConvProblem* probs, const float* const* w_hosts
               } else if (co < p.Cout) {
                 w = w_hosts[cls][((size_t)tap * p.Cin + kc * 32 + kphys) * p.Cout_pad + co];
               }
-              const float hi = (nsplit == 3) ? tf32_round_h(w) : w;
+              const size_t off = (size_t)fmt.offset(r, k);
+              if (fmt.mode == 1) {   // FP16, round to nearest even; a weight FP16 cannot hold is refused, not made infinite
+                if (!(std::fabs(w) <= 65504.f)) return kTcWeightRange;
+                const __half h = __float2half_rn(w);
+                memcpy(blk + off, &h, 2);
+                continue;
+              }
+              const float hi = (fmt.mode == 2) ? tf32_round_h(w) : w;
               const float lo = w - hi;
-              const size_t off = (size_t)r * 128 + (size_t)(((k >> 2) ^ (r & 7)) << 4) + (size_t)(k & 3) * 4;
               memcpy(blk + off, &hi, 4);
-              if (nsplit == 3) memcpy(blk + (size_t)rows * 128 + off, &lo, 4);
+              if (fmt.mode == 2) memcpy(blk + (size_t)rows * 128 + off, &lo, 4);
             }
           }
         }
@@ -1109,14 +1165,21 @@ static int launch_n(const HaloPlan* plan, const HaloParams& prm, int grid, cudaS
 
 template <bool PER_TAP, bool CIN8, int NCLS>
 static int launch_mode(const HaloPlan* plan, const HaloParams& prm, int grid, cudaStream_t stream) {
-  return prm.mode == 0 ? launch_n<PER_TAP, CIN8, 0, NCLS>(plan, prm, grid, stream) : launch_n<PER_TAP, CIN8, 2, NCLS>(plan, prm, grid, stream);
+  switch (prm.mode) {
+    case 0: return launch_n<PER_TAP, CIN8, 0, NCLS>(plan, prm, grid, stream);
+    case 1: return launch_n<PER_TAP, CIN8, 1, NCLS>(plan, prm, grid, stream);
+    default: return launch_n<PER_TAP, CIN8, 2, NCLS>(plan, prm, grid, stream);
+  }
 }
 
 template <int FOLD, int N>
 static int launch_fold(const HaloPlan* plan, const HaloParams& prm, int grid, cudaStream_t stream) {
   if (prm.fold_n != N) return fail(DEMON_E_STATE, "conv_tc_halo: no fold kernel for %d taps at N %d", prm.fold, prm.fold_n);
-  return prm.mode == 0 ? launch_variant<false, false, 0, N, 1, FOLD>(plan, prm, grid, stream)
-                       : launch_variant<false, false, 2, N, 1, FOLD>(plan, prm, grid, stream);
+  switch (prm.mode) {
+    case 0: return launch_variant<false, false, 0, N, 1, FOLD>(plan, prm, grid, stream);
+    case 1: return launch_variant<false, false, 1, N, 1, FOLD>(plan, prm, grid, stream);
+    default: return launch_variant<false, false, 2, N, 1, FOLD>(plan, prm, grid, stream);
+  }
 }
 
 int conv_tc_launch(const TcLayer& t, const ConvProblem* probs, cudaStream_t stream) {

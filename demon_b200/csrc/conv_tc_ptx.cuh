@@ -62,6 +62,18 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   return d;
 }
 
+// The same with 64-byte swizzle (the FP16 weight blocks: a 32-channel row is 64 bytes): 8-row groups 512 bytes apart,
+// 16-byte chunk c of row r at chunk c ^ ((r >> 1) & 3), layout type 2 = SWIZZLE_64B.  Advancing the start address by 32
+// bytes selects the next K = 16 slice.
+__device__ __forceinline__ uint64_t wgmma_desc_sw64(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);   // start address, bits [0,14)
+  d |= (uint64_t)1 << 16;                        // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)(512 >> 4) << 32;               // stride byte offset, bits [32,46)
+  d |= (uint64_t)2 << 62;                        // SWIZZLE_64B
+  return d;
+}
+
 // elect.sync: exactly one lane of the (converged) warp gets `true`.  Unlike `lane == 0`, the compiler then KNOWS the
 // region runs with a single active thread and emits the uniform-datapath instructions (UTMALDG, UBLKCP, ...)
 // directly instead of wrapping each one in a per-thread serialisation loop.

@@ -685,6 +685,9 @@ int upload_layer(Layer& l, const float* k, const float* bias_host, int B, int pr
     ConvProblem probs[4];
     const int nclass = build_problems(l, B, probs);
     rc = tc_prepare(l.tc, probs, w_hosts, nclass, precision);
+    if (rc == kTcWeightRange)
+      return fail(DEMON_E_INVALID, "variable %s/kernel: a value is not finite or above 65504 in magnitude, which FP16 cannot hold",
+                  l.name.c_str());
     if (rc != kTcNoPlan) return rc;   // on the tensor cores, or an error
   }
   for (int c = 0; c < nw; ++c)
@@ -1186,7 +1189,7 @@ static int net_create(demon_net** out, int batch, int refine_h, int refine_w, in
   DEMON_REQUIRE(out, "demon_net_create: null out");
   DEMON_REQUIRE(batch >= 1 && batch <= 4096, "demon_net_create: batch %d", batch);
   DEMON_REQUIRE(refine_h >= 4 && refine_w >= 4 && refine_h % 4 == 0 && refine_w % 4 == 0, "demon_net_create: refine size %dx%d must be a multiple of 4", refine_h, refine_w);
-  DEMON_REQUIRE(precision >= 0 && precision <= 2, "demon_net_create: precision %d", precision);
+  DEMON_REQUIRE(precision >= 0 && precision <= DEMON_PREC_FP16, "demon_net_create: precision %d", precision);
   std::unique_ptr<demon_net> n(new demon_net());
   n->B = batch; n->RH = refine_h; n->RW = refine_w; n->precision = precision; n->variant = variant;
   DEMON_CHECK_CUDA(cudaGetDevice(&n->device));
@@ -1940,7 +1943,7 @@ int demon_debug_describe_layers(const demon_net* n, char* buf, int buflen) {
 int demon_debug_describe_plan(int variant, int batch, int refine_h, int refine_w, int precision, char* buf, int buflen) {
   DEMON_REQUIRE(variant == 1 || variant == 2, "describe_plan: variant %d", variant);
   DEMON_REQUIRE(batch >= 1 && refine_h >= 4 && refine_w >= 4 && refine_h % 4 == 0 && refine_w % 4 == 0, "describe_plan: shape");
-  DEMON_REQUIRE(precision >= 0 && precision <= 2, "describe_plan: precision %d", precision);
+  DEMON_REQUIRE(precision >= 0 && precision <= DEMON_PREC_FP16, "describe_plan: precision %d", precision);
   std::unique_ptr<demon_net> n(new demon_net());
   n->B = batch; n->RH = refine_h; n->RW = refine_w; n->precision = precision; n->variant = variant;
   if (variant == 2) build_plan_v2(n.get());
@@ -1968,6 +1971,7 @@ int demon_debug_trace_layers(demon_net* n, float* const* in, float* const* out) 
 int demon_debug_describe_conv(int B, int H, int W, int Cin, int in_pitch, int Cout, int out_pitch, int kh, int kw, int sy, int sx, int deconv,
                               int precision, char* buf, int buflen) {
   DEMON_REQUIRE(buf && buflen > 0, "describe: null");
+  DEMON_REQUIRE(precision >= 0 && precision <= DEMON_PREC_FP16, "describe: precision %d", precision);
   StandaloneLayer s(nullptr, nullptr, H, W, Cin, in_pitch, Cout, out_pitch, kh, kw, sy, sx, deconv != 0, false);
   return describe_layer(s.layer, B, precision, buf, buflen);
 }
@@ -1985,6 +1989,7 @@ static int standalone_conv(const float* in, int in_pitch, float* out, int out_pi
   if (deconv) DEMON_REQUIRE(kh == 4 && kw == 4 && sy == 2 && sx == 2, "deconv: only k4 s2");
   else DEMON_REQUIRE(kh >= 1 && kw >= 1 && kh * kw <= kMaxTaps && (kh & 1) && (kw & 1), "conv: kernel %dx%d", kh, kw);
   DEMON_REQUIRE(sy >= 1 && sx >= 1, "conv: stride");
+  DEMON_REQUIRE(precision >= 0 && precision <= DEMON_PREC_FP16, "conv: precision %d", precision);
   std::vector<void*> allocs;
   StandaloneLayer s(in, out, H, W, Cin, in_pitch, Cout, out_pitch, kh, kw, sy, sx, deconv, leaky != 0);
   Layer& l = s.layer;

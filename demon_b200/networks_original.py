@@ -22,7 +22,7 @@ import torch
 from . import _lib
 from ._lib import check_errors  # noqa: F401  (re-exported: networks_original.check_errors())
 
-PRECISIONS = {"fp32": 0, "3xtf32": 1, "tf32": 2}
+PRECISIONS = {"fp32": 0, "3xtf32": 1, "tf32": 2, "fp16": 3}
 DEFAULT_PRECISION = "3xtf32"
 
 

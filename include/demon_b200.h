@@ -430,6 +430,13 @@ typedef struct demon_net demon_net;
 #define DEMON_PREC_FP32_SIMT  0   /* CUDA-core fp32 FFMA for every layer                           */
 #define DEMON_PREC_3XTF32     1   /* wgmma kind tf32 with error compensation (fp32-grade)         */
 #define DEMON_PREC_TF32       2   /* single-pass wgmma kind tf32 (fast mode, ~1e-3 relative)      */
+#define DEMON_PREC_FP16       3   /* wgmma kind f16, FP32 accumulators (fast mode, ~1e-3 relative)
+ * FP16: the tensor-core layers round their weights and input activations to FP16 (round to nearest even, 2^-11 relative);
+ * accumulation, bias, activations in memory and the layers without a tensor-core plan (dense, small outputs) stay fp32.
+ * demon_net_finalize refuses (DEMON_E_INVALID, naming the variable) a tensor-core layer's kernel with a value FP16 cannot
+ * hold: |w| > 65504 or not finite.  An input activation is converted as IEEE does: a magnitude of 65520 (65504 + half an
+ * FP16 ulp) or more becomes +-inf, so an out-of-range activation shows up as non-finite outputs, not as wrong finite
+ * ones. */
 
 /* replaces BootstrapNet/IterativeNet/RefinementNet.__init__ (networks_original.py:22-57,92-152,202-234).
  * refine_h/refine_w: input size of the refinement block (192, 256 for the standard pipeline). */

@@ -1,5 +1,5 @@
 """Offline (no GPU): which kernel family and tiling plan every convolution shape of the DeMoN graphs gets at a batch size.
-Usage: python tools/describe_plan.py [batch] [precision 0|1|2]"""
+Usage: python tools/describe_plan.py [batch] [precision 0|1|2|3]"""
 import ctypes
 import os
 import sys
