@@ -70,6 +70,10 @@ PROTOTYPES = {
     "demon_point_cloud_scratch_bytes": [c_int, c_int, c_int],
     "demon_point_cloud_f32": [_P] * 7 + [c_int] * 3 + [_P] * 6,
     "demon_point_cloud_inverse_f32": [_P] * 7 + [c_int] * 3 + [_P] * 6,
+    "demon_tsdf_integrate_f32": [_P] * 3 + [c_int] * 3 + [_P, c_float, c_float] + [_P] * 5 + [c_int] * 3 + [_P],
+    "demon_marching_cubes_scratch_bytes": [c_int, c_int, c_int],
+    "demon_marching_cubes_count_f32": [_P, _P, c_int, c_int, c_int, _P, _P, _P],
+    "demon_marching_cubes_f32": [_P] * 3 + [c_int] * 3 + [_P, c_float] + [_P] * 5,
     "demon_net_create": [ctypes.POINTER(c_void_p), c_int, c_int, c_int, c_int],
     "demon_net_destroy": [_P],
     "demon_net_set_weight": [_P, c_char_p, _P, _P, c_int],
@@ -149,6 +153,7 @@ _RESTYPES = {
     "demon_loss_ground_truth_workspace_bytes": c_int64,
     "demon_flow_warp_grad_workspace_bytes": c_int64,
     "demon_point_cloud_scratch_bytes": c_int64,
+    "demon_marching_cubes_scratch_bytes": c_int64,
     "demon_last_error": c_char_p,
     "demon_version": c_char_p,
     "demon_launch_count": c_int64,

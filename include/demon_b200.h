@@ -331,6 +331,33 @@ int demon_point_cloud_inverse_f32(const float* inverse_depth, const float* K, co
                                   float* normals_out, uint8_t* colors_out, int* counts, void* stream);
 
 /* ------------------------------------------------------------------------
+ * Fusion of depth maps into one surface (demon_b200/sequence.py): a TSDF volume and marching cubes.
+ * The volume is caller-owned, nx x ny x nz voxels with x fastest: tsdf [nz,ny,nx] and weight [nz,ny,nx] float32, color
+ * [nz,ny,nx,3] float32 or NULL.  Voxel (i,j,k) is the point origin + voxel_size*(i,j,k); origin is a HOST float[3].  At least
+ * 2 voxels per axis and fewer than 2^31 in all.  Every float operation is round-to-nearest in the order given here.
+ * ---------------------------------------------------------------------- */
+/* Adds n frames to the volume, in frame order: depth [n,h,w] camera z, K [n,3,3], R [n,3,3], t [n,3] world-to-camera (float32
+ * device arrays), image [n,h,w,3] uint8 (HWC RGB) with color, or NULL without.  For every voxel and frame: X_c = R X + t,
+ * u = fx x/z + cx, v = fy y/z + cy, pixel (floor(u), floor(v)); the frame is skipped when z <= 0, the pixel is outside the
+ * image, d is not finite or not > 0, or sdf = d - z < -trunc; otherwise f = min(1, sdf/trunc), tsdf = (tsdf W + f)/(W + 1),
+ * color likewise with the pixel's bytes, W = W + 1.  voxel_size and trunc finite and > 0; h*w < 2^24. */
+int demon_tsdf_integrate_f32(float* tsdf, float* weight, float* color, int nx, int ny, int nz, const float* origin, float voxel_size,
+                             float trunc, const float* depth, const float* K, const float* R, const float* t, const uint8_t* image,
+                             int n, int h, int w, void* stream);
+/* bytes of device scratch the marching-cubes entries need (0 for an invalid volume) */
+int64_t demon_marching_cubes_scratch_bytes(int nx, int ny, int nz);
+/* Marching cubes, step 1: the number of triangles into *triangles (device int64), and in scratch where each tile of cubes
+ * starts.  A cube is skipped when any of its 8 corners has weight 0; corner q of the cube is inside when its tsdf < 0. */
+int demon_marching_cubes_count_f32(const float* tsdf, const float* weight, int nx, int ny, int nz, void* scratch, int64_t* triangles,
+                                   void* stream);
+/* Step 2, on the scratch step 1 filled and the same volume: the triangle soup, in the order of the cube's linear index and
+ * then the standard Lorensen-Cline table's triangle order.  For T triangles: vertices [3T,3] float32, colors [3T,3] uint8
+ * (with color; NULL without), faces [T,3] int32 = 0, 1, 2, ...  A vertex on the edge from corner p0 (the lower grid
+ * coordinate) to p1 is p0 + (f0/(f0 - f1))(p1 - p0), its colour c0 + (f0/(f0 - f1))(c1 - c0) rounded half to even. */
+int demon_marching_cubes_f32(const float* tsdf, const float* weight, const float* color, int nx, int ny, int nz, const float* origin,
+                             float voxel_size, const void* scratch, float* vertices, uint8_t* colors, int* faces, void* stream);
+
+/* ------------------------------------------------------------------------
  * Image input (examples/example.py:15-42 resizes every image with PIL.Image.resize).
  * ---------------------------------------------------------------------- */
 /* resample filters, with Pillow's enum values (PIL.Image.Resampling) */
