@@ -3,7 +3,7 @@ Correlation1DGrad (lmbspecialops/src/correlation{,_1d}.cc and correlation{,_1d}_
 oracle/correlation.mk into oracle/_ref/libref_correlation.so, a git-ignored build product) run on the current CUDA device.
 
 Where the library is absent (no reference tree when it was built), every call returns the stored RESULT DIGESTS of the same
-call (shape, dtype, SHA-256 with NaNs canonicalised, oracle/ref.py:digest) from tests/golden/correlation_digests.json, keyed
+call (shape, dtype, SHA-256 with NaNs canonicalised, oracle/recorded.py:digest) from tests/golden/correlation_digests.json, keyed
 by a hash of the op, its attributes and its inputs; record them from the compiled kernels with DEMON_REF_RECORD=<json path>.
 
 Never call the reference with single_dir = -1: its kernels then read before the start of their padded buffer (the first
@@ -13,17 +13,15 @@ Only tests/ and tools/ may import this module.
 """
 import ctypes
 import hashlib
-import json
 import os
-import subprocess
 
 import numpy as np
 
-from .ref import REF_SRC, Recorded, digest
+from .recorded import REF_SRC, Recorded, Store, build_artefact, entry, record
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "_ref", "libref_correlation.so")
-_GOLDEN = os.path.join(os.path.dirname(_HERE), "tests", "golden", "correlation_digests.json")
+_STORE = Store("correlation_digests.json")
 _SOURCES = ["correlation.cc", "correlation_1d.cc", "correlation_cuda.cu", "correlation_1d_cuda.cu"]
 _DEPS = ["correlation_harness.cu", "correlation.mk", "ref_stub_gpu/tf_gpu_stub.h", "ref_stub_gpu/cuda_helper_shim.h",
          "ref_stub/tf_stub.h"]
@@ -31,33 +29,20 @@ _DEPS = ["correlation_harness.cu", "correlation.mk", "ref_stub_gpu/tf_gpu_stub.h
 
 def build(force=False):
     """Compile _ref/libref_correlation.so if the reference tree is present; returns the path or None."""
-    have_src = bool(REF_SRC) and all(os.path.isfile(os.path.join(REF_SRC, s)) for s in _SOURCES)
-    if not have_src:
-        return _LIB_PATH if os.path.isfile(_LIB_PATH) else None
-    deps = [os.path.join(REF_SRC, s) for s in _SOURCES] + [os.path.join(_HERE, f) for f in _DEPS]
-    if force or not os.path.isfile(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(os.path.getmtime(d) for d in deps):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-B", "-f", "correlation.mk", "correlation", "REF_SRC=" + REF_SRC])
-    return _LIB_PATH
+    return build_artefact(_LIB_PATH, [os.path.join(REF_SRC, s) for s in _SOURCES], _DEPS,
+                          ["-f", "correlation.mk", "correlation"], force)
 
 
 _lib = None
-_golden = None
 
 
 def have_library():
     return build() is not None
 
 
-def _golden_db():
-    global _golden
-    if _golden is None:
-        _golden = json.load(open(_GOLDEN)) if os.path.isfile(_GOLDEN) else {}
-    return _golden
-
-
 def available():
     """The reference kernels can be run here, or their recorded results are stored."""
-    return have_library() or bool(_golden_db())
+    return have_library() or bool(_STORE.entries())
 
 
 def lib():
@@ -73,16 +58,6 @@ def lib():
         L.ref_correlation_run.restype = I
         _lib = L
     return _lib
-
-
-def _record(key, value):
-    path = os.environ.get("DEMON_REF_RECORD")
-    if not path:
-        return
-    db = json.load(open(path)) if os.path.isfile(path) else {}
-    db[key] = value
-    with open(path, "w") as f:
-        json.dump(db, f, indent=0, sort_keys=True)
 
 
 def _attrs(corr_type, kernel_size, max_displacement, stride1, stride2, pad_size, do_abs, single_dir):
@@ -106,10 +81,7 @@ def run(op, arrays, attrs, out_shapes):
         raise ValueError("the reference's kernels read out of bounds with single_dir = -1; use oracle/correlation.py")
     key = _key(op, attrs, arrays)
     if not have_library():
-        db = _golden_db()
-        if key not in db:
-            raise RuntimeError("no stored reference result for this %s call (record it with DEMON_REF_RECORD)" % op)
-        return [Recorded(d) for d in db[key]]
+        return [Recorded(d) for d in _STORE.lookup(key, "reference result for this %s call" % op)]
     import torch
     dev = [torch.from_numpy(a).cuda() for a in arrays]
     outs = [torch.empty(tuple(max(0, s) for s in shp), dtype=torch.float32, device="cuda") for shp in out_shapes]
@@ -127,7 +99,7 @@ def run(op, arrays, attrs, out_shapes):
     if tuple(oshape) != tuple(out_shapes[0]):
         raise RuntimeError("reference kernel %s made shape %s, expected %s" % (op, tuple(oshape), tuple(out_shapes[0])))
     res = [o.cpu().numpy() for o in outs]
-    _record(key, [{"shape": list(r.shape), "dtype": r.dtype.str, "sha256": digest(r)} for r in res])
+    record(key, [entry(r) for r in res])
     return res
 
 

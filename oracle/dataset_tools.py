@@ -27,7 +27,7 @@ import numpy as np
 from PIL import Image
 
 from . import view_tools as vt
-from .ref import REF_SRC
+from .recorded import REF_SRC, Recorded, Store, entry, record
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 DATASET_TOOLS = (os.path.normpath(os.path.join(REF_SRC, "..", "..", "python", "depthmotionnet", "dataset_tools")) if REF_SRC
@@ -45,24 +45,8 @@ def have_reference():
 
 
 # ---- compute_depth_ratios (view_tools_cython.pyx:107-191) -------------------------------------------------------------
-_GOLDEN_RATIOS = os.path.join(os.path.dirname(_HERE), "tests", "golden", "dataset_tools_digests.json")
-_golden_ratios = None
-
-
-def nan_digest(a):
-    """SHA-256 of the array's bytes with every NaN replaced by the default NaN: ratio maps compare with all NaNs equal."""
-    a = np.array(a, copy=True, order="C")
-    if a.dtype.kind == "f":
-        a[np.isnan(a)] = np.nan
-    return hashlib.sha256(a.tobytes()).hexdigest()
-
-
-class RecordedRatios(vt.Recorded):
-    """Digest of a stored reference ratio map, NaNs canonicalised."""
-
-    def matches(self, a):
-        a = np.asarray(a)
-        return a.shape == self.shape and a.dtype == self.dtype and nan_digest(a) == self.sha256
+_RATIOS = Store("dataset_tools_digests.json")
+RecordedRatios = Recorded   # the digest of a stored ratio map: NaNs canonicalised like every other
 
 
 def depth_ratios_numpy(depth1, depth2, K1, R1, t1, P2):
@@ -106,21 +90,14 @@ def depth_ratios_numpy(depth1, depth2, K1, R1, t1, P2):
     return ratios, out_of_array
 
 
-def _golden_ratio_db():
-    global _golden_ratios
-    if _golden_ratios is None:
-        _golden_ratios = json.load(open(_GOLDEN_RATIOS)) if os.path.isfile(_GOLDEN_RATIOS) else {}
-    return _golden_ratios
-
-
 def ratios_available():
-    return vt.have_module() or bool(_golden_ratio_db())
+    return vt.have_module() or bool(_RATIOS.entries())
 
 
 def reference_depth_ratios(depth1, depth2, K1, R1, t1, K2, R2, t2):
     """compute_depth_ratios(view1, view2) of the reference's Cython for one ordered view pair (float32 camera-z depths of one
     size, float64 cameras).  The pixels the .pyx reads past depth2 for (depth_ratios_numpy's out_of_array) are set to NaN,
-    so the result is defined.  Returns the float32 map, or its RecordedRatios digest (tests/golden/dataset_tools_digests.json,
+    so the result is defined.  Returns the float32 map, or its Recorded digest (tests/golden/dataset_tools_digests.json,
     recorded with DEMON_REF_RECORD=<json path>)."""
     depth1 = np.ascontiguousarray(depth1, dtype=np.float32)
     depth2 = np.ascontiguousarray(depth2, dtype=np.float32)
@@ -132,16 +109,13 @@ def reference_depth_ratios(depth1, depth2, K1, R1, t1, K2, R2, t2):
         h.update(a.tobytes())
     key = h.hexdigest()
     if not vt.have_module():
-        db = _golden_ratio_db()
-        if key not in db:
-            raise RuntimeError("no stored result for this compute_depth_ratios call (record it with DEMON_REF_RECORD)")
-        return RecordedRatios(db[key])
+        return Recorded(_RATIOS.lookup(key, "result for this compute_depth_ratios call"))
     v1 = vt.View(R=np.asarray(R1), t=np.asarray(t1), K=np.asarray(K1), image=None, depth=depth1, depth_metric='camera_z')
     v2 = vt.View(R=np.asarray(R2), t=np.asarray(t2), K=np.asarray(K2), image=None, depth=depth2, depth_metric='camera_z')
     ratios = np.array(vt.module().compute_depth_ratios(v1, v2), dtype=np.float32)
     _, oob = depth_ratios_numpy(depth1, depth2, *vt.operands(K1, R1, t1, K2, R2, t2))
     ratios[oob] = np.nan
-    vt._record(key, {"shape": list(ratios.shape), "dtype": ratios.dtype.str, "sha256": nan_digest(ratios)})
+    record(key, entry(ratios))
     return ratios
 
 

@@ -6,7 +6,7 @@ Two families:
   * the CPU kernels (FlowWarp, FlowWarpGrad, FlowOutOfFrame; `*_cpu` below) run on host buffers and need no device;
   * the GPU kernels (FlowWarp, FlowWarpGrad, Resample; `*_gpu`) run on the current CUDA device.
 Where the library is absent (no reference tree when it was built), every call returns the stored RESULT DIGESTS of the same
-call (shape, dtype, SHA-256 with NaNs canonicalised, oracle/ref.py:digest) from tests/golden/flow_ops_digests.json, keyed by
+call (shape, dtype, SHA-256 with NaNs canonicalised, oracle/recorded.py:digest) from tests/golden/flow_ops_digests.json, keyed by
 a hash of the kernel, its attributes and its inputs; record them from the compiled kernels with DEMON_REF_RECORD=<json path>.
 
 Never call the reference's NEAREST resample where its source pixel leaves the image (`nearest_in_range` False): it then
@@ -17,17 +17,15 @@ Only tests/ and tools/ may import this module.
 """
 import ctypes
 import hashlib
-import json
 import os
-import subprocess
 
 import numpy as np
 
-from .ref import REF_SRC, Recorded, digest
+from .recorded import REF_SRC, Recorded, Store, build_artefact, entry, record
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "_ref", "libref_flow_ops.so")
-_GOLDEN = os.path.join(os.path.dirname(_HERE), "tests", "golden", "flow_ops_digests.json")
+_STORE = Store("flow_ops_digests.json")
 _SOURCES = ["flowwarp.cc", "flow_out_of_frame.cc", "resample.cc", "flowwarp_cuda.cu", "resample_cuda.cu"]
 _DEPS = ["flow_ops_harness.cu", "flow_ops.mk", "flow_ops_stub.h", "ref_stub_gpu/cuda_helper_shim.h", "ref_stub/tf_stub.h",
          "ref_stub/tensorflow/core/framework/common_shape_fns.h"]
@@ -36,33 +34,20 @@ RESAMPLE_TYPES = ("NEAREST", "CUBIC", "LINEAR")
 
 def build(force=False):
     """Compile _ref/libref_flow_ops.so if the reference tree is present; returns the path or None."""
-    have_src = bool(REF_SRC) and all(os.path.isfile(os.path.join(REF_SRC, s)) for s in _SOURCES)
-    if not have_src:
-        return _LIB_PATH if os.path.isfile(_LIB_PATH) else None
-    deps = [os.path.join(REF_SRC, s) for s in _SOURCES] + [os.path.join(_HERE, f) for f in _DEPS]
-    if force or not os.path.isfile(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(os.path.getmtime(d) for d in deps):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-B", "-f", "flow_ops.mk", "flow_ops", "REF_SRC=" + REF_SRC])
-    return _LIB_PATH
+    return build_artefact(_LIB_PATH, [os.path.join(REF_SRC, s) for s in _SOURCES], _DEPS,
+                          ["-f", "flow_ops.mk", "flow_ops"], force)
 
 
 _lib = None
-_golden = None
 
 
 def have_library():
     return build() is not None
 
 
-def _golden_db():
-    global _golden
-    if _golden is None:
-        _golden = json.load(open(_GOLDEN)) if os.path.isfile(_GOLDEN) else {}
-    return _golden
-
-
 def available():
     """The reference kernels can be run here, or their recorded results are stored."""
-    return have_library() or bool(_golden_db())
+    return have_library() or bool(_STORE.entries())
 
 
 def lib():
@@ -77,16 +62,6 @@ def lib():
         L.ref_flow_run.restype = I
         _lib = L
     return _lib
-
-
-def _record(key, value):
-    path = os.environ.get("DEMON_REF_RECORD")
-    if not path:
-        return
-    db = json.load(open(path)) if os.path.isfile(path) else {}
-    db[key] = value
-    with open(path, "w") as f:
-        json.dump(db, f, indent=0, sort_keys=True)
 
 
 def _key(kernel, attrs, arrays):
@@ -104,10 +79,7 @@ def run(kernel, arrays, attrs, out_shapes):
     arrays = [np.ascontiguousarray(a, dtype=dt) for a in arrays]
     key = _key(kernel, attrs, arrays)
     if not have_library():
-        db = _golden_db()
-        if key not in db:
-            raise RuntimeError("no stored reference result for this %s call (record it with DEMON_REF_RECORD)" % kernel)
-        return [Recorded(d) for d in db[key]]
+        return [Recorded(d) for d in _STORE.lookup(key, "reference result for this %s call" % kernel)]
     gpu = "/GPU/" in kernel
     min_elems = max(a.size for a in arrays)   # FlowWarpGrad_CPU clears n*c*h*w elements of its [n,2,h,w] output
     outs = [np.zeros(tuple(max(0, s) for s in shp), dtype=dt) for shp in out_shapes]
@@ -134,7 +106,7 @@ def run(kernel, arrays, attrs, out_shapes):
     if tuple(oshape) != tuple(out_shapes[0]):
         raise RuntimeError("reference kernel %s made shape %s, expected %s" % (kernel, tuple(oshape), tuple(out_shapes[0])))
     res = [t.cpu().numpy() for t in dev_out] if gpu else outs
-    _record(key, [{"shape": list(r.shape), "dtype": r.dtype.str, "sha256": digest(r)} for r in res])
+    record(key, [entry(r) for r in res])
     return res
 
 

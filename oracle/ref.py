@@ -14,58 +14,25 @@ The tests' bit comparisons accept either form, so they stay bit exact without th
 """
 import ctypes
 import hashlib
-import json
 import os
-import subprocess
 
 import numpy as np
 
+from .recorded import REF_SRC, Recorded, Store, build_artefact, digest, entry, record  # noqa: F401  (digest: re-exported)
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "_ref", "libref_ops.so")
-REF_SRC = os.environ.get("DEMON_REF_SRC", "")   # the reference's lmbspecialops/src; unset: use the stored results
-_GOLDEN = os.path.join(os.path.dirname(_HERE), "tests", "golden", "reference_ops.json")
+_STORE = Store("reference_ops.json")
 _SOURCES = ["warp2d.cc", "median3x3downsample.cc", "scaleinvariantgradient.cc", "leakyrelu.cc", "depthtoflow.cc", "replacenonfinite.cc", "depthtonormals.cc"]
 
 
 def build(force=False):
     """Compile _ref/libref_ops.so if the reference tree is present; returns the path or None."""
-    have_src = bool(REF_SRC) and all(os.path.isfile(os.path.join(REF_SRC, s)) for s in _SOURCES)
-    if not have_src:
-        return _LIB_PATH if os.path.isfile(_LIB_PATH) else None
-    deps = [os.path.join(REF_SRC, s) for s in _SOURCES] + [os.path.join(_HERE, f) for f in (
-        "ref_harness.cc", "ref_stub/tf_stub.h", "ref_stub/eigen_stub.h", "Makefile")]
-    if force or not os.path.isfile(_LIB_PATH) or os.path.getmtime(_LIB_PATH) < max(os.path.getmtime(d) for d in deps):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-B", "ref", "REF_SRC=" + REF_SRC])   # this function decided it is stale (make does not see Makefile edits)
-    return _LIB_PATH
+    return build_artefact(_LIB_PATH, [os.path.join(REF_SRC, s) for s in _SOURCES],
+                          ["ref_harness.cc", "ref_stub/tf_stub.h", "ref_stub/eigen_stub.h", "Makefile"], ["ref"], force)
 
 
 _lib = None
-_golden = None
-
-
-class Recorded:
-    """Digest of a reference kernel's output, from tests/golden/reference_ops.json."""
-
-    def __init__(self, d):
-        self.shape, self.dtype, self.sha256 = tuple(d["shape"]), np.dtype(d["dtype"]), d["sha256"]
-
-    def matches(self, a):
-        a = np.asarray(a)
-        return a.shape == self.shape and a.dtype == self.dtype and digest(a) == self.sha256
-
-
-def digest(a):
-    """SHA-256 of the array's bytes with every NaN replaced by the default NaN (payloads are not part of the contract)."""
-    a = np.array(a, copy=True, order="C")
-    a[np.isnan(a)] = np.nan
-    return hashlib.sha256(a.tobytes()).hexdigest()
-
-
-def _golden_db():
-    global _golden
-    if _golden is None:
-        _golden = json.load(open(_GOLDEN)) if os.path.isfile(_GOLDEN) else {}
-    return _golden
 
 
 def _call_key(op, arrs, attrs):
@@ -83,7 +50,7 @@ def have_library():
 
 def available():
     """The reference kernels can be run here, or their recorded results are stored."""
-    return have_library() or bool(_golden_db())
+    return have_library() or bool(_STORE.entries())
 
 
 def lib():
@@ -97,23 +64,13 @@ def lib():
     return _lib
 
 
-def _record(key, value):
-    path = os.environ.get("DEMON_REF_RECORD")
-    if not path:
-        return
-    db = json.load(open(path)) if os.path.isfile(path) else {}
-    db[key] = value
-    with open(path, "w") as f:
-        json.dump(db, f, indent=0, sort_keys=True)
-
-
 def kernels():
     if not have_library():
-        return _golden_db()["kernels"]
+        return _STORE.entries()["kernels"]
     buf = ctypes.create_string_buffer(4096)
     lib().ref_list(buf, 4096)
     ks = sorted(k for k in buf.value.decode().split(";") if k)
-    _record("kernels", ks)
+    record("kernels", ks)
     return ks
 
 
@@ -125,10 +82,7 @@ def run(op, inputs, attrs="", out_elems=None):
         raise TypeError("reference kernels take float32 or float64 tensors of one type")
     key = _call_key(op, arrs, attrs)
     if not have_library():
-        db = _golden_db()
-        if key not in db:
-            raise RuntimeError("no stored reference result for this %s call (record it with DEMON_REF_RECORD)" % op)
-        return Recorded(db[key])
+        return Recorded(_STORE.lookup(key, "reference result for this %s call" % op))
     n = len(arrs)
     data = (ctypes.c_void_p * n)(*[a.ctypes.data for a in arrs])
     shapes = [d for a in arrs for d in a.shape]
@@ -145,7 +99,7 @@ def run(op, inputs, attrs="", out_elems=None):
         raise RuntimeError("reference kernel %s: %s" % (op, err.value.decode()))
     shape = tuple(oshape[i] for i in range(orank.value))
     res = out[:int(np.prod(shape)) if shape else 1].reshape(shape).copy()
-    _record(key, {"shape": list(res.shape), "dtype": res.dtype.str, "sha256": digest(res)})
+    record(key, entry(res))
     return res
 
 

@@ -12,21 +12,19 @@ Only tests/, __graft_entry__ and tools/ may import this module.
 """
 import hashlib
 import importlib.util
-import json
 import os
-import subprocess
 import sys
 from collections import namedtuple
 
 import numpy as np
 
-from .ref import REF_SRC
+from .recorded import REF_SRC, Recorded, Store, build_artefact, digest, entry, record  # noqa: F401  (digest: re-exported)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _EXT_PATH = os.path.join(_HERE, "_ref", "view_tools_cython.so")
 PYX = (os.path.normpath(os.path.join(REF_SRC, "..", "..", "python", "depthmotionnet", "dataset_tools", "view_tools_cython.pyx"))
        if REF_SRC else "")
-_GOLDEN = os.path.join(os.path.dirname(_HERE), "tests", "golden", "view_tools_digests.json")
+_STORE = Store("view_tools_digests.json")
 
 # dataset_tools/view.py:25
 View = namedtuple('View', ['R', 't', 'K', 'image', 'depth', 'depth_metric'])
@@ -34,17 +32,11 @@ View = namedtuple('View', ['R', 't', 'K', 'image', 'depth', 'depth_metric'])
 
 def build(force=False):
     """Compile _ref/view_tools_cython.so if the reference tree is present; returns the path or None."""
-    if not (PYX and os.path.isfile(PYX)):
-        return _EXT_PATH if os.path.isfile(_EXT_PATH) else None
-    deps = [PYX, os.path.join(_HERE, "view_tools.mk")]
-    if force or not os.path.isfile(_EXT_PATH) or os.path.getmtime(_EXT_PATH) < max(os.path.getmtime(d) for d in deps):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-B", "-f", "view_tools.mk", "view_tools", "REF_SRC=" + REF_SRC,
-                               "PYTHON=" + sys.executable])
-    return _EXT_PATH
+    return build_artefact(_EXT_PATH, [PYX], ["view_tools.mk"],
+                          ["-f", "view_tools.mk", "view_tools", "PYTHON=" + sys.executable], force)
 
 
 _mod = None
-_golden = None
 
 
 def have_module():
@@ -63,30 +55,8 @@ def module():
     return _mod
 
 
-class Recorded:
-    """Digest of a stored reference mask (shape, dtype, SHA-256 of the bytes)."""
-
-    def __init__(self, d):
-        self.shape, self.dtype, self.sha256 = tuple(d["shape"]), np.dtype(d["dtype"]), d["sha256"]
-
-    def matches(self, a):
-        a = np.asarray(a)
-        return a.shape == self.shape and a.dtype == self.dtype and digest(a) == self.sha256
-
-
-def digest(a):
-    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
-
-
-def _golden_db():
-    global _golden
-    if _golden is None:
-        _golden = json.load(open(_GOLDEN)) if os.path.isfile(_GOLDEN) else {}
-    return _golden
-
-
 def available():
-    return have_module() or bool(_golden_db())
+    return have_module() or bool(_STORE.entries())
 
 
 def _key(arrays, ints):
@@ -98,16 +68,6 @@ def _key(arrays, ints):
     return h.hexdigest()
 
 
-def _record(key, value):
-    path = os.environ.get("DEMON_REF_RECORD")
-    if not path:
-        return
-    db = json.load(open(path)) if os.path.isfile(path) else {}
-    db[key] = value
-    with open(path, "w") as f:
-        json.dump(db, f, indent=0, sort_keys=True)
-
-
 def reference_mask(depth, K1, R1, t1, K2, R2, t2, borderx=0, bordery=0):
     """compute_visible_points_mask(view1, view2, borderx, bordery) of the reference's Cython for one view pair: depth [h,w]
     float32 camera z of view 1 (view 2 has the same size).  Returns the uint8 mask, or its Recorded digest."""
@@ -115,14 +75,11 @@ def reference_mask(depth, K1, R1, t1, K2, R2, t2, borderx=0, bordery=0):
     arrays = [depth] + [np.asarray(a) for a in (K1, R1, t1, K2, R2, t2)]
     key = _key(arrays, (int(borderx), int(bordery)))
     if not have_module():
-        db = _golden_db()
-        if key not in db:
-            raise RuntimeError("no stored result for this compute_visible_points_mask call (record it with DEMON_REF_RECORD)")
-        return Recorded(db[key])
+        return Recorded(_STORE.lookup(key, "result for this compute_visible_points_mask call"))
     v1 = View(R=np.asarray(R1), t=np.asarray(t1), K=np.asarray(K1), image=None, depth=depth, depth_metric='camera_z')
     v2 = View(R=np.asarray(R2), t=np.asarray(t2), K=np.asarray(K2), image=None, depth=depth, depth_metric='camera_z')
     mask = np.asarray(module().compute_visible_points_mask(v1, v2, borderx, bordery))
-    _record(key, {"shape": list(mask.shape), "dtype": mask.dtype.str, "sha256": digest(mask)})
+    record(key, entry(mask))
     return mask
 
 

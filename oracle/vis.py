@@ -8,24 +8,22 @@ in two forms:
 * `point_cloud_numpy`, a numpy restatement of the .pyx loop (float32 element-wise operations in the .pyx's order), which
   the CPU tests hold to the Cython bit for bit and the GPU tests hold the device to.
 
-Digests hash the arrays with every NaN canonicalised (oracle/ref.py:digest): a rotated NaN normal or an overflowing point
+Digests hash the arrays with every NaN canonicalised (oracle/recorded.py:digest): a rotated NaN normal or an overflowing point
 carries an x86 NaN payload the GPU does not reproduce.  Only tests/, __graft_entry__ and tools/ may import this module.
 """
 import hashlib
 import importlib.util
-import json
 import os
-import subprocess
 import sys
 
 import numpy as np
 
-from .ref import REF_SRC
+from .recorded import REF_SRC, Recorded, Store, build_artefact, digest, entry, record  # noqa: F401  (digest: re-exported)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _EXT_PATH = os.path.join(_HERE, "_ref", "vis_cython.so")
 PYX = (os.path.normpath(os.path.join(REF_SRC, "..", "..", "python", "depthmotionnet", "vis_cython.pyx")) if REF_SRC else "")
-_GOLDEN = os.path.join(os.path.dirname(_HERE), "tests", "golden", "vis_digests.json")
+_STORE = Store("vis_digests.json")
 
 # vis.py:252
 SUN3D_INTRINSICS = (0.89115971, 1.18821287, 0.5, 0.5)
@@ -33,17 +31,10 @@ SUN3D_INTRINSICS = (0.89115971, 1.18821287, 0.5, 0.5)
 
 def build(force=False):
     """Compile _ref/vis_cython.so if the reference tree is present; returns the path or None."""
-    if not (PYX and os.path.isfile(PYX)):
-        return _EXT_PATH if os.path.isfile(_EXT_PATH) else None
-    deps = [PYX, os.path.join(_HERE, "vis.mk")]
-    if force or not os.path.isfile(_EXT_PATH) or os.path.getmtime(_EXT_PATH) < max(os.path.getmtime(d) for d in deps):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-B", "-f", "vis.mk", "vis", "REF_SRC=" + REF_SRC,
-                               "PYTHON=" + sys.executable])
-    return _EXT_PATH
+    return build_artefact(_EXT_PATH, [PYX], ["vis.mk"], ["-f", "vis.mk", "vis", "PYTHON=" + sys.executable], force)
 
 
 _mod = None
-_golden = None
 
 
 def have_module():
@@ -62,34 +53,8 @@ def module():
     return _mod
 
 
-class Recorded:
-    """Digest of a stored reference array (shape, dtype, SHA-256 of the bytes with NaNs canonicalised)."""
-
-    def __init__(self, d):
-        self.shape, self.dtype, self.sha256 = tuple(d["shape"]), np.dtype(d["dtype"]), d["sha256"]
-
-    def matches(self, a):
-        a = np.asarray(a)
-        return a.shape == self.shape and a.dtype == self.dtype and digest(a) == self.sha256
-
-
-def digest(a):
-    """SHA-256 of the array's bytes, floating-point arrays with every NaN replaced by the default NaN (oracle/ref.py:digest)."""
-    a = np.array(a, copy=True, order="C")
-    if a.dtype.kind == "f":
-        a[np.isnan(a)] = np.nan
-    return hashlib.sha256(a.tobytes()).hexdigest()
-
-
-def _golden_db():
-    global _golden
-    if _golden is None:
-        _golden = json.load(open(_GOLDEN)) if os.path.isfile(_GOLDEN) else {}
-    return _golden
-
-
 def available():
-    return have_module() or bool(_golden_db())
+    return have_module() or bool(_STORE.entries())
 
 
 def _key(arrays):
@@ -104,16 +69,6 @@ def _key(arrays):
     return h.hexdigest()
 
 
-def _record(key, value):
-    path = os.environ.get("DEMON_REF_RECORD")
-    if not path:
-        return
-    db = json.load(open(path)) if os.path.isfile(path) else {}
-    db[key] = value
-    with open(path, "w") as f:
-        json.dump(db, f, indent=0, sort_keys=True)
-
-
 def reference_point_cloud(depth, K, R, t, normals=None, colors=None):
     """The reference's compute_point_cloud_from_depthmap for one view: depth [h,w] float32, K [3,3], R [3,3], t [3],
     normals [3,h,w] float32 or None, colors [3,h,w] uint8 or None.  Returns its dict of arrays, or a dict of their
@@ -122,13 +77,11 @@ def reference_point_cloud(depth, K, R, t, normals=None, colors=None):
     K, R, t = (np.asarray(a) for a in (K, R, t))
     key = _key([depth, K, R, t, normals, colors])
     if not have_module():
-        db = _golden_db()
-        if key not in db:
-            raise RuntimeError("no stored result for this compute_point_cloud_from_depthmap call (record it with DEMON_REF_RECORD)")
-        return {name: Recorded(v) for name, v in db[key].items()}
+        stored = _STORE.lookup(key, "result for this compute_point_cloud_from_depthmap call")
+        return {name: Recorded(v) for name, v in stored.items()}
     out = module().compute_point_cloud_from_depthmap(depth, K, R, t, normals, colors)
     out = {name: np.asarray(v) for name, v in out.items()}
-    _record(key, {name: {"shape": list(v.shape), "dtype": v.dtype.str, "sha256": digest(v)} for name, v in out.items()})
+    record(key, {name: entry(v) for name, v in out.items()})
     return out
 
 

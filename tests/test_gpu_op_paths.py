@@ -27,6 +27,7 @@ Every output is allocated in a block filled with SENTINEL just before the call (
 import collections
 import os
 import re
+import time
 import zlib
 from typing import NamedTuple
 
@@ -44,6 +45,7 @@ F, D = np.float32, np.float64
 CTYPE = {F: "float", D: "double"}
 CHUNK = 32768                       # planes per launch of the chunked launchers
 SENTINEL = -1.5e38                  # a value none of the ops computes from the data below
+WINDOW_MARGIN_S = 0.005
 CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "demon_b200", "csrc")
 
 
@@ -89,8 +91,13 @@ class Trace:
         prof = profile(activities=[ProfilerActivity.CUDA])
         try:
             with prof:
+                # the profiler keeps only device activity inside its capture window, timed on the host's clock: keep the
+                # calls clear of the window's edges, so that a small offset between the host and device clocks drops none
+                torch.cuda.synchronize()
+                time.sleep(WINDOW_MARGIN_S)
                 out = fn()
                 torch.cuda.synchronize()
+                time.sleep(WINDOW_MARGIN_S)
         finally:
             ours, other = device_kernels(prof)
             self.kernels.update(ours)
