@@ -74,6 +74,14 @@ PROTOTYPES = {
     "demon_marching_cubes_scratch_bytes": [c_int, c_int, c_int],
     "demon_marching_cubes_count_f32": [_P, _P, c_int, c_int, c_int, _P, _P, _P],
     "demon_marching_cubes_f32": [_P] * 3 + [c_int] * 3 + [_P, c_float] + [_P] * 5,
+    "demon_sparse_tsdf_rehash": [_P, _P, c_int64, _P, _P, c_int64, _P, _P],
+    "demon_sparse_tsdf_allocate_f32": [_P, _P, c_int64, _P, _P, c_float, c_float] + [_P] * 4 + [c_int] * 3 + [_P],
+    "demon_sparse_tsdf_gather_new": [_P, _P, c_int64, _P, _P, _P],
+    "demon_sparse_tsdf_commit": [_P, _P, c_int64, _P, c_int, c_int, _P, _P],
+    "demon_sparse_tsdf_integrate_f32": [_P] * 4 + [c_int, _P, c_float, c_float] + [_P] * 5 + [c_int] * 3 + [_P],
+    "demon_sparse_tsdf_mesh_scratch_bytes": [c_int],
+    "demon_sparse_tsdf_mesh_count_f32": [_P] * 3 + [c_int, _P, _P, c_int64, _P, _P, _P],
+    "demon_sparse_tsdf_mesh_f32": [_P] * 4 + [c_int, _P, c_float] + [_P] * 5,
     "demon_net_create": [ctypes.POINTER(c_void_p), c_int, c_int, c_int, c_int],
     "demon_net_destroy": [_P],
     "demon_net_set_weight": [_P, c_char_p, _P, _P, c_int],
@@ -154,6 +162,7 @@ _RESTYPES = {
     "demon_flow_warp_grad_workspace_bytes": c_int64,
     "demon_point_cloud_scratch_bytes": c_int64,
     "demon_marching_cubes_scratch_bytes": c_int64,
+    "demon_sparse_tsdf_mesh_scratch_bytes": c_int64,
     "demon_last_error": c_char_p,
     "demon_version": c_char_p,
     "demon_launch_count": c_int64,

@@ -4,7 +4,7 @@ trajectory, and their depth maps fused into a TSDF volume and meshed (csrc/fusio
     res = reconstruct(pipeline, frames, K)                  # CUDA uint8 [T,H,W,3] frames, K in pixels
     export_sequence_to_ply('out/seq', res)                  # out/seq_mesh.ply, out/seq_cameras.ply
     ch = chain_pairs(out['predict_depth0'], out['predict_rotation'], out['predict_translation'])
-    vol = TsdfVolume((256, 256, 256), origin, voxel_size)
+    vol = TsdfVolume((256, 256, 256), origin, voxel_size)   # or SparseTsdfVolume(voxel_size): hashed 8^3 blocks, no box
     vol.integrate(ch['depth'], K, ch['R'][:-1], ch['t'][:-1], image)
     vertices, colors, faces = vol.mesh()
 
@@ -150,6 +150,44 @@ def chain_pairs(inverse_depth, rotation, translation, intrinsics=None, min_ratio
     return {"scales": scales, "sigma": sigma, "R": R, "t": t, "depth": sig / inv}
 
 
+def _grid(origin, voxel_size, trunc):
+    """float32 origin [3], voxel_size and trunc (default 3 voxels) of a volume, checked."""
+    org = np.asarray(origin, dtype=np.float32).reshape(-1)
+    if org.shape != (3,) or not np.all(np.isfinite(org)):
+        raise ValueError("origin must be 3 finite numbers, got %r" % (origin,))
+    vs = np.float32(voxel_size)
+    tr = np.float32(3 * vs if trunc is None else trunc)
+    if not (np.isfinite(vs) and vs > 0 and np.isfinite(tr) and tr > 0):
+        raise ValueError("voxel_size and trunc must be finite and > 0, got %r and %r" % (voxel_size, trunc))
+    return org, vs, tr
+
+
+def _frames(depth, K, R, t, image, color):
+    """The frames of an integrate call as CUDA tensors: depth [n,h,w] float32, K, R [n,3,3], t [n,3] float32 and image
+    [n,h,w,3] uint8 or None.  The shapes, and image against `color`, are checked before anything touches a device."""
+    s = _shape(depth)
+    if len(s) == 4 and s[1] == 1:
+        s = (s[0],) + tuple(s[2:])
+    if len(s) != 3:
+        raise ValueError("depth must be [n,h,w] or [n,1,h,w], got %s" % (_shape(depth),))
+    n, h, w = s
+    if h * w >= 2 ** 24:
+        raise ValueError("depth: %dx%d pixels is too many (h*w must be below 2^24)" % (h, w))
+    for name, x, shape in (("K", K, (3, 3)), ("R", R, (3, 3)), ("t", t, (3,))):
+        if _shape(x) not in (shape, (n,) + shape):
+            raise ValueError("%s has shape %s; want %s or %s" % (name, _shape(x), shape, (n,) + shape))
+    if (image is None) == color:
+        raise ValueError("image is required with a colour volume and refused without one")
+    if image is not None:
+        if not vis._is_uint8(image):
+            raise ValueError("image must be uint8, got %s" % (image.dtype,))
+        if _shape(image) != (n, h, w, 3):
+            raise ValueError("image: expected %s, got %s" % ((n, h, w, 3), _shape(image)))
+    d = _cuda(depth, torch.float32).reshape(n, h, w)
+    im = None if image is None else _cuda(image, torch.uint8)
+    return d, vis._per_view(K, n, (3, 3), "K"), vis._per_view(R, n, (3, 3), "R"), vis._per_view(t, n, (3,), "t"), im
+
+
 class TsdfVolume:
     """A truncated signed distance volume on the device (include/demon_b200.h: demon_tsdf_integrate_f32): dims (nx, ny, nz)
     voxels, voxel (i,j,k) at origin + voxel_size*(i,j,k), truncation `trunc` (default 3 voxels), and a colour average with
@@ -163,13 +201,7 @@ class TsdfVolume:
             raise ValueError("dims must be (nx, ny, nz), got %r" % (dims,))
         if min(nx, ny, nz) < 2 or nx * ny * nz >= 2 ** 31 or 15 * (nx - 1) * (ny - 1) * (nz - 1) >= 2 ** 31:
             raise ValueError("dims %s: at least 2 voxels per axis and a volume the mesh indices fit" % ((nx, ny, nz),))
-        org = np.asarray(origin, dtype=np.float32).reshape(-1)
-        if org.shape != (3,) or not np.all(np.isfinite(org)):
-            raise ValueError("origin must be 3 finite numbers, got %r" % (origin,))
-        vs = np.float32(voxel_size)
-        tr = np.float32(3 * vs if trunc is None else trunc)
-        if not (np.isfinite(vs) and vs > 0 and np.isfinite(tr) and tr > 0):
-            raise ValueError("voxel_size and trunc must be finite and > 0, got %r and %r" % (voxel_size, trunc))
+        org, vs, tr = _grid(origin, voxel_size, trunc)
         self.dims, self.origin, self.voxel_size, self.trunc = (nx, ny, nz), org, vs, tr
         dev = _device()
         self.tsdf = torch.zeros((nz, ny, nx), dtype=torch.float32, device=dev)
@@ -183,24 +215,8 @@ class TsdfVolume:
         """Adds n frames in order: depth [n,h,w] (or [n,1,h,w]) float32 camera z, K [n,3,3] pixels (or one [3,3]), R [n,3,3]
         and t [n,3] world-to-camera, image [n,h,w,3] uint8 RGB (required with a colour volume, refused without).  Asynchronous
         on the current stream."""
-        d = _cuda(depth, torch.float32)
-        if d.dim() == 4 and d.shape[1] == 1:
-            d = d[:, 0]
-        if d.dim() != 3:
-            raise ValueError("depth must be [n,h,w] or [n,1,h,w], got %s" % (_shape(d),))
+        d, Kd, Rd, td, im = _frames(depth, K, R, t, image, self.color is not None)
         n, h, w = d.shape
-        if h * w >= 2 ** 24:
-            raise ValueError("depth: %dx%d pixels is too many (h*w must be below 2^24)" % (h, w))
-        Kd, Rd, td = vis._per_view(K, n, (3, 3), "K"), vis._per_view(R, n, (3, 3), "R"), vis._per_view(t, n, (3,), "t")
-        if (image is None) != (self.color is None):
-            raise ValueError("image is required with a colour volume and refused without one")
-        im = None
-        if image is not None:
-            if not vis._is_uint8(image):
-                raise ValueError("image must be uint8, got %s" % (image.dtype,))
-            im = _cuda(image, torch.uint8)
-            if _shape(im) != (n, h, w, 3):
-                raise ValueError("image: expected %s, got %s" % ((n, h, w, 3), _shape(im)))
         nx, ny, nz = self.dims
         with torch.cuda.device(self.tsdf.device):
             _lib.check(_lib.load().demon_tsdf_integrate_f32(
@@ -234,6 +250,173 @@ class TsdfVolume:
         return vertices, colors, faces
 
 
+class SparseTsdfVolume:
+    """A TSDF volume of 8x8x8 voxel blocks kept in a hash table on the device, allocated where depth is seen
+    (include/demon_b200.h: demon_sparse_tsdf_*), so memory and integration work follow the observed surface rather than a
+    bounding box.  Voxel g = 8 b + l (block b, |b| < 2^20 per axis) is the point origin + voxel_size * g, with
+    TsdfVolume's arithmetic; `trunc` defaults to 3 voxels.
+
+    State, CUDA tensors in allocation order, views of a pool that doubles as it fills (m = the number of blocks):
+      blocks [m,3] int32 (bx, by, bz), tsdf and weight [m,8,8,8] float32 (z, y, x; x fastest), color [m,8,8,8,3] float32
+      or None.
+    `integrate` first allocates, one thread per pixel, every block within 2 voxels of the pixel's band cell (its pixel square
+    between camera z d - trunc and d + trunc); a pixel whose cell would span more than DEMON_SPARSE_TSDF_MAX_SPAN (4) blocks
+    along an axis, or leaves the key range, allocates nothing and is counted in `last_skipped_pixels`.  The call's new
+    blocks are sorted by key and appended, then every block integrates the call's frames exactly as TsdfVolume does.  So a
+    block holds the dense integration of every frame from the call that allocated it onward: blocks of the first call equal
+    a dense volume's voxels bit for bit, and a block first seen in a later call has missed the free-space updates of the
+    earlier calls, as in every voxel-hashing fusion."""
+
+    MAX_SPAN = 4   # DEMON_SPARSE_TSDF_MAX_SPAN
+    _POOL_BLOCKS = 64
+    _TABLE_SLOTS = 1024
+
+    def __init__(self, voxel_size, origin=(0, 0, 0), trunc=None, color=True):
+        self.origin, self.voxel_size, self.trunc = _grid(origin, voxel_size, trunc)
+        self._color = bool(color)
+        self.last_skipped_pixels = 0
+        self._m = 0
+        self._pool = None    # blocks, tsdf, weight, color: the device state, made by the first call that needs it
+        self._table = None   # keys, values, counters
+
+    def _state(self):
+        if self._pool is None:
+            dev = _device()
+            with torch.cuda.device(dev):
+                self._pool = self._new_pool(self._POOL_BLOCKS, dev)
+                self._table = self._rehash(self._TABLE_SLOTS, dev)
+        return self._pool
+
+    def _new_pool(self, capacity, dev):
+        pool = {"blocks": torch.zeros((capacity, 3), dtype=torch.int32, device=dev),
+                "tsdf": torch.zeros((capacity, 8, 8, 8), dtype=torch.float32, device=dev),
+                "weight": torch.zeros((capacity, 8, 8, 8), dtype=torch.float32, device=dev),
+                "color": torch.zeros((capacity, 8, 8, 8, 3), dtype=torch.float32, device=dev) if self._color else None}
+        if self._pool is not None:
+            for k, v in pool.items():
+                if v is not None:
+                    v[:self._m] = self._pool[k][:self._m]
+        return pool
+
+    def _rehash(self, slots, dev):
+        """A table of `slots` slots holding the current table's entries."""
+        old = self._table
+        keys = torch.empty((slots,), dtype=torch.int64, device=dev)
+        values = torch.empty((slots,), dtype=torch.int32, device=dev)
+        counters = old[2] if old is not None else torch.empty((4,), dtype=torch.int64, device=dev)
+        _lib.check(_lib.load().demon_sparse_tsdf_rehash(
+            None if old is None else old[0].data_ptr(), None if old is None else old[1].data_ptr(), 0 if old is None else old[0].numel(),
+            keys.data_ptr(), values.data_ptr(), slots, counters.data_ptr(), _stream()))
+        return keys, values, counters
+
+    def _view(self, name):
+        t = self._state()[name]
+        return None if t is None else t[:self._m]
+
+    @property
+    def blocks(self):
+        return self._view("blocks")
+
+    @property
+    def tsdf(self):
+        return self._view("tsdf")
+
+    @property
+    def weight(self):
+        return self._view("weight")
+
+    @property
+    def color(self):
+        return self._view("color") if self._color else None
+
+    @property
+    def capacity(self):
+        """Blocks the pool holds before it doubles again."""
+        return self._state()["blocks"].shape[0]
+
+    @property
+    def table_slots(self):
+        self._state()
+        return self._table[0].numel()
+
+    @property
+    def nbytes(self):
+        """Device bytes of the pool and the hash table."""
+        tensors = list(self._state().values()) + list(self._table)
+        return sum(t.numel() * t.element_size() for t in tensors if t is not None)
+
+    def _origin(self):
+        return ctypes.cast((ctypes.c_float * 3)(*(float(v) for v in self.origin)), ctypes.c_void_p)
+
+    def integrate(self, depth, K, R, t, image=None):
+        """Adds n frames in order, with TsdfVolume.integrate's arguments: allocates their blocks, then integrates them into
+        every block.  Synchronises once, to read the number of new blocks and grow the pool (and once more each time the
+        hash table has to double)."""
+        d, Kd, Rd, td, im = _frames(depth, K, R, t, image, self._color)
+        n, h, w = d.shape
+        pool = self._state()
+        lib = _lib.load()
+        dev = pool["tsdf"].device
+        args = (self._origin(), float(self.voxel_size), float(self.trunc), d.data_ptr(), Kd.data_ptr(), Rd.data_ptr(), td.data_ptr())
+        with torch.cuda.device(dev):
+            while True:
+                keys, values, counters = self._table
+                _lib.check(lib.demon_sparse_tsdf_allocate_f32(keys.data_ptr(), values.data_ptr(), keys.numel(), counters.data_ptr(),
+                                                              *args, n, h, w, _stream()))
+                occupied, overflow, skipped = counters[:3].tolist()
+                if not overflow:
+                    break
+                self._table = self._rehash(2 * keys.numel(), dev)
+            new = occupied - self._m
+            if new:
+                fresh = torch.empty((new,), dtype=torch.int64, device=dev)
+                _lib.check(lib.demon_sparse_tsdf_gather_new(keys.data_ptr(), values.data_ptr(), keys.numel(), counters.data_ptr(),
+                                                            fresh.data_ptr(), _stream()))
+                fresh = torch.sort(fresh).values
+                cap = pool["blocks"].shape[0]
+                if self._m + new > cap:
+                    while cap < self._m + new:
+                        cap *= 2
+                    pool = self._pool = self._new_pool(cap, dev)
+                _lib.check(lib.demon_sparse_tsdf_commit(keys.data_ptr(), values.data_ptr(), keys.numel(), fresh.data_ptr(), new, self._m,
+                                                        pool["blocks"].data_ptr(), _stream()))
+                self._m += new
+            self.last_skipped_pixels = skipped
+            _lib.check(lib.demon_sparse_tsdf_integrate_f32(
+                pool["tsdf"].data_ptr(), pool["weight"].data_ptr(), None if pool["color"] is None else pool["color"].data_ptr(),
+                pool["blocks"].data_ptr(), self._m, *args, None if im is None else im.data_ptr(), n, h, w, _stream()))
+        return self
+
+    def mesh(self):
+        """TsdfVolume.mesh on the blocks: a cube is skipped when a corner lies in a block that is not allocated or has weight
+        0; the order is the block's pool index, the cube's local linear index (x fastest), then the table's.  Faces are
+        int32, so a mesh of 2^31 vertices or more raises ValueError.  Reads the triangle count back, so it synchronises."""
+        pool = self._state()
+        lib = _lib.load()
+        dev, m = pool["tsdf"].device, self._m
+        with torch.cuda.device(dev):
+            tri = 0
+            if m:
+                keys, values, _ = self._table
+                scratch = torch.empty((lib.demon_sparse_tsdf_mesh_scratch_bytes(m),), dtype=torch.uint8, device=dev)
+                total = torch.empty((1,), dtype=torch.int64, device=dev)
+                _lib.check(lib.demon_sparse_tsdf_mesh_count_f32(pool["tsdf"].data_ptr(), pool["weight"].data_ptr(), pool["blocks"].data_ptr(),
+                                                                m, keys.data_ptr(), values.data_ptr(), keys.numel(), scratch.data_ptr(),
+                                                                total.data_ptr(), _stream()))
+                tri = int(total.item())
+                if 3 * tri >= 2 ** 31:
+                    raise ValueError("the mesh has %d triangles: its int32 faces cannot index 3x that many vertices" % tri)
+            vertices = torch.empty((3 * tri, 3), dtype=torch.float32, device=dev)
+            colors = None if pool["color"] is None else torch.empty((3 * tri, 3), dtype=torch.uint8, device=dev)
+            faces = torch.empty((tri, 3), dtype=torch.int32, device=dev)
+            if tri:
+                _lib.check(lib.demon_sparse_tsdf_mesh_f32(
+                    pool["tsdf"].data_ptr(), pool["weight"].data_ptr(), None if colors is None else pool["color"].data_ptr(),
+                    pool["blocks"].data_ptr(), m, self._origin(), float(self.voxel_size), scratch.data_ptr(), vertices.data_ptr(),
+                    None if colors is None else colors.data_ptr(), faces.data_ptr(), _stream()))
+        return vertices, colors, faces
+
+
 def volume_from_points(points, dims=(256, 256, 256), low=5.0, high=95.0, color=True):
     """A TsdfVolume of at most `dims` voxels with cubic voxels around the `low`..`high` percentile box of points [m,3]
     (CUDA float32), each axis's percentiles taken on its own (torch.kthvalue, so any m works)."""
@@ -256,16 +439,16 @@ def reconstruct(pipeline, frames, intrinsics, volume=None, resample="bicubic", m
     (images.adjust_intrinsics), and its 64x48 image2_2 resized from the adapted frame with `resample`, as forward_views makes
     it.  The pairs (k, k+1) run through pipeline.forward_u8 (DemonPipeline or DemonPipelineV2) batch_size at a time; a
     partial last batch repeats its last pair, whose outputs are dropped.  The pairs are chained (chain_pairs) and the P
-    depth maps integrated, coloured by adapted frame k, into `volume` (a TsdfVolume, which is added to) or, by default, a
-    new 256^3 volume around the 5th..95th percentiles of the chained points.
+    depth maps integrated, coloured by adapted frame k, into `volume` (a TsdfVolume or a SparseTsdfVolume, which is added to)
+    or, by default, a new 256^3 TsdfVolume around the 5th..95th percentiles of the chained points.
 
     Returns a dict: chain_pairs' scales, sigma, R, t and depth, inverse_depth / rotation / translation [P,...] of the pairs,
     the adapted frames [T,192,256,3] and their status (images.adjust_intrinsics), K [3,3] of the adapted frames in pixels,
     volume, and the mesh: vertices, colors, faces."""
     if not (isinstance(frames, torch.Tensor) and frames.dim() == 4 and frames.shape[0] >= 2):
         raise ValueError("frames: expected a CUDA uint8 tensor [T,H,W,3] with T >= 2, got %s" % (_shape(frames),))
-    if volume is not None and not isinstance(volume, TsdfVolume):
-        raise ValueError("volume must be a TsdfVolume or None")
+    if volume is not None and not isinstance(volume, (TsdfVolume, SparseTsdfVolume)):
+        raise ValueError("volume must be a TsdfVolume, a SparseTsdfVolume or None")
     adapted, K_new, status = images.adjust_intrinsics(frames, intrinsics)
     small = images.resize(adapted, (64, 48), resample)
     T, b = frames.shape[0], pipeline.batch_size

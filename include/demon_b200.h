@@ -358,6 +358,59 @@ int demon_marching_cubes_f32(const float* tsdf, const float* weight, const float
                              float voxel_size, const void* scratch, float* vertices, uint8_t* colors, int* faces, void* stream);
 
 /* ------------------------------------------------------------------------
+ * A sparse TSDF volume (demon_b200/sequence.py: SparseTsdfVolume): voxel blocks of 8x8x8 stored where depth was seen.
+ * Block b = (bx, by, bz), |b| <= DEMON_SPARSE_TSDF_MAX_COORD per axis, holds voxels g = 8b + (0..7) at origin +
+ * voxel_size*g, with the dense volume's arithmetic.  The caller owns the state: blocks [m,3] int32 in pool order, tsdf and
+ * weight [m,8,8,8] float32 (z, y, x; x fastest), color [m,8,8,8,3] float32 or NULL; and a hash table of `capacity` slots
+ * (a power of 2) from a block's key to its pool index: keys int64 [capacity] (-1 empty), values int32 [capacity] (-1 for a
+ * block inserted and not yet committed), and counters int64 [4] (0: occupied slots, 1: set when the allocation found the
+ * table half full, 2: the pixels the allocation skipped, 3: scratch).  The table never holds more than capacity/2 keys.
+ * A call that adds frames runs allocate, reads the counters (doubling the table with rehash and allocating again when it
+ * was half full), gather_new, sorts the new keys ascending, commit, and integrate.
+ * ---------------------------------------------------------------------- */
+#define DEMON_SPARSE_TSDF_MAX_COORD ((1 << 20) - 1)
+/* a pixel whose widened cell spans more blocks than this along an axis allocates nothing */
+#define DEMON_SPARSE_TSDF_MAX_SPAN 4
+/* Fills keys and values with -1 and zeroes counters, then moves every entry of the old table (old_capacity <= capacity/2
+ * slots; 0 and NULL for none) into it and counts them in counters[0]. */
+int demon_sparse_tsdf_rehash(const int64_t* old_keys, const int* old_values, int64_t old_capacity, int64_t* keys, int* values,
+                             int64_t capacity, int64_t* counters, void* stream);
+/* Inserts the blocks of n frames (depth [n,h,w], K, R, t as demon_tsdf_integrate_f32 takes them) into the table.  One
+ * thread per pixel with finite d > 0 takes its band cell: the pixel square [px,px+1] x [py,py+1] between camera z d - trunc
+ * and d + trunc, the near face replaced by the camera centre when d - trunc <= 0.  In this float order: zf = d + trunc,
+ * zn = d - trunc; for each corner (u, v), a = (u - cx)/fx and b = (v - cy)/fy, camera points (a zf, b zf, zf) and, when
+ * zn > 0, (a zn, b zn, zn); (0, 0, 0) when zn <= 0; world X_i = (R_0i (x - t_0) + R_1i (y - t_1)) + R_2i (z - t_2).  Over
+ * the AABB [lo, hi] of those points, blocks floor(((lo - o)/vs - 2) * 0.125) .. floor(((hi - o)/vs + 2) * 0.125) per axis
+ * are inserted.  A pixel with a non-finite point, a block past +-DEMON_SPARSE_TSDF_MAX_COORD or a range wider than
+ * DEMON_SPARSE_TSDF_MAX_SPAN blocks inserts nothing and is counted in counters[2].  Every block an update with
+ * f < 1 of a counted-in pixel reaches, and every voxel within one voxel of it, then lies in an inserted block.  New keys
+ * get value -1; when an insertion would fill more than half the table it stops and sets counters[1].  Idempotent. */
+int demon_sparse_tsdf_allocate_f32(int64_t* keys, const int* values, int64_t capacity, int64_t* counters, const float* origin,
+                                   float voxel_size, float trunc, const float* depth, const float* K, const float* R, const float* t,
+                                   int n, int h, int w, void* stream);
+/* Writes the keys with value -1 to new_keys [counters[0] - m], in no particular order. */
+int demon_sparse_tsdf_gather_new(const int64_t* keys, const int* values, int64_t capacity, int64_t* counters, int64_t* new_keys,
+                                 void* stream);
+/* Gives sorted_keys[i] the pool index first + i and writes its block coordinates to blocks[first + i]. */
+int demon_sparse_tsdf_commit(const int64_t* keys, int* values, int64_t capacity, const int64_t* sorted_keys, int count, int first,
+                             int* blocks, void* stream);
+/* demon_tsdf_integrate_f32 on every voxel of the m blocks: one thread per voxel, the same per-frame update and order. */
+int demon_sparse_tsdf_integrate_f32(float* tsdf, float* weight, float* color, const int* blocks, int m, const float* origin, float voxel_size,
+                                    float trunc, const float* depth, const float* K, const float* R, const float* t, const uint8_t* image,
+                                    int n, int h, int w, void* stream);
+/* bytes of device scratch the sparse marching-cubes entries need for m >= 1 blocks */
+int64_t demon_sparse_tsdf_mesh_scratch_bytes(int m);
+/* Marching cubes on the blocks, step 1: resolves each block's 7 positive neighbours through the table and counts the
+ * triangles into *triangles (device int64).  Cube l of block b has its corner 0 at voxel 8b + l; it is skipped when a corner
+ * lies in a block that is not stored or has weight 0. */
+int demon_sparse_tsdf_mesh_count_f32(const float* tsdf, const float* weight, const int* blocks, int m, const int64_t* keys, const int* values,
+                                     int64_t capacity, void* scratch, int64_t* triangles, void* stream);
+/* Step 2, on the scratch step 1 filled: demon_marching_cubes_f32's triangle soup, in the order of the block's pool index,
+ * the cube's local linear index (x fastest) and the table's triangle order. */
+int demon_sparse_tsdf_mesh_f32(const float* tsdf, const float* weight, const float* color, const int* blocks, int m, const float* origin,
+                               float voxel_size, const void* scratch, float* vertices, uint8_t* colors, int* faces, void* stream);
+
+/* ------------------------------------------------------------------------
  * Image input (examples/example.py:15-42 resizes every image with PIL.Image.resize).
  * ---------------------------------------------------------------------- */
 /* resample filters, with Pillow's enum values (PIL.Image.Resampling) */
