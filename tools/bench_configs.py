@@ -1,12 +1,8 @@
 """Latency / throughput of the BASELINE.json configurations other than the bench workload:
 configs[1] full pipeline at batch 1 (latency), configs[4] RefinementNet at 1024x768 batch 8, plus batch 8 and 16."""
-import os
-import sys
-
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from benchkit import span_ms
 from demon_b200 import weights as W
 from demon_b200.networks_original import Session, DemonPipeline, RefinementNet
 
@@ -18,31 +14,12 @@ def main():
         pipe = DemonPipeline(sess, B, 3)
         x = torch.rand(B, 6, 192, 256, device="cuda") - 0.5
         outs = pipe.forward(x, None)
-        for _ in range(5):
-            pipe.forward(x, None, outs)
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        n = 30
-        e0.record()
-        for _ in range(n):
-            pipe.forward(x, None, outs)
-        e1.record()
-        torch.cuda.synchronize()
-        ms = e0.elapsed_time(e1) / n
+        ms = span_ms(lambda: pipe.forward(x, None, outs), 30, warmup=5)
         print("full pipeline batch %2d: %.3f ms per call (CUDA graph replay, device resident) = %.0f pairs/s" % (B, ms, B / ms * 1e3))
     net = RefinementNet(sess, "channels_first", 8, image_size=(768, 1024))
     img = torch.rand(8, 3, 768, 1024, device="cuda") - 0.5
     d2 = torch.rand(8, 1, 192, 256, device="cuda") + 0.3
-    for _ in range(3):
-        net.eval(img, d2)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(10):
-        net.eval(img, d2)
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / 10
+    ms = span_ms(lambda: net.eval(img, d2), 10)
     macs = W.macs_per_pair()["refine_fn"](768, 1024) * 8
     print("RefinementNet 1024x768 batch 8: %.3f ms per call = %.1f algorithmic TFLOP/s (98.675 GFLOP per image)" % (ms, 2 * macs / (ms / 1e3) / 1e12))
 

@@ -14,17 +14,12 @@ same call.
     python tools/bench_correlation.py [--reps 20] [--out profiles/h100_correlation.jsonl]
 """
 import argparse
-import json
-import os
-import subprocess
 import sys
 
 import numpy as np
 import torch
-from torch.profiler import ProfilerActivity, profile
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from benchkit import Rows, device_events, span_ms
 from demon_b200 import lmbspecialops as ops
 from oracle import correlation_ref as cref
 from oracle.ref import digest
@@ -37,39 +32,15 @@ ROWS = [
 ]
 
 
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clock = (s.strip() for s in out.split(","))
-        return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
-    except Exception:
-        return {"gpu": torch.cuda.get_device_name(), "power_limit": None, "max_sm_clock": None}
-
-
-def event_ms(fn, reps, warmup=3):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
-
-
 def reference_device_ms(fn, reps):
     """mean summed device time (kernels and memsets) of one reference call"""
     fn()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+
+    def calls():
         for _ in range(reps):
             fn()
-        torch.cuda.synchronize()
-    us = sum(e.device_time_total for e in prof.events()
-             if e.device_type == torch.autograd.DeviceType.CUDA and "Memcpy" not in e.name)
-    return us / 1e3 / reps
+    _, events = device_events(calls)
+    return sum(e.device_time_total for e in events if "Memcpy" not in e.name) / 1e3 / reps
 
 
 def main():
@@ -81,8 +52,7 @@ def main():
     assert torch.cuda.is_available(), "this benchmark measures the GPU"
     if not cref.have_library():
         sys.exit("oracle/_ref/libref_correlation.so is not built (build() with DEMON_REF_SRC set)")
-    info = gpu_info()
-    lines = []
+    rows = Rows(args.out)
     for name, one_d, n, attrs in ROWS:
         rng = np.random.RandomState(0)
         shape = (n, 256, 48, 64)
@@ -99,8 +69,8 @@ def main():
         ours_g = grad(g, a, b, **attrs)
         same = (digest(top.cpu().numpy()) == digest(rfwd(x1, x2, **attrs))
                 and all(digest(o.cpu().numpy()) == digest(r) for o, r in zip(ours_g, rgrad(gnp, x1, x2, **attrs))))
-        fwd_ms = event_ms(lambda: fwd(a, b, **attrs), args.reps)
-        grad_ms = event_ms(lambda: grad(g, a, b, **attrs), args.reps)
+        fwd_ms = span_ms(lambda: fwd(a, b, **attrs), args.reps)
+        grad_ms = span_ms(lambda: grad(g, a, b, **attrs), args.reps)
         ref_fwd_ms = reference_device_ms(lambda: rfwd(x1, x2, **attrs), args.ref_reps)
         ref_grad_ms = reference_device_ms(lambda: rgrad(gnp, x1, x2, **attrs), args.ref_reps)
         _, tc, th, tw = top.shape
@@ -114,15 +84,10 @@ def main():
             row[what] = {"ms": round(ms, 4), "reference_ms": round(rms, 4), "speedup": round(rms / ms, 2),
                          "gflop": round(flop / 1e9, 3), "tflops": round(flop / ms / 1e9, 2), "mbytes": round(nbytes / 1e6, 1),
                          "share_of_peak": round(max(t_c, t_m) * 1e3 / ms, 3), "bound": "fp32" if t_c >= t_m else "hbm"}
-        row.update(info)
-        lines.append(row)
-        print(json.dumps(row), flush=True)
+        rows.add(row)
         del a, b, top, g, ours_g
         torch.cuda.empty_cache()
-    if args.out:
-        with open(args.out, "w") as f:
-            for r in lines:
-                f.write(json.dumps(r) + "\n")
+    rows.save()
 
 
 if __name__ == "__main__":

@@ -13,18 +13,12 @@ for _v in ("OMP_NUM_THREADS", "OPENBLAS_NUM_THREADS", "MKL_NUM_THREADS"):   # th
     os.environ[_v] = "1"
 
 import argparse   # noqa: E402
-import json       # noqa: E402
-import sys        # noqa: E402
 import time       # noqa: E402
 
 import numpy as np   # noqa: E402
 import torch         # noqa: E402
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from bench_v2 import device_info, time_ms                  # noqa: E402
+from benchkit import ROOT, Rows, call_times, summary       # noqa: E402
 from demon_b200 import datareader as dr                    # noqa: E402
 from demon_b200.dataset_tools import View                  # noqa: E402
 from oracle import datareader as od                        # noqa: E402
@@ -44,23 +38,16 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_datareader needs a CUDA device")
-    info = device_info()
-    lines = []
-
-    def emit(d):
-        d.update(info)
-        print(json.dumps(d), flush=True)
-        lines.append(d)
-
+    rows = Rows(args.out)
     raw = od.synthetic_views(64, 480, 640, 0)
     views = [View(*v) for v in raw]
     pool = dr.ViewPool(256, 192)
     pool.add(views)   # warm-up and the pool the batches read
-    t = time_ms(lambda: dr.ViewPool(256, 192).add(views), args.reps)
+    t = summary(call_times(lambda: dr.ViewPool(256, 192).add(views), args.reps))
     nbytes = 64 * (480 * 640 * (3 + 4) + 192 * 256 * (3 + 4))
-    emit({"bench": "datareader_add", "views": 64, "source": [480, 640], "scaled": [192, 256], "ms": t[0], "ms_min": t[1], "ms_max": t[2],
-          "bytes": nbytes, "gb_per_s": nbytes / (t[0] * 1e-3) / 1e9,
-          "note": "whole call: host staging, one upload of the 640x480 sources, one launch, pool allocation"})
+    rows.add({"bench": "datareader_add", "views": 64, "source": [480, 640], "scaled": [192, 256], "ms": t["ms"], "ms_min": t["ms_min"],
+              "ms_max": t["ms_max"], "bytes": nbytes, "gb_per_s": nbytes / (t["ms"] * 1e-3) / 1e9,
+              "note": "whole call: host staging, one upload of the 640x480 sources, one launch, pool allocation"})
 
     rng = np.random.default_rng(1)
     colour_params = {'aug_hsv_hue': {'normal': {'mean': 0, 'stddev': 10}}, 'aug_contrast': {'uniform': {'a': 0.8, 'b': 1.2}},
@@ -71,11 +58,11 @@ def main():
                   'top_output': dr.OUTPUTS}
         for colour in (False, True):
             aug = dr.draw_augmentation(dict(params, **(colour_params if colour else {})), b, rng)
-            t = time_ms(lambda: dr.build_batch(pool, pairs, params, aug), args.reps)
+            t = summary(call_times(lambda: dr.build_batch(pool, pairs, params, aug), args.reps))
             nbytes = batch_bytes(b, 192, 256)
-            emit({"bench": "datareader_build_batch", "batch": b, "colour": colour, "outputs": list(dr.OUTPUTS), "ms": t[0], "ms_min": t[1],
-                  "ms_max": t[2], "bytes": nbytes, "gb_per_s": nbytes / (t[0] * 1e-3) / 1e9,
-                  "note": "whole call: host pose math, one table upload, one launch, output allocation"})
+            rows.add({"bench": "datareader_build_batch", "batch": b, "colour": colour, "outputs": list(dr.OUTPUTS), "ms": t["ms"],
+                      "ms_min": t["ms_min"], "ms_max": t["ms_max"], "bytes": nbytes, "gb_per_s": nbytes / (t["ms"] * 1e-3) / 1e9,
+                      "note": "whole call: host pose math, one table upload, one launch, output allocation"})
         if b == 8:
             prepared = [od.prepare(img, d, K, R, t_, m, 256, 192) for R, t_, K, img, d, m in raw[:max(max(p) for p in pairs) + 1]]
             p = dr.reader_params(params)
@@ -86,12 +73,9 @@ def main():
                     t0 = time.perf_counter()
                     od.build_batch(prepared, pairs, p, aug.rot180, aug.mirror_x, aug.colour)
                     times.append((time.perf_counter() - t0) * 1e3)
-                emit({"bench": "datareader_oracle_build_batch", "batch": b, "colour": colour, "ms": float(np.median(times)),
-                      "note": "numpy oracle on one host core (BLAS threads 1), median of 3"})
-    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    with open(args.out, "a") as fh:
-        for d in lines:
-            fh.write(json.dumps(d) + "\n")
+                rows.add({"bench": "datareader_oracle_build_batch", "batch": b, "colour": colour, "ms": float(np.median(times)),
+                          "note": "numpy oracle on one host core (BLAS threads 1), median of 3"})
+    rows.save()
 
 
 if __name__ == "__main__":

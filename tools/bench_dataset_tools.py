@@ -6,9 +6,7 @@ per pair from oracle/_ref, where it was built).  Appends JSON lines to --out (de
     python tools/bench_dataset_tools.py [--reps 20] [--host-frames 8] [--host-pairs 8] [--out ...]
 """
 import argparse
-import json
 import os
-import sys
 import time
 
 import numpy as np
@@ -16,23 +14,12 @@ import scipy.ndimage
 import torch
 from PIL import Image
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-
-from bench_eval import device_info, time_ms   # noqa: E402
-from demon_b200 import _lib                   # noqa: E402
-from demon_b200 import dataset_tools as dt    # noqa: E402
-from oracle import view_tools as vt           # noqa: E402
+from benchkit import ROOT, Rows, call_times, library_launches, summary
+from demon_b200 import _lib
+from demon_b200 import dataset_tools as dt
+from oracle import view_tools as vt
 
 HBM_BYTES_PER_S = 3.35e12   # H100 SXM data sheet
-
-
-def launches(fn):
-    lib = _lib.load()
-    n0 = lib.demon_launch_count()
-    fn()
-    return int(lib.demon_launch_count() - n0)
 
 
 def views(n, h, w, seed=0):
@@ -58,19 +45,19 @@ def main():
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_dataset_tools.jsonl"))
     args = ap.parse_args()
     assert torch.cuda.is_available(), "the benchmark needs a GPU"
-    info = device_info()
-    lines = []
+    rows = Rows(args.out)
 
     # sharpness: 256 frames of 480x640 RGB
     n, h, w = 256, 480, 640
     rng = np.random.RandomState(1)
     host = rng.randint(0, 256, (n, h, w, 3)).astype(np.uint8)
     frames = torch.from_numpy(host).cuda()
-    med, lo, hi = time_ms(lambda: dt.sharpness(frames), args.reps, warmup=3)
+    tm = summary(call_times(lambda: dt.sharpness(frames), args.reps, warmup=3))
+    med = tm["ms"]
     moved = 2 * n * h * w * 3 + 4 * n   # the frames read once per pass, the results
-    line = {"bench": "sharpness", "frames": n, "size": [h, w], "device_ms": med, "device_ms_min": lo, "device_ms_max": hi,
-            "reps": args.reps, "bytes_moved": moved, "achieved_GBps": moved / (med * 1e-3) / 1e9,
-            "hbm_share": moved / (med * 1e-3) / HBM_BYTES_PER_S, "launches_per_call": launches(lambda: dt.sharpness(frames))}
+    line = {"bench": "sharpness", "frames": n, "size": [h, w], "device_ms": med, "device_ms_min": tm["ms_min"],
+            "device_ms_max": tm["ms_max"], "reps": args.reps, "bytes_moved": moved, "achieved_GBps": moved / (med * 1e-3) / 1e9,
+            "hbm_share": moved / (med * 1e-3) / HBM_BYTES_PER_S, "launches_per_call": library_launches(lambda: dt.sharpness(frames))}
     k = min(args.host_frames, n)
     if k > 0:
         t0 = time.perf_counter()
@@ -79,9 +66,7 @@ def main():
         per = (time.perf_counter() - t0) * 1e3 / k
         line.update({"host_ms_per_frame": per, "host_ms_per_batch": per * n, "host_frames_timed": k,
                      "host_note": "measure_sharpness's numpy / scipy / Pillow calls, one host thread"})
-    line.update(info)
-    lines.append(line)
-    print(json.dumps(line), flush=True)
+    rows.add(line)
 
     # consistency counts: 512 pair-directions among 64 views of 480x640
     nv, npairs = 64, 256
@@ -100,12 +85,13 @@ def main():
         _lib.check(lib.demon_depth_consistency_counts_f32(depth.data_ptr(), K.data_ptr(), R.data_ptr(), t.data_ptr(), P.data_ptr(), nv, h,
                                                           w, pr.data_ptr(), len(pairs), float(lo_t), float(hi_t), counts.data_ptr(),
                                                           dt._stream()))
-    med, lo, hi = time_ms(run, args.reps, warmup=3)
+    tm = summary(call_times(run, args.reps, warmup=3))
+    med = tm["ms"]
     moved = len(pairs) * h * w * 4 * 2   # depth i streamed, depth j gathered (at least once per pair)
     line = {"bench": "consistency_counts", "pair_directions": len(pairs), "views": nv, "size": [h, w], "device_ms": med,
-            "device_ms_min": lo, "device_ms_max": hi, "reps": args.reps, "bytes_moved": moved,
+            "device_ms_min": tm["ms_min"], "device_ms_max": tm["ms_max"], "reps": args.reps, "bytes_moved": moved,
             "achieved_GBps": moved / (med * 1e-3) / 1e9, "hbm_share": moved / (med * 1e-3) / HBM_BYTES_PER_S,
-            "launches_per_call": launches(run),
+            "launches_per_call": library_launches(run),
             "bytes_note": "two depth maps per pair direction; the 64 views' 79 MB mostly stay in L2, so this is L2-level traffic"}
     if vt.have_module() and args.host_pairs > 0:
         m = vt.module()
@@ -118,13 +104,8 @@ def main():
         per = (time.perf_counter() - t0) * 1e3 / k
         line.update({"host_cython_ms_per_pair": per, "host_cython_ms_per_call": per * len(pairs), "host_pairs_timed": k,
                      "host_note": "reference Cython compute_depth_ratios (-O2) and check_depth_consistency's numpy, one host thread"})
-    line.update(info)
-    lines.append(line)
-    print(json.dumps(line), flush=True)
-    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    with open(args.out, "a") as f:
-        for line in lines:
-            f.write(json.dumps(line) + "\n")
+    rows.add(line)
+    rows.save()
 
 
 if __name__ == "__main__":

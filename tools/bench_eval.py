@@ -5,51 +5,23 @@ with numpy / scipy for comparison.  Appends JSON lines to --out (default profile
     python tools/bench_eval.py [--batch 64] [--reps 20] [--host-samples 4] [--out profiles/h100_eval.jsonl]
 """
 import argparse
-import json
 import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 import scipy.ndimage
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-from demon_b200 import evaluation as ev            # noqa: E402
-from demon_b200 import lmbspecialops as sops       # noqa: E402
-from demon_b200 import weights as W                # noqa: E402
-from demon_b200.networks_original import DemonPipeline, Session   # noqa: E402
-from oracle import view_tools as vt                # noqa: E402
+from benchkit import ROOT, Rows, call_times, summary
+from demon_b200 import evaluation as ev
+from demon_b200 import lmbspecialops as sops
+from demon_b200 import weights as W
+from demon_b200.networks_original import DemonPipeline, Session
+from oracle import view_tools as vt
 
 
-def device_info():
-    info = {"gpu": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
-                           text=True, timeout=30).stdout.strip().splitlines()[0]
-        info["power_limit"], info["max_sm_clock"] = [s.strip() for s in q.split(",")]
-    except Exception as e:   # the figure is still a measurement; say that the power limit could not be read
-        info["power_limit"] = "unknown (%s)" % type(e).__name__
-    return info
-
-
-def time_ms(fn, reps, warmup=3):
-    """Median per-call time over `reps` calls, each bracketed by CUDA events on the current stream."""
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    times = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        times.append(a.elapsed_time(b))
-    return float(np.median(times)), float(np.min(times)), float(np.max(times))
+def median_ms(fn, reps):
+    return summary(call_times(fn, reps))["ms"]
 
 
 def host_errors(pred, gt):
@@ -76,14 +48,7 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_eval needs a CUDA device")
     B, reps = args.batch, args.reps
-    info = device_info()
-    lines = []
-
-    def emit(d):
-        d.update(info)
-        print(json.dumps(d), flush=True)
-        lines.append(d)
-
+    rows = Rows(args.out)
     sess = Session()
     sess.load_weights(W.synthetic_weights(0))
     pipe = DemonPipeline(sess, batch_size=B, iterations=3)
@@ -91,15 +56,15 @@ def main():
     ip = (torch.rand(B, 6, 192, 256, generator=g) - 0.5).cuda()
     pipe.stage(ip)
     # alternate the three calls in one window so that drift on a shared host hits all of them alike
-    t_fwd = time_ms(lambda: pipe.forward_staged(), reps)
-    t_snap = time_ms(lambda: pipe.forward_snapshots(ip, refine=False), reps)
-    t_snap_r = time_ms(lambda: pipe.forward_snapshots(ip, refine=True), reps)
-    t_fwd2 = time_ms(lambda: pipe.forward_staged(), reps)
-    emit({"bench": "forward_snapshots", "batch": B, "iterations": 3, "precision": sess.precision,
-          "forward_ms": min(t_fwd[0], t_fwd2[0]), "forward_ms_runs": [t_fwd, t_fwd2],
-          "snapshots_ms": t_snap[0], "snapshots_refined_ms": t_snap_r[0],
-          "snapshots_refined_over_forward": t_snap_r[0] / min(t_fwd[0], t_fwd2[0]),
-          "launches_forward": pipe.launches(), "launches_snapshots_refined": pipe.snapshot_launches()})
+    t_fwd = summary(call_times(lambda: pipe.forward_staged(), reps))
+    t_snap = median_ms(lambda: pipe.forward_snapshots(ip, refine=False), reps)
+    t_snap_r = median_ms(lambda: pipe.forward_snapshots(ip, refine=True), reps)
+    t_fwd2 = summary(call_times(lambda: pipe.forward_staged(), reps))
+    fwd = min(t_fwd["ms"], t_fwd2["ms"])
+    rows.add({"bench": "forward_snapshots", "batch": B, "iterations": 3, "precision": sess.precision, "forward_ms": fwd,
+              "forward_ms_runs": [[t["ms"], t["ms_min"], t["ms_max"]] for t in (t_fwd, t_fwd2)],
+              "snapshots_ms": t_snap, "snapshots_refined_ms": t_snap_r, "snapshots_refined_over_forward": t_snap_r / fwd,
+              "launches_forward": pipe.launches(), "launches_snapshots_refined": pipe.snapshot_launches()})
 
     # ground truth of the batch: 480x640 inverse depth with holes, motions, intrinsics
     n, gh, gw = B, 480, 640
@@ -137,12 +102,11 @@ def main():
     def run_motion():
         for k in range(4):
             ev.motion_errors(preds["predict_rotation"][k], preds["predict_translation"][k], motion_d)
-    t_mask, t_flow, t_sums, t_mot = (time_ms(f, reps) for f in (run_mask, run_flow, run_sums, run_motion))
-    t_batch = time_ms(lambda: ev.evaluate_batch(preds, inv_d, motion_d, intr, depthmask=True), max(5, reps // 2))
-    emit({"bench": "ground_truth_work", "samples": n, "gt": [gh, gw], "depthmask": True, "mask_ms": t_mask[0], "flow_gt_ms": t_flow[0],
-          "sums_8_snapshots_ms": t_sums[0], "motion_ms": t_mot[0],
-          "device_ms": t_mask[0] + t_flow[0] + t_sums[0] + t_mot[0],
-          "evaluate_batch_ms": t_batch[0], "evaluate_batch_note": "whole call: host operand construction, launches, one copy, host table"})
+    t_mask, t_flow, t_sums, t_mot = (median_ms(f, reps) for f in (run_mask, run_flow, run_sums, run_motion))
+    t_batch = median_ms(lambda: ev.evaluate_batch(preds, inv_d, motion_d, intr, depthmask=True), max(5, reps // 2))
+    rows.add({"bench": "ground_truth_work", "samples": n, "gt": [gh, gw], "depthmask": True, "mask_ms": t_mask, "flow_gt_ms": t_flow,
+              "sums_8_snapshots_ms": t_sums, "motion_ms": t_mot, "device_ms": t_mask + t_flow + t_sums + t_mot,
+              "evaluate_batch_ms": t_batch, "evaluate_batch_note": "whole call: host operand construction, launches, one copy, host table"})
 
     # the same per sample on the host: numpy mask, scipy zoom of 8 depth snapshots and 4 flows, numpy errors
     hp = {k: v[:, :args.host_samples].cpu().numpy() for k, v in preds.items()}
@@ -163,12 +127,9 @@ def main():
                 epe[np.isfinite(epe) & (epe > 0)].mean()
                 ev.compute_motion_errors(np.concatenate([hp["predict_rotation"][k, i], hp["predict_translation"][k, i]]), motion[i], True)
     host_ms = (time.perf_counter() - t0) * 1000 / args.host_samples
-    emit({"bench": "ground_truth_work_host", "samples_timed": args.host_samples, "per_sample_ms": host_ms,
-          "per_64_samples_ms": host_ms * 64, "cpu": os.cpu_count(), "note": "numpy / scipy on one host thread per sample"})
-    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    with open(args.out, "a") as f:
-        for d in lines:
-            f.write(json.dumps(d) + "\n")
+    rows.add({"bench": "ground_truth_work_host", "samples_timed": args.host_samples, "per_sample_ms": host_ms,
+              "per_64_samples_ms": host_ms * 64, "cpu": os.cpu_count(), "note": "numpy / scipy on one host thread per sample"})
+    rows.save()
 
 
 if __name__ == "__main__":

@@ -8,17 +8,15 @@ steps) and kernel launches per step (counted by torch.profiler).  One JSON line 
     python tools/bench_losses.py [--steps K] [--warmup W] [--out profiles/h100_losses.jsonl]
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from demon_b200 import lmbspecialops as sops   # noqa: E402
-from demon_b200.v2 import losses as L          # noqa: E402
+from benchkit import Rows, call_times, profiled_kernels, summary
+from demon_b200 import lmbspecialops as sops
+from demon_b200.v2 import losses as L
 
 N, H, W = 32, 192, 256
 FLOW = dict(flow_weight=1000.0, conf_weight=1000.0, flow_sig_weight=1000.0, conf_sig_weight=1000.0, conf_diff_scale=10, level5_factor=0)
@@ -80,39 +78,9 @@ def c_refine_block(g, d0, n0, a):
 
 
 # ---- measurement ---------------------------------------------------------------------------------------------------------------
-def timed(fn, steps, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
-    for a, b in ev:
-        a.record()
-        fn()
-        b.record()
-    torch.cuda.synchronize()
-    return float(np.median([a.elapsed_time(b) for a, b in ev]))
-
-
-def launches(fn):
-    from torch.profiler import ProfilerActivity, profile
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    return sum(1 for e in prof.events() if e.device_type.name == "CUDA" and not e.name.startswith(("Memcpy", "Memset")))
-
-
 def agree(a, b, rtol):
     a, b = float(a.detach()), float(b.detach())
     return abs(a - b) <= rtol * max(abs(b), 1e-30)
-
-
-def power_limit():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
-                              timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        return ""
 
 
 def main():
@@ -172,18 +140,18 @@ def main():
             return total
         return run
 
-    rows = []
-    gpu = power_limit()
+    rows = Rows(args.out)
+
+    def timed(fn):
+        return round(summary(call_times(fn, args.steps, args.warmup, sync_each=False))["ms"], 4)
 
     def row(name, fused, composed, check):
         with torch.no_grad() if "backward" not in name else torch.enable_grad():
             ok = check()
-            rec = {"row": name, "batch": N, "depth_hw": [H, W], "fused_ms": round(timed(fused, args.steps, args.warmup), 4),
-                   "composed_ms": round(timed(composed, args.steps, args.warmup), 4), "fused_launches": launches(fused),
-                   "composed_launches": launches(composed), "agree": bool(ok), "gpu": gpu}
+            rec = {"row": name, "batch": N, "depth_hw": [H, W], "fused_ms": timed(fused), "composed_ms": timed(composed),
+                   "fused_launches": profiled_kernels(fused), "composed_launches": profiled_kernels(composed), "agree": bool(ok)}
         rec["speedup"] = round(rec["composed_ms"] / rec["fused_ms"], 2)
-        print(json.dumps(rec))
-        rows.append(rec)
+        rows.add(rec)
 
     row("prepare_ground_truth", lambda: L.prepare_ground_truth_tensors(depth, rot_gt, tr_gt, k), lambda: c_ground_truth(depth, rot_gt, tr_gt, k),
         lambda: all(torch.equal(a.view(torch.int32), b.view(torch.int32)) for a, b in
@@ -202,11 +170,7 @@ def main():
         return all(torch.allclose(ga[key], leaf[key].grad, rtol=1e-3, atol=1e-6 * float(leaf[key].grad.abs().max())) for key in keys)
     row("4_iterative_forward_backward", fused_it, comp_it, lambda: grads_agree(fused_it, comp_it, ("f2", "f5", "c2", "c5", "d2", "n2", "rot", "tr")))
     row("5_refine_forward_backward", fused_rf, comp_rf, lambda: grads_agree(fused_rf, comp_rf, ("d0", "n0")))
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as fh:
-            for r in rows:
-                fh.write(json.dumps(r) + "\n")
+    rows.save()
     if not all(r["agree"] for r in rows):
         sys.exit("the fused and composed results disagree")
 

@@ -5,28 +5,25 @@ before timing).  The batch comes from datareader.build_batch over synthetic view
 weights are v2.weights.synthetic_weights (no trained v2 weights are published).
 
 Each row: milliseconds per call (median of CUDA-event timed calls, after warm-up) and the library's kernel launches per
-call (demon_launch_count; torch's own small ops of the composition are not counted), with the card's name and power
+call (its own launch counter; torch's own small ops of the composition are not counted), with the card's name and power
 limit read in the same run.  One JSON line per evolution:
     python tools/bench_objective.py [--steps K] [--warmup W] [--precision 3xtf32] [--out profiles/h100_objective.jsonl]
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 
 import numpy as np
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from demon_b200 import _lib                     # noqa: E402
-from demon_b200 import datareader as dr        # noqa: E402
-from demon_b200 import images                  # noqa: E402
-from demon_b200.dataset_tools import View      # noqa: E402
-from demon_b200.v2 import blocks, objective    # noqa: E402
-from demon_b200.v2 import weights as W2        # noqa: E402
-from demon_b200.v2.networks import Session     # noqa: E402
-from oracle.datareader import synthetic_views  # noqa: E402
+from benchkit import Rows, call_times, library_launches, summary
+from demon_b200 import datareader as dr
+from demon_b200 import images
+from demon_b200.dataset_tools import View
+from demon_b200.v2 import blocks, objective
+from demon_b200.v2 import weights as W2
+from demon_b200.v2.networks import Session
+from oracle.datareader import synthetic_views
 
 BATCH, NEW = 32, 8   # training.py:92-94 and its queue of _simulated_iterations - 1 = 3 earlier batches
 
@@ -42,35 +39,6 @@ def training_batch(b, seed):
     return dr.build_batch(pool, pairs, params, aug)
 
 
-def timed(fn, steps, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
-    for a, b in ev:
-        a.record()
-        fn()
-        b.record()
-    torch.cuda.synchronize()
-    return float(np.median([a.elapsed_time(b) for a, b in ev]))
-
-
-def launches(fn):
-    """Kernels the library launches in one call (its own counter, demon_launch_count); the torch ops of the composition
-    (contiguous copies of channel slices, concatenations, scalar adds) come on top."""
-    lib = _lib.load()
-    n0 = lib.demon_launch_count()
-    fn()
-    return int(lib.demon_launch_count() - n0)
-
-
-def gpu_info():
-    out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
-                         timeout=30, check=True).stdout.strip().splitlines()[0]
-    name, limit = (s.strip() for s in out.split(","))
-    return name, limit
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
@@ -80,7 +48,7 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_objective needs a CUDA device")
-    name, limit = gpu_info()
+    rows = Rows(args.out)
     session = Session(precision=args.precision)
     session.load_weights(W2.synthetic_weights(0))
     batch = training_batch(BATCH, 3)
@@ -90,7 +58,6 @@ def main():
     fc2 = blocks.flow_block(ip[NEW:], scope='netFlow1', session=session)['predict_flowconf2']
     earlier = blocks.depthmotion_block(ip[NEW:], i22, fc2[:, 0:2], fc2, scope='netDM1', session=session)
     session.kernel_l2()   # once per load_weights, not part of a call
-    rows = []
     for evo in objective.EVOLUTIONS:
         prev = earlier if evo >= '4_iterative' else None
 
@@ -98,17 +65,11 @@ def main():
             return objective.objective(session, batch, evo, prev)
         res = call()
         torch.cuda.synchronize()
-        rec = {"row": "objective", "evolution": evo, "batch": BATCH, "new_samples": NEW if prev is not None else BATCH,
-               "precision": args.precision, "ms": round(timed(call, args.steps, args.warmup), 3), "library_launches": launches(call),
-               "total": float(res["total"]), "finite": bool(all(torch.isfinite(v).item() for v in res.values())),
-               "gpu": name, "power_limit": limit}
-        print(json.dumps(rec), flush=True)
-        rows.append(rec)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as fh:
-            for r in rows:
-                fh.write(json.dumps(r) + "\n")
+        ms = summary(call_times(call, args.steps, args.warmup, sync_each=False))["ms"]
+        rows.add({"row": "objective", "evolution": evo, "batch": BATCH, "new_samples": NEW if prev is not None else BATCH,
+                  "precision": args.precision, "ms": round(ms, 3), "library_launches": library_launches(call),
+                  "total": float(res["total"]), "finite": bool(all(torch.isfinite(v).item() for v in res.values()))})
+    rows.save()
     if not all(r["finite"] for r in rows):
         sys.exit("a loss is not finite")
 

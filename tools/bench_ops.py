@@ -2,26 +2,11 @@
 hot-path size ([64,*,48,64]): CUDA-event time per launch, algorithmic bytes / time, fraction of the measured copy peak."""
 import json
 import os
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from benchkit import ROOT, span_ms
 from demon_b200 import lmbspecialops as ops
-
-
-def timeit(fn, n=20):
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(n):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / n
 
 
 def main():
@@ -52,7 +37,7 @@ def main():
             ("leaky_relu", lambda: ops.leaky_relu(img), 2 * 3 * 4 * px),
         ]
         for name, fn, nbytes in cases:
-            ms = timeit(fn)
+            ms = span_ms(fn, 20)
             gbs = nbytes / (ms / 1e3) / 1e9
             rows.append((tag, name, ms, nbytes / 1e6, gbs, gbs / peak))
     print("| size | op | ms / launch (incl. output allocation) | algorithmic MB | GB/s | fraction of measured copy peak (%.0f GB/s) |" % peak)

@@ -6,21 +6,15 @@ Cython (oracle/_ref/vis_cython.so, where it was built) on the host for the same 
     python tools/bench_pointcloud.py [--reps 50] [--host-views 4] [--out profiles/h100_pointcloud.jsonl]
 """
 import argparse
-import json
 import os
-import sys
 import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-
-from bench_eval import device_info, time_ms   # noqa: E402
-from demon_b200 import vis                    # noqa: E402
-from oracle import vis as ov                  # noqa: E402
+from benchkit import ROOT, Rows, call_times, summary
+from demon_b200 import vis
+from oracle import vis as ov
 
 HBM_BYTES_PER_S = 3.35e12   # H100 SXM data sheet
 
@@ -49,8 +43,7 @@ def main():
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_pointcloud.jsonl"))
     args = ap.parse_args()
     assert torch.cuda.is_available(), "the benchmark needs a GPU"
-    info = device_info()
-    lines = []
+    rows = Rows(args.out)
     for n, h, w, normals in ((64, 192, 256, False), (64, 192, 256, True), (8, 768, 1024, False)):
         inv, img, nrm, K = inputs(n, h, w)
         dev = dict(d=torch.from_numpy(inv).cuda(), i=torch.from_numpy(img).cuda(), n=torch.from_numpy(nrm).cuda(),
@@ -59,11 +52,12 @@ def main():
         def run():
             return vis.point_clouds(dev['d'], dev['K'], dev['R'], dev['t'], normals=dev['n'] if normals else None, image=dev['i'],
                                     inverse_depth=True)
-        med, lo, hi = time_ms(run, args.reps, warmup=5)
+        tm = summary(call_times(run, args.reps, warmup=5))
+        med = tm["ms"]
         valid = int(run()['counts'].sum())
         moved = bytes_moved(n, h, w, valid, normals)
         line = {"bench": "point_clouds", "views": n, "size": [h, w], "normals": normals, "colors": "image", "inverse_depth": True,
-                "device_ms": med, "device_ms_min": lo, "device_ms_max": hi, "reps": args.reps, "points": valid,
+                "device_ms": med, "device_ms_min": tm["ms_min"], "device_ms_max": tm["ms_max"], "reps": args.reps, "points": valid,
                 "bytes_moved": moved, "achieved_GBps": moved / (med * 1e-3) / 1e9,
                 "hbm_share": moved / (med * 1e-3) / HBM_BYTES_PER_S, "launches_per_call": 2}
         if ov.have_module() and args.host_views > 0:
@@ -79,13 +73,8 @@ def main():
             per_view = (time.perf_counter() - t0) * 1e3 / k
             line.update({"host_cython_ms_per_view": per_view, "host_cython_ms_per_batch": per_view * n, "host_views_timed": k,
                          "host_note": "reference Cython (-O2), one host thread, including 1/inverse depth and the uint8 cast"})
-        line.update(info)
-        lines.append(line)
-        print(json.dumps(line), flush=True)
-    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    with open(args.out, "a") as f:
-        for line in lines:
-            f.write(json.dumps(line) + "\n")
+        rows.add(line)
+    rows.save()
 
 
 if __name__ == "__main__":

@@ -10,36 +10,19 @@ profiles/h100_precision.jsonl).
     python tools/bench_precision.py [--reps 20] [--out profiles/h100_precision.jsonl]
 """
 import argparse
-import json
 import os
 import re
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-from demon_b200 import weights as W1                                             # noqa: E402
-from demon_b200.networks_original import DemonPipeline, RefinementNet, Session   # noqa: E402
-from demon_b200.v2 import weights as W2                                          # noqa: E402
-from demon_b200.v2.networks import DemonPipelineV2, Session as SessionV2         # noqa: E402
+from benchkit import ROOT, Rows, call_times, device_events, summary
+from demon_b200 import weights as W1
+from demon_b200.networks_original import DemonPipeline, RefinementNet, Session
+from demon_b200.v2 import weights as W2
+from demon_b200.v2.networks import DemonPipelineV2, Session as SessionV2
 
 PRECS = ("fp16", "tf32", "3xtf32")
-
-
-def device_info():
-    """The card's name and power limit, read in the same call as the timings."""
-    info = {"gpu": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        info["power_limit"], info["max_sm_clock"] = [s.strip() for s in q.split(",")]
-    except Exception as e:   # the figure is still a measurement; say that the power limit could not be read
-        info["power_limit"] = "unknown (%s)" % type(e).__name__
-    return info
 
 
 def alternate(steps, reps, warmup=3):
@@ -48,21 +31,11 @@ def alternate(steps, reps, warmup=3):
     for _ in range(warmup):
         for fn in steps.values():
             fn()
-    torch.cuda.synchronize()
     times = {p: [] for p in steps}
     for _ in range(reps):
         for p, fn in steps.items():
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            fn()
-            b.record()
-            b.synchronize()
-            times[p].append(a.elapsed_time(b))
+            times[p] += call_times(fn, 1, warmup=0)
     return times
-
-
-def summary(ts):
-    return dict(ms=float(np.median(ts)), ms_min=float(np.min(ts)), ms_max=float(np.max(ts)), steps=len(ts))
 
 
 def kernel_kind(name):
@@ -73,14 +46,8 @@ def kernel_kind(name):
 def profile_conv_kernels(fn):
     """Device time of conv_tc_halo_kernel per kind over one call of fn, and every other kernel's, from torch.profiler."""
     fn()
-    torch.cuda.synchronize()
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
     out = {"halo": 0.0, "per-tap": 0.0, "other": 0.0}
-    for ev in prof.events():
-        if ev.device_type != torch.autograd.DeviceType.CUDA:
-            continue
+    for ev in device_events(fn)[1]:
         out[kernel_kind(ev.name) or "other"] += ev.device_time_total / 1000.0
     return out
 
@@ -88,7 +55,7 @@ def profile_conv_kernels(fn):
 def cublas_fp16_tflops(n=8192, reps=20):
     a = torch.randn(n, n, device="cuda", dtype=torch.float16)
     b = torch.randn(n, n, device="cuda", dtype=torch.float16)
-    ts = alternate({"gemm": lambda: torch.matmul(a, b)}, reps)["gemm"]
+    ts = call_times(lambda: torch.matmul(a, b), reps)
     return 2.0 * n ** 3 / (float(np.median(ts)) * 1e-3) / 1e12
 
 
@@ -99,8 +66,7 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_precision needs a CUDA device")
-    info = device_info()
-    lines = []
+    rows = Rows(args.out)
     g = torch.Generator().manual_seed(1234)
     s1 = {p: Session(p) for p in PRECS}
     s2 = {p: SessionV2(p) for p in PRECS}
@@ -113,9 +79,8 @@ def main():
         base = summary(times["3xtf32"])["ms"]
         for p in PRECS:
             sm = summary(times[p])
-            lines.append(dict(bench=bench, precision=p, **sm, **{unit: per_step * 1000.0 / sm["ms"]},
-                              speedup_vs_3xtf32=base / sm["ms"], speedup_vs_tf32=summary(times["tf32"])["ms"] / sm["ms"], **extra, **info))
-            print(json.dumps(lines[-1]))
+            rows.add(dict(bench=bench, precision=p, **sm, **{unit: per_step * 1000.0 / sm["ms"]},
+                          speedup_vs_3xtf32=base / sm["ms"], speedup_vs_tf32=summary(times["tf32"])["ms"] / sm["ms"], **extra))
 
     for batch in (64, 1):
         x = (torch.rand(batch, 6, 192, 256, generator=g) - 0.5).cuda()
@@ -140,21 +105,15 @@ def main():
     for p in PRECS:
         pipe = DemonPipeline(s1[p], batch_size=64, iterations=3)
         k = profile_conv_kernels(lambda: pipe.forward(x))
-        lines.append(dict(bench="v1_pipeline_kernels", precision=p, batch=64, conv_tc_halo_ms=k["halo"], conv_tc_per_tap_ms=k["per-tap"],
-                          other_kernels_ms=k["other"], note="torch.profiler device time of one step, outside the timed runs",
-                          **info))
-        print(json.dumps(lines[-1]))
+        rows.add(dict(bench="v1_pipeline_kernels", precision=p, batch=64, conv_tc_halo_ms=k["halo"], conv_tc_per_tap_ms=k["per-tap"],
+                      other_kernels_ms=k["other"], note="torch.profiler device time of one step, outside the timed runs"))
         del pipe
     gflop = 2 * W1.macs_per_pair()["pipeline"] / 1e9
-    fp16_b64 = [ln for ln in lines if ln["bench"] == "v1_pipeline" and ln["precision"] == "fp16" and ln["batch"] == 64][0]
-    lines.append(dict(bench="cublas_fp16_gemm", m=8192, n=8192, k=8192, tflops=tflops,
-                      v1_b64_fp16_tflops=gflop * 64 / fp16_b64["ms"], v1_b64_fp16_share_of_cublas=gflop * 64 / fp16_b64["ms"] / tflops,
-                      note="torch.matmul fp16 (cuBLAS), median of 20; the pipeline's rate counts 2 x its multiply-accumulates",
-                      **info))
-    print(json.dumps(lines[-1]))
-    with open(args.out, "a") as f:
-        for ln in lines:
-            f.write(json.dumps(ln) + "\n")
+    fp16_b64 = [ln for ln in rows if ln["bench"] == "v1_pipeline" and ln["precision"] == "fp16" and ln["batch"] == 64][0]
+    rows.add(dict(bench="cublas_fp16_gemm", m=8192, n=8192, k=8192, tflops=tflops,
+                  v1_b64_fp16_tflops=gflop * 64 / fp16_b64["ms"], v1_b64_fp16_share_of_cublas=gflop * 64 / fp16_b64["ms"] / tflops,
+                  note="torch.matmul fp16 (cuBLAS), median of 20; the pipeline's rate counts 2 x its multiply-accumulates"))
+    rows.save()
 
 
 if __name__ == "__main__":

@@ -6,47 +6,23 @@ name and power limit.
     python tools/bench_prepare.py [--pairs 64] [--reps 50] [--out FILE]
 """
 import argparse
-import json
-import os
-import subprocess
-import sys
 import time
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from benchkit import Rows, span_ms
 from demon_b200 import images
 
 SIZES = [(640, 480), (1920, 1080)]
 FILTERS = ["nearest", "bilinear", "bicubic"]
 
 
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clock = (s.strip() for s in out.split(","))
-        return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
-    except Exception:
-        return {"gpu": torch.cuda.get_device_name(), "power_limit": None, "max_sm_clock": None}
-
-
 def device_ms(pairs, reps, f):
     """CUDA-event milliseconds of one batch's resizes, averaged over `reps` batches after a warm-up"""
     run = lambda: images.resize(images.resize(pairs.reshape(-1, *pairs.shape[2:]), (256, 192), f).view(pairs.shape[0], 2, 192, 256, 3)[:, 1],
                                 (64, 48), f)
-    for _ in range(3):
-        run()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        run()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
+    return span_ms(run, reps)
 
 
 def host_ms(pairs_np, f):
@@ -73,24 +49,18 @@ def main():
         pil_version = PIL.__version__
     except ImportError:
         pil_version = None
-    info = gpu_info()
-    lines = []
+    rows = Rows(a.out)
     for (w, h) in SIZES:
         pairs_np = np.random.default_rng(0).integers(0, 256, (a.pairs, 2, h, w, 3), dtype=np.uint8)
         pairs = torch.from_numpy(pairs_np).cuda()
         for f in FILTERS:
             rec = {"source": "%dx%d" % (w, h), "filter": f, "pairs": a.pairs, "device_ms_per_batch": round(device_ms(pairs, a.reps, f), 4),
                    "host_pillow_ms_per_batch": round(host_ms(pairs_np, f), 1) if pil_version else None,
-                   "pillow": pil_version, **info}
+                   "pillow": pil_version}
             if rec["host_pillow_ms_per_batch"] is not None:
                 rec["host_over_device"] = round(rec["host_pillow_ms_per_batch"] / rec["device_ms_per_batch"], 1)
-            print(json.dumps(rec), flush=True)
-            lines.append(rec)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as fh:
-            for r in lines:
-                fh.write(json.dumps(r) + "\n")
+            rows.add(rec)
+    rows.save()
 
 
 if __name__ == "__main__":

@@ -15,21 +15,15 @@ once per call, so its time includes that host round trip).
     python tools/bench_sparse_tsdf.py [--reps 10] [--out profiles/h100_sparse_tsdf.jsonl]
 """
 import argparse
-import json
 import os
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from demon_b200 import sequence                                   # noqa: E402
-from bench_sequence import device_info, orbit_frames, timed       # noqa: E402
-import sequence_oracle as so                                      # noqa: E402
+from benchkit import ROOT, Rows, call_times, summary
+from bench_sequence import orbit_frames
+from demon_b200 import sequence
+import sequence_oracle as so
 
 
 def corridor_frames(n, h=192, w=256):
@@ -52,14 +46,7 @@ def main():
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "h100_sparse_tsdf.jsonl"))
     args = ap.parse_args()
-    info = device_info()
-    rows = []
-
-    def emit(row):
-        row.update(info)
-        rows.append(row)
-        print(json.dumps(row), flush=True)
-
+    rows = Rows(args.out)
     dims, origin, vs = (256, 256, 256), (-1.25, -1.25, -1.25), 2.5 / 255
     d, K, R, t, img = orbit_frames(256)
     dev = {k: torch.from_numpy(v).cuda() for k, v in dict(d=d, K=K, R=R, t=t, img=img).items()}
@@ -67,25 +54,26 @@ def main():
         for color in (False, True):
             fr = (dev["d"][:n], dev["K"], dev["R"][:n], dev["t"][:n], dev["img"][:n] if color else None)
             dense = sequence.TsdfVolume(dims, origin, vs, color=color)
-            ms, lo, hi = timed(lambda: dense.integrate(*fr), args.reps)
+            tm = summary(call_times(lambda: dense.integrate(*fr), args.reps, warmup=1))
             dense = sequence.TsdfVolume(dims, origin, vs, color=color).integrate(*fr)
-            mesh_ms, _, _ = timed(dense.mesh, args.reps)
+            mesh_ms = summary(call_times(dense.mesh, args.reps, warmup=1))["ms"]
             nbytes = sum(x.numel() * x.element_size() for x in (dense.tsdf, dense.weight, dense.color) if x is not None)
-            emit({"bench": "orbit", "volume": "dense", "frames": n, "color": color, "voxel_size": vs, "dims": dims,
-                  "integrate_ms": ms, "integrate_ms_min": lo, "integrate_ms_max": hi, "mesh_ms": mesh_ms,
-                  "triangles": int(dense.mesh()[2].shape[0]), "voxels": int(np.prod(dims)), "state_bytes": nbytes})
+            rows.add({"bench": "orbit", "volume": "dense", "frames": n, "color": color, "voxel_size": vs, "dims": dims,
+                      "integrate_ms": tm["ms"], "integrate_ms_min": tm["ms_min"], "integrate_ms_max": tm["ms_max"], "mesh_ms": mesh_ms,
+                      "triangles": int(dense.mesh()[2].shape[0]), "voxels": int(np.prod(dims)), "state_bytes": nbytes})
             del dense
-            first_ms, flo, fhi = timed(lambda: sequence.SparseTsdfVolume(vs, origin, color=color).integrate(*fr), args.reps)
+            first = summary(call_times(lambda: sequence.SparseTsdfVolume(vs, origin, color=color).integrate(*fr), args.reps, warmup=1))
             sp = sequence.SparseTsdfVolume(vs, origin, color=color).integrate(*fr)
-            ms, lo, hi = timed(lambda: sp.integrate(*fr), args.reps)
+            again = summary(call_times(lambda: sp.integrate(*fr), args.reps, warmup=1))
             sp = sequence.SparseTsdfVolume(vs, origin, color=color).integrate(*fr)
-            mesh_ms, _, _ = timed(sp.mesh, args.reps)
+            mesh_ms = summary(call_times(sp.mesh, args.reps, warmup=1))["ms"]
             m = int(sp.blocks.shape[0])
-            emit({"bench": "orbit", "volume": "sparse", "frames": n, "color": color, "voxel_size": vs,
-                  "integrate_first_ms": first_ms, "integrate_first_ms_min": flo, "integrate_first_ms_max": fhi,
-                  "integrate_again_ms": ms, "integrate_again_ms_min": lo, "integrate_again_ms_max": hi, "mesh_ms": mesh_ms,
-                  "triangles": int(sp.mesh()[2].shape[0]), "blocks": m, "voxels": 512 * m, "capacity_blocks": sp.capacity,
-                  "table_slots": sp.table_slots, "state_bytes": sp.nbytes, "skipped_pixels": sp.last_skipped_pixels})
+            rows.add({"bench": "orbit", "volume": "sparse", "frames": n, "color": color, "voxel_size": vs,
+                      "integrate_first_ms": first["ms"], "integrate_first_ms_min": first["ms_min"],
+                      "integrate_first_ms_max": first["ms_max"], "integrate_again_ms": again["ms"],
+                      "integrate_again_ms_min": again["ms_min"], "integrate_again_ms_max": again["ms_max"], "mesh_ms": mesh_ms,
+                      "triangles": int(sp.mesh()[2].shape[0]), "blocks": m, "voxels": 512 * m, "capacity_blocks": sp.capacity,
+                      "table_slots": sp.table_slots, "state_bytes": sp.nbytes, "skipped_pixels": sp.last_skipped_pixels})
             del sp
             torch.cuda.empty_cache()
 
@@ -97,24 +85,15 @@ def main():
     vol = sequence.SparseTsdfVolume(cvs, box[0], color=False)
     for s in range(0, n, chunk):
         sl = slice(s, s + chunk)
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        vol.integrate(dev["d"][sl], dev["K"], dev["R"][sl], dev["t"][sl])
-        b.record()
-        b.synchronize()
-        ms = a.elapsed_time(b)
+        ms, = call_times(lambda: vol.integrate(dev["d"][sl], dev["K"], dev["R"][sl], dev["t"][sl]), 1, warmup=0)
         m = int(vol.blocks.shape[0])
-        emit({"bench": "corridor_integrate", "frames": [s, s + chunk], "voxel_size": cvs, "box": box, "dense_voxels_of_box": dense_voxels,
-              "ms": ms, "ms_per_frame": ms / chunk, "blocks": m, "voxels": 512 * m, "state_bytes": vol.nbytes,
-              "skipped_pixels": vol.last_skipped_pixels, "pixels": chunk * d.shape[1] * d.shape[2]})
-    mesh_ms, lo, hi = timed(vol.mesh, max(3, args.reps // 3))
-    emit({"bench": "corridor_mesh", "frames": n, "voxel_size": cvs, "blocks": int(vol.blocks.shape[0]), "ms": mesh_ms, "ms_min": lo,
-          "ms_max": hi, "triangles": int(vol.mesh()[2].shape[0]), "state_bytes": vol.nbytes})
-
-    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    with open(args.out, "a") as fh:
-        for r in rows:
-            fh.write(json.dumps(r) + "\n")
+        rows.add({"bench": "corridor_integrate", "frames": [s, s + chunk], "voxel_size": cvs, "box": box, "dense_voxels_of_box": dense_voxels,
+                  "ms": ms, "ms_per_frame": ms / chunk, "blocks": m, "voxels": 512 * m, "state_bytes": vol.nbytes,
+                  "skipped_pixels": vol.last_skipped_pixels, "pixels": chunk * d.shape[1] * d.shape[2]})
+    tm = summary(call_times(vol.mesh, max(3, args.reps // 3), warmup=1))
+    rows.add({"bench": "corridor_mesh", "frames": n, "voxel_size": cvs, "blocks": int(vol.blocks.shape[0]), "ms": tm["ms"],
+              "ms_min": tm["ms_min"], "ms_max": tm["ms_max"], "triangles": int(vol.mesh()[2].shape[0]), "state_bytes": vol.nbytes})
+    rows.save()
 
 
 if __name__ == "__main__":

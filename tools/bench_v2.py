@@ -7,47 +7,14 @@ GFLOP per pair are counted like demon_b200.weights.layer_macs counts v1's (2 x m
 """
 import argparse
 import ctypes
-import json
 import os
-import subprocess
-import sys
 
-import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-from demon_b200 import _lib                                   # noqa: E402
-from demon_b200.v2 import weights as W2                        # noqa: E402
-from demon_b200.v2.networks import DemonPipelineV2, RefinementNet, Session   # noqa: E402
-
-
-def device_info():
-    info = {"gpu": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
-                           text=True, timeout=30).stdout.strip().splitlines()[0]
-        info["power_limit"], info["max_sm_clock"] = [s.strip() for s in q.split(",")]
-    except Exception as e:   # the figure is still a measurement; say that the power limit could not be read
-        info["power_limit"] = "unknown (%s)" % type(e).__name__
-    return info
-
-
-def time_ms(fn, reps, warmup=3):
-    """Median, min and max per-call time over `reps` calls, each bracketed by CUDA events on the current stream."""
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    times = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        times.append(a.elapsed_time(b))
-    return float(np.median(times)), float(np.min(times)), float(np.max(times))
+from benchkit import ROOT, Rows, call_times, summary
+from demon_b200 import _lib
+from demon_b200.v2 import weights as W2
+from demon_b200.v2.networks import DemonPipelineV2, RefinementNet, Session
 
 
 def main():
@@ -57,8 +24,7 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_v2 needs a CUDA device")
-    info = device_info()
-    lines = []
+    rows = Rows(args.out)
     s = Session("3xtf32")
     s.load_weights(W2.synthetic_weights(0))
     macs = W2.macs_per_pair()
@@ -67,18 +33,18 @@ def main():
     for batch in (64, 1):
         pipe = DemonPipelineV2(s, batch_size=batch, iterations=3)
         x = (torch.rand(batch, 6, 192, 256, generator=g) - 0.5).cuda()
-        med, lo, hi = time_ms(lambda: pipe.forward(x), args.reps)
-        lines.append(dict(bench="v2_pipeline", batch=batch, iterations=3, precision="3xtf32", ms=med, ms_min=lo, ms_max=hi,
-                          pairs_per_s=batch * 1000.0 / med, gflop_per_pair=gflop_pair, tflops=gflop_pair * batch / med,
-                          launches=pipe.launches(), **info))
+        t = summary(call_times(lambda: pipe.forward(x), args.reps))
+        rows.add(dict(bench="v2_pipeline", batch=batch, iterations=3, precision="3xtf32", ms=t["ms"], ms_min=t["ms_min"],
+                      ms_max=t["ms_max"], pairs_per_s=batch * 1000.0 / t["ms"], gflop_per_pair=gflop_pair,
+                      tflops=gflop_pair * batch / t["ms"], launches=pipe.launches()))
     # refinement block at 1024x768, batch 8
     rn = RefinementNet(s, "channels_first", 8, image_size=(768, 1024))
     im = (torch.rand(8, 3, 768, 1024, generator=g) - 0.5).cuda()
     d2 = (torch.rand(8, 1, 192, 256, generator=g) * 0.6 + 0.2).cuda()
-    med, lo, hi = time_ms(lambda: rn.eval(im, d2, None), args.reps)
+    t = summary(call_times(lambda: rn.eval(im, d2, None), args.reps))
     gflop_ref = 2 * sum(v for k, v in W2.layer_macs((768, 1024)).items() if k.startswith("netRefine/")) / 1e9
-    lines.append(dict(bench="v2_refine", batch=8, size=[768, 1024], precision="3xtf32", ms=med, ms_min=lo, ms_max=hi,
-                      images_per_s=8 * 1000.0 / med, gflop_per_image=gflop_ref, **info))
+    rows.add(dict(bench="v2_refine", batch=8, size=[768, 1024], precision="3xtf32", ms=t["ms"], ms_min=t["ms_min"],
+                  ms_max=t["ms_max"], images_per_s=8 * 1000.0 / t["ms"], gflop_per_image=gflop_ref))
     # dense5 at batch 1: per-layer CUDA events of the stage-wise bootstrap (demon_net_profile_*)
     lib = _lib.load()
     net = s.net(1)
@@ -102,13 +68,10 @@ def main():
             if calls.value == 0 or ms.value <= 0:
                 raise RuntimeError("no device time recorded for %s (calls %d, ms %g)" % (name, calls.value, ms.value))
             per = ms.value / calls.value
-            lines.append(dict(bench="v2_dense5", layer=name, batch=1, ms=per, weight_mb=4608 * 4608 * 4 / 1e6,
-                              gb_per_s=4608 * 4608 * 4 / (per * 1e-3) / 1e9,
-                              note="the dense kernel and its split-K reduction, without the gather / scatter copies", **info))
-    with open(args.out, "a") as f:
-        for ln in lines:
-            f.write(json.dumps(ln) + "\n")
-            print(json.dumps(ln))
+            rows.add(dict(bench="v2_dense5", layer=name, batch=1, ms=per, weight_mb=4608 * 4608 * 4 / 1e6,
+                          gb_per_s=4608 * 4608 * 4 / (per * 1e-3) / 1e9,
+                          note="the dense kernel and its split-K reduction, without the gather / scatter copies"))
+    rows.save()
 
 
 if __name__ == "__main__":

@@ -5,9 +5,9 @@ import json
 import os
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
 import torch
+
+from benchkit import ROOT, span_ms
 from demon_b200 import _lib, weights as W
 from demon_b200.networks_original import Session, DemonPipeline
 
@@ -27,13 +27,7 @@ def main():
         pipe.forward(x, None)
     torch.cuda.synchronize()
     _lib.check(lib.demon_net_profile_begin(pipe.net.ptr))
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(steps):
-        pipe.forward(x, None)
-    e1.record()
-    torch.cuda.synchronize()
-    total = e0.elapsed_time(e1) / steps
+    total = span_ms(lambda: pipe.forward(x, None), steps, warmup=0)
     _lib.check(lib.demon_net_profile_end(pipe.net.ptr))
     lm = W.layer_macs()
     rows = []
