@@ -13,6 +13,19 @@ _DEFAULT = os.path.join(_HERE, "lib", "libdemon_b200.so")
 c_void_p, c_int, c_int64, c_float, c_double, c_char_p = (
     ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_double, ctypes.c_char_p)
 
+
+class PipelineArgs(ctypes.Structure):
+    """demon_pipeline_args: one fused-pipeline call, every field 64 bits wide (include/demon_b200.h)."""
+    _fields_ = [("input", c_int64), ("images", c_void_p), ("image2_2", c_void_p), ("image2_2_mode", c_int64),
+                ("sn", c_int64), ("si", c_int64), ("sy", c_int64), ("h", c_int64), ("w", c_int64), ("resample", c_int64),
+                ("K", c_void_p), ("status", c_void_p), ("iterations", c_int64), ("snapshots", c_int64),
+                ("depth0", c_void_p), ("normal0", c_void_p), ("rotation", c_void_p), ("translation", c_void_p),
+                ("flow2", c_void_p), ("depth2", c_void_p), ("normal2", c_void_p)]
+
+
+# PipelineArgs.input (DEMON_INPUT_*)
+INPUT_F32, INPUT_U8, INPUT_RESIZE_U8, INPUT_VIEWS_U8 = range(4)
+
 # name -> argtypes; every function returns int unless listed in _RESTYPES
 _P = c_void_p
 PROTOTYPES = {
@@ -98,27 +111,11 @@ PROTOTYPES = {
     "demon_refine_forward_v2": [_P] * 6 + [c_int, _P],
     "demon_flow_block_forward_v2": [_P, c_char_p] + [_P] * 9 + [c_int, _P],
     "demon_depthmotion_block_forward_v2": [_P, c_char_p] + [_P] * 12 + [c_int, _P],
-    "demon_pipeline_forward_v2": [_P, _P, _P, c_int] + [_P] * 7 + [_P],
+    "demon_pipeline_run": [_P, ctypes.POINTER(PipelineArgs), _P],
+    "demon_pipeline_run_host": [_P, ctypes.POINTER(PipelineArgs), c_int, _P],
     "demon_debug_describe_plan": [c_int] * 5 + [_P, c_int],
-    "demon_pipeline_forward": [_P, _P, _P, c_int] + [_P] * 6 + [_P],
-    "demon_pipeline_forward_snapshots": [_P, _P, _P, c_int] + [_P] * 6 + [_P],
-    "demon_pipeline_forward_host": [_P, _P, _P, c_int, _P, _P, _P, _P],
-    "demon_pipeline_forward_host_async": [_P, _P, _P, c_int, _P, _P, _P, _P],
-    "demon_pipeline_forward_u8": [_P, _P, _P, c_int] + [_P] * 6 + [_P],
-    "demon_pipeline_forward_host_u8": [_P, _P, _P, c_int, _P, _P, _P, _P],
-    "demon_pipeline_forward_host_u8_async": [_P, _P, _P, c_int, _P, _P, _P, _P],
     "demon_resize_u8": [_P, c_int64, c_int64, c_int, c_int, c_int, _P, c_int, c_int, c_int, _P],
-    "demon_pipeline_forward_images_u8": [_P, _P, c_int64, c_int64, c_int64] + [c_int] * 5 + [_P] * 6 + [_P],
     "demon_adjust_intrinsics_u8": [_P, c_int64, c_int64, c_int, c_int, c_int, _P] + [c_double] * 4 + [_P, c_int, c_int, _P, _P],
-    "demon_pipeline_forward_views_u8": [_P, _P, c_int64, c_int64, c_int64, c_int, c_int, _P, _P] + [c_int] * 3 + [_P] * 6 + [_P],
-    "demon_pipeline_forward_snapshots_v2": [_P, _P, _P, c_int, c_int] + [_P] * 7 + [_P],
-    "demon_pipeline_forward_u8_v2": [_P, _P, _P, c_int, c_int] + [_P] * 7 + [_P],
-    "demon_pipeline_forward_images_u8_v2": [_P, _P, c_int64, c_int64, c_int64] + [c_int] * 5 + [_P] * 7 + [_P],
-    "demon_pipeline_forward_views_u8_v2": [_P, _P, c_int64, c_int64, c_int64, c_int, c_int, _P, _P] + [c_int] * 3 + [_P] * 7 + [_P],
-    "demon_pipeline_forward_host_v2": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P],
-    "demon_pipeline_forward_host_async_v2": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P],
-    "demon_pipeline_forward_host_u8_v2": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P],
-    "demon_pipeline_forward_host_u8_async_v2": [_P, _P, _P, c_int, c_int, _P, _P, _P, _P, _P],
     "demon_resize_area_f32": [_P, c_int64, _P] + [c_int] * 6 + [_P],
     "demon_sharpness_u8": [_P, c_int64, c_int64, c_int, c_int, c_int, _P, _P],
     "demon_sun3d_depth_u16": [_P, c_int, c_int, c_int, _P, _P, _P],

@@ -80,31 +80,10 @@ struct Layer {
 // The refinement block has no head (head_end == begin).
 struct Block { int begin = 0, head_end = 0, end = 0; };
 
-// The outputs of a fused-pipeline call, in the C ABI's order; any pointer may be null (normal0: v2 nets only)
-struct PipelineOutputs { float *depth0, *rotation, *translation, *flow2, *depth2, *normal2, *normal0; };
-
-enum PipelineInput : int64_t { IN_FP32, IN_U8, IN_RESIZE, IN_VIEWS };
-// NO_SNAPSHOTS: the last iteration's predictions and the refinement block; otherwise snapshot k (0 = bootstrap, k = after
-// iteration k) of every output is its k-th [B, ...] slice, and SNAPSHOTS_REFINED runs the refinement block on every snapshot
-// (examples/evaluation.py:225-255 refines all four)
-enum SnapshotMode : int64_t { NO_SNAPSHOTS, SNAPSHOTS, SNAPSHOTS_REFINED };
-
-// Everything one demon_pipeline_forward* call depends on, and so also the key of its CUDA graph: every field is 64 bits
-// wide, so the struct has no padding and equal calls are equal bytes.  Entries value-initialise it (unused fields are 0).
-struct PipelineCall {
-  PipelineInput input;
-  const float* image_pair;        // IN_FP32: [B,6,192,256]
-  const float* image2_2;          // IN_FP32: [B,3,48,64] or null (median3x3_downsample twice)
-  const uint8_t* images;          // IN_U8: [B,2,192,256,3]; IN_RESIZE / IN_VIEWS: [B,2,h,w,3] with strides sn, si, sy
-  const uint8_t* image2_2_u8;     // IN_U8: [B,48,64,3] or null
-  int64_t sn, si, sy, h, w, resample, image2_2_mode;
-  const double* K;                // IN_VIEWS: [B,2,4], adapted to the network's intrinsics with status [B,2]
-  uint8_t* status;
-  int64_t iterations;
-  PipelineOutputs out;
-  SnapshotMode snapshots;
-};
-static_assert(std::has_unique_object_representations<PipelineCall>::value, "PipelineCall is compared with memcmp");
+// A validated demon_pipeline_args (check_pipeline_args) is everything one fused-pipeline call depends on, and so also the
+// key of its CUDA graph: equal calls must be equal bytes
+static_assert(std::has_unique_object_representations<demon_pipeline_args>::value, "demon_pipeline_args is compared with memcmp");
+static_assert(sizeof(demon_pipeline_args) == 21 * sizeof(int64_t), "demon_pipeline_args: 21 fields of 64 bits each");
 
 }  // namespace
 }  // namespace demon
@@ -126,9 +105,9 @@ struct demon_net {
   std::map<std::string, std::vector<float>> host_vars;   // the weights set so far, TF layout; uploaded at finalize
   std::vector<void*> dev_allocs;
   int pipeline_launches[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  int snapshot_launches[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // the same for demon_pipeline_forward_snapshots (kept apart: bench.py reads the above)
+  int snapshot_launches[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // the same for the pipeline calls with snapshots (kept apart: bench.py reads the above)
   // CUDA graphs of the fused pipeline, one per distinct call (launch-bound at small batch: ~270 launches)
-  struct GraphEntry { PipelineCall call; cudaGraphExec_t exec; int launches; };
+  struct GraphEntry { demon_pipeline_args call; cudaGraphExec_t exec; int launches; };
   std::vector<GraphEntry> graphs;
   cudaStream_t cap_stream = nullptr;   // capture happens on this private stream (the caller's may be the legacy default stream)
   // optional per-layer timing with CUDA events on the launching stream (bench.py's roofline leg)
@@ -1354,7 +1333,8 @@ int demon_net_layer_profile(const demon_net* n, int i, double* ms, int64_t* call
   return DEMON_OK;
 }
 
-// A forward entry of network variant v (1: the demon_* entries, 2: the demon_*_v2 entries) takes only a net of that variant
+// A stage-wise or block entry of network variant v (1: the demon_* entries, 2: the demon_*_v2 entries) takes only a net of
+// that variant
 #define REQUIRE_READY_AS(n, v)                                                   \
   do {                                                                           \
     DEMON_REQUIRE(n, "null net");                                                \
@@ -1537,34 +1517,33 @@ int demon_depthmotion_block_forward_v2(demon_net* n, const char* scope, const fl
 static const double kNetIntrinsics[4] = {0.89115971 * 256, 1.18821287 * 192, 0.5 * 256, 0.5 * 192};
 
 // The predictions at snapshot point k (0 = bootstrap, k = after iteration k) into the call's outputs, at slice k with
-// snapshots, then the refinement block on them unless the call takes snapshots without it
-static int export_outputs(demon_net* n, const PipelineCall& c, int k, cudaStream_t s) {
+// snapshots, then the refinement block on them unless the call takes snapshots without it (no depth0)
+static int export_outputs(demon_net* n, const demon_pipeline_args& c, int k, cudaStream_t s) {
   const long B = n->B, P2 = 48L * 64, P0 = 192L * 256;
-  const long slice = c.snapshots == NO_SNAPSHOTS ? 0 : k;
+  const long slice = c.snapshots ? k : 0;
   const auto at = [slice](float* p, long per_snapshot) { return p ? p + slice * per_snapshot : nullptr; };
-  const PipelineOutputs& o = c.out;
-  int rc = export_predictions(n, nullptr, at(o.flow2, B * 2 * P2), at(o.depth2, B * P2), at(o.normal2, B * 3 * P2), at(o.rotation, B * 3),
-                              at(o.translation, B * 3), 0, s);
-  if (rc || c.snapshots == SNAPSHOTS) return rc;
+  int rc = export_predictions(n, nullptr, at(c.flow2, B * 2 * P2), at(c.depth2, B * P2), at(c.normal2, B * 3 * P2), at(c.rotation, B * 3),
+                              at(c.translation, B * 3), 0, s);
+  if (rc || (c.snapshots && !c.depth0)) return rc;
   if (n->variant == 2)
-    return run_refine_block_v2(n, n->img8->p, buf_strides(n->img8), n->dn2->p, buf_strides(n->dn2), 48, 64, at(o.depth0, B * P0),
-                               at(o.normal0, B * 3 * P0), 0, s);
+    return run_refine_block_v2(n, n->img8->p, buf_strides(n->img8), n->dn2->p, buf_strides(n->dn2), 48, 64, at(c.depth0, B * P0),
+                               at(c.normal0, B * 3 * P0), 0, s);
   // image1 is read back from img8 (NHWC8: the first three channels), whatever the input kind; no depth0: into rdepth0
-  return run_refine_block(n, n->img8->p, buf_strides(n->img8), n->dn2->p, buf_strides(n->dn2), 48, 64, at(o.depth0, B * P0), s);
+  return run_refine_block(n, n->img8->p, buf_strides(n->img8), n->dn2->p, buf_strides(n->dn2), 48, 64, at(c.depth0, B * P0), s);
 }
 
-static int pipeline_body(demon_net* n, const PipelineCall& c, cudaStream_t s) {
+static int pipeline_body(demon_net* n, const demon_pipeline_args& c, cudaStream_t s) {
   int rc;
   const long P = 192L * 256;
-  const uint8_t* images = c.images;
-  const uint8_t* image2_2_u8 = c.image2_2_u8;
-  if (c.input == IN_RESIZE || c.input == IN_VIEWS) {
+  const uint8_t* images = static_cast<const uint8_t*>(c.images);
+  const uint8_t* image2_2_u8 = static_cast<const uint8_t*>(c.image2_2);
+  if (c.input == DEMON_INPUT_RESIZE_U8 || c.input == DEMON_INPUT_VIEWS_U8) {
     uint8_t* pair = reinterpret_cast<uint8_t*>(n->pair_bytes->p);
-    if (c.input == IN_VIEWS)
-      rc = adjust_intrinsics_launch(c.images, c.sn, c.si, 2, c.sy, 2 * n->B, (int)c.h, (int)c.w, c.K, kNetIntrinsics, pair, 192, 256,
+    if (c.input == DEMON_INPUT_VIEWS_U8)
+      rc = adjust_intrinsics_launch(images, c.sn, c.si, 2, c.sy, 2 * n->B, (int)c.h, (int)c.w, c.K, kNetIntrinsics, pair, 192, 256,
                                     c.status, s);
     else
-      rc = resize_u8_launch(c.images, c.sn, c.si, 2, c.sy, 2 * n->B, (int)c.h, (int)c.w, pair, 192, 256, (int)c.resample, s);
+      rc = resize_u8_launch(images, c.sn, c.si, 2, c.sy, 2 * n->B, (int)c.h, (int)c.w, pair, 192, 256, (int)c.resample, s);
     if (rc) return rc;
     images = pair;
     if (c.image2_2_mode == 1) {
@@ -1573,7 +1552,7 @@ static int pipeline_body(demon_net* n, const PipelineCall& c, cudaStream_t s) {
       image2_2_u8 = i22;
     }
   }
-  if (c.input != IN_FP32) {
+  if (c.input != DEMON_INPUT_F32) {
     // img8 straight from the bytes; without image2_2, image 2's planes for the median pair
     float* planes2 = image2_2_u8 ? nullptr : n->planes2->p;
     long blocks = ((long)n->B * P + 255) / 256;
@@ -1588,18 +1567,19 @@ static int pipeline_body(demon_net* n, const PipelineCall& c, cudaStream_t s) {
       return rc;
     }
   } else {
-    if ((rc = import_image_pair(n, c.image_pair, 0, s))) return rc;
+    const float* image_pair = static_cast<const float*>(c.images);
+    if ((rc = import_image_pair(n, image_pair, 0, s))) return rc;
     if (c.image2_2) {
-      if ((rc = import_image2_2(n, c.image2_2, 0, s))) return rc;
+      if ((rc = import_image2_2(n, static_cast<const float*>(c.image2_2), 0, s))) return rc;
     } else {
-      if ((rc = downsample_image2_2(n, c.image_pair + 3 * P, 6 * P, c.image2_2_mode, s))) return rc;
+      if ((rc = downsample_image2_2(n, image_pair + 3 * P, 6 * P, c.image2_2_mode, s))) return rc;
     }
   }
   // k = 0: the bootstrap blocks; k > 0: iteration k
   for (int k = 0; k <= c.iterations; ++k) {
     if ((rc = run_flow_block(n, k ? n->flow2 : n->flow1, k > 0, s, k == 0))) return rc;
     if ((rc = run_dm_block(n, k ? n->dm2 : n->dm1, k > 0, s, k == 0))) return rc;
-    if ((c.snapshots != NO_SNAPSHOTS || k == c.iterations) && (rc = export_outputs(n, c, k, s))) return rc;
+    if ((c.snapshots || k == c.iterations) && (rc = export_outputs(n, c, k, s))) return rc;
     // conv1 / conv2 of netFlow2 and netDM2 read only the image pair and fixed weights: once per call instead of once per
     // iteration (bit identical; 2 x 2 x 221.7 MMAC per pair less to execute at three iterations)
     if (k == 0 && c.iterations > 0) {
@@ -1610,19 +1590,47 @@ static int pipeline_body(demon_net* n, const PipelineCall& c, cudaStream_t s) {
   return DEMON_OK;
 }
 
-// The fused pipeline is not traced: a graph captured with the trace's copies inside would replay them after it is cleared
-static int refuse_while_tracing(const demon_net* n) {
+// The one check of a fused-pipeline call, shared by both entries and done before anything is launched.  The network
+// variant comes from the handle.  A field the input kind does not read must be 0 / NULL: the struct is the call's CUDA-graph
+// key, and a stray value there would capture a second graph of the same call.
+static int check_pipeline_args(const demon_net* n, const demon_pipeline_args* a) {
+  DEMON_REQUIRE(n && a, "pipeline: null net or args");
+  if (!n->finalized) return fail(DEMON_E_STATE, "forward before demon_net_finalize");
+  int dev = -1;
+  cudaGetDevice(&dev);
+  if (dev != n->device) return fail(DEMON_E_STATE, "net handle belongs to CUDA device %d but device %d is current", n->device, dev);
+  // The fused pipeline is not traced: a graph captured with the trace's copies inside would replay them after it is cleared
   if (n->tracing) return fail(DEMON_E_STATE, "pipeline: a layer trace is set (demon_debug_trace_layers); only the stage-wise entries are traced");
-  return DEMON_OK;
+  DEMON_REQUIRE(n->RH == 192 && n->RW == 256, "pipeline: net was created with a %dx%d refinement block", n->RH, n->RW);
+  DEMON_REQUIRE(a->iterations >= 0 && a->iterations <= 7, "pipeline: iterations %lld", (long long)a->iterations);
+  DEMON_REQUIRE(a->input >= DEMON_INPUT_F32 && a->input <= DEMON_INPUT_VIEWS_U8, "pipeline: no input kind %lld", (long long)a->input);
+  DEMON_REQUIRE(a->images, "pipeline: null images");
+  DEMON_REQUIRE(a->snapshots == 0 || a->snapshots == 1, "pipeline: snapshots %lld is not 0 or 1", (long long)a->snapshots);
+  DEMON_REQUIRE(!a->normal0 || n->variant == 2, "pipeline: normal0 needs a v2 net (demon_net_create_v2)");
+  DEMON_REQUIRE(!a->snapshots || a->depth0 || !a->normal0, "pipeline: normal0 without depth0 in snapshots (normal0 comes out of the refinement block)");
+  const bool views = a->input == DEMON_INPUT_VIEWS_U8, any_size = views || a->input == DEMON_INPUT_RESIZE_U8;
+  // image2_2_mode 2 (area) is v2's only: it is the input training/v2/training.py feeds v2, and v1 never saw it
+  DEMON_REQUIRE(a->image2_2_mode == 0 || (a->image2_2_mode == 1 && any_size) || (a->image2_2_mode == 2 && n->variant == 2),
+                "pipeline: image2_2_mode %lld is not 0 (median)%s%s", (long long)a->image2_2_mode,
+                any_size ? ", 1 (resize)" : "", n->variant == 2 ? ", 2 (area)" : "");
+  DEMON_REQUIRE(a->image2_2_mode != 2 || !a->image2_2, "pipeline: image2_2_mode 2 (area) computes image2_2, which must then be NULL");
+  DEMON_REQUIRE(!a->K == !views && !a->status == !views, "pipeline: K and status come with DEMON_INPUT_VIEWS_U8, and only with it");
+  if (!any_size) {
+    DEMON_REQUIRE(!a->sn && !a->si && !a->sy && !a->h && !a->w && !a->resample,
+                  "pipeline: sn, si, sy, h, w and resample are for DEMON_INPUT_RESIZE_U8 / DEMON_INPUT_VIEWS_U8 only");
+    return DEMON_OK;
+  }
+  DEMON_REQUIRE(!a->image2_2, "pipeline: DEMON_INPUT_RESIZE_U8 / DEMON_INPUT_VIEWS_U8 make image2_2 as image2_2_mode says; it must be NULL");
+  DEMON_REQUIRE(a->sn >= 0 && a->si >= 0 && a->sy >= 0, "pipeline: negative stride");
+  DEMON_REQUIRE(a->h == (int)a->h && a->w == (int)a->w && a->resample == (int)a->resample, "pipeline: h, w or resample out of range");
+  if (!views) return resize_u8_check((int)a->h, (int)a->w, 192, 256, (int)a->resample, "pipeline_images_u8");
+  if (int rc = adjust_intrinsics_check((int)a->h, (int)a->w, kNetIntrinsics, 192, 256, "pipeline_views_u8")) return rc;
+  return resize_u8_check(192, 256, 48, 64, (int)a->resample, "pipeline_views_u8");
 }
 
-static int pipeline_forward_impl(demon_net* n, const PipelineCall& c, void* stream) {
-  if (int rc = refuse_while_tracing(n)) return rc;
-  DEMON_REQUIRE(c.iterations >= 0 && c.iterations <= 7, "pipeline: iterations %d", (int)c.iterations);
-  int* launch_record = c.snapshots != NO_SNAPSHOTS ? n->snapshot_launches : n->pipeline_launches;
-  DEMON_REQUIRE(n->RH == 192 && n->RW == 256, "pipeline: net was created with a %dx%d refinement block", n->RH, n->RW);
-  cudaStream_t s = (cudaStream_t)stream;
-  // The call is one CUDA graph per distinct PipelineCall (DEMON_GRAPH=0 disables): the first call with a new one runs
+static int pipeline_forward_impl(demon_net* n, const demon_pipeline_args& c, cudaStream_t s) {
+  int* launch_record = c.snapshots ? n->snapshot_launches : n->pipeline_launches;
+  // The call is one CUDA graph per distinct demon_pipeline_args (DEMON_GRAPH=0 disables): the first call with a new one runs
   // eagerly, the second captures, later ones replay.  Not used while per-layer profiling is on or when the caller is itself
   // capturing this stream.
   static const bool graphs_on = []() { const char* e = getenv("DEMON_GRAPH"); return !(e && e[0] == '0'); }();
@@ -1664,190 +1672,42 @@ static int pipeline_forward_impl(demon_net* n, const PipelineCall& c, void* stre
   return DEMON_OK;
 }
 
-int demon_pipeline_forward(demon_net* n, const float* image_pair, const float* image2_2, int iterations, float* depth0, float* rotation,
-                           float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
-  REQUIRE_READY(n);
-  DEMON_REQUIRE(image_pair, "pipeline: null image_pair");
-  PipelineCall c{};
-  c.input = IN_FP32; c.image_pair = image_pair; c.image2_2 = image2_2; c.iterations = iterations;
-  c.out = {depth0, rotation, translation, flow2, depth2, normal2};
-  return pipeline_forward_impl(n, c, stream);
+int demon_pipeline_run(demon_net* n, const demon_pipeline_args* args, void* stream) {
+  if (int rc = check_pipeline_args(n, args)) return rc;
+  return pipeline_forward_impl(n, *args, (cudaStream_t)stream);
 }
 
-int demon_pipeline_forward_v2(demon_net* n, const float* image_pair, const float* image2_2, int iterations, float* depth0, float* normal0,
-                              float* rotation, float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
-  REQUIRE_READY_AS(n, 2);
-  DEMON_REQUIRE(image_pair, "pipeline_v2: null image_pair");
-  PipelineCall c{};
-  c.input = IN_FP32; c.image_pair = image_pair; c.image2_2 = image2_2; c.iterations = iterations;
-  c.out = {depth0, rotation, translation, flow2, depth2, normal2, normal0};
-  return pipeline_forward_impl(n, c, stream);
-}
-
-// The image2_2 source of a v2 entry that takes pairs at the network's size (uint8 or float32): 0 (the given image2_2, or
-// the median pair without one) or 2 (resize_area of image 2; then there is no given image2_2)
-static int check_pair_mode(int image2_2_mode, const void* image2_2, const char* who) {
-  DEMON_REQUIRE(image2_2_mode == 0 || image2_2_mode == 2, "%s: image2_2_mode %d is not 0 (median) or 2 (area)", who, image2_2_mode);
-  DEMON_REQUIRE(image2_2_mode == 0 || !image2_2, "%s: image2_2_mode 2 (area) computes image2_2, which must then be NULL", who);
-  return DEMON_OK;
-}
-
-// snapshot k of every output at slice k; the refinement block runs on every snapshot iff depth0 is given
-static int snapshots_impl(demon_net* n, const float* image_pair, const float* image2_2, int image2_2_mode, int iterations,
-                          const PipelineOutputs& o, void* stream) {
-  DEMON_REQUIRE(image_pair, "pipeline_snapshots: null image_pair");
-  DEMON_REQUIRE(o.depth0 || !o.normal0, "pipeline_snapshots: normal0 without depth0 (normal0 comes out of the refinement block)");
-  PipelineCall c{};
-  c.input = IN_FP32; c.image_pair = image_pair; c.image2_2 = image2_2; c.image2_2_mode = image2_2_mode; c.iterations = iterations;
-  c.out = o;
-  c.snapshots = o.depth0 ? SNAPSHOTS_REFINED : SNAPSHOTS;
-  return pipeline_forward_impl(n, c, stream);
-}
-
-int demon_pipeline_forward_snapshots(demon_net* n, const float* image_pair, const float* image2_2, int iterations, float* flow2,
-                                     float* depth2, float* normal2, float* rotation, float* translation, float* depth0, void* stream) {
-  REQUIRE_READY(n);
-  return snapshots_impl(n, image_pair, image2_2, 0, iterations, {depth0, rotation, translation, flow2, depth2, normal2}, stream);
-}
-
-int demon_pipeline_forward_snapshots_v2(demon_net* n, const float* image_pair, const float* image2_2, int image2_2_mode, int iterations,
-                                        float* depth0, float* normal0, float* rotation, float* translation, float* flow2, float* depth2,
-                                        float* normal2, void* stream) {
-  REQUIRE_READY_AS(n, 2);
-  if (int rc = check_pair_mode(image2_2_mode, image2_2, "pipeline_snapshots_v2")) return rc;
-  return snapshots_impl(n, image_pair, image2_2, image2_2_mode, iterations, {depth0, rotation, translation, flow2, depth2, normal2, normal0},
-                        stream);
-}
-
-static int u8_impl(demon_net* n, const uint8_t* images, const uint8_t* image2_2, int image2_2_mode, int iterations, const PipelineOutputs& o,
-                   void* stream) {
-  DEMON_REQUIRE(images, "pipeline_u8: null images");
-  PipelineCall c{};
-  c.input = IN_U8; c.images = images; c.image2_2_u8 = image2_2; c.image2_2_mode = image2_2_mode; c.iterations = iterations;
-  c.out = o;
-  return pipeline_forward_impl(n, c, stream);
-}
-
-int demon_pipeline_forward_u8(demon_net* n, const uint8_t* images, const uint8_t* image2_2, int iterations, float* depth0, float* rotation,
-                              float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
-  REQUIRE_READY(n);
-  return u8_impl(n, images, image2_2, 0, iterations, {depth0, rotation, translation, flow2, depth2, normal2}, stream);
-}
-
-int demon_pipeline_forward_u8_v2(demon_net* n, const uint8_t* images, const uint8_t* image2_2, int image2_2_mode, int iterations,
-                                 float* depth0, float* normal0, float* rotation, float* translation, float* flow2, float* depth2,
-                                 float* normal2, void* stream) {
-  REQUIRE_READY_AS(n, 2);
-  if (int rc = check_pair_mode(image2_2_mode, image2_2, "pipeline_u8_v2")) return rc;
-  return u8_impl(n, images, image2_2, image2_2_mode, iterations, {depth0, rotation, translation, flow2, depth2, normal2, normal0}, stream);
-}
-
-// The argument checks shared by the entries that take uint8 pairs of any size, which then fill the source fields of `c`.
-// image2_2_mode 2 (area) is v2's only: it is the input training/v2/training.py feeds v2, and v1 never saw it
-static int set_source(const demon_net* n, PipelineCall& c, PipelineInput input, const uint8_t* images, int64_t sn, int64_t si, int64_t sy,
-                      int h, int w, int resample, int image2_2_mode, const char* who) {
-  DEMON_REQUIRE(sn >= 0 && si >= 0 && sy >= 0, "%s: negative stride", who);
-  if (n->variant == 2)
-    DEMON_REQUIRE(image2_2_mode >= 0 && image2_2_mode <= 2, "%s: image2_2_mode %d is not 0 (median), 1 (resize) or 2 (area)", who,
-                  image2_2_mode);
-  else
-    DEMON_REQUIRE(image2_2_mode == 0 || image2_2_mode == 1, "%s: image2_2_mode %d is not 0 (median) or 1 (resize)", who, image2_2_mode);
-  c.input = input; c.images = images; c.sn = sn; c.si = si; c.sy = sy; c.h = h; c.w = w; c.resample = resample;
-  c.image2_2_mode = image2_2_mode;
-  return DEMON_OK;
-}
-
-static int images_impl(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, int resample,
-                       int image2_2_mode, int iterations, const PipelineOutputs& o, void* stream) {
-  DEMON_REQUIRE(images, "pipeline_images_u8: null images");
-  PipelineCall c{};
-  int rc = set_source(n, c, IN_RESIZE, images, sn, si, sy, h, w, resample, image2_2_mode, "pipeline_images_u8");
-  if (rc || (rc = resize_u8_check(h, w, 192, 256, resample, "pipeline_images_u8"))) return rc;
-  c.iterations = iterations;
-  c.out = o;
-  return pipeline_forward_impl(n, c, stream);
-}
-
-int demon_pipeline_forward_images_u8(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, int resample,
-                                     int image2_2_mode, int iterations, float* depth0, float* rotation, float* translation, float* flow2,
-                                     float* depth2, float* normal2, void* stream) {
-  REQUIRE_READY(n);
-  return images_impl(n, images, sn, si, sy, h, w, resample, image2_2_mode, iterations, {depth0, rotation, translation, flow2, depth2, normal2},
-                     stream);
-}
-
-int demon_pipeline_forward_images_u8_v2(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, int resample,
-                                        int image2_2_mode, int iterations, float* depth0, float* normal0, float* rotation, float* translation,
-                                        float* flow2, float* depth2, float* normal2, void* stream) {
-  REQUIRE_READY_AS(n, 2);
-  return images_impl(n, images, sn, si, sy, h, w, resample, image2_2_mode, iterations,
-                     {depth0, rotation, translation, flow2, depth2, normal2, normal0}, stream);
-}
-
-static int views_impl(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, const double* K, uint8_t* status,
-                      int resample, int image2_2_mode, int iterations, const PipelineOutputs& o, void* stream) {
-  DEMON_REQUIRE(images && K && status, "pipeline_views_u8: null images, K or status");
-  PipelineCall c{};
-  int rc = set_source(n, c, IN_VIEWS, images, sn, si, sy, h, w, resample, image2_2_mode, "pipeline_views_u8");
-  if (rc || (rc = adjust_intrinsics_check(h, w, kNetIntrinsics, 192, 256, "pipeline_views_u8"))) return rc;
-  if ((rc = resize_u8_check(192, 256, 48, 64, resample, "pipeline_views_u8"))) return rc;
-  c.K = K; c.status = status; c.iterations = iterations;
-  c.out = o;
-  return pipeline_forward_impl(n, c, stream);
-}
-
-int demon_pipeline_forward_views_u8(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, const double* K,
-                                    uint8_t* status, int resample, int image2_2_mode, int iterations, float* depth0, float* rotation,
-                                    float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
-  REQUIRE_READY(n);
-  return views_impl(n, images, sn, si, sy, h, w, K, status, resample, image2_2_mode, iterations,
-                    {depth0, rotation, translation, flow2, depth2, normal2}, stream);
-}
-
-int demon_pipeline_forward_views_u8_v2(demon_net* n, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w, const double* K,
-                                       uint8_t* status, int resample, int image2_2_mode, int iterations, float* depth0, float* normal0,
-                                       float* rotation, float* translation, float* flow2, float* depth2, float* normal2, void* stream) {
-  REQUIRE_READY_AS(n, 2);
-  return views_impl(n, images, sn, si, sy, h, w, K, status, resample, image2_2_mode, iterations,
-                    {depth0, rotation, translation, flow2, depth2, normal2, normal0}, stream);
-}
-
-// H2D of the inputs into the staging buffers (build_plan, build_plan_v2), the pipeline of network `variant`, D2H of depth0 /
+// H2D of the host inputs into the staging buffers (build_plan, build_plan_v2), the pipeline on them, D2H of depth0 /
 // normal0 (v2) / rotation / translation
-static int pipeline_host(demon_net* n, int variant, const void* images_host, const void* image2_2_host, bool u8, int image2_2_mode,
-                         int iterations, float* depth0_host, float* normal0_host, float* rotation_host, float* translation_host, void* stream,
-                         bool sync) {
-  REQUIRE_READY_AS(n, variant);
-  if (int rc = refuse_while_tracing(n)) return rc;
-  DEMON_REQUIRE(images_host && depth0_host, "pipeline_host: null pointer");
-  if (variant == 2)
-    if (int rc = check_pair_mode(image2_2_mode, image2_2_host, "pipeline_host_v2")) return rc;
+int demon_pipeline_run_host(demon_net* n, const demon_pipeline_args* args, int synchronize, void* stream) {
+  if (int rc = check_pipeline_args(n, args)) return rc;
+  const demon_pipeline_args& h = *args;
+  const bool u8 = h.input == DEMON_INPUT_U8;
+  DEMON_REQUIRE(u8 || h.input == DEMON_INPUT_F32, "pipeline_run_host: input %lld is not DEMON_INPUT_F32 or DEMON_INPUT_U8", (long long)h.input);
+  DEMON_REQUIRE(!h.snapshots, "pipeline_run_host: takes no snapshots");
+  DEMON_REQUIRE(h.depth0, "pipeline_run_host: null depth0");
+  DEMON_REQUIRE(!h.flow2 && !h.depth2 && !h.normal2, "pipeline_run_host: flow2, depth2 and normal2 are not copied back and must be NULL");
   cudaStream_t s = (cudaStream_t)stream;
   const size_t px = (size_t)n->B * 192 * 256;
   const size_t ip_bytes = u8 ? px * 6 : px * 6 * sizeof(float);
   const size_t i22_bytes = (size_t)n->B * 3 * 48 * 64 * (u8 ? 1 : sizeof(float));
-  void* ip_dev = n->pair_bytes->p;
-  void* i22_dev = image2_2_host ? n->i22_bytes->p : nullptr;
-  DEMON_CHECK_CUDA(cudaMemcpyAsync(ip_dev, images_host, ip_bytes, cudaMemcpyHostToDevice, s));
-  if (i22_dev) DEMON_CHECK_CUDA(cudaMemcpyAsync(i22_dev, image2_2_host, i22_bytes, cudaMemcpyHostToDevice, s));
   float* rt_dev = n->host_motion->p;
-  PipelineCall c{};
-  if (u8) { c.input = IN_U8; c.images = static_cast<const uint8_t*>(ip_dev); c.image2_2_u8 = static_cast<const uint8_t*>(i22_dev); }
-  else { c.input = IN_FP32; c.image_pair = static_cast<const float*>(ip_dev); c.image2_2 = static_cast<const float*>(i22_dev); }
-  c.image2_2_mode = image2_2_mode;
-  c.iterations = iterations;
-  c.out.depth0 = n->host_depth0->p;
-  c.out.normal0 = normal0_host ? n->host_normal0->p : nullptr;
-  c.out.rotation = rotation_host ? rt_dev : nullptr;
-  c.out.translation = translation_host ? rt_dev + 3 * n->B : nullptr;
-  int rc = pipeline_forward_impl(n, c, stream);
-  if (rc) return rc;
-  DEMON_CHECK_CUDA(cudaMemcpyAsync(depth0_host, c.out.depth0, px * sizeof(float), cudaMemcpyDeviceToHost, s));
-  if (normal0_host) DEMON_CHECK_CUDA(cudaMemcpyAsync(normal0_host, c.out.normal0, px * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
-  if (rotation_host) DEMON_CHECK_CUDA(cudaMemcpyAsync(rotation_host, rt_dev, (size_t)n->B * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
-  if (translation_host)
-    DEMON_CHECK_CUDA(cudaMemcpyAsync(translation_host, rt_dev + 3 * n->B, (size_t)n->B * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
-  if (sync) {
+  demon_pipeline_args c = h;   // the same call on the staging buffers
+  c.images = n->pair_bytes->p;
+  c.image2_2 = h.image2_2 ? n->i22_bytes->p : nullptr;
+  c.depth0 = n->host_depth0->p;
+  c.normal0 = h.normal0 ? n->host_normal0->p : nullptr;
+  c.rotation = h.rotation ? rt_dev : nullptr;
+  c.translation = h.translation ? rt_dev + 3 * n->B : nullptr;
+  DEMON_CHECK_CUDA(cudaMemcpyAsync(n->pair_bytes->p, h.images, ip_bytes, cudaMemcpyHostToDevice, s));
+  if (h.image2_2) DEMON_CHECK_CUDA(cudaMemcpyAsync(n->i22_bytes->p, h.image2_2, i22_bytes, cudaMemcpyHostToDevice, s));
+  if (int rc = pipeline_forward_impl(n, c, s)) return rc;
+  DEMON_CHECK_CUDA(cudaMemcpyAsync(h.depth0, c.depth0, px * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if (h.normal0) DEMON_CHECK_CUDA(cudaMemcpyAsync(h.normal0, c.normal0, px * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if (h.rotation) DEMON_CHECK_CUDA(cudaMemcpyAsync(h.rotation, c.rotation, (size_t)n->B * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if (h.translation)
+    DEMON_CHECK_CUDA(cudaMemcpyAsync(h.translation, c.translation, (size_t)n->B * 3 * sizeof(float), cudaMemcpyDeviceToHost, s));
+  if (synchronize) {
     DEMON_CHECK_CUDA(cudaStreamSynchronize(s));
     if (tc_read_error_flag(true))
       return fail(DEMON_E_STATE, "a pipeline wait inside a tensor-core convolution kernel timed out: the outputs are invalid");
@@ -1855,55 +1715,6 @@ static int pipeline_host(demon_net* n, int variant, const void* images_host, con
   return DEMON_OK;
 }
 
-int demon_pipeline_forward_host(demon_net* n, const float* image_pair_host, const float* image2_2_host, int iterations, float* depth0_host,
-                                float* rotation_host, float* translation_host, void* stream) {
-  return pipeline_host(n, 1, image_pair_host, image2_2_host, false, 0, iterations, depth0_host, nullptr, rotation_host, translation_host,
-                       stream, true);
-}
-
-int demon_pipeline_forward_host_async(demon_net* n, const float* image_pair_host, const float* image2_2_host, int iterations,
-                                      float* depth0_host, float* rotation_host, float* translation_host, void* stream) {
-  return pipeline_host(n, 1, image_pair_host, image2_2_host, false, 0, iterations, depth0_host, nullptr, rotation_host, translation_host,
-                       stream, false);
-}
-
-int demon_pipeline_forward_host_u8(demon_net* n, const uint8_t* images_host, const uint8_t* image2_2_host, int iterations, float* depth0_host,
-                                   float* rotation_host, float* translation_host, void* stream) {
-  return pipeline_host(n, 1, images_host, image2_2_host, true, 0, iterations, depth0_host, nullptr, rotation_host, translation_host, stream,
-                       true);
-}
-
-int demon_pipeline_forward_host_u8_async(demon_net* n, const uint8_t* images_host, const uint8_t* image2_2_host, int iterations,
-                                         float* depth0_host, float* rotation_host, float* translation_host, void* stream) {
-  return pipeline_host(n, 1, images_host, image2_2_host, true, 0, iterations, depth0_host, nullptr, rotation_host, translation_host, stream,
-                       false);
-}
-
-int demon_pipeline_forward_host_v2(demon_net* n, const float* image_pair_host, const float* image2_2_host, int image2_2_mode, int iterations,
-                                   float* depth0_host, float* normal0_host, float* rotation_host, float* translation_host, void* stream) {
-  return pipeline_host(n, 2, image_pair_host, image2_2_host, false, image2_2_mode, iterations, depth0_host, normal0_host, rotation_host,
-                       translation_host, stream, true);
-}
-
-int demon_pipeline_forward_host_async_v2(demon_net* n, const float* image_pair_host, const float* image2_2_host, int image2_2_mode,
-                                         int iterations, float* depth0_host, float* normal0_host, float* rotation_host,
-                                         float* translation_host, void* stream) {
-  return pipeline_host(n, 2, image_pair_host, image2_2_host, false, image2_2_mode, iterations, depth0_host, normal0_host, rotation_host,
-                       translation_host, stream, false);
-}
-
-int demon_pipeline_forward_host_u8_v2(demon_net* n, const uint8_t* images_host, const uint8_t* image2_2_host, int image2_2_mode, int iterations,
-                                      float* depth0_host, float* normal0_host, float* rotation_host, float* translation_host, void* stream) {
-  return pipeline_host(n, 2, images_host, image2_2_host, true, image2_2_mode, iterations, depth0_host, normal0_host, rotation_host,
-                       translation_host, stream, true);
-}
-
-int demon_pipeline_forward_host_u8_async_v2(demon_net* n, const uint8_t* images_host, const uint8_t* image2_2_host, int image2_2_mode,
-                                            int iterations, float* depth0_host, float* normal0_host, float* rotation_host,
-                                            float* translation_host, void* stream) {
-  return pipeline_host(n, 2, images_host, image2_2_host, true, image2_2_mode, iterations, depth0_host, normal0_host, rotation_host,
-                       translation_host, stream, false);
-}
 
 // resize_area over NCHW planes (area_planes_kernel): input [N,C,h,w] with `in_sn` floats between samples -> packed
 // [N,C,oh,ow]; h / oh and w / ow must be integers

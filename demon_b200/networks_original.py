@@ -149,11 +149,6 @@ def _ptr(x):
     return x.data_ptr() if isinstance(x, torch.Tensor) else x.ctypes.data
 
 
-# the output pointers of the fused-pipeline entries, in C ABI order
-_OUTPUTS = ("predict_depth0", "predict_rotation", "predict_translation", "predict_flow2", "predict_depth2", "predict_normal2")
-_SNAPSHOT_OUTPUTS = ("predict_flow2", "predict_depth2", "predict_normal2", "predict_rotation", "predict_translation", "predict_depth0")
-
-
 class _NetBase:
     def __init__(self, session, data_format="channels_first", batch_size=1):
         self.session = session if session is not None else default_session()
@@ -245,14 +240,10 @@ class RefinementNet(_NetBase):
 
 class _Pipeline:
     """The fused pipeline's methods, written once for DemonPipeline (networks_original) and DemonPipelineV2 (v2.networks).
-    A subclass names its network handle, the suffix of its C entries, its output keys in C ABI order and the image2_2 modes
-    it takes; v2's entries also take an image2_2_mode and return normal0."""
+    A subclass names its network handle, its outputs (_output_shapes) and the image2_2 modes it takes; every call is one
+    demon_pipeline_run or demon_pipeline_run_host with a PipelineArgs."""
 
     _handle = _NetHandle
-    _suffix = ""                                 # C entry names: demon_pipeline_forward<kind><suffix>
-    _keys = _OUTPUTS                             # outputs of the device entries, in C ABI order
-    _snapshot_keys = _SNAPSHOT_OUTPUTS
-    _host_keys = ("predict_depth0", "predict_rotation", "predict_translation")
     _modes = {"resize": 1, "median": 0}          # image2_2 of forward_images / forward_views -> image2_2_mode
     _area = False                                # image2_2='area' (tf.image.resize_area of image 2, v2 only)
 
@@ -268,10 +259,6 @@ class _Pipeline:
         self._ip = self._i22 = self._out = None
         self._snap = self._snap_refined = None
         self._K = self._status = None   # forward_views: intrinsics staging [B,2,4] float64 and status [B,2] uint8
-
-    def _mode_args(self, mode):
-        """The image2_2_mode argument of the entries at the network's input size: v1's take none (mode 0 only)."""
-        return ()
 
     def _image2_2_source(self, image2_2):
         """image2_2 of the uint8 and host entries -> (the tensor or None, image2_2_mode)."""
@@ -325,15 +312,19 @@ class _Pipeline:
     def own_outputs(self):
         return self._own("_out", self._output_shapes())
 
-    def _run(self, entry, args, outputs=None, keys=None, iterations=None):
-        """Calls the C entry `entry` (+ the class's suffix) on the net with `args`, the iteration count, the pointers of
-        `outputs` (default: the pipeline's own) in the order of `keys` (default: the class's; null for a missing one) and the
-        current stream; raises on an error code."""
+    def _args(self, outputs, iterations=None, **fields):
+        """The PipelineArgs of one call: `fields`, the iteration count (default: the pipeline's) and the pointer of every
+        output of the network by name (predict_depth0 -> depth0; NULL for one `outputs` lacks)."""
+        args = _lib.PipelineArgs(iterations=self.iterations if iterations is None else int(iterations), **fields)
+        for key in self._output_shapes():
+            setattr(args, key[len("predict_"):], _ptr(outputs.get(key)))
+        return args
+
+    def _run(self, outputs=None, iterations=None, **fields):
+        """demon_pipeline_run on the current stream with `outputs` (default: the pipeline's own); raises on an error code."""
         if outputs is None:
             outputs = self.own_outputs()
-        fn = getattr(_lib.load(), entry + self._suffix)
-        it = self.iterations if iterations is None else int(iterations)
-        _lib.check(fn(self.net.ptr, *args, it, *(_ptr(outputs.get(k)) for k in (keys or self._keys)), _stream()))
+        _lib.check(_lib.load().demon_pipeline_run(self.net.ptr, self._args(outputs, iterations, **fields), _stream()))
         return outputs
 
     def forward(self, image_pair, image2_2=None, outputs=None, stage_inputs=True):
@@ -353,7 +344,7 @@ class _Pipeline:
             i2 = self._stage_image2_2(ip, image2_2) if isinstance(image2_2, str) else image2_2
             if i2 is not None and i2 is not self._i22:
                 i2, _ = _to_dev(i2, (self.batch_size, 3, 48, 64), "image2_2")
-        return self._run("demon_pipeline_forward", (ip.data_ptr(), _ptr(i2)), outputs, iterations=iterations)
+        return self._run(outputs, iterations, input=_lib.INPUT_F32, images=ip.data_ptr(), image2_2=_ptr(i2))
 
     def forward_staged(self, outputs=None, ip=None, i2=None, use_image2_2=False):
         """The pipeline on inputs that are already in place: by default the pipeline's own staging buffers (filled by
@@ -363,7 +354,7 @@ class _Pipeline:
             if self._ip is None:
                 raise RuntimeError("forward_staged() before stage()")
             ip, i2 = self._ip, (self._i22 if use_image2_2 else None)
-        return self._run("demon_pipeline_forward", (ip.data_ptr(), _ptr(i2)), outputs)
+        return self._run(outputs, input=_lib.INPUT_F32, images=ip.data_ptr(), image2_2=_ptr(i2))
 
     def own_snapshot_outputs(self, refine=True):
         """The persistent output buffers of forward_snapshots (S = iterations + 1 snapshots); one set per `refine`."""
@@ -384,8 +375,8 @@ class _Pipeline:
         if outputs is None:
             outputs = self.own_snapshot_outputs(refine)
         # without `refine` no depth0 pointer, which is what skips the refinement
-        self._run("demon_pipeline_forward_snapshots", (ip.data_ptr(), _ptr(i2)) + self._mode_args(0),
-                  outputs if refine else dict(outputs, predict_depth0=None, predict_normal0=None), self._snapshot_keys)
+        self._run(outputs if refine else dict(outputs, predict_depth0=None, predict_normal0=None), input=_lib.INPUT_F32,
+                  images=ip.data_ptr(), image2_2=_ptr(i2), snapshots=1)
         return outputs
 
     def snapshot_launches(self):
@@ -405,7 +396,7 @@ class _Pipeline:
         images = images.contiguous()
         if image2_2 is not None:
             image2_2 = image2_2.contiguous()
-        return self._run("demon_pipeline_forward_u8", (images.data_ptr(), _ptr(image2_2)) + self._mode_args(mode), outputs)
+        return self._run(outputs, input=_lib.INPUT_U8, images=images.data_ptr(), image2_2=_ptr(image2_2), image2_2_mode=mode)
 
     def _check_pairs(self, images, resample, image2_2):
         """The checks of forward_images / forward_views; returns h, w, the resample code and the image2_2 mode."""
@@ -426,7 +417,9 @@ class _Pipeline:
         'median' (median3x3_downsample twice, examples/evaluation.py:170-173).  Same outputs as forward_u8 on the resized
         bytes, bit for bit."""
         h, w, code, mode = self._check_pairs(images, resample, image2_2)
-        return self._run("demon_pipeline_forward_images_u8", (images.data_ptr(), *images.stride()[:3], h, w, code, mode), outputs)
+        sn, si, sy = images.stride()[:3]
+        return self._run(outputs, input=_lib.INPUT_RESIZE_U8, images=images.data_ptr(), sn=sn, si=si, sy=sy, h=h, w=w, resample=code,
+                         image2_2_mode=mode)
 
     def forward_views(self, images, intrinsics, resample="bicubic", image2_2="resize", outputs=None):
         """The pipeline on photos from any calibrated camera: images CUDA uint8 [B,2,h,w,3] as in forward_images, intrinsics
@@ -446,29 +439,29 @@ class _Pipeline:
             self._K = torch.empty((b, 2, 4), dtype=torch.float64, device=images.device)
             self._status = torch.empty((b, 2), dtype=torch.uint8, device=images.device)
         self._K.copy_(k, non_blocking=True)
-        out = self._run("demon_pipeline_forward_views_u8",
-                        (images.data_ptr(), *images.stride()[:3], h, w, self._K.data_ptr(), self._status.data_ptr(), code, mode), outputs)
+        sn, si, sy = images.stride()[:3]
+        out = self._run(outputs, input=_lib.INPUT_VIEWS_U8, images=images.data_ptr(), sn=sn, si=si, sy=sy, h=h, w=w,
+                        K=self._K.data_ptr(), status=self._status.data_ptr(), resample=code, image2_2_mode=mode)
         return dict(out, status=self._status)
 
-    def _host(self, entry, inputs, image2_2, outputs, stream):
-        """A host entry: `inputs` and `image2_2` host buffers (image2_2 may also be None or a mode name), `outputs` the host
-        buffers by key (the class's _host_keys; depth0 is required)."""
+    def _host(self, kind, sync, inputs, image2_2, outputs, stream):
+        """demon_pipeline_run_host: `inputs` and `image2_2` host buffers of input kind `kind` (image2_2 may also be None or a
+        mode name), `outputs` the host buffers by key (depth0 is required), synchronised iff `sync`."""
         image2_2, mode = self._image2_2_source(image2_2)
         s = ctypes.c_void_p((stream or torch.cuda.current_stream()).cuda_stream)
-        fn = getattr(_lib.load(), entry + self._suffix)
-        _lib.check(fn(self.net.ptr, _ptr(inputs), _ptr(image2_2), *self._mode_args(mode), self.iterations,
-                      *(_ptr(outputs.get(k)) for k in self._host_keys), s))
+        args = self._args(outputs, input=kind, images=_ptr(inputs), image2_2=_ptr(image2_2), image2_2_mode=mode)
+        _lib.check(_lib.load().demon_pipeline_run_host(self.net.ptr, args, int(sync), s))
 
     def forward_host_u8(self, images, image2_2, depth0, rotation, translation, stream=None, sync=True):
         """End to end from HOST uint8 images [B,2,192,256,3] (numpy or pinned torch CPU uint8): H2D of the bytes, the
         pipeline, D2H of depth0 / rotation / translation.  sync=False: asynchronous on `stream` like forward_host_async."""
-        self._host("demon_pipeline_forward_host_u8" if sync else "demon_pipeline_forward_host_u8_async", images, image2_2,
+        self._host(_lib.INPUT_U8, sync, images, image2_2,
                    {"predict_depth0": depth0, "predict_rotation": rotation, "predict_translation": translation}, stream)
 
     def forward_host(self, image_pair, image2_2, depth0, rotation, translation):
         """End-to-end call on HOST buffers (pinned torch CPU tensors or numpy arrays): H2D, pipeline, D2H and a
         stream synchronise inside the C call."""
-        self._host("demon_pipeline_forward_host", image_pair, image2_2,
+        self._host(_lib.INPUT_F32, True, image_pair, image2_2,
                    {"predict_depth0": depth0, "predict_rotation": rotation, "predict_translation": translation}, None)
         # (the C call synchronises and returns DEMON_E_STATE itself if a tensor-core pipeline wait timed out)
 
@@ -476,7 +469,7 @@ class _Pipeline:
         """forward_host without the final synchronisation, on `stream` (a torch.cuda.Stream; default: current).  The host
         buffers must be pinned and are valid after `stream.synchronize()`.  Two DemonPipeline objects on two Sessions'
         nets and two streams overlap one batch's copies with the other's compute."""
-        self._host("demon_pipeline_forward_host_async", image_pair, image2_2,
+        self._host(_lib.INPUT_F32, False, image_pair, image2_2,
                    {"predict_depth0": depth0, "predict_rotation": rotation, "predict_translation": translation}, stream)
 
     def launches(self):

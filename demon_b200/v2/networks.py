@@ -132,10 +132,8 @@ class RefinementNet(_NetBase):
         return self._finish(out, t1 and t2)
 
 
-# output pointers of the stage-wise entries and of demon_pipeline_forward_v2, in C ABI order
+# output pointers of the stage-wise entries, in C ABI order
 _STAGE_OUTPUTS = ("predict_flow5", "predict_flow2", "predict_depth2", "predict_normal2", "predict_rotation", "predict_translation")
-_OUTPUTS = ("predict_depth0", "predict_normal0", "predict_rotation", "predict_translation", "predict_flow2", "predict_depth2",
-            "predict_normal2")
 
 
 class DemonPipelineV2(_v1._Pipeline):
@@ -150,17 +148,11 @@ class DemonPipelineV2(_v1._Pipeline):
     images, views and host entries compute it inside the pipeline from image 2's float planes (x/255 - 0.5 for uint8)."""
 
     _handle = _NetHandleV2
-    _suffix = "_v2"
-    _keys = _snapshot_keys = _OUTPUTS
-    _host_keys = ("predict_depth0", "predict_normal0", "predict_rotation", "predict_translation")
     _modes = {"resize": 1, "median": 0, "area": 2}
     _area = True
 
     def __init__(self, session=None, batch_size=1, iterations=3, private_net=False):
         super().__init__(session if session is not None else default_session(), batch_size, iterations, private_net)
-
-    def _mode_args(self, mode):
-        return (mode,)
 
     def _output_shapes(self):
         return dict(super()._output_shapes(), predict_normal0=(self.batch_size, 3, 192, 256))
@@ -178,19 +170,19 @@ class DemonPipelineV2(_v1._Pipeline):
 
     def forward_host_u8(self, images, image2_2, depth0, rotation, translation, stream=None, sync=True, normal0=None):
         """DemonPipeline.forward_host_u8 with v2's optional normal0 [B,3,192,256] host buffer; image2_2 may be 'area'."""
-        self._host("demon_pipeline_forward_host_u8" if sync else "demon_pipeline_forward_host_u8_async", images, image2_2,
+        self._host(_lib.INPUT_U8, sync, images, image2_2,
                    {"predict_depth0": depth0, "predict_normal0": normal0, "predict_rotation": rotation, "predict_translation": translation},
                    stream)
 
     def forward_host(self, image_pair, image2_2, depth0, rotation, translation, normal0=None):
         """DemonPipeline.forward_host with v2's optional normal0 [B,3,192,256] host buffer; image2_2 may be 'area'."""
-        self._host("demon_pipeline_forward_host", image_pair, image2_2,
+        self._host(_lib.INPUT_F32, True, image_pair, image2_2,
                    {"predict_depth0": depth0, "predict_normal0": normal0, "predict_rotation": rotation, "predict_translation": translation},
                    None)
 
     def forward_host_async(self, image_pair, image2_2, depth0, rotation, translation, stream=None, normal0=None):
         """DemonPipeline.forward_host_async with v2's optional normal0 [B,3,192,256] host buffer; image2_2 may be 'area'."""
-        self._host("demon_pipeline_forward_host_async", image_pair, image2_2,
+        self._host(_lib.INPUT_F32, False, image_pair, image2_2,
                    {"predict_depth0": depth0, "predict_normal0": normal0, "predict_rotation": rotation, "predict_translation": translation},
                    stream)
 

@@ -555,20 +555,13 @@ int demon_iterative_forward(demon_net* net, const float* image_pair, const float
 int demon_refine_forward(demon_net* net, const float* image1, const float* depth2, float* depth0,
                          int data_format, void* stream);
 
-/* The whole of examples/example.py:87-99 without leaving the device: bootstrap, `iterations` x
- * iterative, refinement.  image2_2 may be NULL: it is then computed as
- * median3x3_downsample(median3x3_downsample(image_pair[:,3:6])) (examples/evaluation.py:170-173).
- * Any output pointer may be NULL.  channels_first only. */
-int demon_pipeline_forward(demon_net* net, const float* image_pair, const float* image2_2, int iterations,
-                           float* depth0, float* rotation, float* translation,
-                           float* flow2, float* depth2, float* normal2, void* stream);
-
 /* ------------------------------------------------------------------------
  * The v2 network (python/depthmotionnet/v2/networks.py, the one training/v2/training.py trains): a second plan over the
  * same kernels, with TF 'same' padding, the dense5 layer of every trunk, the motion branch of v2 and a refinement block
- * that also predicts normal0.  demon_net_set_weight / _num_variables / _variable_name / _finalize / _destroy, the profile
- * and the debug entries take either kind of handle; every forward entry takes one kind only and returns DEMON_E_INVALID
- * for the other (the entries above are v1's, the *_v2 entries below v2's).  float32 device entries only.
+ * that also predicts normal0.  demon_net_set_weight / _num_variables / _variable_name / _finalize / _destroy, the fused
+ * pipeline, the profile and the debug entries take either kind of handle; every stage-wise or block entry takes one kind
+ * only and returns DEMON_E_INVALID for the other (the entries above are v1's, the *_v2 entries below v2's).  float32
+ * device entries only.
  * ---------------------------------------------------------------------- */
 int demon_net_create_v2(demon_net** net, int batch, int refine_h, int refine_w, int precision);
 /* 1 for a handle of demon_net_create, 2 for one of demon_net_create_v2, 0 for NULL */
@@ -605,109 +598,79 @@ int demon_depthmotion_block_forward_v2(demon_net* net, const char* scope, const 
                                        const float* prev_flow2, const float* prev_flowconf2, const float* prev_rotation,
                                        const float* prev_translation, const float* intrinsics, float* depth2, float* normal2,
                                        float* rotation, float* translation, float* scale, int data_format, void* stream);
-/* bootstrap, `iterations` x iterative and refinement of v2 in one call, as demon_pipeline_forward (one CUDA graph per
- * distinct call, image2_2 may be NULL, any output may be NULL); normal0 [B,3,192,256].  channels_first only. */
-int demon_pipeline_forward_v2(demon_net* net, const float* image_pair, const float* image2_2, int iterations,
-                              float* depth0, float* normal0, float* rotation, float* translation,
-                              float* flow2, float* depth2, float* normal2, void* stream);
 
-/* The pipeline as examples/evaluation.py:225-255 runs it for an accuracy table: every intermediate prediction is kept.
- * Snapshot k = 0 is the bootstrap block's output, snapshot k = 1..iterations the output after iteration k; the arrays hold
- * S = iterations + 1 snapshots of the batch: flow2 [S,B,2,48,64], depth2 [S,B,1,48,64], normal2 [S,B,3,48,64],
- * rotation / translation [S,B,3].  depth0 [S,B,1,192,256], if not NULL, is the refinement block run on every snapshot's
- * depth2 (evaluation.py:249).  Inputs, image2_2 = NULL and the CUDA graph cache as demon_pipeline_forward; snapshot k
- * equals the stage-wise entries after k iterations bit for bit.  Any output pointer may be NULL. */
-int demon_pipeline_forward_snapshots(demon_net* net, const float* image_pair, const float* image2_2, int iterations,
-                                     float* flow2, float* depth2, float* normal2, float* rotation, float* translation,
-                                     float* depth0, void* stream);
+/* ------------------------------------------------------------------------
+ * The fused pipeline: bootstrap, `iterations` x iterative and refinement in one call that never leaves the device, the
+ * whole of examples/example.py:87-99 (v2: examples/example_v2.py), on a handle of either kind; the handle says which
+ * network runs.  One call is described by one demon_pipeline_args.
+ * ---------------------------------------------------------------------- */
+/* input kinds */
+enum { DEMON_INPUT_F32 = 0, DEMON_INPUT_U8 = 1, DEMON_INPUT_RESIZE_U8 = 2, DEMON_INPUT_VIEWS_U8 = 3 };
 
-/* Same, HOST buffers in and out (pinned or pageable): H2D copies, the pipeline, D2H copies and a
- * stream synchronisation, all inside the call.  This is the end-to-end path bench.py times. */
-int demon_pipeline_forward_host(demon_net* net, const float* image_pair_host, const float* image2_2_host,
-                                int iterations, float* depth0_host, float* rotation_host,
-                                float* translation_host, void* stream);
-/* Same without the final synchronisation: the host outputs are valid once `stream` has been synchronised.  With PINNED
- * host buffers and two nets on two streams a caller overlaps the copies of one batch with the compute of the other. */
-int demon_pipeline_forward_host_async(demon_net* net, const float* image_pair_host, const float* image2_2_host,
-                                      int iterations, float* depth0_host, float* rotation_host,
-                                      float* translation_host, void* stream);
-
-/* The same pipeline on uint8 images, the form examples/example.py:15-42 starts from (PIL RGB, HWC): images [B,2,192,256,3]
- * (image 1 then image 2 of every pair), image2_2 [B,48,64,3] (the resized second image) or NULL (then it is computed with
- * median3x3_downsample twice, examples/evaluation.py:170-173).  `x/255 - 0.5` and the pair concat happen on the device in
- * the kernel that feeds conv1y, with numpy's two float32 operations, so the outputs equal the fp32 entry's bit for bit;
- * the host variants move 4x fewer input bytes. */
-int demon_pipeline_forward_u8(demon_net* net, const uint8_t* images, const uint8_t* image2_2, int iterations, float* depth0,
-                              float* rotation, float* translation, float* flow2, float* depth2, float* normal2, void* stream);
-int demon_pipeline_forward_host_u8(demon_net* net, const uint8_t* images_host, const uint8_t* image2_2_host, int iterations,
-                                   float* depth0_host, float* rotation_host, float* translation_host, void* stream);
-int demon_pipeline_forward_host_u8_async(demon_net* net, const uint8_t* images_host, const uint8_t* image2_2_host, int iterations,
-                                         float* depth0_host, float* rotation_host, float* translation_host, void* stream);
-
-/* The same pipeline on image pairs of any size, resized on the device first, the whole of examples/example.py:15-42:
- * images [B,2,h,w,3] uint8 RGB with `sn`, `si`, `sy` bytes between samples, between the two images of a pair and between
- * rows (pixel stride 3, channel stride 1, so a cropped view is read in place), 1 <= h, w <= 8192.  Both images are resized
- * to 256x192 with `resample` exactly like PIL.Image.resize (demon_resize_u8), then image2_2 is
- *   image2_2_mode 0: median3x3_downsample twice of the resized second image (examples/evaluation.py:170-173), or
- *   image2_2_mode 1: the resized second image resized to 64x48 with the same filter (examples/example.py:22).
- * The outputs equal demon_pipeline_forward_u8 on the resized bytes, bit for bit. */
-int demon_pipeline_forward_images_u8(demon_net* net, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w,
-                                     int resample, int image2_2_mode, int iterations, float* depth0, float* rotation,
-                                     float* translation, float* flow2, float* depth2, float* normal2, void* stream);
-
-/* The same pipeline on photos from any calibrated camera: images as in demon_pipeline_forward_images_u8 with their
- * intrinsics K [B,2,4] (fx, fy, cx, cy in pixels, DEVICE doubles).  Every image is adapted to the network's intrinsics,
- * K_new = (0.89115971 * 256, 1.18821287 * 192, 0.5 * 256, 0.5 * 192) at 256x192, exactly like demon_adjust_intrinsics_u8
- * (status [B,2] as there); image2_2 is made from the adapted second image as image2_2_mode says.  The outputs equal
- * demon_pipeline_forward_u8 on the adapted bytes, bit for bit.  K and status are part of the CUDA-graph key: a replay
- * reads the K buffer's current values. */
-int demon_pipeline_forward_views_u8(demon_net* net, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w,
-                                    const double* K, uint8_t* status, int resample, int image2_2_mode, int iterations, float* depth0,
-                                    float* rotation, float* translation, float* flow2, float* depth2, float* normal2, void* stream);
-
-/* The entries above for a v2 handle (demon_net_create_v2).  Arguments as their v1 twins, with two differences: the outputs
- * come in demon_pipeline_forward_v2's order with normal0 [B,3,192,256] (snapshots: [S,B,3,192,256]) after depth0, and every
- * entry takes an image2_2_mode:
- *   0: the given image2_2, or without one median3x3_downsample twice of image 2 (examples/evaluation.py:170-173);
- *   1: image 2 resized to 64x48 with the call's filter (examples/example_v2.py) -- images_u8 / views_u8 only;
+/* One fused-pipeline call.  Every field is 64 bits wide, so the struct has no padding and equal calls are equal bytes: the
+ * library keeps one CUDA graph per distinct call (the first call runs eagerly, the second captures, later ones replay),
+ * keyed by these bytes.  A field the input kind does not read must be 0 / NULL, otherwise the call is refused.
+ *
+ * input, images, image2_2:
+ *   DEMON_INPUT_F32: images float [B,6,192,256], the image pair; image2_2 float [B,3,48,64] or NULL.
+ *   DEMON_INPUT_U8: images uint8 [B,2,192,256,3], image 1 then image 2 of every pair as PIL gives them (HWC RGB,
+ *     examples/example.py:15-42); image2_2 uint8 [B,48,64,3] (the resized second image) or NULL.  `x/255 - 0.5` and the
+ *     pair concat happen on the device in the kernel that feeds conv1y, with numpy's two float32 operations, so the outputs
+ *     equal the F32 call's bit for bit; the host entry moves 4x fewer input bytes.
+ *   DEMON_INPUT_RESIZE_U8: images uint8 [B,2,h,w,3] of any size with `sn`, `si`, `sy` bytes between samples, between the two
+ *     images of a pair and between rows (pixel stride 3, channel stride 1, so a cropped view is read in place),
+ *     1 <= h, w <= 8192.  Both images are resized to 256x192 with `resample` exactly like PIL.Image.resize
+ *     (demon_resize_u8).  image2_2 NULL.  The outputs equal the U8 call on the resized bytes, bit for bit.
+ *   DEMON_INPUT_VIEWS_U8: photos from any calibrated camera: images as for RESIZE_U8 with their intrinsics K [B,2,4] (fx,
+ *     fy, cx, cy in pixels, DEVICE doubles).  Every image is adapted to the network's intrinsics, K_new = (0.89115971 * 256,
+ *     1.18821287 * 192, 0.5 * 256, 0.5 * 192) at 256x192, exactly like demon_adjust_intrinsics_u8, with its status [B,2].
+ *     image2_2 NULL.  The outputs equal the U8 call on the adapted bytes, bit for bit.  K and status are part of the
+ *     CUDA-graph key: a replay reads the K buffer's current values.
+ * image2_2_mode, how image2_2 is made when it is not given:
+ *   0: median3x3_downsample twice of image 2 (examples/evaluation.py:170-173);
+ *   1: image 2 resized to 64x48 with the call's filter (examples/example.py:22) -- RESIZE_U8 / VIEWS_U8 only;
  *   2: tf.image.resize_area of image 2's float planes to 48x64, the input training/v2/training.py:179 trains v2 on
- *      (demon_resize_area_f32 on x/255 - 0.5 for uint8 input); image2_2 must then be NULL.
- * The v1 entries refuse mode 2.  Any device output may be NULL.  demon_pipeline_forward_snapshots_v2 runs the refinement block
- * on every snapshot iff depth0 is given, and refuses normal0 without depth0.  The host entries need depth0_host; normal0_host,
- * rotation_host and translation_host may be NULL. */
-int demon_pipeline_forward_snapshots_v2(demon_net* net, const float* image_pair, const float* image2_2, int image2_2_mode, int iterations,
-                                        float* depth0, float* normal0, float* rotation, float* translation, float* flow2, float* depth2,
-                                        float* normal2, void* stream);
-int demon_pipeline_forward_u8_v2(demon_net* net, const uint8_t* images, const uint8_t* image2_2, int image2_2_mode, int iterations,
-                                 float* depth0, float* normal0, float* rotation, float* translation, float* flow2, float* depth2,
-                                 float* normal2, void* stream);
-int demon_pipeline_forward_images_u8_v2(demon_net* net, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w,
-                                        int resample, int image2_2_mode, int iterations, float* depth0, float* normal0, float* rotation,
-                                        float* translation, float* flow2, float* depth2, float* normal2, void* stream);
-int demon_pipeline_forward_views_u8_v2(demon_net* net, const uint8_t* images, int64_t sn, int64_t si, int64_t sy, int h, int w,
-                                       const double* K, uint8_t* status, int resample, int image2_2_mode, int iterations, float* depth0,
-                                       float* normal0, float* rotation, float* translation, float* flow2, float* depth2, float* normal2,
-                                       void* stream);
-int demon_pipeline_forward_host_v2(demon_net* net, const float* image_pair_host, const float* image2_2_host, int image2_2_mode,
-                                   int iterations, float* depth0_host, float* normal0_host, float* rotation_host, float* translation_host,
-                                   void* stream);
-int demon_pipeline_forward_host_async_v2(demon_net* net, const float* image_pair_host, const float* image2_2_host, int image2_2_mode,
-                                         int iterations, float* depth0_host, float* normal0_host, float* rotation_host,
-                                         float* translation_host, void* stream);
-int demon_pipeline_forward_host_u8_v2(demon_net* net, const uint8_t* images_host, const uint8_t* image2_2_host, int image2_2_mode,
-                                      int iterations, float* depth0_host, float* normal0_host, float* rotation_host, float* translation_host,
-                                      void* stream);
-int demon_pipeline_forward_host_u8_async_v2(demon_net* net, const uint8_t* images_host, const uint8_t* image2_2_host, int image2_2_mode,
-                                            int iterations, float* depth0_host, float* normal0_host, float* rotation_host,
-                                            float* translation_host, void* stream);
+ *      (demon_resize_area_f32 on x/255 - 0.5 for uint8 input) -- v2 handles only; image2_2 must be NULL.
+ * iterations: 0..7.
+ * Outputs, float32 channels_first, each may be NULL: depth0 [B,1,192,256], normal0 [B,3,192,256] (v2 handles only),
+ *   rotation / translation [B,3], flow2 [B,2,48,64], depth2 [B,1,48,64], normal2 [B,3,48,64].
+ * snapshots 0: the outputs after the last iteration and the refinement block.  snapshots 1: every intermediate prediction,
+ *   as examples/evaluation.py:225-255 keeps them for an accuracy table.  Snapshot k = 0 is the bootstrap block's output,
+ *   snapshot k = 1..iterations the output after iteration k; every output holds S = iterations + 1 snapshots [S,B,...].  The
+ *   refinement block runs on every snapshot's depth2 iff depth0 is given (evaluation.py:249), and normal0 needs depth0.
+ *   Snapshot k equals the stage-wise entries after k iterations bit for bit. */
+typedef struct demon_pipeline_args {
+  int64_t input;                       /* DEMON_INPUT_* */
+  const void* images;
+  const void* image2_2;
+  int64_t image2_2_mode;
+  int64_t sn, si, sy, h, w, resample;  /* RESIZE_U8 / VIEWS_U8 */
+  const double* K;                     /* VIEWS_U8 */
+  uint8_t* status;                     /* VIEWS_U8 */
+  int64_t iterations;
+  int64_t snapshots;
+  float *depth0, *normal0, *rotation, *translation, *flow2, *depth2, *normal2;
+} demon_pipeline_args;
+
+/* The call on DEVICE pointers, asynchronous on `stream`.  Calls on one handle must not overlap.
+ * DEMON_E_INVALID for an argument the struct's rules above refuse, a null images, or a net whose refinement block is not
+ * 192x256; DEMON_E_STATE for a net that is not finalized, belongs to another device or has a layer trace set.  A refused
+ * call launches nothing. */
+int demon_pipeline_run(demon_net* net, const demon_pipeline_args* args, void* stream);
+/* The same on HOST buffers in and out (pinned or pageable): F32 or U8 input, snapshots 0, depth0 required, flow2, depth2
+ * and normal2 NULL.  H2D copies into the net's staging buffers, the pipeline, D2H copies of depth0, normal0, rotation and
+ * translation, all inside the call.  With `synchronize` the call also synchronises the stream and returns DEMON_E_STATE if
+ * a tensor-core pipeline wait timed out (demon_check_errors); this is the end-to-end path bench.py times.  Without it the
+ * host outputs are valid once `stream` has been synchronised: with PINNED host buffers and two nets on two streams a caller
+ * overlaps the copies of one batch with the compute of the other. */
+int demon_pipeline_run_host(demon_net* net, const demon_pipeline_args* args, int synchronize, void* stream);
 
 /* introspection for tests and bench */
 int demon_net_batch(const demon_net* net);
 int64_t demon_net_workspace_bytes(const demon_net* net);
-/* number of kernel launches of one demon_pipeline_forward with `iterations` */
+/* number of kernel launches of the last fused-pipeline call without snapshots with `iterations` */
 int demon_net_pipeline_launches(const demon_net* net, int iterations);
-/* the same for the last demon_pipeline_forward_snapshots with `iterations` (counted apart: snapshot calls leave the value
- * above untouched) */
+/* the same for the last call with snapshots (counted apart: snapshot calls leave the value above untouched) */
 int demon_net_snapshot_launches(const demon_net* net, int iterations);
 /* 1 if layer `tf_name` (e.g. "netRefine/conv1_1") runs on the tensor-core path */
 int demon_net_layer_uses_tensor_cores(const demon_net* net, const char* tf_name);
@@ -755,8 +718,9 @@ int demon_debug_describe_plan(int variant, int batch, int refine_h, int refine_w
  * runs) to in[i] and its output slice (cout channels, just after) to out[i], as dense float32 [B,H,W,C] (dense layers:
  * [B,cin_buf] in the buffer's NHWC order and [B,cout]), on the launching stream; a null pointer skips that copy.  The last
  * refinement layer's output is read from the caller's depth0.  `in` and `out` are arrays of demon_net_num_layers(net)
- * device pointers in layer order (demon_net_layer_name); in == out == NULL clears the trace.  While a trace is set, every
- * demon_pipeline_forward* entry returns DEMON_E_STATE, so that no CUDA graph is captured with the copies inside it.
+ * device pointers in layer order (demon_net_layer_name); in == out == NULL clears the trace.  While a trace is set,
+ * demon_pipeline_run and demon_pipeline_run_host return DEMON_E_STATE, so that no CUDA graph is captured with the copies
+ * inside it.
  * Without a trace the forward passes are unchanged. */
 int demon_debug_trace_layers(demon_net* net, float* const* in, float* const* out);
 

@@ -1,6 +1,7 @@
 """CPU: the C-ABI library loads and exports every symbol include/demon_b200.h declares; the Python
 mirrors validate shapes like the reference's shape functions without needing a GPU; the product never
 falls back to a CPU implementation."""
+import ctypes
 import os
 import re
 
@@ -27,6 +28,21 @@ def test_header_symbols_are_exported_and_bound(lib):
         assert hasattr(lib, name), "library does not export %s" % name
     assert declared == set(_lib.PROTOTYPES), declared ^ set(_lib.PROTOTYPES)
     assert lib.demon_version().decode().endswith("sm_90a")
+
+
+def test_pipeline_args_layout_matches_the_header():
+    """_lib.PipelineArgs has demon_pipeline_args' fields in the header's order, each 8 bytes wide (the C side asserts the
+    struct's size), so the binding and the library read the same bytes."""
+    header = open(os.path.join(ROOT, "include", "demon_b200.h")).read()
+    body = re.search(r"typedef struct demon_pipeline_args \{(.*?)\} demon_pipeline_args;", header, re.S).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    names = []
+    for decl in body.split(";")[:-1]:
+        first, *rest = decl.split(",")
+        names += [re.search(r"(\w+)\s*$", d).group(1) for d in [first] + rest]
+    assert names == [f for f, _ in _lib.PipelineArgs._fields_]
+    assert all(ctypes.sizeof(t) == 8 for _, t in _lib.PipelineArgs._fields_)
+    assert ctypes.sizeof(_lib.PipelineArgs) == 8 * len(names)
 
 
 def test_library_is_sm90a_only():

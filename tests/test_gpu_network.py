@@ -239,7 +239,7 @@ def test_uint8_entry_equals_fp32_entry_bit_for_bit(sessions, synthetic_weights):
 
 
 def test_cuda_graph_replay_equals_eager(sessions, random_pairs):
-    """demon_pipeline_forward replays a CUDA graph from the third call with the same pointer arguments on; the result
+    """demon_pipeline_run replays a CUDA graph from the third call with the same pointer arguments on; the result
     must equal the eager first call bit for bit, also after the input buffer's CONTENT changes."""
     from demon_b200.networks_original import DemonPipeline
     ip, i22 = random_pairs

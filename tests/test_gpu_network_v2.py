@@ -124,7 +124,7 @@ def test_clip_of_depth_from_flow_with_adversarial_weights(weights):
 
 
 def test_pipeline_equals_stagewise_chain_and_graph_replay(sessions, pairs):
-    """demon_pipeline_forward_v2 == bootstrap, three iterations and refinement through the stage-wise entries, bit for
+    """demon_pipeline_run on a v2 handle == bootstrap, three iterations and refinement through the stage-wise entries, bit for
     bit; image2_2=None is the median pair; the replayed CUDA graph equals the eager first call, also on new content."""
     from demon_b200.v2.networks import BootstrapNet, DemonPipelineV2, IterativeNet, RefinementNet
     ip, i22 = pairs
@@ -200,9 +200,10 @@ def test_refinement_sizes(sessions, weights, hw):
     assert np.abs(o["predict_normal0"] - r["predict_normal0"].numpy()).mean() < TOL
 
 
-def test_entries_refuse_the_other_kind_of_handle(sessions, weights, pairs):
-    """v1 forward entries refuse a v2 handle and v2 entries a v1 handle (DEMON_E_INVALID); the variable table, describe,
-    trace and profile entries take both."""
+def test_stage_entries_refuse_the_other_kind_and_the_pipeline_takes_both(sessions, weights, pairs):
+    """v1 forward entries refuse a v2 handle and v2 entries a v1 handle (DEMON_E_INVALID); the fused pipeline takes both and
+    refuses what only v2 has on a v1 handle (normal0, image2_2_mode 2); the variable table, describe, trace and profile
+    entries take both."""
     from demon_b200.networks_original import Session as SessionV1
     from demon_b200 import weights as W1
     lib = _lib.load()
@@ -217,10 +218,13 @@ def test_entries_refuse_the_other_kind_of_handle(sessions, weights, pairs):
     o = [torch.zeros(1, 8, 192, 256, device="cuda") for _ in range(7)]
     s = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     assert lib.demon_bootstrap_forward(v2.ptr, x.data_ptr(), i2.data_ptr(), *(t.data_ptr() for t in o[:6]), 0, s) == -1
-    assert lib.demon_pipeline_forward(v2.ptr, x.data_ptr(), None, 1, *(t.data_ptr() for t in o[:6]), s) == -1
     assert lib.demon_refine_forward(v2.ptr, x.data_ptr(), i2.data_ptr(), o[0].data_ptr(), 0, s) == -1
     assert lib.demon_bootstrap_forward_v2(v1.ptr, x.data_ptr(), i2.data_ptr(), *(t.data_ptr() for t in o[:6]), 0, s) == -1
-    assert lib.demon_pipeline_forward_v2(v1.ptr, x.data_ptr(), None, 1, *(t.data_ptr() for t in o), s) == -1
+    outs = dict(zip(("depth0", "normal0", "rotation", "translation", "flow2", "depth2", "normal2"), (t.data_ptr() for t in o)))
+    assert lib.demon_pipeline_run(v1.ptr, _lib.PipelineArgs(input=_lib.INPUT_F32, images=x.data_ptr(), iterations=1, **outs), s) == -1
+    del outs["normal0"]
+    assert lib.demon_pipeline_run(v1.ptr, _lib.PipelineArgs(input=_lib.INPUT_F32, images=x.data_ptr(), image2_2_mode=2, iterations=1,
+                                                            **outs), s) == -1
     assert lib.demon_refine_forward_v2(v1.ptr, x.data_ptr(), i2.data_ptr(), None, o[0].data_ptr(), None, 0, s) == -1
     buf = ctypes.create_string_buffer(1 << 20)
     assert lib.demon_debug_describe_layers(v2.ptr, buf, len(buf)) > 0

@@ -1,6 +1,6 @@
 """GPU: the v2 pipeline's input paths (DemonPipelineV2: uint8, resized photos, calibrated views, host buffers, snapshots),
 image2_2='area' (tf.image.resize_area, images.resize_area) against the numpy oracle, the handle-kind and mode refusals of
-the _v2 C entries, and Evaluator on a v2 Session.  Synthetic v2 weights at 3xTF32; every comparison is bit for bit except
+the pipeline's C entries, and Evaluator on a v2 Session.  Synthetic v2 weights at 3xTF32; every comparison is bit for bit except
 the evaluation table's non-depth columns (1e-12, as for v1)."""
 import ctypes
 
@@ -198,7 +198,7 @@ def median_i22(ip):
     return sops.median3x3_downsample(sops.median3x3_downsample(ip[:, 3:6].contiguous()))
 
 
-def test_snapshots_equal_stagewise_and_forward(session):
+def test_pipeline_snapshots_equal_stagewise_forward_and_area_mode(session):
     pipe = pipeline(session)
     ip = random_pair(11)
     plain = cloned(pipe.forward(ip, None))
@@ -235,9 +235,9 @@ def test_snapshots_equal_stagewise_and_forward(session):
             assert torch.equal(a[key][k], want3[k][key]), ("area", k, key)
     own = pipe.own_snapshot_outputs(True)
     c = {key: torch.empty_like(v) for key, v in own.items()}
-    _lib.check(_lib.load().demon_pipeline_forward_snapshots_v2(
-        pipe.net.ptr, pipe._ip.data_ptr(), None, 2, ITER, *(c[key].data_ptr() for key in KEYS),
-        ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
+    args = _lib.PipelineArgs(input=_lib.INPUT_F32, images=pipe._ip.data_ptr(), image2_2_mode=2, iterations=ITER, snapshots=1,
+                             **{key[len("predict_"):]: c[key].data_ptr() for key in KEYS})
+    _lib.check(_lib.load().demon_pipeline_run(pipe.net.ptr, args, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)))
     assert_same(c, a)
     assert pipe.launches() == plain_launches and pipe.snapshot_launches() > 0
 
@@ -280,7 +280,7 @@ def test_interleaved_call_kinds_equal_their_eager_results(session):
     _lib.check_errors()
 
 
-def test_refusals(session, synthetic_weights):
+def test_pipeline_args_refusals_launch_nothing(session, synthetic_weights):
     from demon_b200.networks_original import DemonPipeline, Session as SessionV1
     lib = _lib.load()
     v2 = session.net(1)
@@ -293,34 +293,48 @@ def test_refusals(session, synthetic_weights):
     u22 = torch.zeros(1, 48, 64, 3, dtype=torch.uint8, device="cuda")
     K = torch.full((1, 2, 4), 300.0, dtype=torch.float64, device="cuda")
     st = torch.zeros(1, 2, dtype=torch.uint8, device="cuda")
-    o = [torch.zeros(4, 3, 192, 256, device="cuda").data_ptr() for _ in range(7)]
+    o = dict(zip(("depth0", "normal0", "rotation", "translation", "flow2", "depth2", "normal2"),
+                 (torch.zeros(4, 3, 192, 256, device="cuda").data_ptr() for _ in range(7))))
     h_f, h_u8 = np.zeros((1, 6, 192, 256), np.float32), np.zeros((1, 2, 192, 256, 3), np.uint8)
-    h_o = [np.zeros((1, 3, 192, 256), np.float32).ctypes.data for _ in range(4)]
-    v2_calls = {
-        "snapshots": lambda n, m, i22=None: lib.demon_pipeline_forward_snapshots_v2(n, f.data_ptr(), i22, m, 1, *o, s),
-        "u8": lambda n, m, i22=None: lib.demon_pipeline_forward_u8_v2(n, u8.data_ptr(), i22, m, 1, *o, s),
-        "images": lambda n, m, i22=None: lib.demon_pipeline_forward_images_u8_v2(n, u8.data_ptr(), *u8.stride()[:3], 192, 256, 3, m, 1, *o, s),
-        "views": lambda n, m, i22=None: lib.demon_pipeline_forward_views_u8_v2(n, u8.data_ptr(), *u8.stride()[:3], 192, 256, K.data_ptr(),
-                                                                               st.data_ptr(), 3, m, 1, *o, s),
-        "host": lambda n, m, i22=None: lib.demon_pipeline_forward_host_v2(n, h_f.ctypes.data, i22, m, 1, *h_o, s),
-        "host_async": lambda n, m, i22=None: lib.demon_pipeline_forward_host_async_v2(n, h_f.ctypes.data, i22, m, 1, *h_o, s),
-        "host_u8": lambda n, m, i22=None: lib.demon_pipeline_forward_host_u8_v2(n, h_u8.ctypes.data, i22, m, 1, *h_o, s),
-        "host_u8_async": lambda n, m, i22=None: lib.demon_pipeline_forward_host_u8_async_v2(n, h_u8.ctypes.data, i22, m, 1, *h_o, s),
+    h_o = {k: np.zeros((1, 3, 192, 256), np.float32).ctypes.data for k in ("depth0", "normal0", "rotation", "translation")}
+    sizes = dict(zip(("sn", "si", "sy"), u8.stride()[:3]), h=192, w=256, resample=3)
+    run = lambda n, a: lib.demon_pipeline_run(n, a, s)
+    run_host = lambda sync: lambda n, a: lib.demon_pipeline_run_host(n, a, sync, s)
+    calls = {   # call kind -> (entry, the fields of its PipelineArgs)
+        "snapshots": (run, dict(input=_lib.INPUT_F32, images=f.data_ptr(), snapshots=1, **o)),
+        "u8": (run, dict(input=_lib.INPUT_U8, images=u8.data_ptr(), **o)),
+        "images": (run, dict(input=_lib.INPUT_RESIZE_U8, images=u8.data_ptr(), **sizes, **o)),
+        "views": (run, dict(input=_lib.INPUT_VIEWS_U8, images=u8.data_ptr(), K=K.data_ptr(), status=st.data_ptr(), **sizes, **o)),
+        "host": (run_host(1), dict(input=_lib.INPUT_F32, images=h_f.ctypes.data, **h_o)),
+        "host_async": (run_host(0), dict(input=_lib.INPUT_F32, images=h_f.ctypes.data, **h_o)),
+        "host_u8": (run_host(1), dict(input=_lib.INPUT_U8, images=h_u8.ctypes.data, **h_o)),
+        "host_u8_async": (run_host(0), dict(input=_lib.INPUT_U8, images=h_u8.ctypes.data, **h_o)),
     }
+
+    def call(name, net, mode, i22=None, **change):
+        entry, fields = calls[name]
+        return entry(net, _lib.PipelineArgs(image2_2=i22, image2_2_mode=mode, iterations=1, **dict(fields, **change)))
+
     n0 = lib.demon_launch_count()
-    for name, call in v2_calls.items():
-        assert call(v1.ptr, 0) == -1, name                      # a v1 handle
-        assert call(v2.ptr, 7) == -1, name                      # no such mode
+    for name in calls:
+        assert call(name, v1.ptr, 0) == -1, name                     # normal0 on a v1 handle
+        assert "normal0" in lib.demon_last_error().decode(), name
+        assert call(name, v1.ptr, 2, normal0=None) == -1, name       # area on a v1 handle
+        assert "image2_2_mode" in lib.demon_last_error().decode(), name
+        assert call(name, v2.ptr, 7) == -1, name                     # no such mode
         if name not in ("images", "views"):
-            assert call(v2.ptr, 1) == -1, name                  # resize: images / views only
-            assert call(v2.ptr, 2, u22.data_ptr()) == -1, name  # area and a given image2_2
+            assert call(name, v2.ptr, 1) == -1, name                 # resize: images / views only
+            assert call(name, v2.ptr, 2, u22.data_ptr()) == -1, name  # area and a given image2_2
     # snapshots: normal0 needs depth0
-    assert lib.demon_pipeline_forward_snapshots_v2(v2.ptr, f.data_ptr(), None, 0, 1, None, *o[1:], s) == -1
-    # every v1 entry that takes a mode refuses area
-    assert lib.demon_pipeline_forward_images_u8(v1.ptr, u8.data_ptr(), *u8.stride()[:3], 192, 256, 3, 2, 1, *o[:6], s) == -1
-    assert lib.demon_pipeline_forward_views_u8(v1.ptr, u8.data_ptr(), *u8.stride()[:3], 192, 256, K.data_ptr(), st.data_ptr(), 3, 2, 1,
-                                               *o[:6], s) == -1
-    assert lib.demon_launch_count() == n0                       # nothing was launched
+    assert call("snapshots", v2.ptr, 0, depth0=None) == -1
+    # a field the input kind does not read, and what the host entry does not take
+    assert call("u8", v2.ptr, 0, K=K.data_ptr()) == -1
+    assert call("snapshots", v2.ptr, 0, sn=1) == -1
+    assert call("images", v2.ptr, 0, u22.data_ptr()) == -1
+    assert call("u8", v2.ptr, 0, snapshots=2) == -1
+    for change in (dict(snapshots=1), dict(flow2=o["flow2"]), dict(depth0=None), dict(input=_lib.INPUT_RESIZE_U8, **sizes)):
+        assert call("host_u8", v2.ptr, 0, **change) == -1, change
+    assert lib.demon_launch_count() == n0                            # nothing was launched
     pipe1 = DemonPipeline(s1, batch_size=1, iterations=1)
     for call in (lambda: pipe1.forward(f, "area"), lambda: pipe1.forward_snapshots(f, "area"), lambda: pipe1.forward_u8(u8, "area"),
                  lambda: pipe1.forward_images(u8, image2_2="area"), lambda: pipe1.forward_views(u8, K, image2_2="area"),

@@ -78,7 +78,7 @@ def test_prepare_input_data_argument_errors():
         images.prepare_input_data(ok, ok)
 
 
-def test_c_entries_reject_bad_arguments_before_any_device_work():
+def test_resize_and_pipeline_args_reject_bad_arguments_before_any_device_work():
     dbuild.build()
     lib = _lib.load()
     buf = (ctypes.c_uint8 * 16)()
@@ -98,4 +98,5 @@ def test_c_entries_reject_bad_arguments_before_any_device_work():
         assert lib.demon_resize_u8(*args, None) == -1, args
     assert lib.demon_resize_u8(p, 24, 24, 1, 8, 8, p, 4, 4, 1, None) == -1
     assert "resample 1" in lib.demon_last_error().decode()
-    assert lib.demon_pipeline_forward_images_u8(None, p, 0, 0, 0, 480, 640, 3, 1, 3, *([None] * 6), None) == -1
+    args = _lib.PipelineArgs(input=_lib.INPUT_RESIZE_U8, images=p, h=480, w=640, resample=3, image2_2_mode=1, iterations=3)
+    assert lib.demon_pipeline_run(None, args, None) == -1

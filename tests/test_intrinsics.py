@@ -224,7 +224,7 @@ def test_intrinsics4_forms():
     assert np.array_equal(images.intrinsics4(K33.reshape(3, 1, 3, 3).repeat(2, 1), (3, 2), "K"), np.repeat(K4[:, None], 2, 1))
 
 
-def test_c_entries_reject_bad_arguments_before_any_device_work():
+def test_adjust_and_pipeline_args_reject_bad_arguments_before_any_device_work():
     dbuild.build()
     lib = _lib.load()
     buf = (ctypes.c_uint8 * 64)()
@@ -245,4 +245,6 @@ def test_c_entries_reject_bad_arguments_before_any_device_work():
     ]
     for args in calls:
         assert lib.demon_adjust_intrinsics_u8(*args, None) == -1, args
-    assert lib.demon_pipeline_forward_views_u8(None, p, 0, 0, 0, 480, 640, p, p, 3, 1, 3, *([None] * 6), None) == -1
+    args = _lib.PipelineArgs(input=_lib.INPUT_VIEWS_U8, images=p, h=480, w=640, K=p, status=p, resample=3, image2_2_mode=1,
+                             iterations=3)
+    assert lib.demon_pipeline_run(None, args, None) == -1
