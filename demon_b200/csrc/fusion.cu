@@ -449,17 +449,19 @@ struct DenseVolume {
 __device__ __forceinline__ unsigned long long block_key(int bx, int by, int bz);
 __device__ __forceinline__ long find_slot(const unsigned long long* __restrict__ keys, long mask, unsigned long long key);
 
-// The cubes of the hashed blocks: cube c has its lower corner at local voxel c % 512 (x fastest) of block c / 512, and
-// its corners past the block's last voxel lie in the +x, +y, +z neighbours nbr[8 b + (dx | dy << 1 | dz << 2)].
+// The cubes of the hashed blocks first, first + 1, ...: cube c has its lower corner at local voxel c % 512 (x fastest) of
+// block first + c / 512, and its corners past the block's last voxel lie in the +x, +y, +z neighbours
+// nbr[8 (b - first) + (dx | dy << 1 | dz << 2)], which may be any block of the pool.
 struct SparseVolume {
   const float* tsdf;
   const float* weight;
   const int* blocks;   // [m,3] block coordinates
-  const int* nbr;      // [m,8] pool index of block b + (dx, dy, dz), or -1
+  const int* nbr;      // [count,8] pool index of block b + (dx, dy, dz), or -1
   long ncubes;
   const unsigned long long* keys;   // the hash table, for `at` only
   const int* values;
   long mask;
+  int first;           // the first block of the cubes `locate` enumerates
   struct Cube {
     int b;      // pool index
     int l[3];   // local voxel of corner 0
@@ -484,7 +486,7 @@ struct SparseVolume {
     }
     if (B[0] != cur.B[0] || B[1] != cur.B[1] || B[2] != cur.B[2]) {
       const long s = find_slot(keys, mask, block_key(B[0], B[1], B[2]));
-      cur.b = s < 0 ? -1 : __ldg(values + s);
+      cur.b = s < 0 ? -1 : __ldg(values + s);   // negative (new, or on the host): not stored
 #pragma unroll
       for (int a = 0; a < 3; ++a) cur.B[a] = B[a];
     }
@@ -493,7 +495,7 @@ struct SparseVolume {
   }
   __device__ bool locate(long c, Cube& cb) const {
     if (c >= ncubes) return false;
-    cb.b = (int)(c >> 9);
+    cb.b = first + (int)(c >> 9);
     const int r = (int)(c & 511);
     cb.l[0] = r & 7;
     cb.l[1] = (r >> 3) & 7;
@@ -506,7 +508,7 @@ struct SparseVolume {
   __device__ long corner(const Cube& cb, int q) const {
     const int x = cb.l[0] + kCorner[q][0], y = cb.l[1] + kCorner[q][1], z = cb.l[2] + kCorner[q][2];
     const int nb = (x >> 3) | ((y >> 3) << 1) | ((z >> 3) << 2);
-    const int blk = nb ? __ldg(nbr + 8 * cb.b + nb) : cb.b;
+    const int blk = nb ? __ldg(nbr + 8L * (cb.b - first) + nb) : cb.b;
     if (blk < 0) return -1;
     return ((long)blk << 9) + ((z & 7) << 6) + ((y & 7) << 3) + (x & 7);
   }
@@ -666,8 +668,10 @@ DenseVolume make_volume(const float* tsdf, const float* weight, int nx, int ny, 
 // ---- sparse volume: voxel blocks in a hash table -------------------------------------------------------------------------
 // Block (bx, by, bz), |b| <= kMaxBlockCoord per axis, holds voxels 8 b + (0..7) in the pool at its index: tsdf and weight
 // [m,8,8,8] (z, y, x; x fastest), colour [m,8,8,8,3].  The table maps the packed key of a block to its pool index, by open
-// addressing with linear probing over `capacity` (a power of 2) slots: key -1 marks an empty slot, value -1 a block
-// inserted by the running call's allocation and not yet given a pool index.
+// addressing with linear probing over `capacity` (a power of 2) slots: key -1 marks an empty slot.  A value >= 0 is the
+// block's pool index, -1 a block inserted by the running call's allocation and not yet given a pool index, and -2 - s a
+// block streamed out to host slot s (SparseTsdfVolume's max_device_blocks): every reader below takes a negative value
+// as "not stored on the device".
 constexpr int kSparseThreads = 256;
 constexpr int kMaxBlockCoord = DEMON_SPARSE_TSDF_MAX_COORD;
 constexpr int kMaxSpan = DEMON_SPARSE_TSDF_MAX_SPAN;
@@ -825,7 +829,7 @@ __global__ void __launch_bounds__(kSparseThreads) sparse_gather_kernel(const uns
   const long s = (long)blockIdx.x * kSparseThreads + threadIdx.x;
   if (s >= capacity) return;
   const unsigned long long key = keys[s];
-  if (key != kEmptyKey && values[s] < 0) out[atomicAdd(counters + kCursor, 1ull)] = (int64_t)key;
+  if (key != kEmptyKey && values[s] == -1) out[atomicAdd(counters + kCursor, 1ull)] = (int64_t)key;
 }
 
 // Key i of the sorted new keys gets pool index first + i.
@@ -862,18 +866,20 @@ __global__ void __launch_bounds__(kFuseThreads) sparse_tsdf_integrate_kernel(
   if (active) store_state<kColor>(tsdf, weight, color, vox, st);
 }
 
-// nbr[8 b + q] = the pool index of block b + (q & 1, q >> 1 & 1, q >> 2), or -1.
+// nbr[8 (b - first) + q] = the pool index of block b + (q & 1, q >> 1 & 1, q >> 2), or -1, for blocks first .. first+count-1.
 __global__ void __launch_bounds__(kSparseThreads) sparse_neighbours_kernel(const unsigned long long* __restrict__ keys,
                                                                            const int* __restrict__ values, long mask,
-                                                                           const int* __restrict__ blocks, int m, int* __restrict__ nbr) {
+                                                                           const int* __restrict__ blocks, int first, int count,
+                                                                           int* __restrict__ nbr) {
   const long e = (long)blockIdx.x * kSparseThreads + threadIdx.x;
-  if (e >= 8L * m) return;
-  const long b = e >> 3;
+  if (e >= 8L * count) return;
+  const long b = first + (e >> 3);
   const int q = (int)(e & 7);
   const int bx = blocks[3 * b] + (q & 1), by = blocks[3 * b + 1] + ((q >> 1) & 1), bz = blocks[3 * b + 2] + (q >> 2);
   long s = -1;
   if (bx <= kMaxBlockCoord && by <= kMaxBlockCoord && bz <= kMaxBlockCoord) s = find_slot(keys, mask, block_key(bx, by, bz));
-  nbr[e] = s < 0 ? -1 : __ldg(values + s);
+  const int v = s < 0 ? -1 : __ldg(values + s);
+  nbr[e] = v < 0 ? -1 : v;   // a block on the host is not stored
 }
 
 // ---- ray casting ------------------------------------------------------------------------------------------------------
@@ -1106,6 +1112,176 @@ __global__ void sparse_far_decode_kernel(float* far, int n) {
   far[f] = __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
 }
 
+
+// ---- streaming blocks between the device and host memory (SparseTsdfVolume's max_device_blocks) -----------------------
+// The reach rule decides which blocks a call's cameras can touch; the evict and restore kernels move whole blocks between
+// pool slots and host slots of mapped pinned memory (zero-copy: one warp per block, coalesced 16-byte accesses over the
+// PCIe link) and rewrite the blocks' table values in the same pass.  The rule is in include/demon_b200.h
+// (demon_sparse_tsdf_reach_f32) and its guarantee in DESIGN.md §3.9.
+constexpr int kDepthTile = 8;
+constexpr int kMoveThreads = 256;
+
+// tiles[f, ty, tx] = the largest finite depth > 0 of the tile's pixels, -inf when there is none.
+__global__ void __launch_bounds__(kSparseThreads) sparse_depth_tiles_kernel(const float* __restrict__ depth, int n, int h, int w, int th,
+                                                                            int tw, float* __restrict__ tiles) {
+  const long e = (long)blockIdx.x * kSparseThreads + threadIdx.x;
+  if (e >= (long)n * th * tw) return;
+  const int f = (int)(e / ((long)th * tw));
+  const int r = (int)(e - (long)f * th * tw), ty = r / tw, tx = r - ty * tw;
+  const float* df = depth + (long)f * h * w;
+  float mx = -INFINITY;
+  for (int y = kDepthTile * ty; y < min(h, kDepthTile * ty + kDepthTile); ++y)
+    for (int x = kDepthTile * tx; x < min(w, kDepthTile * tx + kDepthTile); ++x) {
+      const float d = __ldg(df + (long)y * w + x);
+      if (isfinite(d) && d > 0.0f) mx = fmaxf(mx, d);
+    }
+  tiles[e] = mx;
+}
+
+// One thread per block and frame: out[b] = mark when frame f reaches block b (the rule of demon_sparse_tsdf_reach_f32).
+__global__ void __launch_bounds__(kSparseThreads) sparse_reach_kernel(const int* __restrict__ blocks, int m, Grid gr, float trunc,
+                                                                      const float* __restrict__ tiles, const float* __restrict__ K,
+                                                                      const float* __restrict__ R, const float* __restrict__ t, int n,
+                                                                      int h, int w, int* __restrict__ out, int mark) {
+  const long e = (long)blockIdx.x * kSparseThreads + threadIdx.x;
+  if (e >= (long)m * n) return;
+  const int f = (int)(e / m), b = (int)(e - (long)f * m);
+  float lo[3], hi[3];
+  const float tr2 = fadd(trunc, trunc);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const int g = 8 * __ldg(blocks + 3 * b + a);
+    lo[a] = fsub(fadd(gr.o[a], fmul(gr.vs, (float)(g - 3))), tr2);
+    hi[a] = fadd(fadd(gr.o[a], fmul(gr.vs, (float)(g + 10))), tr2);
+  }
+  const float* Rf = R + 9 * f;
+  const float* tf = t + 3 * f;
+  const float fx = __ldg(K + 9 * f), cx = __ldg(K + 9 * f + 2), fy = __ldg(K + 9 * f + 4), cy = __ldg(K + 9 * f + 5);
+  float zmin = INFINITY, zmax = -INFINITY, umin = INFINITY, umax = -INFINITY, vmin = INFINITY, vmax = -INFINITY;
+  bool behind = false;
+#pragma unroll
+  for (int q = 0; q < 8; ++q) {
+    const float X0 = (q & 1) ? hi[0] : lo[0], X1 = (q & 2) ? hi[1] : lo[1], X2 = (q & 4) ? hi[2] : lo[2];
+    const float z = fadd(fadd(fadd(fmul(__ldg(Rf + 6), X0), fmul(__ldg(Rf + 7), X1)), fmul(__ldg(Rf + 8), X2)), __ldg(tf + 2));
+    zmin = fminf(zmin, z);
+    zmax = fmaxf(zmax, z);
+    if (!(z > gr.vs)) {
+      behind = true;
+      continue;
+    }
+    const float x = fadd(fadd(fadd(fmul(__ldg(Rf), X0), fmul(__ldg(Rf + 1), X1)), fmul(__ldg(Rf + 2), X2)), __ldg(tf));
+    const float y = fadd(fadd(fadd(fmul(__ldg(Rf + 3), X0), fmul(__ldg(Rf + 4), X1)), fmul(__ldg(Rf + 5), X2)), __ldg(tf + 1));
+    const float u = fadd(fdiv(fmul(fx, x), z), cx), v = fadd(fdiv(fmul(fy, y), z), cy);
+    umin = fminf(umin, u);
+    umax = fmaxf(umax, u);
+    vmin = fminf(vmin, v);
+    vmax = fmaxf(vmax, v);
+  }
+  if (!(zmax > gr.vs)) return;   // wholly behind the camera
+  int x0 = 0, x1 = w - 1, y0 = 0, y1 = h - 1;
+  if (behind) {
+    zmin = 0.0f;
+  } else {
+    const float u0 = floorf(umin) - 1.0f, u1 = floorf(umax) + 1.0f, v0 = floorf(vmin) - 1.0f, v1 = floorf(vmax) + 1.0f;
+    if (!(u1 >= 0.0f && u0 <= (float)(w - 1) && v1 >= 0.0f && v0 <= (float)(h - 1))) return;
+    x0 = (int)fmaxf(u0, 0.0f);
+    x1 = (int)fminf(u1, (float)(w - 1));
+    y0 = (int)fmaxf(v0, 0.0f);
+    y1 = (int)fminf(v1, (float)(h - 1));
+  }
+  const int tw = (w + kDepthTile - 1) / kDepthTile, th = (h + kDepthTile - 1) / kDepthTile;
+  const float* T = tiles + (long)f * th * tw;
+  for (int ty = y0 / kDepthTile; ty <= y1 / kDepthTile; ++ty)
+    for (int tx = x0 / kDepthTile; tx <= x1 / kDepthTile; ++tx)
+      if (fadd(__ldg(T + ty * tw + tx), trunc) >= zmin) {
+        out[b] = mark;
+        return;
+      }
+}
+
+// Warp i moves pool block src[i] to host slot slots[i] and gives its key the value -2 - slots[i].
+__global__ void __launch_bounds__(kMoveThreads) sparse_evict_kernel(const float4* __restrict__ tsdf, const float4* __restrict__ weight,
+                                                                    const float4* __restrict__ color, const int* __restrict__ blocks,
+                                                                    const int* __restrict__ stamps, const unsigned long long* __restrict__ keys,
+                                                                    int* __restrict__ values, long mask, const int* __restrict__ src,
+                                                                    const int* __restrict__ slots, int count, float4* __restrict__ htsdf,
+                                                                    float4* __restrict__ hweight, float4* __restrict__ hcolor,
+                                                                    int* __restrict__ hblocks, int* __restrict__ hstamps) {
+  const int i = (int)(((long)blockIdx.x * kMoveThreads + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (i >= count) return;
+  const long s = __ldg(src + i), d = __ldg(slots + i);
+  for (int j = lane; j < 128; j += 32) {
+    htsdf[128 * d + j] = __ldg(tsdf + 128 * s + j);
+    hweight[128 * d + j] = __ldg(weight + 128 * s + j);
+  }
+  if (color)
+    for (int j = lane; j < 384; j += 32) hcolor[384 * d + j] = __ldg(color + 384 * s + j);
+  if (lane < 3) hblocks[3 * d + lane] = __ldg(blocks + 3 * s + lane);
+  if (lane == 0) {
+    hstamps[d] = __ldg(stamps + s);
+    const long sl = find_slot(keys, mask, block_key(__ldg(blocks + 3 * s), __ldg(blocks + 3 * s + 1), __ldg(blocks + 3 * s + 2)));
+    if (sl >= 0) values[sl] = -2 - (int)d;
+  }
+}
+
+// Warp i moves host slot slots[i] to pool block dst[i]: its coordinates, optionally its stamp, and its table value.
+__global__ void __launch_bounds__(kMoveThreads) sparse_restore_kernel(const float4* __restrict__ htsdf, const float4* __restrict__ hweight,
+                                                                      const float4* __restrict__ hcolor, const int* __restrict__ hblocks,
+                                                                      const int* __restrict__ slots, const int* __restrict__ dst, int count,
+                                                                      float4* __restrict__ tsdf, float4* __restrict__ weight,
+                                                                      float4* __restrict__ color, int* __restrict__ blocks,
+                                                                      int* __restrict__ stamps, int stamp,
+                                                                      const unsigned long long* __restrict__ keys, int* __restrict__ values,
+                                                                      long mask) {
+  const int i = (int)(((long)blockIdx.x * kMoveThreads + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (i >= count) return;
+  const long s = __ldg(slots + i), d = __ldg(dst + i);
+  for (int j = lane; j < 128; j += 32) {
+    tsdf[128 * d + j] = htsdf[128 * s + j];
+    weight[128 * d + j] = hweight[128 * s + j];
+  }
+  if (color)
+    for (int j = lane; j < 384; j += 32) color[384 * d + j] = hcolor[384 * s + j];
+  if (lane < 3) blocks[3 * d + lane] = __ldg(hblocks + 3 * s + lane);
+  if (lane == 0) {
+    if (stamps) stamps[d] = stamp;
+    if (keys) {
+      const long sl = find_slot(keys, mask, block_key(__ldg(hblocks + 3 * s), __ldg(hblocks + 3 * s + 1), __ldg(hblocks + 3 * s + 2)));
+      if (sl >= 0) values[sl] = (int)d;
+    }
+  }
+}
+
+// values[key of block b] = b for blocks first .. first+count-1, inserting the key when the table lacks it.
+__global__ void __launch_bounds__(kSparseThreads) sparse_index_kernel(unsigned long long* __restrict__ keys, int* __restrict__ values,
+                                                                      long mask, const int* __restrict__ blocks, int first, int count) {
+  const int i = blockIdx.x * kSparseThreads + threadIdx.x;
+  if (i >= count) return;
+  const long b = (long)first + i;
+  const unsigned long long key = block_key(blocks[3 * b], blocks[3 * b + 1], blocks[3 * b + 2]);
+  for (long q = key_slot(key, mask);; q = (q + 1) & mask) {
+    unsigned long long k = *(volatile unsigned long long*)(keys + q);
+    if (k == kEmptyKey) k = atomicCAS(keys + q, kEmptyKey, key);
+    if (k == kEmptyKey || k == key) {
+      values[q] = (int)b;
+      return;
+    }
+  }
+}
+
+// The device address of mapped pinned host memory, or an error for memory the device cannot reach.
+int mapped(const char* name, const void* p, void** dev) {
+  if (!p) {
+    *dev = nullptr;
+    return DEMON_OK;
+  }
+  cudaPointerAttributes at;
+  DEMON_CHECK_CUDA(cudaPointerGetAttributes(&at, p));
+  DEMON_REQUIRE(at.type == cudaMemoryTypeHost && at.devicePointer, "%s: the host store must be pinned host memory the device can map", name);
+  *dev = at.devicePointer;
+  return DEMON_OK;
+}
+
 int check_raycast(const char* name, const float* origin, float voxel_size, float step, int n, int h, int w) {
   DEMON_REQUIRE(n >= 0 && h >= 1 && w >= 1 && (long)h * w < (1L << 24), "%s: bad size %d frames of %dx%d", name, n, h, w);
   DEMON_REQUIRE(origin && std::isfinite(origin[0]) && std::isfinite(origin[1]) && std::isfinite(origin[2]), "%s: the origin must be finite",
@@ -1301,36 +1477,41 @@ int64_t demon_sparse_tsdf_mesh_scratch_bytes(int m) {
   return sparse_mc_tiles(m) * (int64_t)(sizeof(int64_t) + sizeof(int)) + 8LL * m * sizeof(int);
 }
 
-int demon_sparse_tsdf_mesh_count_f32(const float* tsdf, const float* weight, const int* blocks, int m, const int64_t* keys, const int* values,
-                                     int64_t capacity, void* scratch, int64_t* triangles, void* stream) {
+int demon_sparse_tsdf_mesh_range_count_f32(const float* tsdf, const float* weight, const int* blocks, int m, int first, int count,
+                                           const int64_t* keys, const int* values, int64_t capacity, void* scratch, int64_t* triangles,
+                                           void* stream) {
   if (int rc = check_table("sparse_tsdf_mesh_count", keys, values, capacity)) return rc;
-  DEMON_REQUIRE(m >= 1 && 512LL * m * 15 < (1LL << 40), "sparse_tsdf_mesh_count: bad block count %d", m);
+  DEMON_REQUIRE(m >= 1 && first >= 0 && count >= 1 && (int64_t)first + count <= m && 512LL * count * 15 < (1LL << 40),
+                "sparse_tsdf_mesh_count: bad blocks %d..%d of %d", first, first + count - 1, m);
   DEMON_REQUIRE(tsdf && weight && blocks && scratch && triangles, "sparse_tsdf_mesh_count: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  const int tiles = (int)sparse_mc_tiles(m);
-  int64_t* tile_first = static_cast<int64_t*>(scratch);   // scratch: tile_first [tiles], tile_counts [tiles], nbr [m,8]
+  const int tiles = (int)sparse_mc_tiles(count);
+  int64_t* tile_first = static_cast<int64_t*>(scratch);   // scratch: tile_first [tiles], tile_counts [tiles], nbr [count,8]
   int* tile_counts = reinterpret_cast<int*>(tile_first + tiles);
   int* nbr = tile_counts + tiles;
-  sparse_neighbours_kernel<<<(unsigned)ceil_div64(8LL * m, kSparseThreads), kSparseThreads, 0, st>>>(
-      reinterpret_cast<const unsigned long long*>(keys), values, capacity - 1, blocks, m, nbr);
+  sparse_neighbours_kernel<<<(unsigned)ceil_div64(8LL * count, kSparseThreads), kSparseThreads, 0, st>>>(
+      reinterpret_cast<const unsigned long long*>(keys), values, capacity - 1, blocks, first, count, nbr);
   DEMON_LAUNCH_CHECK();
-  mc_count_kernel<<<tiles, kMcThreads, 0, st>>>(SparseVolume{tsdf, weight, blocks, nbr, 512L * m}, tile_counts);
+  const SparseVolume vol{tsdf, weight, blocks, nbr, 512L * count, nullptr, nullptr, 0, first};
+  mc_count_kernel<<<tiles, kMcThreads, 0, st>>>(vol, tile_counts);
   DEMON_LAUNCH_CHECK();
   mc_offsets_kernel<<<1, kScanThreads, 0, st>>>(tile_counts, tiles, tile_first, triangles);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
 }
 
-int demon_sparse_tsdf_mesh_f32(const float* tsdf, const float* weight, const float* color, const int* blocks, int m, const float* origin,
-                               float voxel_size, const void* scratch, float* vertices, uint8_t* colors, int* faces, void* stream) {
-  DEMON_REQUIRE(m >= 1 && 512LL * m * 15 < (1LL << 40), "sparse_tsdf_mesh: bad block count %d", m);
+int demon_sparse_tsdf_mesh_range_f32(const float* tsdf, const float* weight, const float* color, const int* blocks, int m, int first,
+                                     int count, const float* origin, float voxel_size, const void* scratch, float* vertices, uint8_t* colors,
+                                     int* faces, void* stream) {
+  DEMON_REQUIRE(m >= 1 && first >= 0 && count >= 1 && (int64_t)first + count <= m && 512LL * count * 15 < (1LL << 40),
+                "sparse_tsdf_mesh: bad blocks %d..%d of %d", first, first + count - 1, m);
   DEMON_REQUIRE(origin && std::isfinite(voxel_size) && voxel_size > 0.0f, "sparse_tsdf_mesh: bad origin or voxel_size %g", voxel_size);
   DEMON_REQUIRE(!color == !colors, "sparse_tsdf_mesh: color and colors go together");
   DEMON_REQUIRE(tsdf && weight && blocks && scratch && vertices && faces, "sparse_tsdf_mesh: null pointer");
-  const int tiles = (int)sparse_mc_tiles(m);
+  const int tiles = (int)sparse_mc_tiles(count);
   const int64_t* tile_first = static_cast<const int64_t*>(scratch);
   const int* nbr = reinterpret_cast<const int*>(tile_first + tiles) + tiles;
-  const SparseVolume vol{tsdf, weight, blocks, nbr, 512L * m};
+  const SparseVolume vol{tsdf, weight, blocks, nbr, 512L * count, nullptr, nullptr, 0, first};
   if (color)
     mc_scatter_kernel<true><<<tiles, kMcThreads, 0, (cudaStream_t)stream>>>(vol, color, origin[0], origin[1], origin[2], voxel_size,
                                                                            tile_first, vertices, colors, faces);
@@ -1339,6 +1520,16 @@ int demon_sparse_tsdf_mesh_f32(const float* tsdf, const float* weight, const flo
                                                                             tile_first, vertices, nullptr, faces);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
+}
+
+int demon_sparse_tsdf_mesh_count_f32(const float* tsdf, const float* weight, const int* blocks, int m, const int64_t* keys, const int* values,
+                                     int64_t capacity, void* scratch, int64_t* triangles, void* stream) {
+  return demon_sparse_tsdf_mesh_range_count_f32(tsdf, weight, blocks, m, 0, m, keys, values, capacity, scratch, triangles, stream);
+}
+
+int demon_sparse_tsdf_mesh_f32(const float* tsdf, const float* weight, const float* color, const int* blocks, int m, const float* origin,
+                               float voxel_size, const void* scratch, float* vertices, uint8_t* colors, int* faces, void* stream) {
+  return demon_sparse_tsdf_mesh_range_f32(tsdf, weight, color, blocks, m, 0, m, origin, voxel_size, scratch, vertices, colors, faces, stream);
 }
 
 int demon_tsdf_raycast_f32(const float* tsdf, const float* weight, const float* color, int nx, int ny, int nz, const float* origin,
@@ -1386,10 +1577,92 @@ int demon_sparse_tsdf_raycast_f32(const float* tsdf, const float* weight, const 
   cudaStream_t st = (cudaStream_t)stream;
   int* nbr = static_cast<int*>(scratch);   // scratch: nbr [m,8]
   sparse_neighbours_kernel<<<(unsigned)ceil_div64(8LL * m, kSparseThreads), kSparseThreads, 0, st>>>(
-      reinterpret_cast<const unsigned long long*>(keys), values, capacity - 1, blocks, m, nbr);
+      reinterpret_cast<const unsigned long long*>(keys), values, capacity - 1, blocks, 0, m, nbr);
   DEMON_LAUNCH_CHECK();
-  const SparseVolume vol{tsdf, weight, blocks, nbr, 512L * m, reinterpret_cast<const unsigned long long*>(keys), values, (long)capacity - 1};
+  const SparseVolume vol{tsdf, weight, blocks, nbr, 512L * m, reinterpret_cast<const unsigned long long*>(keys), values, (long)capacity - 1, 0};
   return launch_raycast(vol, color, origin, voxel_size, K, R, t, near, far, step, n, h, w, depth, normals, colors, st);
+}
+
+int demon_sparse_tsdf_depth_tiles_f32(const float* depth, int n, int h, int w, float* tiles, void* stream) {
+  DEMON_REQUIRE(n >= 0 && h >= 1 && w >= 1 && (long)h * w < (1L << 24), "sparse_tsdf_depth_tiles: bad size %d frames of %dx%d", n, h, w);
+  if (n == 0) return DEMON_OK;
+  DEMON_REQUIRE(depth && tiles, "sparse_tsdf_depth_tiles: null pointer");
+  const int th = ceil_div(h, kDepthTile), tw = ceil_div(w, kDepthTile);
+  sparse_depth_tiles_kernel<<<(unsigned)ceil_div64((int64_t)n * th * tw, kSparseThreads), kSparseThreads, 0, (cudaStream_t)stream>>>(
+      depth, n, h, w, th, tw, tiles);
+  DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
+}
+
+int demon_sparse_tsdf_reach_f32(const int* blocks, int m, const float* origin, float voxel_size, float trunc, const float* tiles, const float* K,
+                                const float* R, const float* t, int n, int h, int w, int* out, int mark, void* stream) {
+  DEMON_REQUIRE(m >= 0 && n >= 0 && h >= 1 && w >= 1 && (long)h * w < (1L << 24), "sparse_tsdf_reach: bad size %d blocks, %d frames of %dx%d",
+                m, n, h, w);
+  DEMON_REQUIRE(origin && std::isfinite(origin[0]) && std::isfinite(origin[1]) && std::isfinite(origin[2]) && std::isfinite(voxel_size) &&
+                    voxel_size > 0.0f && std::isfinite(trunc) && trunc >= 0.0f,
+                "sparse_tsdf_reach: bad origin, voxel_size %g or trunc %g", voxel_size, trunc);
+  if (m == 0 || n == 0) return DEMON_OK;
+  DEMON_REQUIRE(blocks && tiles && K && R && t && out, "sparse_tsdf_reach: null pointer");
+  const Grid gr{{origin[0], origin[1], origin[2]}, voxel_size};
+  sparse_reach_kernel<<<(unsigned)ceil_div64((int64_t)m * n, kSparseThreads), kSparseThreads, 0, (cudaStream_t)stream>>>(
+      blocks, m, gr, trunc, tiles, K, R, t, n, h, w, out, mark);
+  DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
+}
+
+int demon_sparse_tsdf_evict(const float* tsdf, const float* weight, const float* color, const int* blocks, const int* stamps, const int64_t* keys,
+                            int* values, int64_t capacity, const int* src, const int* slots, int count, float* host_tsdf, float* host_weight,
+                            float* host_color, int* host_blocks, int* host_stamps, void* stream) {
+  if (int rc = check_table("sparse_tsdf_evict", keys, values, capacity)) return rc;
+  DEMON_REQUIRE(count >= 0, "sparse_tsdf_evict: bad count %d", count);
+  DEMON_REQUIRE(!color == !host_color, "sparse_tsdf_evict: color and host_color go together");
+  if (count == 0) return DEMON_OK;
+  DEMON_REQUIRE(tsdf && weight && blocks && stamps && src && slots && host_tsdf && host_weight && host_blocks && host_stamps,
+                "sparse_tsdf_evict: null pointer");
+  void *ht, *hw, *hc;
+  if (int rc = mapped("sparse_tsdf_evict", host_tsdf, &ht)) return rc;
+  if (int rc = mapped("sparse_tsdf_evict", host_weight, &hw)) return rc;
+  if (int rc = mapped("sparse_tsdf_evict", host_color, &hc)) return rc;
+  sparse_evict_kernel<<<(unsigned)ceil_div64(32LL * count, kMoveThreads), kMoveThreads, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const float4*>(tsdf), reinterpret_cast<const float4*>(weight), reinterpret_cast<const float4*>(color), blocks, stamps,
+      reinterpret_cast<const unsigned long long*>(keys), values, capacity - 1, src, slots, count, static_cast<float4*>(ht),
+      static_cast<float4*>(hw), static_cast<float4*>(hc), host_blocks, host_stamps);
+  DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
+}
+
+int demon_sparse_tsdf_restore(const float* host_tsdf, const float* host_weight, const float* host_color, const int* host_blocks, const int* slots,
+                              const int* dst, int count, float* tsdf, float* weight, float* color, int* blocks, int* stamps, int stamp,
+                              const int64_t* keys, int* values, int64_t capacity, void* stream) {
+  if (keys) {
+    if (int rc = check_table("sparse_tsdf_restore", keys, values, capacity)) return rc;
+  }
+  DEMON_REQUIRE(count >= 0, "sparse_tsdf_restore: bad count %d", count);
+  DEMON_REQUIRE(!color == !host_color, "sparse_tsdf_restore: color and host_color go together");
+  if (count == 0) return DEMON_OK;
+  DEMON_REQUIRE(host_tsdf && host_weight && host_blocks && slots && dst && tsdf && weight && blocks, "sparse_tsdf_restore: null pointer");
+  void *ht, *hw, *hc;
+  if (int rc = mapped("sparse_tsdf_restore", host_tsdf, &ht)) return rc;
+  if (int rc = mapped("sparse_tsdf_restore", host_weight, &hw)) return rc;
+  if (int rc = mapped("sparse_tsdf_restore", host_color, &hc)) return rc;
+  sparse_restore_kernel<<<(unsigned)ceil_div64(32LL * count, kMoveThreads), kMoveThreads, 0, (cudaStream_t)stream>>>(
+      static_cast<const float4*>(ht), static_cast<const float4*>(hw), static_cast<const float4*>(hc), host_blocks, slots, dst, count,
+      reinterpret_cast<float4*>(tsdf), reinterpret_cast<float4*>(weight), reinterpret_cast<float4*>(color), blocks, stamps, stamp,
+      reinterpret_cast<const unsigned long long*>(keys), values, keys ? capacity - 1 : 0);
+  DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
+}
+
+int demon_sparse_tsdf_index(int64_t* keys, int* values, int64_t capacity, const int* blocks, int first, int count, void* stream) {
+  if (int rc = check_table("sparse_tsdf_index", keys, values, capacity)) return rc;
+  DEMON_REQUIRE(first >= 0 && count >= 0 && (int64_t)first + count < (1LL << 31) && count < capacity, "sparse_tsdf_index: bad blocks %d + %d",
+                first, count);
+  if (count == 0) return DEMON_OK;
+  DEMON_REQUIRE(blocks, "sparse_tsdf_index: null pointer");
+  sparse_index_kernel<<<ceil_div(count, kSparseThreads), kSparseThreads, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<unsigned long long*>(keys), values, capacity - 1, blocks, first, count);
+  DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
 }
 
 }  // extern "C"

@@ -364,19 +364,37 @@ class SparseTsdfVolume:
     blocks are sorted by key and appended, then every block integrates the call's frames exactly as TsdfVolume does.  So a
     block holds the dense integration of every frame from the call that allocated it onward: blocks of the first call equal
     a dense volume's voxels bit for bit, and a block first seen in a later call has missed the free-space updates of the
-    earlier calls, as in every voxel-hashing fusion."""
+    earlier calls, as in every voxel-hashing fusion.
+
+    With `max_device_blocks` (an integer >= 1; default None: every block stays on the device), the blocks beyond that many
+    stream to pinned host memory after each integrate and raycast call, least recently reached first (ties by ascending
+    packed key, z then y then x), and every host block a call's cameras reach (include/demon_b200.h:
+    demon_sparse_tsdf_reach_f32) comes back before the call does any work, appended in key order.  A call that reaches
+    more blocks than the budget keeps them all until it ends (`peak_device_blocks`).  The table still indexes every block
+    and the host blocks' coordinates stay on the device, so the union of device and host blocks equals an unbudgeted
+    volume fed the same calls, voxel for voxel, and raycast and mesh return what it returns.  `blocks`, `tsdf`, `weight`,
+    `color`, `capacity` and `nbytes` describe the device; `host`, `host_nbytes`, `last_blocks_in` and `last_blocks_out`
+    the rest.  A long video is fused in bounded device memory by calling integrate once per chunk of frames."""
 
     MAX_SPAN = 4   # DEMON_SPARSE_TSDF_MAX_SPAN
     _POOL_BLOCKS = 64
     _TABLE_SLOTS = 1024
 
-    def __init__(self, voxel_size, origin=(0, 0, 0), trunc=None, color=True):
+    def __init__(self, voxel_size, origin=(0, 0, 0), trunc=None, color=True, max_device_blocks=None):
         self.origin, self.voxel_size, self.trunc = _grid(origin, voxel_size, trunc)
+        if max_device_blocks is not None and (isinstance(max_device_blocks, bool) or not isinstance(max_device_blocks, (int, np.integer))
+                                              or max_device_blocks < 1):
+            raise ValueError("max_device_blocks must be an integer >= 1 or None, got %r" % (max_device_blocks,))
+        self.max_device_blocks = None if max_device_blocks is None else int(max_device_blocks)
         self._color = bool(color)
         self.last_skipped_pixels = 0
         self._m = 0
-        self._pool = None    # blocks, tsdf, weight, color: the device state, made by the first call that needs it
+        self._pool = None    # blocks, tsdf, weight, color (and stamp with a budget): the device state, made by the first call
         self._table = None   # keys, values, counters
+        # with a budget: the host store (pinned tsdf, weight, color; device blocks, stamp, live), its slots in use
+        # [0, _hend) and the free ones among them (ascending), and the index of the last integrate or raycast call
+        self._host, self._hend, self._free, self._calls = None, 0, [], 0
+        self.last_blocks_in = self.last_blocks_out = self.peak_device_blocks = 0
 
     def _state(self):
         if self._pool is None:
@@ -391,6 +409,8 @@ class SparseTsdfVolume:
                 "tsdf": torch.zeros((capacity, 8, 8, 8), dtype=torch.float32, device=dev),
                 "weight": torch.zeros((capacity, 8, 8, 8), dtype=torch.float32, device=dev),
                 "color": torch.zeros((capacity, 8, 8, 8, 3), dtype=torch.float32, device=dev) if self._color else None}
+        if self.max_device_blocks is not None:
+            pool["stamp"] = torch.zeros((capacity,), dtype=torch.int32, device=dev)   # the last call that reached the block
         if self._pool is not None:
             for k, v in pool.items():
                 if v is not None:
@@ -444,6 +464,131 @@ class SparseTsdfVolume:
         tensors = list(self._state().values()) + list(self._table)
         return sum(t.numel() * t.element_size() for t in tensors if t is not None)
 
+    @property
+    def host(self):
+        """The blocks on the host in slot order, as CPU tensors: blocks [h,3] int32, tsdf and weight [h,8,8,8], color
+        [h,8,8,8,3] or None.  Synchronises (the transfers are asynchronous)."""
+        if self._host is None:
+            return {"blocks": torch.zeros((0, 3), dtype=torch.int32), "tsdf": torch.zeros((0, 8, 8, 8)), "weight": torch.zeros((0, 8, 8, 8)),
+                    "color": torch.zeros((0, 8, 8, 8, 3)) if self._color else None}
+        hs = self._host
+        torch.cuda.current_stream(hs["blocks"].device).synchronize()
+        live = torch.nonzero(hs["live"][:self._hend]).reshape(-1)
+        idx = live.cpu()
+        return {"blocks": hs["blocks"][live].cpu(), "tsdf": hs["tsdf"][idx], "weight": hs["weight"][idx],
+                "color": None if hs["color"] is None else hs["color"][idx]}
+
+    @property
+    def host_nbytes(self):
+        """Bytes of the pinned host store (it doubles as it fills; slots freed by returning blocks are reused)."""
+        if self._host is None:
+            return 0
+        return sum(self._host[k].numel() * self._host[k].element_size() for k in ("tsdf", "weight", "color") if self._host[k] is not None)
+
+    def _host_blocks(self):
+        return self._hend - len(self._free)
+
+    def _grow_host(self, slots, dev):
+        """Makes the host store hold `slots` slots: the smallest doubling of its capacity that does."""
+        old = self._host
+        cap = 0 if old is None else old["tsdf"].shape[0]
+        if slots <= cap:
+            return
+        new = max(cap, 1)
+        while new < slots:
+            new *= 2
+        store = {"tsdf": torch.empty((new, 8, 8, 8), dtype=torch.float32, pin_memory=True),
+                 "weight": torch.empty((new, 8, 8, 8), dtype=torch.float32, pin_memory=True),
+                 "color": torch.empty((new, 8, 8, 8, 3), dtype=torch.float32, pin_memory=True) if self._color else None,
+                 "blocks": torch.zeros((new, 3), dtype=torch.int32, device=dev), "stamp": torch.zeros((new,), dtype=torch.int32, device=dev),
+                 "live": torch.zeros((new,), dtype=torch.bool, device=dev)}
+        if old is not None:
+            torch.cuda.current_stream(dev).synchronize()   # the device has written the old store
+            for k, v in store.items():
+                if v is not None:
+                    v[:cap] = old[k]
+        self._host = store
+
+    def _reach(self, blocks, m, trunc, tiles, cams, n, h, w, out, mark):
+        Kd, Rd, td = cams
+        _lib.check(_lib.load().demon_sparse_tsdf_reach_f32(blocks.data_ptr(), m, self._origin(), float(self.voxel_size), float(trunc),
+                                                            tiles.data_ptr(), Kd.data_ptr(), Rd.data_ptr(), td.data_ptr(), n, h, w,
+                                                            out.data_ptr(), mark, _stream()))
+
+    def _bring_back(self, tiles, trunc, cams, n, h, w):
+        """A new call: stamps the device blocks its cameras reach and brings back the host blocks they reach, in key order."""
+        self._calls += 1
+        pool, dev = self._pool, self._pool["tsdf"].device
+        self._reach(pool["blocks"], self._m, trunc, tiles, cams, n, h, w, pool["stamp"], self._calls)
+        r = 0
+        if self._host_blocks():
+            hs = self._host
+            flags = torch.zeros((self._hend,), dtype=torch.int32, device=dev)
+            self._reach(hs["blocks"], self._hend, trunc, tiles, cams, n, h, w, flags, 1)
+            slots = torch.nonzero((flags > 0) & hs["live"][:self._hend]).reshape(-1)
+            r = slots.numel()
+            if r:
+                slots = slots[torch.argsort(_packed_keys(hs["blocks"][slots]))]
+                src = slots.to(torch.int32)   # named: a pointer's tensor must outlive the call
+                cap = pool["blocks"].shape[0]
+                if self._m + r > cap:
+                    while cap < self._m + r:
+                        cap *= 2
+                    pool = self._pool = self._new_pool(cap, dev)
+                keys, values, _ = self._table
+                dst = torch.arange(self._m, self._m + r, dtype=torch.int32, device=dev)
+                _lib.check(_lib.load().demon_sparse_tsdf_restore(
+                    hs["tsdf"].data_ptr(), hs["weight"].data_ptr(), None if hs["color"] is None else hs["color"].data_ptr(),
+                    hs["blocks"].data_ptr(), src.data_ptr(), dst.data_ptr(), r, pool["tsdf"].data_ptr(),
+                    pool["weight"].data_ptr(), None if pool["color"] is None else pool["color"].data_ptr(), pool["blocks"].data_ptr(),
+                    pool["stamp"].data_ptr(), self._calls, keys.data_ptr(), values.data_ptr(), keys.numel(), _stream()))
+                hs["live"][slots] = False
+                self._free = sorted(self._free + slots.tolist())
+                while self._free and self._free[-1] == self._hend - 1:
+                    self._free.pop()
+                    self._hend -= 1
+                self._m += r
+        self.last_blocks_in = r
+
+    def _stream_out(self):
+        """The end of a call: moves the device blocks beyond the budget to the host, least recently reached first (ties
+        by key), and compacts the pool in order."""
+        pool, m, dev = self._pool, self._m, self._pool["tsdf"].device
+        self.peak_device_blocks = max(self.peak_device_blocks, m)
+        e = m - self.max_device_blocks
+        self.last_blocks_out = max(e, 0)
+        if e <= 0:
+            return
+        order = torch.argsort(_packed_keys(pool["blocks"][:m]))
+        order = order[torch.sort(pool["stamp"][:m][order], stable=True).indices]
+        out = order[:e]
+        src = out.to(torch.int32)
+        reuse = min(e, len(self._free))
+        slots = self._free[:reuse] + list(range(self._hend, self._hend + e - reuse))
+        self._free = self._free[reuse:]
+        self._hend += e - reuse
+        self._grow_host(self._hend, dev)
+        hs = self._host
+        slots = torch.tensor(slots, dtype=torch.int32, device=dev)
+        keys, values, _ = self._table
+        _lib.check(_lib.load().demon_sparse_tsdf_evict(
+            pool["tsdf"].data_ptr(), pool["weight"].data_ptr(), None if pool["color"] is None else pool["color"].data_ptr(),
+            pool["blocks"].data_ptr(), pool["stamp"].data_ptr(), keys.data_ptr(), values.data_ptr(), keys.numel(),
+            src.data_ptr(), slots.data_ptr(), e, hs["tsdf"].data_ptr(), hs["weight"].data_ptr(),
+            None if hs["color"] is None else hs["color"].data_ptr(), hs["blocks"].data_ptr(), hs["stamp"].data_ptr(), _stream()))
+        hs["live"][slots.long()] = True
+        keep = torch.ones((m,), dtype=torch.bool, device=dev)
+        keep[out] = False
+        first = int(out.min())   # blocks before it keep their index
+        tail = torch.nonzero(keep[first:]).reshape(-1) + first
+        for v in pool.values():
+            if v is not None:
+                v[first:m - e] = v[tail]
+                v[m - e:m] = 0   # new blocks are committed onto zeroed slots
+        self._m = m - e
+        _lib.check(_lib.load().demon_sparse_tsdf_index(keys.data_ptr(), values.data_ptr(), keys.numel(), pool["blocks"].data_ptr(), first,
+                                                       self._m - first, _stream()))
+
     def _origin(self):
         return ctypes.cast((ctypes.c_float * 3)(*(float(v) for v in self.origin)), ctypes.c_void_p)
 
@@ -458,6 +603,11 @@ class SparseTsdfVolume:
         dev = pool["tsdf"].device
         args = (self._origin(), float(self.voxel_size), float(self.trunc), d.data_ptr(), Kd.data_ptr(), Rd.data_ptr(), td.data_ptr())
         with torch.cuda.device(dev):
+            if self.max_device_blocks is not None:
+                tiles = torch.empty((n, -(-h // 8), -(-w // 8)), dtype=torch.float32, device=dev)
+                _lib.check(lib.demon_sparse_tsdf_depth_tiles_f32(d.data_ptr(), n, h, w, tiles.data_ptr(), _stream()))
+                self._bring_back(tiles, self.trunc, (Kd, Rd, td), n, h, w)
+                pool = self._pool
             while True:
                 keys, values, counters = self._table
                 _lib.check(lib.demon_sparse_tsdf_allocate_f32(keys.data_ptr(), values.data_ptr(), keys.numel(), counters.data_ptr(),
@@ -466,7 +616,7 @@ class SparseTsdfVolume:
                 if not overflow:
                     break
                 self._table = self._rehash(2 * keys.numel(), dev)
-            new = occupied - self._m
+            new = occupied - self._m - self._host_blocks()   # the table also holds the blocks on the host
             if new:
                 fresh = torch.empty((new,), dtype=torch.int64, device=dev)
                 _lib.check(lib.demon_sparse_tsdf_gather_new(keys.data_ptr(), values.data_ptr(), keys.numel(), counters.data_ptr(),
@@ -479,17 +629,27 @@ class SparseTsdfVolume:
                     pool = self._pool = self._new_pool(cap, dev)
                 _lib.check(lib.demon_sparse_tsdf_commit(keys.data_ptr(), values.data_ptr(), keys.numel(), fresh.data_ptr(), new, self._m,
                                                         pool["blocks"].data_ptr(), _stream()))
+                if self.max_device_blocks is not None:
+                    pool["stamp"][self._m:self._m + new] = self._calls
                 self._m += new
             self.last_skipped_pixels = skipped
             _lib.check(lib.demon_sparse_tsdf_integrate_f32(
                 pool["tsdf"].data_ptr(), pool["weight"].data_ptr(), None if pool["color"] is None else pool["color"].data_ptr(),
                 pool["blocks"].data_ptr(), self._m, *args, None if im is None else im.data_ptr(), n, h, w, _stream()))
+            if self.max_device_blocks is not None:
+                self._stream_out()
         return self
 
     def mesh(self):
         """TsdfVolume.mesh on the blocks: a cube is skipped when a corner lies in a block that is not allocated or has weight
         0; the order is the block's pool index, the cube's local linear index (x fastest), then the table's.  Faces are
-        int32, so a mesh of 2^31 vertices or more raises ValueError.  Reads the triangle count back, so it synchronises."""
+        int32, so a mesh of 2^31 vertices or more raises ValueError.  Reads the triangle count back, so it synchronises.
+
+        With blocks on the host, every block is meshed: all blocks in ascending key order, max_device_blocks at a time, each
+        chunk copied with the neighbours its cubes need into a scratch pool on the device; the result is the chunk meshes
+        concatenated, faces offset.  The volume's state does not change."""
+        if self._host_blocks():
+            return self._mesh_chunks()
         pool = self._state()
         lib = _lib.load()
         dev, m = pool["tsdf"].device, self._m
@@ -515,14 +675,102 @@ class SparseTsdfVolume:
                     None if colors is None else colors.data_ptr(), faces.data_ptr(), _stream()))
         return vertices, colors, faces
 
+    def _mesh_chunks(self):
+        pool, hs, lib, m = self._pool, self._host, _lib.load(), self._m
+        dev = pool["tsdf"].device
+        out = ([], [], [])
+        with torch.cuda.device(dev):
+            slots = torch.nonzero(hs["live"][:self._hend]).reshape(-1)
+            coords = torch.cat([pool["blocks"][:m], hs["blocks"][slots]])
+            where = torch.cat([torch.arange(m, device=dev), -2 - slots])   # pool index, or -2 - host slot, as the table has it
+            keys = _packed_keys(coords)
+            order = torch.argsort(keys)
+            keys, coords, where = keys[order], coords[order], where[order]
+            total, vertices = keys.numel(), 0
+            for c0 in range(0, total, self.max_device_blocks):
+                c1 = min(total, c0 + self.max_device_blocks)
+                nk = []
+                for q in range(1, 8):   # the +x, +y, +z neighbours the chunk's cubes read
+                    step = [(q >> a) & 1 for a in range(3)]
+                    ok = ((coords[c0:c1] + torch.tensor(step, dtype=torch.int32, device=dev)) <= _MAX_COORD).all(dim=1)
+                    nk.append(keys[c0:c1][ok] + (step[0] + (step[1] << 21) + (step[2] << 42)))
+                nk = torch.unique(torch.cat(nk))
+                pos = torch.searchsorted(keys, nk).clamp_(max=total - 1)
+                pos = pos[(keys[pos] == nk) & ((pos < c0) | (pos >= c1))]
+                sel = torch.cat([torch.arange(c0, c1, device=dev), pos])
+                chunk = self._chunk_pool(coords[sel].contiguous(), where[sel])
+                v, c, f = self._mesh_range(chunk, c1 - c0)
+                if vertices + v.shape[0] >= 2 ** 31:
+                    raise ValueError("the mesh has %d or more vertices: its int32 faces cannot index them" % (vertices + v.shape[0]))
+                out[0].append(v)
+                out[1].append(c)
+                out[2].append(f + vertices)
+                vertices += v.shape[0]
+        return torch.cat(out[0]), torch.cat(out[1]) if self._color else None, torch.cat(out[2])
+
+    def _chunk_pool(self, blocks, where):
+        """A scratch pool of the blocks [t,3] (where: their pool index or -2 - host slot) with its own table."""
+        pool, hs, lib = self._pool, self._host, _lib.load()
+        dev, t = blocks.device, blocks.shape[0]
+        chunk = {"blocks": blocks, "tsdf": torch.empty((t, 8, 8, 8), dtype=torch.float32, device=dev),
+                 "weight": torch.empty((t, 8, 8, 8), dtype=torch.float32, device=dev),
+                 "color": torch.empty((t, 8, 8, 8, 3), dtype=torch.float32, device=dev) if self._color else None}
+        on = torch.nonzero(where >= 0).reshape(-1)
+        for k in ("tsdf", "weight", "color"):
+            if chunk[k] is not None:
+                chunk[k][on] = pool[k][where[on]]
+        off = torch.nonzero(where < 0).reshape(-1)
+        if off.numel():
+            src, dst = (-2 - where[off]).to(torch.int32), off.to(torch.int32)
+            _lib.check(lib.demon_sparse_tsdf_restore(
+                hs["tsdf"].data_ptr(), hs["weight"].data_ptr(), None if hs["color"] is None else hs["color"].data_ptr(), hs["blocks"].data_ptr(),
+                src.data_ptr(), dst.data_ptr(), off.numel(), chunk["tsdf"].data_ptr(),
+                chunk["weight"].data_ptr(), None if chunk["color"] is None else chunk["color"].data_ptr(), blocks.data_ptr(), None, 0, None,
+                None, 0, _stream()))
+        slots = 1024
+        while slots < 2 * t:
+            slots *= 2
+        keys = torch.empty((slots,), dtype=torch.int64, device=dev)
+        values = torch.empty((slots,), dtype=torch.int32, device=dev)
+        counters = torch.empty((4,), dtype=torch.int64, device=dev)
+        _lib.check(lib.demon_sparse_tsdf_rehash(None, None, 0, keys.data_ptr(), values.data_ptr(), slots, counters.data_ptr(), _stream()))
+        _lib.check(lib.demon_sparse_tsdf_index(keys.data_ptr(), values.data_ptr(), slots, blocks.data_ptr(), 0, t, _stream()))
+        chunk["table"] = (keys, values)
+        return chunk
+
+    def _mesh_range(self, chunk, count):
+        """The mesh of the chunk pool's first `count` blocks (demon_sparse_tsdf_mesh_range_*)."""
+        lib, t = _lib.load(), chunk["blocks"].shape[0]
+        dev = chunk["tsdf"].device
+        keys, values = chunk["table"]
+        scratch = torch.empty((lib.demon_sparse_tsdf_mesh_scratch_bytes(count),), dtype=torch.uint8, device=dev)
+        total = torch.empty((1,), dtype=torch.int64, device=dev)
+        _lib.check(lib.demon_sparse_tsdf_mesh_range_count_f32(chunk["tsdf"].data_ptr(), chunk["weight"].data_ptr(), chunk["blocks"].data_ptr(), t,
+                                                              0, count, keys.data_ptr(), values.data_ptr(), keys.numel(), scratch.data_ptr(),
+                                                              total.data_ptr(), _stream()))
+        tri = int(total.item())
+        vertices = torch.empty((3 * tri, 3), dtype=torch.float32, device=dev)
+        colors = None if chunk["color"] is None else torch.empty((3 * tri, 3), dtype=torch.uint8, device=dev)
+        faces = torch.empty((tri, 3), dtype=torch.int32, device=dev)
+        if tri:
+            _lib.check(lib.demon_sparse_tsdf_mesh_range_f32(
+                chunk["tsdf"].data_ptr(), chunk["weight"].data_ptr(), None if colors is None else chunk["color"].data_ptr(),
+                chunk["blocks"].data_ptr(), t, 0, count, self._origin(), float(self.voxel_size), scratch.data_ptr(), vertices.data_ptr(),
+                None if colors is None else colors.data_ptr(), faces.data_ptr(), _stream()))
+        return vertices, colors, faces
+
     def default_far(self, R, t):
         """CUDA float32 [n]: raycast's default far, the largest camera z of the 8 corners origin + voxel_size*(8b + (0 or 8))
-        of every allocated block b (include/demon_b200.h: demon_sparse_tsdf_far_f32), for each world-to-camera R [n,3,3]
-        (CUDA float32) and t [n,3].  The volume must hold a block."""
+        of every allocated block b, on the device or the host (include/demon_b200.h: demon_sparse_tsdf_far_f32), for each
+        world-to-camera R [n,3,3] (CUDA float32) and t [n,3].  The volume must hold a block."""
         pool = self._state()
         n = R.shape[0]
+        blocks, m = pool["blocks"], self._m
+        if self._host_blocks():
+            blocks = torch.cat([blocks[:m], self._host["blocks"][:self._hend][self._host["live"][:self._hend]]])
+            m = blocks.shape[0]
         far = torch.empty((n,), dtype=torch.float32, device=R.device)
-        _lib.check(_lib.load().demon_sparse_tsdf_far_f32(pool["blocks"].data_ptr(), self._m, self._origin(), float(self.voxel_size),
+        _lib.check(_lib.load().demon_sparse_tsdf_far_f32(blocks.data_ptr(), m, self._origin(), float(self.voxel_size),
                                                         R.data_ptr(), t.data_ptr(), n, far.data_ptr(), _stream()))
         return far
 
@@ -531,25 +779,46 @@ class SparseTsdfVolume:
         its cube's 8 corners lie in allocated blocks with weight > 0, and far defaults to the largest camera z of the
         corners of every allocated block, reduced on the device.  The march jumps over blocks that are not allocated, with
         the result of evaluating every sample.  An empty volume renders no hit without a launch.  Asynchronous on the
-        current stream."""
+        current stream, except with max_device_blocks: the host blocks its cameras reach (every tile at far, trunc 0) come
+        back first, and the blocks beyond the budget stream out after it, which synchronises."""
         rq = _Render(K, R, t, height, width, near, far, step)
         dev = self._pool["tsdf"].device if self._pool is not None else _device()
         with torch.cuda.device(dev):
             out = rq.outputs(self._color, dev)
-            if rq.n == 0 or self._m == 0:
+            if rq.n == 0 or self._m + self._host_blocks() == 0:
                 return out
-            pool, lib, m = self._pool, _lib.load(), self._m
-            keys, values, _ = self._table
             Kd, Rd, td = rq.cameras()
             nr, fr = rq.limits(dev, None if rq.far is not None else self.default_far(Rd, td))
-            scratch = torch.empty((lib.demon_sparse_tsdf_raycast_scratch_bytes(m),), dtype=torch.uint8, device=dev)
-            _lib.check(lib.demon_sparse_tsdf_raycast_f32(
-                pool["tsdf"].data_ptr(), pool["weight"].data_ptr(), None if pool["color"] is None else pool["color"].data_ptr(),
-                pool["blocks"].data_ptr(), m, keys.data_ptr(), values.data_ptr(), keys.numel(), scratch.data_ptr(), self._origin(),
-                float(self.voxel_size), Kd.data_ptr(), Rd.data_ptr(), td.data_ptr(), nr.data_ptr(), fr.data_ptr(), float(rq.step), rq.n,
-                rq.h, rq.w, out["depth"].data_ptr(), out["normals"].data_ptr(),
-                None if out["colors"] is None else out["colors"].data_ptr(), _stream()))
+            if self.max_device_blocks is not None:
+                tiles = fr[:, None, None].expand(rq.n, -(-rq.h // 8), -(-rq.w // 8)).contiguous()
+                self._bring_back(tiles, 0.0, (Kd, Rd, td), rq.n, rq.h, rq.w)
+                if self._m:
+                    self._launch_raycast(rq, Kd, Rd, td, nr, fr, out)
+                self._stream_out()
+            else:
+                self._launch_raycast(rq, Kd, Rd, td, nr, fr, out)
         return out
+
+    def _launch_raycast(self, rq, Kd, Rd, td, nr, fr, out):
+        pool, lib, m, dev = self._pool, _lib.load(), self._m, self._pool["tsdf"].device
+        keys, values, _ = self._table
+        scratch = torch.empty((lib.demon_sparse_tsdf_raycast_scratch_bytes(m),), dtype=torch.uint8, device=dev)
+        _lib.check(lib.demon_sparse_tsdf_raycast_f32(
+            pool["tsdf"].data_ptr(), pool["weight"].data_ptr(), None if pool["color"] is None else pool["color"].data_ptr(),
+            pool["blocks"].data_ptr(), m, keys.data_ptr(), values.data_ptr(), keys.numel(), scratch.data_ptr(), self._origin(),
+            float(self.voxel_size), Kd.data_ptr(), Rd.data_ptr(), td.data_ptr(), nr.data_ptr(), fr.data_ptr(), float(rq.step), rq.n,
+            rq.h, rq.w, out["depth"].data_ptr(), out["normals"].data_ptr(),
+            None if out["colors"] is None else out["colors"].data_ptr(), _stream()))
+
+
+_MAX_COORD = (1 << 20) - 1   # DEMON_SPARSE_TSDF_MAX_COORD
+
+
+def _packed_keys(blocks):
+    """int64 [m]: the table's packed key of each block [m,3] int32, 21 bits per axis offset by 2^20, z highest (fusion.cu's
+    block_key), so ascending keys are ascending (z, y, x)."""
+    b = blocks.long() + (1 << 20)
+    return (b[:, 2] << 42) | (b[:, 1] << 21) | b[:, 0]
 
 
 def volume_from_points(points, dims=(256, 256, 256), low=5.0, high=95.0, color=True):

@@ -448,6 +448,56 @@ int demon_sparse_tsdf_raycast_f32(const float* tsdf, const float* weight, const 
                                   const int* values, int64_t capacity, void* scratch, const float* origin, float voxel_size, const float* K,
                                   const float* R, const float* t, const float* near, const float* far, float step, int n, int h, int w,
                                   float* depth, float* normals, uint8_t* colors, void* stream);
+/* Marching cubes of the cubes of pool blocks first .. first+count-1 only (1 <= count, first + count <= m), their
+ * neighbours resolved among all m blocks: demon_sparse_tsdf_mesh_count_f32 and demon_sparse_tsdf_mesh_f32 are these with
+ * first = 0, count = m.  Scratch: demon_sparse_tsdf_mesh_scratch_bytes(count). */
+int demon_sparse_tsdf_mesh_range_count_f32(const float* tsdf, const float* weight, const int* blocks, int m, int first, int count,
+                                           const int64_t* keys, const int* values, int64_t capacity, void* scratch, int64_t* triangles,
+                                           void* stream);
+int demon_sparse_tsdf_mesh_range_f32(const float* tsdf, const float* weight, const float* color, const int* blocks, int m, int first,
+                                     int count, const float* origin, float voxel_size, const void* scratch, float* vertices, uint8_t* colors,
+                                     int* faces, void* stream);
+
+/* ------------------------------------------------------------------------
+ * Streaming a sparse volume's blocks between the device and pinned host memory (SparseTsdfVolume's max_device_blocks).
+ * A table value >= 0 is a pool index, -1 a block new in the running call, and -2 - s a block kept in host slot s; every
+ * entry above reads a negative value as a block that is not stored.  Host slots hold tsdf and weight [8,8,8] float32 and
+ * colour [8,8,8,3] in pinned host memory the device maps (cudaHostAlloc; checked with cudaPointerGetAttributes), and the
+ * slots' coordinates [3] int32 and stamps int32 on the device.
+ * ---------------------------------------------------------------------- */
+/* tiles [n, ceil(h/8), ceil(w/8)] float32: the largest finite depth > 0 of each 8x8 pixel tile, -inf when there is none. */
+int demon_sparse_tsdf_depth_tiles_f32(const float* depth, int n, int h, int w, float* tiles, void* stream);
+/* out[b] = mark for every one of the m blocks that some frame reaches; other entries are not written.  One thread per block
+ * and frame.  Block B reaches frame f by this rule, every step one round-to-nearest float32 operation in the order written:
+ *   1. The block's AABB widened by 3 voxels and 2 trunc: m = trunc + trunc, lo_a = (o_a + vs (float)(8 B_a - 3)) - m,
+ *      hi_a = (o_a + vs (float)(8 B_a + 10)) + m.
+ *   2. For its 8 corners X: z = ((R_20 X_0 + R_21 X_1) + R_22 X_2) + t_2, and x, y likewise with rows 0 and 1 and t_0, t_1;
+ *      zmin and zmax = the least and largest z.  A block with zmax <= vs (not > vs) is not reached.  When a corner has
+ *      z <= vs, the block is tested against every tile with zmin = 0.
+ *      Otherwise u = (fx x)/z + cx and v = (fy y)/z + cy for every corner, and the pixel rectangle is
+ *      floor(min u) - 1 .. floor(max u) + 1 by floor(min v) - 1 .. floor(max v) + 1; a rectangle outside the image does
+ *      not reach, and one inside is clipped to it.
+ *   3. The block is reached when some tile of frame f under the rectangle has tile + trunc >= zmin.
+ * With demon_sparse_tsdf_depth_tiles_f32's tiles and the integration's trunc this reaches every block holding a voxel
+ * demon_sparse_tsdf_integrate_f32 would change; with every tile set to a ray cast's far and trunc 0 it reaches every block
+ * holding a corner of a sample, normal sample or colour lookup of demon_sparse_tsdf_raycast_f32 (DESIGN.md §3.9).
+ * trunc finite and >= 0. */
+int demon_sparse_tsdf_reach_f32(const int* blocks, int m, const float* origin, float voxel_size, float trunc, const float* tiles, const float* K,
+                                const float* R, const float* t, int n, int h, int w, int* out, int mark, void* stream);
+/* One warp per block: copies pool block src[i] (tsdf, weight, colour with color) to host slot slots[i], its coordinates and
+ * stamp to host_blocks and host_stamps, and sets its table value to -2 - slots[i].  The pool is left as it was. */
+int demon_sparse_tsdf_evict(const float* tsdf, const float* weight, const float* color, const int* blocks, const int* stamps, const int64_t* keys,
+                            int* values, int64_t capacity, const int* src, const int* slots, int count, float* host_tsdf, float* host_weight,
+                            float* host_color, int* host_blocks, int* host_stamps, void* stream);
+/* One warp per block: copies host slot slots[i] to pool block dst[i] with its coordinates; with stamps, sets stamps[dst[i]]
+ * = stamp; with keys (a table), sets the block's value to dst[i].  With keys NULL it copies into any pool, such as a
+ * mesh chunk's. */
+int demon_sparse_tsdf_restore(const float* host_tsdf, const float* host_weight, const float* host_color, const int* host_blocks, const int* slots,
+                              const int* dst, int count, float* tsdf, float* weight, float* color, int* blocks, int* stamps, int stamp,
+                              const int64_t* keys, int* values, int64_t capacity, void* stream);
+/* Sets the value of every block first .. first+count-1 of blocks to its index, inserting keys the table lacks (count <
+ * capacity; a fresh table from demon_sparse_tsdf_rehash needs capacity >= 2 count to stay half empty). */
+int demon_sparse_tsdf_index(int64_t* keys, int* values, int64_t capacity, const int* blocks, int first, int count, void* stream);
 
 /* ------------------------------------------------------------------------
  * Image input (examples/example.py:15-42 resizes every image with PIL.Image.resize).
