@@ -704,26 +704,29 @@ __device__ __forceinline__ long find_slot(const unsigned long long* __restrict__
   }
 }
 
-// Inserts key unless present.  A thread takes one of the `limit` slots the table may fill before it claims an empty one, so
-// the table never holds more than `limit` keys and always has an empty slot to end a probe; false when none is left.
+// Inserts key unless present; false when the table would hold more than `limit` keys.  `occupied` counts each key once,
+// after the CAS that inserted it: counting every thread that meets an empty slot (many race on each new key) would raise
+// overflows the keys do not cause.  Slots only go from empty to full, so an empty slot on the probe means the key is
+// absent, and with `limit` keys counted already a new one overflows.  So a launch overflows exactly when the table's keys
+// and the new ones are more than `limit` = capacity/2, and the table's size follows from the key count alone.  An
+// overflowing launch may insert past `limit` before every thread sees the count, so the probe is bounded by the table's
+// size and, every 32 slots, ends once more than `limit` keys are counted (the launch has overflowed then, whatever the
+// key); the host rehashes into a doubled table before anything else reads it.  In a launch that does not overflow the
+// count never passes `limit`, so that check ends no probe.
 __device__ __forceinline__ bool insert_key(unsigned long long* keys, long mask, unsigned long long key, unsigned long long* occupied,
                                            unsigned long long limit) {
-  bool reserved = false;
-  for (long s = key_slot(key, mask);; s = (s + 1) & mask) {
+  long s = key_slot(key, mask);
+  for (long probes = 0; probes <= mask; ++probes, s = (s + 1) & mask) {
+    if ((probes & 31) == 31 && *(volatile unsigned long long*)occupied > limit) return false;
     unsigned long long k = *(volatile unsigned long long*)(keys + s);
     if (k == kEmptyKey) {
-      if (!reserved) {
-        if (atomicAdd(occupied, 1ull) >= limit) return false;
-        reserved = true;
-      }
+      if (*(volatile unsigned long long*)occupied >= limit) return false;
       k = atomicCAS(keys + s, kEmptyKey, key);
-      if (k == kEmptyKey) return true;
+      if (k == kEmptyKey) return atomicAdd(occupied, 1ull) < limit;
     }
-    if (k == key) {
-      if (reserved) atomicAdd(occupied, ~0ull);   // give the slot back
-      return true;
-    }
+    if (k == key) return true;
   }
+  return false;
 }
 
 // The world-space AABB of a pixel's band cell, point by point.

@@ -133,7 +133,10 @@ def test_chunked_calls_grow_the_pool_and_table():
         firsts.append(b.shape[0])
         caps.append(vol.capacity)
     assert caps[0] >= 4 * sequence.SparseTsdfVolume._POOL_BLOCKS and caps[1] > caps[0]
-    assert vol.table_slots > sequence.SparseTsdfVolume._TABLE_SLOTS
+    slots = sequence.SparseTsdfVolume._TABLE_SLOTS   # doubled only as the keys need: at most half full, no more
+    while slots < 2 * len(known):
+        slots *= 2
+    assert vol.table_slots == slots > sequence.SparseTsdfVolume._TABLE_SLOTS
     b = vol.blocks.cpu().numpy()
     for c in range(3):
         blk = b[firsts[c]:firsts[c + 1]]
