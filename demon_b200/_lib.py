@@ -106,6 +106,14 @@ PROTOTYPES = {
     "demon_sparse_tsdf_evict": [_P] * 7 + [c_int64, _P, _P, c_int] + [_P] * 5 + [_P],
     "demon_sparse_tsdf_restore": [_P] * 6 + [c_int] + [_P] * 5 + [c_int, _P, _P, c_int64, _P],
     "demon_sparse_tsdf_index": [_P, _P, c_int64, _P, c_int, c_int, _P],
+    "demon_tsdf_indexed_mesh_scratch_bytes": [c_int, c_int, c_int],
+    "demon_tsdf_indexed_mesh_count_f32": [_P, _P, c_int, c_int, c_int, _P, _P, _P],
+    "demon_tsdf_indexed_mesh_f32": [_P] * 3 + [c_int] * 3 + [_P, c_float] + [_P] * 6,
+    "demon_sparse_tsdf_edge_mark_f32": [_P] * 3 + [c_int] * 3 + [_P, _P, c_int64] + [_P] * 4,
+    "demon_sparse_tsdf_edge_scan_bytes": [c_int],
+    "demon_sparse_tsdf_edge_scan": [_P, c_int] + [_P] * 4,
+    "demon_sparse_tsdf_indexed_mesh_range_count_f32": [_P] * 3 + [c_int] * 3 + [_P, _P, _P, c_int64, _P, _P, _P],
+    "demon_sparse_tsdf_indexed_mesh_range_f32": [_P] * 4 + [c_int] * 3 + [_P, _P, _P, c_int64] + [_P] * 4 + [c_float] + [_P] * 6,
     "demon_net_create": [ctypes.POINTER(c_void_p), c_int, c_int, c_int, c_int],
     "demon_net_destroy": [_P],
     "demon_net_set_weight": [_P, c_char_p, _P, _P, c_int],
@@ -172,6 +180,8 @@ _RESTYPES = {
     "demon_marching_cubes_scratch_bytes": c_int64,
     "demon_sparse_tsdf_mesh_scratch_bytes": c_int64,
     "demon_sparse_tsdf_raycast_scratch_bytes": c_int64,
+    "demon_tsdf_indexed_mesh_scratch_bytes": c_int64,
+    "demon_sparse_tsdf_edge_scan_bytes": c_int64,
     "demon_last_error": c_char_p,
     "demon_version": c_char_p,
     "demon_launch_count": c_int64,

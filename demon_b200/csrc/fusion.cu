@@ -31,6 +31,8 @@ constexpr int kMcWarps = kMcThreads / 32;
 constexpr int kMcRounds = 8;
 constexpr int kMcTile = kMcThreads * kMcRounds;   // round j of thread i handles cube tile * kMcTile + j * kMcThreads + i
 constexpr int kScanThreads = 1024;
+constexpr int kSegWords = 48;   // the indexed mesh's segment of mask words: 8 * 8 * 8 voxels of 3 edges
+constexpr int kSegBits = 32 * kSegWords;
 
 // ---- TSDF integration -------------------------------------------------------------------------------------------------
 // Frame f updates voxel X = origin + voxel_size * (i, j, k):  X_c = R X + t, u = fx x/z + cx, v = fy y/z + cy, pixel
@@ -420,6 +422,7 @@ struct DenseVolume {
   long ncubes;
   struct Cube {
     int g[3];   // grid coordinate of corner 0
+    long s;     // the indexed mesh's segment: its first voxel
   };
   struct Cursor {};
   // the cube whose corner 0 is at grid coordinate c (integer-valued floats): stored when it lies inside the box
@@ -444,6 +447,29 @@ struct DenseVolume {
   __device__ long corner(const Cube& cb, int q) const {
     return ((long)(cb.g[2] + kCorner[q][2]) * ny + (cb.g[1] + kCorner[q][1])) * nx + (cb.g[0] + kCorner[q][0]);
   }
+  // indexed mesh: the bit of edge (corner q, axis a), 3 (linear index) + a
+  __device__ long edge_bit(const Cube& cb, int q, int a) const { return 3 * corner(cb, q) + a; }
+  // mask word t: its segment (512 voxels from cb.s) and the segment-local bit of its bit 0
+  __device__ int word(long t, long& w, Cube& cb) const {
+    w = t;
+    const long s = t / kSegWords;
+    cb.s = 512 * s;
+    return 32 * (int)(t - s * kSegWords);
+  }
+  // g = the segment's voxel l
+  __device__ void seg_voxel(int l, Cube& cb) const {
+    const long v = cb.s + l, plane = (long)nx * ny;
+    cb.g[2] = (int)(v / plane);
+    const long r = v - (long)cb.g[2] * plane;
+    cb.g[1] = (int)(r / nx);
+    cb.g[0] = (int)(r - (long)cb.g[1] * nx);
+  }
+  // the state index of voxel g + d, or -1 outside the box
+  __device__ long voxel(const Cube& cb, int dx, int dy, int dz) const {
+    const int x = cb.g[0] + dx, y = cb.g[1] + dy, z = cb.g[2] + dz;
+    if (x < 0 || x >= nx || y < 0 || y >= ny || z < 0 || z > cz) return -1;
+    return ((long)z * ny + y) * nx + x;
+  }
 };
 
 __device__ __forceinline__ unsigned long long block_key(int bx, int by, int bz);
@@ -462,6 +488,7 @@ struct SparseVolume {
   const int* values;
   long mask;
   int first;           // the first block of the cubes `locate` enumerates
+  const int* rank = nullptr;   // indexed mesh: the key rank of every pool block, its segment
   struct Cube {
     int b;      // pool index
     int l[3];   // local voxel of corner 0
@@ -496,12 +523,7 @@ struct SparseVolume {
   __device__ bool locate(long c, Cube& cb) const {
     if (c >= ncubes) return false;
     cb.b = first + (int)(c >> 9);
-    const int r = (int)(c & 511);
-    cb.l[0] = r & 7;
-    cb.l[1] = (r >> 3) & 7;
-    cb.l[2] = r >> 6;
-#pragma unroll
-    for (int a = 0; a < 3; ++a) cb.g[a] = 8 * __ldg(blocks + 3 * cb.b + a) + cb.l[a];
+    seg_voxel((int)(c & 511), cb);
     return true;
   }
   // the state index of corner q, or -1 when its block is not allocated
@@ -511,6 +533,58 @@ struct SparseVolume {
     const int blk = nb ? __ldg(nbr + 8L * (cb.b - first) + nb) : cb.b;
     if (blk < 0) return -1;
     return ((long)blk << 9) + ((z & 7) << 6) + ((y & 7) << 3) + (x & 7);
+  }
+  // indexed mesh: the bit of edge (corner q, axis a) of a valid cube, in the segment of the block that holds the corner
+  __device__ long edge_bit(const Cube& cb, int q, int a) const {
+    const long o = corner(cb, q);
+    return (long)__ldg(rank + (o >> 9)) * kSegBits + 3 * (o & 511) + a;
+  }
+  // mask word t of blocks first, first + 1, ...: the word of block b's segment, and the segment-local bit of its bit 0
+  __device__ int word(long t, long& w, Cube& cb) const {
+    const int k = (int)(t / kSegWords), i = (int)(t - (long)k * kSegWords);
+    cb.b = first + k;
+    w = (long)__ldg(rank + cb.b) * kSegWords + i;
+    return 32 * i;
+  }
+  // corner 0 of cube (or voxel) l of block cb.b
+  __device__ void seg_voxel(int l, Cube& cb) const {
+    cb.l[0] = l & 7;
+    cb.l[1] = (l >> 3) & 7;
+    cb.l[2] = l >> 6;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) cb.g[a] = 8 * __ldg(blocks + 3 * cb.b + a) + cb.l[a];
+  }
+  // the state index of voxel g + d (|d_i| <= 1, or d = e_a + e_i), or -1 when its block is not stored: the block itself,
+  // its + neighbours through nbr, the others through the table
+  __device__ long voxel(const Cube& cb, int dx, int dy, int dz) const {
+    const int x = cb.l[0] + dx, y = cb.l[1] + dy, z = cb.l[2] + dz;
+    const int sx = x >> 3, sy = y >> 3, sz = z >> 3;   // -1, 0 or 1
+    int blk = cb.b;
+    if (sx | sy | sz) {
+      if (sx >= 0 && sy >= 0 && sz >= 0) {
+        blk = __ldg(nbr + 8L * (cb.b - first) + (sx | (sy << 1) | (sz << 2)));
+      } else {
+        const int bx = (cb.g[0] >> 3) + sx, by = (cb.g[1] >> 3) + sy, bz = (cb.g[2] >> 3) + sz;
+        constexpr int lim = DEMON_SPARSE_TSDF_MAX_COORD;
+        if (bx < -lim || by < -lim || bz < -lim || bx > lim || by > lim || bz > lim) return -1;
+        const long s = find_slot(keys, mask, block_key(bx, by, bz));
+        blk = s < 0 ? -1 : __ldg(values + s);
+      }
+      if (blk < 0) return -1;
+    }
+    return ((long)blk << 9) + ((z & 7) << 6) + ((y & 7) << 3) + (x & 7);
+  }
+};
+
+// SparseVolume whose `locate` enumerates the blocks order[0], order[1], ... (a permutation of first .. first+count-1):
+// the indexed mesh's faces in key order.  A type of its own, so the soup's kernels do not carry the lookup.
+struct KeyOrderVolume : SparseVolume {
+  const int* order;
+  __device__ bool locate(long c, Cube& cb) const {
+    if (c >= ncubes) return false;
+    cb.b = __ldg(order + (c >> 9));
+    seg_voxel((int)(c & 511), cb);
+    return true;
   }
 };
 
@@ -583,16 +657,49 @@ __global__ void __launch_bounds__(kScanThreads) mc_offsets_kernel(const int* __r
   }
 }
 
-template <bool kColor, class V>
-__global__ void __launch_bounds__(kMcThreads) mc_scatter_kernel(V vol, const float* __restrict__ color, float ox, float oy, float oz,
-                                                                 float vs, const int64_t* __restrict__ tile_first,
-                                                                 float* __restrict__ vertices, uint8_t* __restrict__ colors_out,
-                                                                 int* __restrict__ faces) {
+// The soup's output: corner e3 of triangle tri gets its own vertex 3 tri + e3, interpolated on the edge.
+template <bool kColor>
+struct SoupOut {
+  const float* color;
+  float org[3];
+  float vs;
+  float* vertices;
+  uint8_t* colors_out;
+  int* faces;
+  template <class V>
+  __device__ __forceinline__ void operator()(const V& vol, const typename V::Cube& cb, int edge, long tri, int e3) const {
+    const int qa = kEdge[edge][0], qb = kEdge[edge][1];
+    float pa[3], pb[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      const int ia = cb.g[a] + kCorner[qa][a], ib = cb.g[a] + kCorner[qb][a];
+      pa[a] = fadd(org[a], fmul(vs, (float)ia));
+      pb[a] = fadd(org[a], fmul(vs, (float)ib));
+    }
+    const long oa = vol.corner(cb, qa), ob = vol.corner(cb, qb);
+    const float fa = __ldg(vol.tsdf + oa), fb = __ldg(vol.tsdf + ob);
+    const float mu = fdiv(fa, fsub(fa, fb));   // fa and fb lie on either side of 0, so fa - fb != 0
+    const long vtx = 3 * tri + e3;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) vertices[3 * vtx + a] = fadd(pa[a], fmul(mu, fsub(pb[a], pa[a])));
+    if (kColor) {
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        const float ca = __ldg(color + 3 * oa + a), cb = __ldg(color + 3 * ob + a);
+        const int q = __float2int_rn(fadd(ca, fmul(mu, fsub(cb, ca))));   // half to even
+        colors_out[3 * vtx + a] = (uint8_t)min(255, max(0, q));
+      }
+    }
+    faces[vtx] = (int)vtx;
+  }
+};
+
+template <class V, class Out>
+__global__ void __launch_bounds__(kMcThreads) mc_scatter_kernel(V vol, Out out, const int64_t* __restrict__ tile_first) {
   __shared__ int s_warp[kMcWarps];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const long base = (long)blockIdx.x * kMcTile + threadIdx.x;
   long row = tile_first[blockIdx.x];   // first triangle of round r in this tile
-  const float org[3] = {ox, oy, oz};
   for (int r = 0; r < kMcRounds; ++r) {
     typename V::Cube cb;
     const int ci = cube_case(vol, base + r * kMcThreads, cb);
@@ -615,36 +722,169 @@ __global__ void __launch_bounds__(kMcThreads) mc_scatter_kernel(V vol, const flo
     }
     if (cnt) {
       long tri = row + before + incl - cnt;
-      for (int m = 0; m < cnt; ++m, ++tri) {
-        for (int e3 = 0; e3 < 3; ++e3) {
-          const int edge = kTriTable[ci][3 * m + e3];
-          const int qa = kEdge[edge][0], qb = kEdge[edge][1];
-          float pa[3], pb[3];
-#pragma unroll
-          for (int a = 0; a < 3; ++a) {
-            const int ia = cb.g[a] + kCorner[qa][a], ib = cb.g[a] + kCorner[qb][a];
-            pa[a] = fadd(org[a], fmul(vs, (float)ia));
-            pb[a] = fadd(org[a], fmul(vs, (float)ib));
-          }
-          const long oa = vol.corner(cb, qa), ob = vol.corner(cb, qb);
-          const float fa = __ldg(vol.tsdf + oa), fb = __ldg(vol.tsdf + ob);
-          const float mu = fdiv(fa, fsub(fa, fb));   // fa and fb lie on either side of 0, so fa - fb != 0
-          const long vtx = 3 * tri + e3;
-#pragma unroll
-          for (int a = 0; a < 3; ++a) vertices[3 * vtx + a] = fadd(pa[a], fmul(mu, fsub(pb[a], pa[a])));
-          if (kColor) {
-#pragma unroll
-            for (int a = 0; a < 3; ++a) {
-              const float ca = __ldg(color + 3 * oa + a), cb = __ldg(color + 3 * ob + a);
-              const int q = __float2int_rn(fadd(ca, fmul(mu, fsub(cb, ca))));   // half to even
-              colors_out[3 * vtx + a] = (uint8_t)min(255, max(0, q));
-            }
-          }
-          faces[vtx] = (int)vtx;
-        }
-      }
+      for (int m = 0; m < cnt; ++m, ++tri)
+        for (int e3 = 0; e3 < 3; ++e3) out(vol, cb, kTriTable[ci][3 * m + e3], tri, e3);
     }
     row += total;
+  }
+}
+
+template <bool kColor, class V>
+void launch_soup(const V& vol, int tiles, const float* color, const float* origin, float vs, const int64_t* tile_first, float* vertices,
+                 uint8_t* colors, int* faces, cudaStream_t st) {
+  const SoupOut<kColor> out{color, {origin[0], origin[1], origin[2]}, vs, vertices, colors, faces};
+  mc_scatter_kernel<<<tiles, kMcThreads, 0, st>>>(vol, out, tile_first);
+}
+
+// ---- indexed mesh: one vertex per surface edge -------------------------------------------------------------------------
+// Edge (g, a) runs from voxel g to g + e_a.  Every edge has a bit: in a dense box bit 3 (linear index of g) + a; in a
+// sparse volume bit 1536 rank + 3 (local linear index of g) + a, rank the key rank of the block that holds g.  So both
+// storages are runs of 48-word segments (512 voxels of 3 edges), and the vertices are the set bits in ascending order.
+//   1. edge_mark_kernel: every valid cube ORs the bits of its sign-changing edges (the edges its triangles use).  The
+//      owner of a cube's edge is the cube's block or one of its +x, +y, +z neighbours; OR is order-free, so the masks
+//      depend on the volume alone.
+//   2. edge_count_kernel, mc_offsets_kernel, edge_base_kernel: each segment's popcount, their exclusive scan (the
+//      segment's first vertex), and each word's first vertex (the segment's plus the popcounts of the words before it).
+//   3. edge_vertex_kernel: one thread per word writes the vertex of each of its set bits at base[word] + popcount of the
+//      bits below it.  mc_scatter_kernel with IndexOut writes each triangle corner's edge index the same way.
+constexpr int kEdgeThreads = 256;
+__constant__ int8_t kEdgeAxis[12] = {0, 1, 0, 1, 0, 1, 0, 1, 2, 2, 2, 2};
+
+template <class V>
+__global__ void __launch_bounds__(kMcThreads) edge_mark_kernel(V vol, unsigned* __restrict__ masks) {
+  typename V::Cube cb;
+  const int ci = cube_case(vol, (long)blockIdx.x * kMcThreads + threadIdx.x, cb);
+  if (ci <= 0 || ci == 255) return;
+#pragma unroll 1
+  for (int e = 0; e < 12; ++e) {
+    const int qa = kEdge[e][0], qb = kEdge[e][1];
+    if (((ci >> qa) ^ (ci >> qb)) & 1) {
+      const long bit = vol.edge_bit(cb, qa, kEdgeAxis[e]);
+      atomicOr(masks + (bit >> 5), 1u << (bit & 31));
+    }
+  }
+}
+
+// One warp per segment: the number of its set bits.
+__global__ void __launch_bounds__(kEdgeThreads) edge_count_kernel(const unsigned* __restrict__ masks, int segs, int* __restrict__ counts) {
+  const long s = ((long)blockIdx.x * kEdgeThreads + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (s >= segs) return;
+  const unsigned* m = masks + s * kSegWords;
+  int c = __popc(m[lane]) + (lane < kSegWords - 32 ? __popc(m[32 + lane]) : 0);
+#pragma unroll
+  for (int o = 16; o; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+  if (lane == 0) counts[s] = c;
+}
+
+// One warp per segment: base[w] = the first vertex of word w (int32: the caller refuses 2^31 vertices or more).
+__global__ void __launch_bounds__(kEdgeThreads) edge_base_kernel(const unsigned* __restrict__ masks, int segs,
+                                                                 const int64_t* __restrict__ seg_first, int* __restrict__ base) {
+  const long s = ((long)blockIdx.x * kEdgeThreads + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (s >= segs) return;
+  const unsigned* m = masks + s * kSegWords;
+  const int p0 = __popc(m[lane]), p1 = lane < kSegWords - 32 ? __popc(m[32 + lane]) : 0;
+  int i0 = p0, i1 = p1;   // inclusive scans over the lanes
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y0 = __shfl_up_sync(0xffffffffu, i0, o), y1 = __shfl_up_sync(0xffffffffu, i1, o);
+    if (lane >= o) {
+      i0 += y0;
+      i1 += y1;
+    }
+  }
+  const int all0 = __shfl_sync(0xffffffffu, i0, 31);
+  const long first = seg_first[s];
+  base[s * kSegWords + lane] = (int)(first + i0 - p0);
+  if (lane < kSegWords - 32) base[s * kSegWords + 32 + lane] = (int)(first + all0 + i1 - p1);
+}
+
+// The index of the vertex of edge bit `bit`.
+__device__ __forceinline__ int edge_index(const unsigned* __restrict__ masks, const int* __restrict__ base, long bit) {
+  const long w = bit >> 5;
+  return __ldg(base + w) + __popc(__ldg(masks + w) & ((1u << (bit & 31)) - 1u));
+}
+
+// The indexed mesh's faces: corner e3 of triangle tri is the index of its edge's vertex.
+struct IndexOut {
+  const unsigned* masks;
+  const int* base;
+  int* faces;
+  template <class V>
+  __device__ __forceinline__ void operator()(const V& vol, const typename V::Cube& cb, int edge, long tri, int e3) const {
+    faces[3 * tri + e3] = edge_index(masks, base, vol.edge_bit(cb, kEdge[edge][0], kEdgeAxis[edge]));
+  }
+};
+
+// The vertex of edge (g, a) and its colour and normal, with demon_tsdf_indexed_mesh_f32's float order.  cb holds g
+// (`voxel` resolves g + d for |d_i| <= 1 and d = e_a + e_i); the edge's two voxels are stored with weight > 0.
+template <bool kColor, bool kNormals, class V>
+__device__ __forceinline__ void edge_vertex(const V& vol, const typename V::Cube& cb, int a, const float* __restrict__ color,
+                                            const float org[3], float vs, long v, float* __restrict__ vertices,
+                                            float* __restrict__ normals, uint8_t* __restrict__ colors_out) {
+  const int ea[3] = {a == 0, a == 1, a == 2};
+  const long oa = vol.voxel(cb, 0, 0, 0), ob = vol.voxel(cb, ea[0], ea[1], ea[2]);
+  const float fa = __ldg(vol.tsdf + oa), fb = __ldg(vol.tsdf + ob);
+  const float mu = fdiv(fa, fsub(fa, fb));
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const float pa = fadd(org[i], fmul(vs, (float)cb.g[i])), pb = fadd(org[i], fmul(vs, (float)(cb.g[i] + ea[i])));
+    vertices[3 * v + i] = fadd(pa, fmul(mu, fsub(pb, pa)));
+  }
+  if (kColor) {
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      const float ca = __ldg(color + 3 * oa + i), cc = __ldg(color + 3 * ob + i);
+      const int q = __float2int_rn(fadd(ca, fmul(mu, fsub(cc, ca))));
+      colors_out[3 * v + i] = (uint8_t)min(255, max(0, q));
+    }
+  }
+  if (kNormals) {
+    float n[3];
+    bool ok = true;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      float d[2];
+#pragma unroll
+      for (int p = 0; p < 2; ++p) {   // central difference along i at g, then at g + e_a
+        int hi[3] = {p * ea[0], p * ea[1], p * ea[2]}, lo[3] = {p * ea[0], p * ea[1], p * ea[2]};
+        ++hi[i];
+        --lo[i];
+        const long oh = vol.voxel(cb, hi[0], hi[1], hi[2]), ol = vol.voxel(cb, lo[0], lo[1], lo[2]);
+        ok = ok && oh >= 0 && ol >= 0 && __ldg(vol.weight + oh) > 0.0f && __ldg(vol.weight + ol) > 0.0f;
+        d[p] = ok ? fsub(__ldg(vol.tsdf + oh), __ldg(vol.tsdf + ol)) : 0.0f;
+      }
+      n[i] = fadd(d[0], fmul(mu, fsub(d[1], d[0])));
+    }
+    const float len = __fsqrt_rn(fadd(fadd(fmul(n[0], n[0]), fmul(n[1], n[1])), fmul(n[2], n[2])));
+    ok = ok && len > 0.0f;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) normals[3 * v + i] = ok ? fdiv(n[i], len) : __int_as_float(0x7fffffff);
+  }
+}
+
+// One thread per mask word of the voxels `vol.word_voxel` enumerates: the vertex of each set bit.
+template <bool kColor, bool kNormals, class V>
+__global__ void __launch_bounds__(kEdgeThreads) edge_vertex_kernel(V vol, long words, const unsigned* __restrict__ masks,
+                                                                   const int* __restrict__ base, const float* __restrict__ color, float ox,
+                                                                   float oy, float oz, float vs, float* __restrict__ vertices,
+                                                                   float* __restrict__ normals, uint8_t* __restrict__ colors_out) {
+  const long t = (long)blockIdx.x * kEdgeThreads + threadIdx.x;
+  if (t >= words) return;
+  long w;
+  typename V::Cube cb;
+  int lb0 = vol.word(t, w, cb);   // the word's global index, and the segment-local bit of its bit 0
+  unsigned bitsw = __ldg(masks + w);
+  if (!bitsw) return;
+  int v = __ldg(base + w);
+  const float org[3] = {ox, oy, oz};
+  while (bitsw) {
+    const int j = __ffs(bitsw) - 1;
+    bitsw &= bitsw - 1;
+    const int lb = lb0 + j, l = lb / 3, a = lb - 3 * l;
+    vol.seg_voxel(l, cb);
+    edge_vertex<kColor, kNormals>(vol, cb, a, color, org, vs, v++, vertices, normals, colors_out);
   }
 }
 
@@ -1327,6 +1567,99 @@ int check_frames(const char* name, const float* origin, float voxel_size, float 
 
 int64_t sparse_mc_tiles(int m) { return ((int64_t)m * 512 + kMcTile - 1) / kMcTile; }
 
+int check_range(const char* name, int m, int first, int count) {
+  DEMON_REQUIRE(m >= 1 && first >= 0 && count >= 1 && (int64_t)first + count <= m && 512LL * count * 15 < (1LL << 40),
+                "%s: bad blocks %d..%d of %d", name, first, first + count - 1, m);
+  return DEMON_OK;
+}
+
+// The neighbour table of blocks first .. first+count-1 into the sparse mesh scratch (tile_first [tiles], tile_counts
+// [tiles], nbr [count,8]); returns nbr.
+int* sparse_range_neighbours(const int* blocks, int first, int count, const int64_t* keys, const int* values, int64_t capacity, void* scratch,
+                             cudaStream_t st) {
+  const int tiles = (int)sparse_mc_tiles(count);
+  int* nbr = reinterpret_cast<int*>(static_cast<int64_t*>(scratch) + tiles) + tiles;
+  sparse_neighbours_kernel<<<(unsigned)ceil_div64(8LL * count, kSparseThreads), kSparseThreads, 0, st>>>(
+      reinterpret_cast<const unsigned long long*>(keys), values, capacity - 1, blocks, first, count, nbr);
+  return nbr;
+}
+
+// Marching cubes, step 1, on the cubes of blocks first .. first+count-1 enumerated in pool order or, with `order`, in
+// the order order[0], order[1], ... (a permutation of first .. first+count-1).
+int sparse_range_count(const char* name, const float* tsdf, const float* weight, const int* blocks, int m, int first, int count,
+                       const int* order, const int64_t* keys, const int* values, int64_t capacity, void* scratch, int64_t* triangles,
+                       cudaStream_t st) {
+  if (int rc = check_table(name, keys, values, capacity)) return rc;
+  if (int rc = check_range(name, m, first, count)) return rc;
+  DEMON_REQUIRE(tsdf && weight && blocks && scratch && triangles, "%s: null pointer", name);
+  const int tiles = (int)sparse_mc_tiles(count);
+  int64_t* tile_first = static_cast<int64_t*>(scratch);
+  int* tile_counts = reinterpret_cast<int*>(tile_first + tiles);
+  const int* nbr = sparse_range_neighbours(blocks, first, count, keys, values, capacity, scratch, st);
+  DEMON_LAUNCH_CHECK();
+  const SparseVolume vol{tsdf, weight, blocks, nbr, 512L * count, nullptr, nullptr, 0, first};
+  if (order)
+    mc_count_kernel<<<tiles, kMcThreads, 0, st>>>(KeyOrderVolume{vol, order}, tile_counts);
+  else
+    mc_count_kernel<<<tiles, kMcThreads, 0, st>>>(vol, tile_counts);
+  DEMON_LAUNCH_CHECK();
+  mc_offsets_kernel<<<1, kScanThreads, 0, st>>>(tile_counts, tiles, tile_first, triangles);
+  DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
+}
+
+// The indexed mesh, step 2: each segment's vertex count, their scan (the total into *vertices) and each word's first
+// vertex.  scratch: seg_first int64 [segs], counts int [segs].
+int edge_scan(const unsigned* masks, int segs, void* scratch, int* base, int64_t* vertices, cudaStream_t st) {
+  int64_t* seg_first = static_cast<int64_t*>(scratch);
+  int* counts = reinterpret_cast<int*>(seg_first + segs);
+  const unsigned grid = (unsigned)ceil_div64(32LL * segs, kEdgeThreads);
+  edge_count_kernel<<<grid, kEdgeThreads, 0, st>>>(masks, segs, counts);
+  DEMON_LAUNCH_CHECK();
+  mc_offsets_kernel<<<1, kScanThreads, 0, st>>>(counts, segs, seg_first, vertices);
+  DEMON_LAUNCH_CHECK();
+  edge_base_kernel<<<grid, kEdgeThreads, 0, st>>>(masks, segs, seg_first, base);
+  DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
+}
+
+template <class V>
+int launch_edge_vertices(const V& vol, long words, const unsigned* masks, const int* base, const float* color, const float* origin, float vs,
+                         float* vertices, float* normals, uint8_t* colors, cudaStream_t st) {
+  const unsigned grid = (unsigned)ceil_div64(words, kEdgeThreads);
+#define DEMON_EDGE_VERTICES(C, N)                                                                                               \
+  edge_vertex_kernel<C, N><<<grid, kEdgeThreads, 0, st>>>(vol, words, masks, base, color, origin[0], origin[1], origin[2], vs, vertices, \
+                                                          normals, colors)
+  if (color && normals) DEMON_EDGE_VERTICES(true, true);
+  else if (color) DEMON_EDGE_VERTICES(true, false);
+  else if (normals) DEMON_EDGE_VERTICES(false, true);
+  else DEMON_EDGE_VERTICES(false, false);
+#undef DEMON_EDGE_VERTICES
+  DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
+}
+
+// The dense indexed mesh's segments (512 voxels each) and its scratch: tile_first int64 [tiles], seg_first int64 [segs],
+// seg counts int [segs], tile_counts int [tiles], masks [segs,48], base [segs,48].
+long dense_segs(int nx, int ny, int nz) { return ((long)nx * ny * nz + 511) / 512; }
+
+struct DenseEdgeScratch {
+  int64_t* tile_first;
+  int* tile_counts;
+  void* scan;   // seg_first, then the counts
+  unsigned* masks;
+  int* base;
+  DenseEdgeScratch(void* scratch, int tiles, long segs) {
+    tile_first = static_cast<int64_t*>(scratch);
+    int64_t* seg_first = tile_first + tiles;
+    scan = seg_first;
+    // edge_scan's counts follow seg_first; tile_counts follow those
+    tile_counts = reinterpret_cast<int*>(seg_first + segs) + segs;
+    masks = reinterpret_cast<unsigned*>(tile_counts + tiles);
+    base = reinterpret_cast<int*>(masks + segs * kSegWords);
+  }
+};
+
 }  // namespace
 }  // namespace demon
 
@@ -1387,11 +1720,9 @@ int demon_marching_cubes_f32(const float* tsdf, const float* weight, const float
   const DenseVolume vol = make_volume(tsdf, weight, nx, ny, nz);
   const int64_t* tile_first = static_cast<const int64_t*>(scratch);
   if (color)
-    mc_scatter_kernel<true><<<tiles, kMcThreads, 0, (cudaStream_t)stream>>>(vol, color, origin[0], origin[1], origin[2], voxel_size,
-                                                                           tile_first, vertices, colors, faces);
+    launch_soup<true>(vol, tiles, color, origin, voxel_size, tile_first, vertices, colors, faces, (cudaStream_t)stream);
   else
-    mc_scatter_kernel<false><<<tiles, kMcThreads, 0, (cudaStream_t)stream>>>(vol, nullptr, origin[0], origin[1], origin[2], voxel_size,
-                                                                            tile_first, vertices, nullptr, faces);
+    launch_soup<false>(vol, tiles, nullptr, origin, voxel_size, tile_first, vertices, nullptr, faces, (cudaStream_t)stream);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
 }
@@ -1483,24 +1814,8 @@ int64_t demon_sparse_tsdf_mesh_scratch_bytes(int m) {
 int demon_sparse_tsdf_mesh_range_count_f32(const float* tsdf, const float* weight, const int* blocks, int m, int first, int count,
                                            const int64_t* keys, const int* values, int64_t capacity, void* scratch, int64_t* triangles,
                                            void* stream) {
-  if (int rc = check_table("sparse_tsdf_mesh_count", keys, values, capacity)) return rc;
-  DEMON_REQUIRE(m >= 1 && first >= 0 && count >= 1 && (int64_t)first + count <= m && 512LL * count * 15 < (1LL << 40),
-                "sparse_tsdf_mesh_count: bad blocks %d..%d of %d", first, first + count - 1, m);
-  DEMON_REQUIRE(tsdf && weight && blocks && scratch && triangles, "sparse_tsdf_mesh_count: null pointer");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int tiles = (int)sparse_mc_tiles(count);
-  int64_t* tile_first = static_cast<int64_t*>(scratch);   // scratch: tile_first [tiles], tile_counts [tiles], nbr [count,8]
-  int* tile_counts = reinterpret_cast<int*>(tile_first + tiles);
-  int* nbr = tile_counts + tiles;
-  sparse_neighbours_kernel<<<(unsigned)ceil_div64(8LL * count, kSparseThreads), kSparseThreads, 0, st>>>(
-      reinterpret_cast<const unsigned long long*>(keys), values, capacity - 1, blocks, first, count, nbr);
-  DEMON_LAUNCH_CHECK();
-  const SparseVolume vol{tsdf, weight, blocks, nbr, 512L * count, nullptr, nullptr, 0, first};
-  mc_count_kernel<<<tiles, kMcThreads, 0, st>>>(vol, tile_counts);
-  DEMON_LAUNCH_CHECK();
-  mc_offsets_kernel<<<1, kScanThreads, 0, st>>>(tile_counts, tiles, tile_first, triangles);
-  DEMON_LAUNCH_CHECK();
-  return DEMON_OK;
+  return sparse_range_count("sparse_tsdf_mesh_count", tsdf, weight, blocks, m, first, count, nullptr, keys, values, capacity, scratch,
+                            triangles, (cudaStream_t)stream);
 }
 
 int demon_sparse_tsdf_mesh_range_f32(const float* tsdf, const float* weight, const float* color, const int* blocks, int m, int first,
@@ -1516,11 +1831,9 @@ int demon_sparse_tsdf_mesh_range_f32(const float* tsdf, const float* weight, con
   const int* nbr = reinterpret_cast<const int*>(tile_first + tiles) + tiles;
   const SparseVolume vol{tsdf, weight, blocks, nbr, 512L * count, nullptr, nullptr, 0, first};
   if (color)
-    mc_scatter_kernel<true><<<tiles, kMcThreads, 0, (cudaStream_t)stream>>>(vol, color, origin[0], origin[1], origin[2], voxel_size,
-                                                                           tile_first, vertices, colors, faces);
+    launch_soup<true>(vol, tiles, color, origin, voxel_size, tile_first, vertices, colors, faces, (cudaStream_t)stream);
   else
-    mc_scatter_kernel<false><<<tiles, kMcThreads, 0, (cudaStream_t)stream>>>(vol, nullptr, origin[0], origin[1], origin[2], voxel_size,
-                                                                            tile_first, vertices, nullptr, faces);
+    launch_soup<false>(vol, tiles, nullptr, origin, voxel_size, tile_first, vertices, nullptr, faces, (cudaStream_t)stream);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
 }
@@ -1665,6 +1978,113 @@ int demon_sparse_tsdf_index(int64_t* keys, int* values, int64_t capacity, const 
   sparse_index_kernel<<<ceil_div(count, kSparseThreads), kSparseThreads, 0, (cudaStream_t)stream>>>(
       reinterpret_cast<unsigned long long*>(keys), values, capacity - 1, blocks, first, count);
   DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
+}
+
+int64_t demon_tsdf_indexed_mesh_scratch_bytes(int nx, int ny, int nz) {
+  if (check_volume("tsdf_indexed_mesh_scratch_bytes", nx, ny, nz)) return 0;
+  const long segs = dense_segs(nx, ny, nz);
+  return mc_tiles(nx, ny, nz) * (int64_t)(sizeof(int64_t) + sizeof(int)) + segs * (int64_t)(sizeof(int64_t) + sizeof(int)) +
+         segs * kSegWords * (int64_t)(sizeof(unsigned) + sizeof(int));
+}
+
+int demon_tsdf_indexed_mesh_count_f32(const float* tsdf, const float* weight, int nx, int ny, int nz, void* scratch, int64_t* counts,
+                                      void* stream) {
+  if (int rc = check_volume("tsdf_indexed_mesh_count", nx, ny, nz)) return rc;
+  DEMON_REQUIRE(tsdf && weight && scratch && counts, "tsdf_indexed_mesh_count: null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int tiles = (int)mc_tiles(nx, ny, nz);
+  const long segs = dense_segs(nx, ny, nz);
+  const DenseEdgeScratch sc(scratch, tiles, segs);
+  const DenseVolume vol = make_volume(tsdf, weight, nx, ny, nz);
+  DEMON_CHECK_CUDA(cudaMemsetAsync(sc.masks, 0, segs * kSegWords * sizeof(unsigned), st));
+  edge_mark_kernel<<<(unsigned)ceil_div64(vol.ncubes, kMcThreads), kMcThreads, 0, st>>>(vol, sc.masks);
+  DEMON_LAUNCH_CHECK();
+  if (int rc = edge_scan(sc.masks, (int)segs, sc.scan, sc.base, counts, st)) return rc;
+  mc_count_kernel<<<tiles, kMcThreads, 0, st>>>(vol, sc.tile_counts);
+  DEMON_LAUNCH_CHECK();
+  mc_offsets_kernel<<<1, kScanThreads, 0, st>>>(sc.tile_counts, tiles, sc.tile_first, counts + 1);
+  DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
+}
+
+int demon_tsdf_indexed_mesh_f32(const float* tsdf, const float* weight, const float* color, int nx, int ny, int nz, const float* origin,
+                                float voxel_size, const void* scratch, float* vertices, float* normals, uint8_t* colors, int* faces,
+                                void* stream) {
+  if (int rc = check_volume("tsdf_indexed_mesh", nx, ny, nz)) return rc;
+  DEMON_REQUIRE(origin && std::isfinite(voxel_size) && voxel_size > 0.0f, "tsdf_indexed_mesh: bad origin or voxel_size %g", voxel_size);
+  DEMON_REQUIRE(!color == !colors, "tsdf_indexed_mesh: color and colors go together");
+  DEMON_REQUIRE(tsdf && weight && scratch && vertices && faces, "tsdf_indexed_mesh: null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int tiles = (int)mc_tiles(nx, ny, nz);
+  const long segs = dense_segs(nx, ny, nz);
+  const DenseEdgeScratch sc(const_cast<void*>(scratch), tiles, segs);
+  const DenseVolume vol = make_volume(tsdf, weight, nx, ny, nz);
+  if (int rc = launch_edge_vertices(vol, segs * kSegWords, sc.masks, sc.base, color, origin, voxel_size, vertices, normals, colors, st))
+    return rc;
+  mc_scatter_kernel<<<tiles, kMcThreads, 0, st>>>(vol, IndexOut{sc.masks, sc.base, faces}, sc.tile_first);
+  DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
+}
+
+int64_t demon_sparse_tsdf_edge_scan_bytes(int blocks) { return blocks < 1 ? 0 : (int64_t)blocks * (int64_t)(sizeof(int64_t) + sizeof(int)); }
+
+int demon_sparse_tsdf_edge_mark_f32(const float* tsdf, const float* weight, const int* blocks, int m, int first, int count, const int64_t* keys,
+                                    const int* values, int64_t capacity, const int* rank, void* scratch, uint32_t* masks, void* stream) {
+  if (int rc = check_table("sparse_tsdf_edge_mark", keys, values, capacity)) return rc;
+  if (int rc = check_range("sparse_tsdf_edge_mark", m, first, count)) return rc;
+  DEMON_REQUIRE(tsdf && weight && blocks && rank && scratch && masks, "sparse_tsdf_edge_mark: null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int* nbr = sparse_range_neighbours(blocks, first, count, keys, values, capacity, scratch, st);
+  DEMON_LAUNCH_CHECK();
+  SparseVolume vol{tsdf, weight, blocks, nbr, 512L * count, nullptr, nullptr, 0, first};
+  vol.rank = rank;
+  edge_mark_kernel<<<(unsigned)ceil_div64(vol.ncubes, kMcThreads), kMcThreads, 0, st>>>(vol, masks);
+  DEMON_LAUNCH_CHECK();
+  return DEMON_OK;
+}
+
+int demon_sparse_tsdf_edge_scan(const uint32_t* masks, int blocks, void* scratch, int* base, int64_t* vertices, void* stream) {
+  DEMON_REQUIRE(blocks >= 1, "sparse_tsdf_edge_scan: bad block count %d", blocks);
+  DEMON_REQUIRE(masks && scratch && base && vertices, "sparse_tsdf_edge_scan: null pointer");
+  return edge_scan(masks, blocks, scratch, base, vertices, (cudaStream_t)stream);
+}
+
+int demon_sparse_tsdf_indexed_mesh_range_count_f32(const float* tsdf, const float* weight, const int* blocks, int m, int first, int count,
+                                                   const int* order, const int64_t* keys, const int* values, int64_t capacity, void* scratch,
+                                                   int64_t* triangles, void* stream) {
+  return sparse_range_count("sparse_tsdf_indexed_mesh_count", tsdf, weight, blocks, m, first, count, order, keys, values, capacity, scratch,
+                            triangles, (cudaStream_t)stream);
+}
+
+int demon_sparse_tsdf_indexed_mesh_range_f32(const float* tsdf, const float* weight, const float* color, const int* blocks, int m, int first,
+                                             int count, const int* order, const int64_t* keys, const int* values, int64_t capacity,
+                                             const int* rank, const uint32_t* masks, const int* base, const float* origin, float voxel_size,
+                                             const void* scratch, float* vertices, float* normals, uint8_t* colors, int* faces,
+                                             void* stream) {
+  if (int rc = check_table("sparse_tsdf_indexed_mesh", keys, values, capacity)) return rc;
+  if (int rc = check_range("sparse_tsdf_indexed_mesh", m, first, count)) return rc;
+  DEMON_REQUIRE(origin && std::isfinite(voxel_size) && voxel_size > 0.0f, "sparse_tsdf_indexed_mesh: bad origin or voxel_size %g", voxel_size);
+  DEMON_REQUIRE(!color == !colors, "sparse_tsdf_indexed_mesh: color and colors go together");
+  DEMON_REQUIRE(tsdf && weight && blocks && rank && masks && base && scratch, "sparse_tsdf_indexed_mesh: null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int tiles = (int)sparse_mc_tiles(count);
+  const int64_t* tile_first = static_cast<const int64_t*>(scratch);
+  const int* nbr = reinterpret_cast<const int*>(tile_first + tiles) + tiles;
+  SparseVolume vol{tsdf, weight, blocks, nbr, 512L * count, reinterpret_cast<const unsigned long long*>(keys), values, (long)capacity - 1,
+                   first};
+  vol.rank = rank;
+  if (vertices) {
+    if (int rc = launch_edge_vertices(vol, (long)kSegWords * count, masks, base, color, origin, voxel_size, vertices, normals, colors, st))
+      return rc;
+  }
+  if (faces) {
+    if (order)
+      mc_scatter_kernel<<<tiles, kMcThreads, 0, st>>>(KeyOrderVolume{vol, order}, IndexOut{masks, base, faces}, tile_first);
+    else
+      mc_scatter_kernel<<<tiles, kMcThreads, 0, st>>>(vol, IndexOut{masks, base, faces}, tile_first);
+    DEMON_LAUNCH_CHECK();
+  }
   return DEMON_OK;
 }
 

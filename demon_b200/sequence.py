@@ -254,6 +254,25 @@ def _far_of_corners(X, Rd, td):
     return z.amax(dim=1)
 
 
+def _check_normals(normals):
+    if not isinstance(normals, (bool, np.bool_)):
+        raise ValueError("normals must be True or False, got %r" % (normals,))
+
+
+def _ptr(t):
+    return None if t is None else t.data_ptr()
+
+
+def _indexed_outputs(nv, tri, normals, color, dev):
+    """The empty CUDA outputs of an indexed mesh of nv vertices and tri triangles; ValueError past int32 indices."""
+    if nv >= 2 ** 31:
+        raise ValueError("the mesh has %d vertices: its int32 faces cannot index them" % nv)
+    return {"vertices": torch.empty((nv, 3), dtype=torch.float32, device=dev),
+            "normals": torch.empty((nv, 3), dtype=torch.float32, device=dev) if normals else None,
+            "colors": torch.empty((nv, 3), dtype=torch.uint8, device=dev) if color else None,
+            "faces": torch.empty((tri, 3), dtype=torch.int32, device=dev)}
+
+
 class TsdfVolume:
     """A truncated signed distance volume on the device (include/demon_b200.h: demon_tsdf_integrate_f32): dims (nx, ny, nz)
     voxels, voxel (i,j,k) at origin + voxel_size*(i,j,k), truncation `trunc` (default 3 voxels), and a colour average with
@@ -314,6 +333,32 @@ class TsdfVolume:
                     ctypes.cast(self._origin(), ctypes.c_void_p), float(self.voxel_size), scratch.data_ptr(), vertices.data_ptr(),
                     None if colors is None else colors.data_ptr(), faces.data_ptr(), _stream()))
         return vertices, colors, faces
+
+    def indexed_mesh(self, normals=True):
+        """The zero surface as an indexed mesh (include/demon_b200.h: demon_tsdf_indexed_mesh_f32): one vertex per edge
+        that a meshed cube's triangles use, in ascending 3 (linear voxel index) + axis, at the soup's position and colour
+        bit for bit; faces are mesh()'s triangles in its order, each corner the index of its edge's vertex, so
+        vertices[faces] is mesh()'s vertices.  Returns a dict of CUDA tensors: vertices [V,3] float32, normals [V,3] float32
+        (unit, towards free space; NaN where a voxel the central differences read is not stored; None with
+        normals=False), colors [V,3] uint8 (None without colour), faces [T,3] int32.  Reads the counts back, so it
+        synchronises."""
+        _check_normals(normals)
+        lib = _lib.load()
+        nx, ny, nz = self.dims
+        dev = self.tsdf.device
+        with torch.cuda.device(dev):
+            scratch = torch.empty((lib.demon_tsdf_indexed_mesh_scratch_bytes(nx, ny, nz),), dtype=torch.uint8, device=dev)
+            counts = torch.empty((2,), dtype=torch.int64, device=dev)
+            _lib.check(lib.demon_tsdf_indexed_mesh_count_f32(self.tsdf.data_ptr(), self.weight.data_ptr(), nx, ny, nz, scratch.data_ptr(),
+                                                             counts.data_ptr(), _stream()))
+            nv, tri = counts.tolist()
+            out = _indexed_outputs(nv, tri, normals, self.color is not None, dev)
+            if nv:
+                _lib.check(lib.demon_tsdf_indexed_mesh_f32(
+                    self.tsdf.data_ptr(), self.weight.data_ptr(), None if self.color is None else self.color.data_ptr(), nx, ny, nz,
+                    ctypes.cast(self._origin(), ctypes.c_void_p), float(self.voxel_size), scratch.data_ptr(), out["vertices"].data_ptr(),
+                    _ptr(out["normals"]), _ptr(out["colors"]), out["faces"].data_ptr(), _stream()))
+        return out
 
     def default_far(self, R, t):
         """CUDA float32 [n]: raycast's default far, the largest camera z of the box's 8 corners for each world-to-camera
@@ -675,29 +720,42 @@ class SparseTsdfVolume:
                     None if colors is None else colors.data_ptr(), faces.data_ptr(), _stream()))
         return vertices, colors, faces
 
-    def _mesh_chunks(self):
-        pool, hs, lib, m = self._pool, self._host, _lib.load(), self._m
+    def _blocks_by_key(self):
+        """Every block, on the device or the host, in ascending key order: packed keys [B] int64, coordinates [B,3] and
+        where each is (its pool index, or -2 - host slot, as the table has it)."""
+        pool, hs, m = self._pool, self._host, self._m
         dev = pool["tsdf"].device
+        slots = torch.nonzero(hs["live"][:self._hend]).reshape(-1)
+        coords = torch.cat([pool["blocks"][:m], hs["blocks"][slots]])
+        where = torch.cat([torch.arange(m, device=dev), -2 - slots])
+        keys = _packed_keys(coords)
+        order = torch.argsort(keys)
+        return keys[order], coords[order], where[order]
+
+    @staticmethod
+    def _chunk_selection(keys, coords, c0, c1, steps):
+        """The key ranks of blocks c0 .. c1-1 of the key-ordered blocks, then those of their neighbours at `steps` that
+        exist outside the chunk, ascending."""
+        dev, total = keys.device, keys.numel()
+        nk = []
+        for step in steps:
+            st = torch.tensor(step, dtype=torch.int32, device=dev)
+            ok = ((coords[c0:c1] + st) <= _MAX_COORD).all(dim=1) & ((coords[c0:c1] + st) >= -_MAX_COORD).all(dim=1)
+            nk.append(keys[c0:c1][ok] + (step[0] + (step[1] << 21) + (step[2] << 42)))
+        nk = torch.unique(torch.cat(nk))
+        pos = torch.searchsorted(keys, nk).clamp_(max=total - 1)
+        pos = pos[(keys[pos] == nk) & ((pos < c0) | (pos >= c1))]
+        return torch.cat([torch.arange(c0, c1, device=dev), pos])
+
+    def _mesh_chunks(self):
+        dev = self._pool["tsdf"].device
         out = ([], [], [])
         with torch.cuda.device(dev):
-            slots = torch.nonzero(hs["live"][:self._hend]).reshape(-1)
-            coords = torch.cat([pool["blocks"][:m], hs["blocks"][slots]])
-            where = torch.cat([torch.arange(m, device=dev), -2 - slots])   # pool index, or -2 - host slot, as the table has it
-            keys = _packed_keys(coords)
-            order = torch.argsort(keys)
-            keys, coords, where = keys[order], coords[order], where[order]
+            keys, coords, where = self._blocks_by_key()
             total, vertices = keys.numel(), 0
             for c0 in range(0, total, self.max_device_blocks):
                 c1 = min(total, c0 + self.max_device_blocks)
-                nk = []
-                for q in range(1, 8):   # the +x, +y, +z neighbours the chunk's cubes read
-                    step = [(q >> a) & 1 for a in range(3)]
-                    ok = ((coords[c0:c1] + torch.tensor(step, dtype=torch.int32, device=dev)) <= _MAX_COORD).all(dim=1)
-                    nk.append(keys[c0:c1][ok] + (step[0] + (step[1] << 21) + (step[2] << 42)))
-                nk = torch.unique(torch.cat(nk))
-                pos = torch.searchsorted(keys, nk).clamp_(max=total - 1)
-                pos = pos[(keys[pos] == nk) & ((pos < c0) | (pos >= c1))]
-                sel = torch.cat([torch.arange(c0, c1, device=dev), pos])
+                sel = self._chunk_selection(keys, coords, c0, c1, _PLUS_STEPS)   # the neighbours the chunk's cubes read
                 chunk = self._chunk_pool(coords[sel].contiguous(), where[sel])
                 v, c, f = self._mesh_range(chunk, c1 - c0)
                 if vertices + v.shape[0] >= 2 ** 31:
@@ -759,6 +817,77 @@ class SparseTsdfVolume:
                 None if colors is None else colors.data_ptr(), faces.data_ptr(), _stream()))
         return vertices, colors, faces
 
+    def indexed_mesh(self, normals=True):
+        """TsdfVolume.indexed_mesh on the blocks (include/demon_b200.h: demon_sparse_tsdf_indexed_mesh_range_f32): one
+        vertex per edge a meshed cube's triangles use, in ascending (packed key of the block holding the edge's first
+        voxel, its local linear index, axis); faces are mesh()'s triangles moved into ascending block key, then the cube's
+        local index and the table's order.  The result depends on the stored voxels alone, not on the pool's layout or
+        max_device_blocks.  Returns TsdfVolume.indexed_mesh's dict; synchronises.
+
+        With blocks on the host it runs twice over mesh()'s key-ordered chunks of max_device_blocks blocks, each copied
+        with its 26 neighbours into a scratch pool: the first pass marks the edges, a scan over all blocks gives every
+        block its first vertex, and the second writes the chunk's vertices and faces.  The edge masks cover every block
+        (384 bytes per block on the device).  The volume's state does not change."""
+        _check_normals(normals)
+        if self._pool is None or self._m + self._host_blocks() == 0:
+            return _indexed_outputs(0, 0, normals, self._color, self._pool["tsdf"].device if self._pool is not None else _device())
+        dev = self._pool["tsdf"].device
+        with torch.cuda.device(dev):
+            if self._host_blocks():
+                keys, coords, where = self._blocks_by_key()
+                total = keys.numel()
+
+                def chunks():
+                    for c0 in range(0, total, self.max_device_blocks):
+                        c1 = min(total, c0 + self.max_device_blocks)
+                        sel = self._chunk_selection(keys, coords, c0, c1, _ALL_STEPS)
+                        yield self._chunk_pool(coords[sel].contiguous(), where[sel]), c1 - c0, sel.to(torch.int32), None
+                return self._indexed(normals, chunks, total)
+            pool, m = self._pool, self._m
+            order = torch.argsort(_packed_keys(pool["blocks"][:m]))
+            rank = torch.empty_like(order)
+            rank[order] = torch.arange(m, device=dev)
+            whole = dict(pool, table=self._table[:2])
+            return self._indexed(normals, lambda: [(whole, m, rank.to(torch.int32), order.to(torch.int32))], m)
+
+    def _indexed(self, normals, chunks, total):
+        """The indexed mesh of `total` blocks from two passes over chunks(), which yields (pool, count, rank, order): a pool
+        with its table whose first count blocks are the chunk, the key rank of every pool block, and the key order of the
+        chunk's blocks (None: already in key order)."""
+        lib, dev = _lib.load(), self._pool["tsdf"].device
+        masks = torch.zeros((total, 48), dtype=torch.int32, device=dev)
+        for pool, count, rank, _ in chunks():
+            keys, values = pool["table"]
+            scratch = torch.empty((lib.demon_sparse_tsdf_mesh_scratch_bytes(count),), dtype=torch.uint8, device=dev)
+            _lib.check(lib.demon_sparse_tsdf_edge_mark_f32(pool["tsdf"].data_ptr(), pool["weight"].data_ptr(), pool["blocks"].data_ptr(),
+                                                           pool["blocks"].shape[0], 0, count, keys.data_ptr(), values.data_ptr(),
+                                                           keys.numel(), rank.data_ptr(), scratch.data_ptr(), masks.data_ptr(), _stream()))
+        base = torch.empty((total, 48), dtype=torch.int32, device=dev)
+        scan = torch.empty((lib.demon_sparse_tsdf_edge_scan_bytes(total),), dtype=torch.uint8, device=dev)
+        nv = torch.empty((1,), dtype=torch.int64, device=dev)
+        _lib.check(lib.demon_sparse_tsdf_edge_scan(masks.data_ptr(), total, scan.data_ptr(), base.data_ptr(), nv.data_ptr(), _stream()))
+        out = _indexed_outputs(int(nv.item()), 0, normals, self._color, dev)
+        if out["vertices"].shape[0] == 0:   # no vertex, no triangle
+            return out
+        faces = []
+        for pool, count, rank, order in chunks():
+            keys, values = pool["table"]
+            t = pool["blocks"].shape[0]
+            scratch = torch.empty((lib.demon_sparse_tsdf_mesh_scratch_bytes(count),), dtype=torch.uint8, device=dev)
+            tri = torch.empty((1,), dtype=torch.int64, device=dev)
+            _lib.check(lib.demon_sparse_tsdf_indexed_mesh_range_count_f32(
+                pool["tsdf"].data_ptr(), pool["weight"].data_ptr(), pool["blocks"].data_ptr(), t, 0, count, _ptr(order), keys.data_ptr(),
+                values.data_ptr(), keys.numel(), scratch.data_ptr(), tri.data_ptr(), _stream()))
+            f = torch.empty((int(tri.item()), 3), dtype=torch.int32, device=dev)
+            _lib.check(lib.demon_sparse_tsdf_indexed_mesh_range_f32(
+                pool["tsdf"].data_ptr(), pool["weight"].data_ptr(), None if out["colors"] is None else pool["color"].data_ptr(),
+                pool["blocks"].data_ptr(), t, 0, count, _ptr(order), keys.data_ptr(), values.data_ptr(), keys.numel(), rank.data_ptr(),
+                masks.data_ptr(), base.data_ptr(), self._origin(), float(self.voxel_size), scratch.data_ptr(), out["vertices"].data_ptr(),
+                _ptr(out["normals"]), _ptr(out["colors"]), f.data_ptr() if f.shape[0] else None, _stream()))
+            faces.append(f)
+        out["faces"] = torch.cat(faces)
+        return out
+
     def default_far(self, R, t):
         """CUDA float32 [n]: raycast's default far, the largest camera z of the 8 corners origin + voxel_size*(8b + (0 or 8))
         of every allocated block b, on the device or the host (include/demon_b200.h: demon_sparse_tsdf_far_f32), for each
@@ -812,6 +941,8 @@ class SparseTsdfVolume:
 
 
 _MAX_COORD = (1 << 20) - 1   # DEMON_SPARSE_TSDF_MAX_COORD
+_PLUS_STEPS = [[(q >> a) & 1 for a in range(3)] for q in range(1, 8)]   # the +x, +y, +z neighbours of a block
+_ALL_STEPS = [[dx, dy, dz] for dz in (-1, 0, 1) for dy in (-1, 0, 1) for dx in (-1, 0, 1) if dx or dy or dz]
 
 
 def _packed_keys(blocks):
@@ -837,7 +968,7 @@ def volume_from_points(points, dims=(256, 256, 256), low=5.0, high=95.0, color=T
     return TsdfVolume(n, lo, vs, color=color)
 
 
-def reconstruct(pipeline, frames, intrinsics, volume=None, resample="bicubic", min_ratios=1000):
+def reconstruct(pipeline, frames, intrinsics, volume=None, resample="bicubic", min_ratios=1000, indexed_mesh=False):
     """A video end to end: frames CUDA uint8 [T,H,W,3] (T >= 2, HWC RGB) with their intrinsics in pixels ([3,3], [T,3,3] or
     [T,4], as images.adjust_intrinsics takes them).  Every frame is adapted once to DeMoN's camera at 256x192
     (images.adjust_intrinsics), and its 64x48 image2_2 resized from the adapted frame with `resample`, as forward_views makes
@@ -848,7 +979,10 @@ def reconstruct(pipeline, frames, intrinsics, volume=None, resample="bicubic", m
 
     Returns a dict: chain_pairs' scales, sigma, R, t and depth, inverse_depth / rotation / translation [P,...] of the pairs,
     the adapted frames [T,192,256,3] and their status (images.adjust_intrinsics), K [3,3] of the adapted frames in pixels,
-    volume, and the mesh: vertices, colors, faces."""
+    volume, and the mesh: vertices, colors, faces.  With indexed_mesh=True the mesh is volume.indexed_mesh()'s (shared
+    vertices, and a `normals` key) instead of the soup."""
+    if not isinstance(indexed_mesh, (bool, np.bool_)):
+        raise ValueError("indexed_mesh must be True or False, got %r" % (indexed_mesh,))
     if not (isinstance(frames, torch.Tensor) and frames.dim() == 4 and frames.shape[0] >= 2):
         raise ValueError("frames: expected a CUDA uint8 tensor [T,H,W,3] with T >= 2, got %s" % (_shape(frames),))
     if volume is not None and not isinstance(volume, (TsdfVolume, SparseTsdfVolume)):
@@ -878,17 +1012,21 @@ def reconstruct(pipeline, frames, intrinsics, volume=None, resample="bicubic", m
         valid = torch.arange(h * w, device=dev)[None, :] < pc["counts"][:, None].long()
         volume = volume_from_points(pc["points"][valid])
     volume.integrate(ch["depth"], K, R32, t32, adapted[:p] if volume.color is not None else None)
-    vertices, colors, faces = volume.mesh()
-    return dict(ch, inverse_depth=inv, rotation=rot, translation=trans, adapted=adapted, status=status, K=K_new, volume=volume,
-                vertices=vertices, colors=colors, faces=faces)
+    res = dict(ch, inverse_depth=inv, rotation=rot, translation=trans, adapted=adapted, status=status, K=K_new, volume=volume)
+    if indexed_mesh:
+        res.update(volume.indexed_mesh())
+    else:
+        res["vertices"], res["colors"], res["faces"] = volume.mesh()
+    return res
 
 
 def export_sequence_to_ply(prefix, result):
-    """Writes prefix + '_mesh.ply' (the coloured mesh of `result`) and prefix + '_cameras.ply' (vis.camera_mesh of every
+    """Writes prefix + '_mesh.ply' (the coloured mesh of `result`, with its normals when it has them) and prefix + '_cameras.ply' (vis.camera_mesh of every
     pose of result['R'] / result['t'], one mesh), in vis.write_ply's format."""
     col = result.get("colors")
+    nrm = result.get("normals")
     vis.write_ply(prefix + "_mesh.ply", result["vertices"].cpu().numpy(), None if col is None else col.cpu().numpy(),
-                  result["faces"].cpu().numpy())
+                  result["faces"].cpu().numpy(), None if nrm is None else nrm.cpu().numpy())
     verts, faces = [], []
     for k, (R, t) in enumerate(zip(result["R"], result["t"])):
         v, f = vis.camera_mesh(R, t)

@@ -199,9 +199,9 @@ def camera_mesh(R, t):
     return (0.25 * CAMERA_POINTS - np.asarray(t)).dot(np.asarray(R)), CAMERA_TRIANGLES.copy()
 
 
-def write_ply(path, vertices, colors=None, faces=None):
-    """A binary little-endian PLY file: vertices [m,3] as float x y z, colors [m,3] uint8 as uchar red green blue, faces
-    [k,3] as list uchar int vertex_indices.  The header is
+def write_ply(path, vertices, colors=None, faces=None, normals=None):
+    """A binary little-endian PLY file: vertices [m,3] as float x y z, normals [m,3] as float nx ny nz, colors [m,3] uint8
+    as uchar red green blue, faces [k,3] as list uchar int vertex_indices.  The header is
 
         ply
         format binary_little_endian 1.0
@@ -209,6 +209,9 @@ def write_ply(path, vertices, colors=None, faces=None):
         property float x
         property float y
         property float z
+        property float nx           (with normals)
+        property float ny
+        property float nz
         property uchar red          (with colours)
         property uchar green
         property uchar blue
@@ -219,10 +222,17 @@ def write_ply(path, vertices, colors=None, faces=None):
     followed by the m packed vertex records and the k face records (a count byte 3 and three int32 indices)."""
     v = np.asarray(vertices).reshape(-1, 3)
     fields = [('x', '<f4'), ('y', '<f4'), ('z', '<f4')]
+    if normals is not None:
+        fields += [('nx', '<f4'), ('ny', '<f4'), ('nz', '<f4')]
     if colors is not None:
         fields += [('red', 'u1'), ('green', 'u1'), ('blue', 'u1')]
     rec = np.empty(v.shape[0], dtype=np.dtype(fields))
     rec['x'], rec['y'], rec['z'] = v[:, 0], v[:, 1], v[:, 2]
+    if normals is not None:
+        nv = np.asarray(normals, dtype=np.float32).reshape(-1, 3)
+        if nv.shape[0] != v.shape[0]:
+            raise ValueError("%d normals for %d vertices" % (nv.shape[0], v.shape[0]))
+        rec['nx'], rec['ny'], rec['nz'] = nv[:, 0], nv[:, 1], nv[:, 2]
     if colors is not None:
         c = np.asarray(colors, dtype=np.uint8).reshape(-1, 3)
         if c.shape[0] != v.shape[0]:
@@ -230,6 +240,8 @@ def write_ply(path, vertices, colors=None, faces=None):
         rec['red'], rec['green'], rec['blue'] = c[:, 0], c[:, 1], c[:, 2]
     head = ["ply", "format binary_little_endian 1.0", "element vertex %d" % v.shape[0],
             "property float x", "property float y", "property float z"]
+    if normals is not None:
+        head += ["property float nx", "property float ny", "property float nz"]
     if colors is not None:
         head += ["property uchar red", "property uchar green", "property uchar blue"]
     frec = None

@@ -459,6 +459,64 @@ int demon_sparse_tsdf_mesh_range_f32(const float* tsdf, const float* weight, con
                                      int* faces, void* stream);
 
 /* ------------------------------------------------------------------------
+ * The indexed mesh (TsdfVolume.indexed_mesh, SparseTsdfVolume.indexed_mesh): marching cubes' surface with one vertex per
+ * edge instead of one per triangle corner.  Edge (g, a) runs from voxel g to g + e_a, a in {x, y, z}; in a sparse volume
+ * it belongs to the block that holds g.
+ *   1. Vertices: one for each edge that changes sign (tsdf < 0 at one end only) and lies in a cube that is not skipped
+ *      (all 8 corners stored with weight > 0), keyed by the edge, not by its position.  Its position and colour are the
+ *      soup's (demon_marching_cubes_f32) for that edge, bit for bit: mu = f0/(f0 - f1), p0 + mu (p1 - p0).
+ *   2. Order: dense, ascending 3 (linear index of g, x fastest) + a; sparse, ascending (packed key of g's block, local
+ *      linear index of g, a), whatever the pool's layout.
+ *   3. Faces [T,3] int32: the soup's triangles, each corner replaced by its edge's vertex index, winding kept.  Dense: the
+ *      soup's order.  Sparse: ascending block key, then the cube's local index, then the table's order.
+ *   4. Normals (world frame, towards increasing tsdf): with d_i(p) = f(p + e_i) - f(p - e_i) at p = g and p = g + e_a,
+ *      n_i = d_i(g) + mu (d_i(g + e_a) - d_i(g)), then n_i / sqrt((n_0 n_0 + n_1 n_1) + n_2 n_2).  NaN when any of the 10
+ *      other voxels it reads is not stored or has weight 0, or when the norm is 0.
+ *   5. Colour as the soup's, rounded half to even and clamped.
+ * Every step is one round-to-nearest float32 operation in the order written.  Faces are int32: callers refuse 2^31
+ * vertices or more (the counts are int64).  The work: every valid cube sets its edges' bits (atomicOr, so the masks do
+ * not depend on scheduling), a scan of the bit counts gives each 48-word segment (512 voxels of 3 edges: a block, or 512
+ * consecutive voxels of a dense box) its first vertex, and vertices and face corners find their index by popcount.
+ * ---------------------------------------------------------------------- */
+/* bytes of device scratch the dense indexed-mesh entries need (0 for an invalid volume) */
+int64_t demon_tsdf_indexed_mesh_scratch_bytes(int nx, int ny, int nz);
+/* Dense, step 1: marks the edges and counts: counts[0] = V vertices, counts[1] = T triangles (device int64 [2]). */
+int demon_tsdf_indexed_mesh_count_f32(const float* tsdf, const float* weight, int nx, int ny, int nz, void* scratch, int64_t* counts,
+                                      void* stream);
+/* Dense, step 2, on the scratch step 1 filled and the same volume: vertices [V,3] float32, normals [V,3] float32 (NULL: not
+ * computed), colors [V,3] uint8 (with color; NULL without), faces [T,3] int32. */
+int demon_tsdf_indexed_mesh_f32(const float* tsdf, const float* weight, const float* color, int nx, int ny, int nz, const float* origin,
+                                float voxel_size, const void* scratch, float* vertices, float* normals, uint8_t* colors, int* faces,
+                                void* stream);
+/* Sparse.  The caller holds, for all B blocks of the volume (on the device or not), masks uint32 [B,48] zeroed, base int32
+ * [B,48], and for the pool it works on a rank map: rank[b] = the key rank (0..B-1) of pool block b.  A pool may be the
+ * volume's own or a scratch pool of a chunk of blocks with their neighbours and its own table; the entries below work on
+ * its blocks first .. first+count-1 and resolve their neighbours among all m.  Scratch:
+ * demon_sparse_tsdf_mesh_scratch_bytes(count).
+ *   mark (every chunk), then scan (once: V into *vertices), then for every chunk range_count and range (vertices of the
+ *   chunk's blocks, wherever their rank puts them, and faces of its cubes).  Every triangle of a chunk's cubes uses edges
+ *   of its blocks and their +x, +y, +z neighbours; normals read all 26 neighbours. */
+int demon_sparse_tsdf_edge_mark_f32(const float* tsdf, const float* weight, const int* blocks, int m, int first, int count, const int64_t* keys,
+                                    const int* values, int64_t capacity, const int* rank, void* scratch, uint32_t* masks, void* stream);
+/* bytes of device scratch demon_sparse_tsdf_edge_scan needs for B >= 1 blocks */
+int64_t demon_sparse_tsdf_edge_scan_bytes(int blocks);
+/* The vertex count of the B blocks' masks into *vertices (device int64), and base: each mask word's first vertex. */
+int demon_sparse_tsdf_edge_scan(const uint32_t* masks, int blocks, void* scratch, int* base, int64_t* vertices, void* stream);
+/* demon_sparse_tsdf_mesh_range_count_f32 with the cubes enumerated block by block in order[0], order[1], ... (a
+ * permutation of first .. first+count-1; NULL: pool order), so the range entry writes faces in that order. */
+int demon_sparse_tsdf_indexed_mesh_range_count_f32(const float* tsdf, const float* weight, const int* blocks, int m, int first, int count,
+                                                   const int* order, const int64_t* keys, const int* values, int64_t capacity, void* scratch,
+                                                   int64_t* triangles, void* stream);
+/* On the scratch range_count filled: the vertices [V,3] (normals and colors as the dense entry) of the blocks first ..
+ * first+count-1 at their global indices (skipped with vertices NULL), and the faces of their cubes (skipped with faces NULL)
+ * from faces[0]. */
+int demon_sparse_tsdf_indexed_mesh_range_f32(const float* tsdf, const float* weight, const float* color, const int* blocks, int m, int first,
+                                             int count, const int* order, const int64_t* keys, const int* values, int64_t capacity,
+                                             const int* rank, const uint32_t* masks, const int* base, const float* origin, float voxel_size,
+                                             const void* scratch, float* vertices, float* normals, uint8_t* colors, int* faces,
+                                             void* stream);
+
+/* ------------------------------------------------------------------------
  * Streaming a sparse volume's blocks between the device and pinned host memory (SparseTsdfVolume's max_device_blocks).
  * A table value >= 0 is a pool index, -1 a block new in the running call, and -2 - s a block kept in host slot s; every
  * entry above reads a negative value as a block that is not stored.  Host slots hold tsdf and weight [8,8,8] float32 and
