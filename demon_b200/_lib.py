@@ -114,6 +114,11 @@ PROTOTYPES = {
     "demon_sparse_tsdf_edge_scan": [_P, c_int] + [_P] * 4,
     "demon_sparse_tsdf_indexed_mesh_range_count_f32": [_P] * 3 + [c_int] * 3 + [_P, _P, _P, c_int64, _P, _P, _P],
     "demon_sparse_tsdf_indexed_mesh_range_f32": [_P] * 4 + [c_int] * 3 + [_P, _P, _P, c_int64] + [_P] * 4 + [c_float] + [_P] * 6,
+    "demon_mesh_components_scratch_bytes": [c_int, c_int64],
+    "demon_mesh_components_count": [_P, c_int64, c_int, _P, _P, _P, _P],
+    "demon_mesh_component_sizes": [_P, c_int64, _P, c_int, c_int64, _P, _P, _P],
+    "demon_mesh_filter_count": [_P, c_int64, _P, c_int, _P, c_int64, _P, _P, _P, _P],
+    "demon_mesh_filter": [_P, c_int64, _P, c_int, _P, c_int64] + [_P] * 10,
     "demon_net_create": [ctypes.POINTER(c_void_p), c_int, c_int, c_int, c_int],
     "demon_net_destroy": [_P],
     "demon_net_set_weight": [_P, c_char_p, _P, _P, c_int],
@@ -182,6 +187,7 @@ _RESTYPES = {
     "demon_sparse_tsdf_raycast_scratch_bytes": c_int64,
     "demon_tsdf_indexed_mesh_scratch_bytes": c_int64,
     "demon_sparse_tsdf_edge_scan_bytes": c_int64,
+    "demon_mesh_components_scratch_bytes": c_int64,
     "demon_last_error": c_char_p,
     "demon_version": c_char_p,
     "demon_launch_count": c_int64,

@@ -10,7 +10,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_DIR = os.path.join(_HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libdemon_b200.so")
-SOURCES = ["geometry_ops.cu", "metrics.cu", "evaluation.cu", "training_ops.cu", "conv_simt.cu", "conv_tc_halo.cu", "images.cu", "vis.cu", "fusion.cu", "dataset_tools.cu",
+SOURCES = ["geometry_ops.cu", "metrics.cu", "evaluation.cu", "training_ops.cu", "conv_simt.cu", "conv_tc_halo.cu", "images.cu", "vis.cu", "fusion.cu", "mesh.cu", "dataset_tools.cu",
            "correlation.cu", "flow_ops.cu", "losses.cu", "datareader.cu", "net.cu"]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17",

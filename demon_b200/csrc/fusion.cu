@@ -16,6 +16,7 @@
 // Every float operation is a round-to-nearest intrinsic in the order the comments give (no contraction into FMAs), so a
 // float32 numpy restatement matches bit for bit.
 #include "common.cuh"
+#include "tile_scan.cuh"
 #include <climits>
 #include <cmath>
 #include <cstdint>
@@ -30,7 +31,6 @@ constexpr int kMcThreads = 256;
 constexpr int kMcWarps = kMcThreads / 32;
 constexpr int kMcRounds = 8;
 constexpr int kMcTile = kMcThreads * kMcRounds;   // round j of thread i handles cube tile * kMcTile + j * kMcThreads + i
-constexpr int kScanThreads = 1024;
 constexpr int kSegWords = 48;   // the indexed mesh's segment of mask words: 8 * 8 * 8 voxels of 3 edges
 constexpr int kSegBits = 32 * kSegWords;
 
@@ -630,33 +630,6 @@ __global__ void __launch_bounds__(kMcThreads) mc_count_kernel(V vol, int* __rest
   }
 }
 
-// One CTA: tile_first[t] = the triangles of tiles 0..t-1, and *total = all of them.
-__global__ void __launch_bounds__(kScanThreads) mc_offsets_kernel(const int* __restrict__ tile_counts, int tiles,
-                                                                  int64_t* __restrict__ tile_first, int64_t* __restrict__ total) {
-  __shared__ int64_t s_sum[kScanThreads];
-  const int seg = (tiles + kScanThreads - 1) / kScanThreads;
-  const int b = threadIdx.x * seg, e = min(tiles, b + seg);
-  int64_t s = 0;
-  for (int q = b; q < e; ++q) s += tile_counts[q];
-  s_sum[threadIdx.x] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {   // 1024 additions: not worth a tree
-    int64_t run = 0;
-    for (int q = 0; q < kScanThreads; ++q) {
-      const int64_t v = s_sum[q];
-      s_sum[q] = run;
-      run += v;
-    }
-    *total = run;
-  }
-  __syncthreads();
-  int64_t run = s_sum[threadIdx.x];
-  for (int q = b; q < e; ++q) {
-    tile_first[q] = run;
-    run += tile_counts[q];
-  }
-}
-
 // The soup's output: corner e3 of triangle tri gets its own vertex 3 tri + e3, interpolated on the edge.
 template <bool kColor>
 struct SoupOut {
@@ -743,7 +716,7 @@ void launch_soup(const V& vol, int tiles, const float* color, const float* origi
 //   1. edge_mark_kernel: every valid cube ORs the bits of its sign-changing edges (the edges its triangles use).  The
 //      owner of a cube's edge is the cube's block or one of its +x, +y, +z neighbours; OR is order-free, so the masks
 //      depend on the volume alone.
-//   2. edge_count_kernel, mc_offsets_kernel, edge_base_kernel: each segment's popcount, their exclusive scan (the
+//   2. edge_count_kernel, tile_offsets_kernel, edge_base_kernel: each segment's popcount, their exclusive scan (the
 //      segment's first vertex), and each word's first vertex (the segment's plus the popcounts of the words before it).
 //   3. edge_vertex_kernel: one thread per word writes the vertex of each of its set bits at base[word] + popcount of the
 //      bits below it.  mc_scatter_kernel with IndexOut writes each triangle corner's edge index the same way.
@@ -1603,7 +1576,7 @@ int sparse_range_count(const char* name, const float* tsdf, const float* weight,
   else
     mc_count_kernel<<<tiles, kMcThreads, 0, st>>>(vol, tile_counts);
   DEMON_LAUNCH_CHECK();
-  mc_offsets_kernel<<<1, kScanThreads, 0, st>>>(tile_counts, tiles, tile_first, triangles);
+  tile_offsets_kernel<<<1, kScanThreads, 0, st>>>(tile_counts, tiles, tile_first, triangles);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
 }
@@ -1616,7 +1589,7 @@ int edge_scan(const unsigned* masks, int segs, void* scratch, int* base, int64_t
   const unsigned grid = (unsigned)ceil_div64(32LL * segs, kEdgeThreads);
   edge_count_kernel<<<grid, kEdgeThreads, 0, st>>>(masks, segs, counts);
   DEMON_LAUNCH_CHECK();
-  mc_offsets_kernel<<<1, kScanThreads, 0, st>>>(counts, segs, seg_first, vertices);
+  tile_offsets_kernel<<<1, kScanThreads, 0, st>>>(counts, segs, seg_first, vertices);
   DEMON_LAUNCH_CHECK();
   edge_base_kernel<<<grid, kEdgeThreads, 0, st>>>(masks, segs, seg_first, base);
   DEMON_LAUNCH_CHECK();
@@ -1705,7 +1678,7 @@ int demon_marching_cubes_count_f32(const float* tsdf, const float* weight, int n
   int* tile_counts = reinterpret_cast<int*>(tile_first + tiles);
   mc_count_kernel<<<tiles, kMcThreads, 0, (cudaStream_t)stream>>>(make_volume(tsdf, weight, nx, ny, nz), tile_counts);
   DEMON_LAUNCH_CHECK();
-  mc_offsets_kernel<<<1, kScanThreads, 0, (cudaStream_t)stream>>>(tile_counts, tiles, tile_first, triangles);
+  tile_offsets_kernel<<<1, kScanThreads, 0, (cudaStream_t)stream>>>(tile_counts, tiles, tile_first, triangles);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
 }
@@ -2003,7 +1976,7 @@ int demon_tsdf_indexed_mesh_count_f32(const float* tsdf, const float* weight, in
   if (int rc = edge_scan(sc.masks, (int)segs, sc.scan, sc.base, counts, st)) return rc;
   mc_count_kernel<<<tiles, kMcThreads, 0, st>>>(vol, sc.tile_counts);
   DEMON_LAUNCH_CHECK();
-  mc_offsets_kernel<<<1, kScanThreads, 0, st>>>(sc.tile_counts, tiles, sc.tile_first, counts + 1);
+  tile_offsets_kernel<<<1, kScanThreads, 0, st>>>(sc.tile_counts, tiles, sc.tile_first, counts + 1);
   DEMON_LAUNCH_CHECK();
   return DEMON_OK;
 }

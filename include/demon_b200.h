@@ -558,6 +558,45 @@ int demon_sparse_tsdf_restore(const float* host_tsdf, const float* host_weight, 
 int demon_sparse_tsdf_index(int64_t* keys, int* values, int64_t capacity, const int* blocks, int first, int count, void* stream);
 
 /* ------------------------------------------------------------------------
+ * Connected components of an indexed mesh, and the removal of the small ones (demon_b200.mesh; csrc/mesh.cu).  The mesh
+ * is V vertices and faces [F,3] int32 with every index in [0, V) (the caller checks this: an index outside it is
+ * undefined behaviour); degenerate faces are allowed.
+ *   1. Connectivity: two vertices are connected when some face contains both, and a component is a class of that
+ *      relation.  It is by index, not by position: coincident vertices stay apart.  A vertex no face uses is a component
+ *      of its own with 0 triangles.
+ *   2. Labels: the components are numbered 0 .. C-1 in ascending order of their smallest vertex index (so vertex 0 is in
+ *      component 0); labels [V] int32 is each vertex's, and a face's is labels[faces[f,0]].  They depend on the faces
+ *      alone, never on scheduling.
+ *   3. Sizes: triangles [C] and vertices [C] int64 count each component's faces and vertices.
+ *   4. Selection: component c is kept when triangles[c] >= min_triangles and, with a selection select [C] uint8 (NULL:
+ *      every component), select[c] != 0.
+ *   5. Filter: the kept vertices in ascending original index, with their vertices, normals and colours copied bit for bit,
+ *      and the kept faces in their original order, each index replaced by its vertex's new index: a boolean-mask
+ *      compaction.
+ * The work: a lock-free union-find (one thread per face, atomicCAS hooking the larger root under the smaller, so a
+ * tree's root is its smallest vertex), a tile scan of the roots for the labels, integer atomics for the sizes, and tile
+ * scans of the kept vertices and faces for the filter.  All four entries take the same scratch.
+ * ---------------------------------------------------------------------- */
+/* bytes of device scratch the entries below need for V vertices and F faces (0 for invalid sizes) */
+int64_t demon_mesh_components_scratch_bytes(int num_vertices, int64_t num_faces);
+/* labels [V] int32 (rule 2) and the component count C into *components (device int64). */
+int demon_mesh_components_count(const int* faces, int64_t num_faces, int num_vertices, void* scratch, int* labels, int64_t* components,
+                                void* stream);
+/* triangles [C] and vertices [C] int64 (rule 3) from the labels of demon_mesh_components_count and its count C. */
+int demon_mesh_component_sizes(const int* faces, int64_t num_faces, const int* labels, int num_vertices, int64_t components,
+                               int64_t* triangles, int64_t* vertices, void* stream);
+/* The filter, step 1: counts[0] = the kept vertices, counts[1] = the kept faces (device int64 [2]), by rule 4 from the
+ * labels and triangle counts above. */
+int demon_mesh_filter_count(const int* faces, int64_t num_faces, const int* labels, int num_vertices, const int64_t* triangles,
+                            int64_t min_triangles, const uint8_t* select, void* scratch, int64_t* counts, void* stream);
+/* The filter, step 2, on the scratch step 1 filled and the same arguments: out_vertices [V',3] float32, out_normals
+ * [V',3] float32 (with normals [V,3]; NULL with NULL), out_colors [V',3] uint8 (with colors [V,3]; NULL with NULL) and
+ * out_faces [F',3] int32 (rule 5; NULL when F' = 0). */
+int demon_mesh_filter(const int* faces, int64_t num_faces, const int* labels, int num_vertices, const int64_t* triangles,
+                      int64_t min_triangles, const uint8_t* select, void* scratch, const float* vertices, const float* normals,
+                      const uint8_t* colors, float* out_vertices, float* out_normals, uint8_t* out_colors, int* out_faces, void* stream);
+
+/* ------------------------------------------------------------------------
  * Image input (examples/example.py:15-42 resizes every image with PIL.Image.resize).
  * ---------------------------------------------------------------------- */
 /* resample filters, with Pillow's enum values (PIL.Image.Resampling) */
